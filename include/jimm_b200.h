@@ -150,7 +150,9 @@ JIMM_API int jimm_comm_status(jimm_model_t* m);
 JIMM_API int jimm_comm_gathered(jimm_model_t* m, float** gathered, int* row_stride);
 
 /* -- per-kernel entry points (device pointers; used by tests/ so every kernel is individually
- *    parity- and profile-testable; SURVEY.md 8b) ------------------------------------------------------------------- */
+ *    parity- and profile-testable; SURVEY.md 8b) -------------------------------------------------------------------
+ * Type codes of these entry points: 0 fp32 | 1 fp16 | 2 bf16 | 3 fp32 rounded to tf32 (round to nearest, ties away from zero;
+ * the operand format of the fp32 compute mode).  Here 3 is NOT JIMM_I32. */
 /* C[M,N] = epi(A[M,K] . B[N,K]^T): impl 0 = wgmma/TMA kernel, 1 = SIMT cross-check.
  * act: 0 none | 1 gelu_tanh | 2 quick_gelu; epi_mode 0 / 1 LSU stores | 2 TMA stores; rows_in>0 remaps output rows. */
 JIMM_API int jimm_k_gemm(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
@@ -162,11 +164,27 @@ JIMM_API int jimm_k_gemm(int impl, int dtype, const void* A, int lda, const void
 JIMM_API int jimm_k_gemm_residual_ln(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, float* x, int ldx,
                             const float* ln_scale, const float* ln_bias, float eps, void* ln_out, int ln_out_type, int ln_ldo, int* counters,
                             void* stream);
+/* Both of the above, as the forward pass runs the GEMM (the two are this call with the extra arguments at their defaults):
+ *   plan_M (0 = M): the rows the plan (its tensor maps) is built for; M <= plan_M rows are run.  With M < plan_M the TMA epilogues
+ *     (epi_mode 2) may write rows [M, roundup(M, 16)) of the output; rows >= roundup(M, 16) are never written.
+ *   reverse: walk the tiles from the last one (same result).
+ *   tok_pad > 0: token scatter of the patch embedding: A row b * tok_pad + p is reduce-added into out[b, p + tok_off, :] of an fp32
+ *     [M / tok_pad, tok_S, N] tensor (residual == out, epi_mode 2, tok_pad a multiple of 16 dividing M and plan_M); rows
+ *     p + tok_off >= tok_S are dropped.
+ *   ln_counters != NULL: fused LayerNorm of jimm_k_gemm_residual_ln (ln_* arguments as there; needs the fp32 reduce-add). */
+JIMM_API int jimm_k_gemm_ex(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
+                            const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
+                            int row_off, int epi_mode, int plan_M, int reverse, int tok_pad, int tok_off, int tok_S, const float* ln_scale,
+                            const float* ln_bias, float ln_eps, void* ln_out, int ln_out_type, int ln_ldo, int* ln_counters, void* stream);
 JIMM_API int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream);
 JIMM_API int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, void* stream);
 JIMM_API int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
+/* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left
+ * untouched) and ldk (row stride in elements, 0 = P*P*C; more = pad columns, written as zeros). */
+JIMM_API int jimm_k_patchify_ex(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, int rows_per_sample,
+                                int ldk, void* stream);
 /* y = act(x) elementwise on device fp32 (act: 1 tanh-GELU == nnx.gelu, 2 QuickGELU == common/transformer.py:12-19). */
 JIMM_API int jimm_k_activation(const float* x, float* y, long long n, int act, void* stream);
 JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream);

@@ -80,10 +80,13 @@ SIGNATURES = {
     "jimm_profile_end": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_longlong)]),
     "jimm_k_gemm": (_i, [_i, _i, _vp, _i, _vp, _i, _i, _i, _i, _fp, _i, _fp, _fp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_gemm_residual_ln": (_i, [_i, _vp, _i, _vp, _i, _i, _i, _i, _fp, _fp, _i, _fp, _fp, _f, _vp, _i, _i, _ip, _vp]),
+    "jimm_k_gemm_ex": (_i, [_i, _i, _vp, _i, _vp, _i, _i, _i, _i, _fp, _i, _fp, _fp, _i, _vp, _i, _i, _i, _i, _i, _i,
+                            _i, _i, _i, _i, _i, _fp, _fp, _f, _vp, _i, _i, _ip, _vp]),
     "jimm_k_layernorm": (_i, [_fp, _i, _i, _i, _ip, _fp, _fp, _f, _vp, _i, _i, _i, _i, _vp]),
     "jimm_k_attention": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
+    "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),

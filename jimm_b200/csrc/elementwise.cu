@@ -209,6 +209,10 @@ int patchify_run(const void* img, int in_type, int B, int H, int W, int C, int P
   const int PPC = P * P * C;
   if (ldk <= 0) ldk = PPC;
   if (ldk < PPC) { set_last_error("patchify: row stride %d < patch_size^2*channels %d", ldk, PPC); return -1; }
+  if (rows_per_sample != 0 && rows_per_sample < (H / P) * (W / P)) {
+    set_last_error("patchify: rows_per_sample %d < patches per image %d", rows_per_sample, (H / P) * (W / P));
+    return -1;
+  }
   if ((P * C) % 4 != 0 || (W * C) % 4 != 0 || ldk != PPC) {
     if (in_type == DT_F32) return patchify_generic_dispatch<float>(img, B, H, W, C, P, out, out_type, stream, rows_per_sample, ldk);
     if (in_type == DT_F16) return patchify_generic_dispatch<__half>(img, B, H, W, C, P, out, out_type, stream, rows_per_sample, ldk);

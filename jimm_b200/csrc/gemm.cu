@@ -604,25 +604,42 @@ int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void
                    const GemmEpilogue& epi) {
   if (M <= 0 || N <= 0 || K <= 0) { set_last_error("gemm: bad shape %dx%dx%d", M, N, K); return -1; }
   if (int rc = check_epi(epi, N)) return rc;
+  // the token scatter exists only as the TMA reduce-add: every other epilogue would ignore tok_* and write the plain row layout
+  if (epi.tok_pad != 0) {
+    if (epi.tok_pad < 0 || epi.tok_pad % EPI_BOX_ROWS != 0 || M % epi.tok_pad != 0 || epi.tok_off < 0 || epi.tok_S <= 0) {
+      set_last_error("gemm: token scatter needs tok_pad a positive multiple of %d dividing M (tok_pad=%d M=%d tok_off=%d tok_S=%d)", EPI_BOX_ROWS,
+                     epi.tok_pad, M, epi.tok_off, epi.tok_S);
+      return -1;
+    }
+    if (epi.residual != epi.out || epi.ldr != epi.ldo || epi.out_type != DT_F32) {
+      set_last_error("gemm: token scatter reduce-adds into an fp32 output that is also the residual");
+      return -1;
+    }
+  }
   if (int rc = make_map(&plan->map_a, dtype, A, M, K, lda, BM)) return rc;
   if (int rc = make_map(&plan->map_b, dtype, B, N, K, ldb, BN)) return rc;
   plan->M = M; plan->N = N; plan->K = K; plan->dtype = dtype; plan->epi = epi;
   memset(&plan->map_c, 0, sizeof(plan->map_c));
   if (plan->epi.mode == 2) {
     const size_t es = dtype_size(epi.out_type);
-    const bool ok = epi.rowadd == nullptr && epi.rows_in == 0 &&
+    // N * es % 16: where a row ends inside a 16-byte chunk, the TMA store wrote columns past N (fp16 / bf16 output, N = 2300,
+    // ldo = 2320, on an H100); with ldo > N they belong to the caller.  Such N take the LSU epilogue.
+    const bool ok = epi.rowadd == nullptr && epi.rows_in == 0 && (static_cast<size_t>(N) * es) % 16 == 0 &&
                     (epi.residual == nullptr || (epi.residual == epi.out && epi.ldr == epi.ldo && epi.out_type == DT_F32)) &&
                     (static_cast<size_t>(epi.ldo) * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(epi.out) & 15) == 0 &&
                     (epi.bias == nullptr || ((reinterpret_cast<uintptr_t>(epi.bias) & 15) == 0 && N % 4 == 0)) &&
                     !(epi.residual && epi.act != ACT_NONE);
     if (ok && epi.tok_pad > 0) {
-      if (epi.tok_pad % EPI_BOX_ROWS != 0 || M % epi.tok_pad != 0 || !epi.residual) { set_last_error("gemm: bad token-scatter epilogue"); return -1; }
       if (int rc = make_map_3d_f32(&plan->map_c, epi.out, M / epi.tok_pad, epi.tok_S, N, epi.ldo)) return rc;
     } else if (ok) {
       if (int rc = make_map(&plan->map_c, epi.out_type, epi.out, M, N, epi.ldo, EPI_BOX_ROWS)) return rc;
     } else {
       plan->epi.mode = 0;
     }
+  }
+  if (epi.tok_pad > 0 && plan->epi.mode != 2) {
+    set_last_error("gemm: the token scatter needs the TMA epilogue (mode 2, no activation, 16-byte aligned output / bias, N %% 4 == 0)");
+    return -1;
   }
   return 0;
 }
@@ -687,6 +704,10 @@ int gemm_fuses_ln(const GemmPlan* p, int /*M_override: any row count*/) {
 
 int gemm_plan_run(const GemmPlan* p0, int M_override, cudaStream_t stream, int reverse) {
   const int M = (M_override > 0 && M_override <= p0->M) ? M_override : p0->M;
+  if (p0->epi.tok_pad > 0 && M % p0->epi.tok_pad != 0) {
+    set_last_error("gemm: token scatter runs whole samples (M=%d, tok_pad=%d)", M, p0->epi.tok_pad);
+    return -1;
+  }
   GemmPlan local;
   const GemmPlan* p = p0;
   if (reverse != p0->epi.reverse) { local = *p0; local.epi.reverse = reverse; p = &local; }

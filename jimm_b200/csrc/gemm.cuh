@@ -30,13 +30,14 @@ struct GemmEpilogue {
   int out_type = DT_F32;
   int ldo = 0;                                   // output row stride (elements)
   // Token-scatter form of the fp32 reduce-add epilogue (patch embedding): A rows are (sample, padded patch index) with
-  // tok_pad rows per sample (multiple of 32); row (b, p) is ADDED to out[b, p + tok_off, :] of a [B, tok_S, N] tensor through a
-  // 3-D tensor map (rows p + tok_off >= tok_S are clipped by TMA).  Requires residual == out (pre-initialised with pos-emb).
+  // tok_pad rows per sample (multiple of 16, dividing M); row (b, p) is ADDED to out[b, p + tok_off, :] of a [B, tok_S, N] tensor through a
+  // 3-D tensor map (rows p + tok_off >= tok_S are clipped by TMA, so the pad rows p >= tok_S - tok_off of A are never added).
+  // Requires residual == out, fp32 (pre-initialised with pos-emb), and the TMA epilogue: gemm_plan_init fails otherwise.
   int tok_pad = 0, tok_off = 0, tok_S = 0;
   int reverse = 0;  // walk the M tiles from the end (L2-resident part of the A operand first; see kernels.cuh)
   int rows_in = 0, rows_out = 0, row_off = 0;    // out_row = (r / rows_in) * rows_out + r % rows_in + row_off (rows_in == 0: identity)
   // 2: TMA epilogue (swizzled smem box -> cp.async.bulk.tensor store, cp.reduce .add for the fp32 residual stream; needs
-  //    no rowadd / row remap and residual == out) -- falls back to 0 when not applicable;
+  //    no rowadd / row remap and residual == out, 16-byte aligned out / ldo and N x element size) -- falls back to 0 when not applicable;
   // 0 / 1: LSU stores straight from the accumulator registers (any shape, row remap, row-add, residual read)
   int mode = 2;
   // Fused LayerNorm of the UPDATED residual rows (fp32 reduce-add epilogue only): when the last column tile of a 32-row group has
@@ -63,7 +64,13 @@ struct GemmPlan {
 // Returns 0 or a negative status (message in jimm_last_error()).
 int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K,
                    const GemmEpilogue& epi);
-// Enqueue on `stream`; M may be overridden (<= planned M) to run on fewer rows of the same buffers.
+// Enqueue on `stream`; M may be overridden (<= planned M) to run on fewer rows of the same buffers.  Rows < M are the same bits a
+// plan built for exactly M rows gives.  The tensor maps still span the planned rows, so with M < planned M:
+//   - the generic epilogue (mode 0 / 1) writes no row >= M;
+//   - the TMA epilogues (mode 2) store / reduce-add whole 16-row boxes: rows [M, roundup(M, 16)) of the output (the residual
+//     stream for the reduce-add) receive values computed from whatever A holds there; rows >= roundup(M, 16) are never written.
+//     A token-scatter plan runs whole samples (M % tok_pad == 0), so its boxes never pass M.
+//   - the fused LayerNorm normalises rows < M only.
 int gemm_plan_run(const GemmPlan* plan, int M_override, cudaStream_t stream, int reverse = 0);
 
 // Simple SIMT reference GEMM (debug / bring-up cross-check on the GPU; never on the product path

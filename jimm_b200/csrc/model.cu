@@ -1452,29 +1452,49 @@ int jimm_profile_end(jimm_model_t* m, double* gemm_ms, double* gemm_flops, long 
 }
 
 // ---- per-kernel entry points ----
-int jimm_k_gemm(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
-                const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
-                int row_off, int epi_mode, void* stream) {
+int jimm_k_gemm_ex(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
+                   const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
+                   int row_off, int epi_mode, int plan_M, int reverse, int tok_pad, int tok_off, int tok_S, const float* ln_scale,
+                   const float* ln_bias, float ln_eps, void* ln_out, int ln_out_type, int ln_ldo, int* ln_counters, void* stream) {
+  if (plan_M <= 0) plan_M = M;
+  if (M <= 0 || M > plan_M) { set_last_error("jimm_k_gemm_ex: need 0 < M <= plan_M (M=%d plan_M=%d)", M, plan_M); return JIMM_EINVAL; }
   GemmEpilogue e;
   e.bias = bias; e.act = act; e.rowadd = rowadd; e.residual = residual; e.ldr = ldr; e.out = out; e.out_type = out_type; e.ldo = ldo;
   e.rows_in = rows_in; e.rows_out = rows_out; e.row_off = row_off; e.mode = epi_mode;
+  e.tok_pad = tok_pad; e.tok_off = tok_off; e.tok_S = tok_S;
+  if (ln_counters) {  // fp32 operands: the normalised rows are the next GEMM's tf32 operand
+    e.ln_scale = ln_scale; e.ln_bias = ln_bias; e.ln_out = ln_out; e.ln_out_type = ln_out_type == JIMM_F32 ? DT_TF32 : ln_out_type; e.ln_ldo = ln_ldo;
+    e.ln_eps = ln_eps; e.ln_cnt = ln_counters;
+  }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (impl == 1) return gemm_simt_run(dtype, A, lda, B, ldb, M, N, K, e, s);
+  if (impl == 1) {
+    if (plan_M != M || reverse || tok_pad || ln_counters) {
+      set_last_error("jimm_k_gemm_ex: the SIMT GEMM has no plan rows, reverse walk, token scatter or fused LayerNorm");
+      return JIMM_EINVAL;
+    }
+    return gemm_simt_run(dtype, A, lda, B, ldb, M, N, K, e, s);
+  }
   GemmPlan p;
-  JIMM_TRY(gemm_plan_init(&p, dtype, A, lda, B, ldb, M, N, K, e));
-  return gemm_plan_run(&p, M, s);
+  JIMM_TRY(gemm_plan_init(&p, dtype, A, lda, B, ldb, plan_M, N, K, e));
+  if (ln_counters && !gemm_fuses_ln(&p, M)) {
+    set_last_error("gemm: this shape does not take the fused LayerNorm path (needs N = 128 x {1,2,3,4,6,8,9,10,12}, aligned operands, "
+                   "LayerNorm output in the operand type)");
+    return JIMM_EINVAL;
+  }
+  return gemm_plan_run(&p, M, s, reverse);
+}
+int jimm_k_gemm(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
+                const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
+                int row_off, int epi_mode, void* stream) {
+  return jimm_k_gemm_ex(impl, dtype, A, lda, B, ldb, M, N, K, bias, act, rowadd, residual, ldr, out, out_type, ldo, rows_in, rows_out, row_off,
+                        epi_mode, M, 0, 0, 0, 0, nullptr, nullptr, 0.f, nullptr, 0, 0, nullptr, stream);
 }
 int jimm_k_gemm_residual_ln(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, float* x, int ldx,
                             const float* ln_scale, const float* ln_bias, float eps, void* ln_out, int ln_out_type, int ln_ldo, int* counters,
                             void* stream) {
-  GemmEpilogue e;
-  e.bias = bias; e.residual = x; e.ldr = ldx; e.out = x; e.out_type = DT_F32; e.ldo = ldx; e.mode = 2;
-  e.ln_scale = ln_scale; e.ln_bias = ln_bias; e.ln_out = ln_out; e.ln_out_type = ln_out_type == JIMM_F32 ? DT_TF32 : ln_out_type; e.ln_ldo = ln_ldo;
-  e.ln_eps = eps; e.ln_cnt = counters;
-  GemmPlan p;
-  JIMM_TRY(gemm_plan_init(&p, dtype, A, lda, B, ldb, M, N, K, e));
-  if (!gemm_fuses_ln(&p, M)) { set_last_error("jimm_k_gemm_residual_ln: this shape does not take the fused path (needs N = 128 x {1,2,3,4,6,8,9,10,12}, aligned operands)"); return JIMM_EINVAL; }
-  return gemm_plan_run(&p, M, static_cast<cudaStream_t>(stream));
+  if (!counters) { set_last_error("jimm_k_gemm_residual_ln: null counters"); return JIMM_EINVAL; }
+  return jimm_k_gemm_ex(0, dtype, A, lda, B, ldb, M, N, K, bias, 0, nullptr, x, ldx, x, JIMM_F32, ldx, 0, 0, 0, 2, M, 0, 0, 0, 0, ln_scale,
+                        ln_bias, eps, ln_out, ln_out_type, ln_ldo, counters, stream);
 }
 int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream) {
@@ -1486,8 +1506,12 @@ int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int 
 int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
   return map_attention_run(q, kv, io_type, out, out_type, B, S, H, static_cast<cudaStream_t>(stream));
 }
+int jimm_k_patchify_ex(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, int rows_per_sample, int ldk,
+                       void* stream) {
+  return patchify_run(img, in_type, B, H, W, C, P, out, out_type, static_cast<cudaStream_t>(stream), rows_per_sample, ldk);
+}
 int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream) {
-  return patchify_run(img, in_type, B, H, W, C, P, out, out_type, static_cast<cudaStream_t>(stream));
+  return jimm_k_patchify_ex(img, in_type, B, H, W, C, P, out, out_type, 0, 0, stream);
 }
 int jimm_k_activation(const float* x, float* y, long long n, int act, void* stream) {
   if (n < 0 || (n > 0 && (!x || !y))) { set_last_error("jimm_k_activation: bad arguments"); return JIMM_EINVAL; }
