@@ -179,6 +179,12 @@ JIMM_API int jimm_k_gemm_ex(int impl, int dtype, const void* A, int lda, const v
 JIMM_API int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream);
 JIMM_API int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, void* stream);
+/* jimm_k_layernorm / jimm_k_attention as the encoder runs them (each of the two is its _ex call with reverse = 0):
+ *   reverse: walk the rows (LayerNorm) or the samples (attention) from the last one; the result is the same, bit for bit. */
+JIMM_API int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
+                                 float eps, void* out, int out_type, int ldy, int rows, int D, int reverse, void* stream);
+JIMM_API int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse,
+                                 void* stream);
 JIMM_API int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
 /* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left

@@ -84,6 +84,8 @@ SIGNATURES = {
                             _i, _i, _i, _i, _i, _fp, _fp, _f, _vp, _i, _i, _ip, _vp]),
     "jimm_k_layernorm": (_i, [_fp, _i, _i, _i, _ip, _fp, _fp, _f, _vp, _i, _i, _i, _i, _vp]),
     "jimm_k_attention": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_layernorm_ex": (_i, [_fp, _i, _i, _i, _ip, _fp, _fp, _f, _vp, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_attention_ex": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),

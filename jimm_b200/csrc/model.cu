@@ -1496,12 +1496,19 @@ int jimm_k_gemm_residual_ln(int dtype, const void* A, int lda, const void* B, in
   return jimm_k_gemm_ex(0, dtype, A, lda, B, ldb, M, N, K, bias, 0, nullptr, x, ldx, x, JIMM_F32, ldx, 0, 0, 0, 2, M, 0, 0, 0, 0, ln_scale,
                         ln_bias, eps, ln_out, ln_out_type, ln_ldo, counters, stream);
 }
+int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
+                        float eps, void* out, int out_type, int ldy, int rows, int D, int reverse, void* stream) {
+  return layernorm_run(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, static_cast<cudaStream_t>(stream), reverse);
+}
 int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream) {
-  return layernorm_run(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, static_cast<cudaStream_t>(stream));
+  return jimm_k_layernorm_ex(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, 0, stream);
+}
+int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse, void* stream) {
+  return attention_run(qkv, io_type, out, out_type, B, S, H, causal, static_cast<cudaStream_t>(stream), reverse);
 }
 int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, void* stream) {
-  return attention_run(qkv, io_type, out, out_type, B, S, H, causal, static_cast<cudaStream_t>(stream));
+  return jimm_k_attention_ex(qkv, io_type, out, out_type, B, S, H, causal, 0, stream);
 }
 int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
   return map_attention_run(q, kv, io_type, out, out_type, B, S, H, static_cast<cudaStream_t>(stream));
