@@ -186,6 +186,12 @@ JIMM_API int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off
 JIMM_API int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse,
                                  void* stream);
 JIMM_API int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream);
+/* jimm_k_attention_ex / jimm_k_map_attention for heads of head_dim columns (D = H * head_dim; the two are these calls with
+ * head_dim = 64).  head_dim: a multiple of 8 from 8 to 128.  Softmax scale 1 / sqrt(head_dim). */
+JIMM_API int jimm_k_attention_hd(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal,
+                                 int reverse, void* stream);
+JIMM_API int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim,
+                                     void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
 /* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left
  * untouched) and ldk (row stride in elements, 0 = P*P*C; more = pad columns, written as zeros). */

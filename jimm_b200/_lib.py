@@ -87,6 +87,8 @@ SIGNATURES = {
     "jimm_k_layernorm_ex": (_i, [_fp, _i, _i, _i, _ip, _fp, _fp, _f, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_attention_ex": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _vp]),
+    "jimm_k_attention_hd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_map_attention_hd": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),

@@ -1,14 +1,17 @@
 // Softmax attention kernels (SURVEY.md 8a row a5, a9).
 //
-// attention_kernel: flash-style fused softmax(q k^T / sqrt(d)) v over the fused qkv buffer, head_dim 64 (every
-// jimm config: vision heads = width // 64, models/clip.py:60, models/siglip.py:59).  One CTA = one warpgroup = 64 query
-// rows of one (sample, head); warp w owns rows 16 w .. 16 w + 15; K/V streamed in 64-key tiles through a double-buffered
-// cp.async ring.  Every tile is 64 rows x 128 B in the 128-byte-swizzle layout, so the tensor cores read it in place:
-// S = Q K^T is wgmma m64n64k16 with both operands in shared memory (K-major), O += P V is wgmma with P straight from the
-// score registers (A fragment) and V in shared memory (MN-major).  Scores and probabilities never leave registers; fp32
-// online softmax with warp-quad shuffles.
+// attention_kernel: flash-style fused softmax(q k^T / sqrt(d)) v over the fused qkv buffer, for any head width d that is a
+// multiple of 8 up to 128 (64 in the CLIP / SigLIP vision towers, models/clip.py:60, models/siglip.py:59; 72 in the SigLIP
+// so400m text tower, 80 in ViT-H/14, 16 in small ViTs).  One CTA = one warpgroup = 64 query rows of one (sample, head); warp w
+// owns rows 16 w .. 16 w + 15; K/V streamed in 64-key tiles through a double-buffered cp.async ring.  The kernel is compiled for
+// a padded width DP (padded_head_dim: 16, 32, 64, 80, 96, 128); every tile is 64 rows x DP columns in a swizzled layout
+// (HeadTile), with columns d .. DP-1 zero-filled, so the tensor cores read it in place: S = Q K^T is wgmma m64n64k16 with both
+// operands in shared memory (K-major), O += P V is wgmma m64nDPk16 with P straight from the score registers (A fragment) and V
+// in shared memory (MN-major).  Scores and probabilities never leave registers; fp32 online softmax with warp-quad shuffles.
 //
-// map_attention_kernel: MAP-head pooling attention with a single precomputed probe query (common/vit.py:96-97).
+// map_attention_kernel: MAP-head pooling attention with a single precomputed probe query (common/vit.py:96-97), any head
+// width the flash kernel takes.
+#include <cmath>
 #include <type_traits>
 
 #include "common.cuh"
@@ -16,9 +19,6 @@
 
 namespace jimm {
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src));
-}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N)); }
@@ -36,54 +36,102 @@ __device__ __forceinline__ uint32_t pack_pair(float a, float b) {
 
 static constexpr int QT = 64;   // query rows per CTA
 static constexpr int KT = 64;   // keys per pipeline stage
-static constexpr int HD = 64;   // head dim
 
-// Copy a 64-row x 128-byte tile (rows s0.. of one head; row stride `ld` elements) into swizzled smem; rows >= S are
-// clamped to S-1 (their scores are masked / their outputs are never stored).
-template <typename T>
-__device__ __forceinline__ void load_tile(uint32_t smem_base, const T* __restrict__ gbase, size_t ld, int s0, int S, int tid) {
+// Shared-memory layout of a 64-row tile of one head, padded to DP columns (DP a multiple of 16).  A row is 2 DP bytes, split into
+// NB column blocks of SW bytes (SW = 128, 64 or 32: the widest swizzle that divides the row).  Block b holds columns
+// [b SW / 2, (b + 1) SW / 2) of all 64 rows, SW bytes per row, in the SW-byte swizzle layout; blocks are 64 SW bytes apart.
+// DP = 64 is one 128-byte-swizzled block of 64 x 128 B.
+template <int DP>
+struct HeadTile {
+  static_assert(DP % 16 == 0 && DP >= 16 && DP <= 128, "padded head width");
+  static constexpr int ROWB = DP * 2;
+  static constexpr int SW = ROWB % 128 == 0 ? 128 : ROWB % 64 == 0 ? 64 : 32;
+  static constexpr int NB = ROWB / SW;
+  static constexpr int CH = SW / 16;        // 16-byte chunks per block row
+  static constexpr int NCH = DP / 8;        // 16-byte chunks per row
+  static constexpr int BYTES = QT * ROWB;   // QT == KT
+  static constexpr int SMEM = 5 * BYTES;    // Q + double-buffered K and V
+  // byte offset of 16-byte chunk `ch` (columns 8 ch .. 8 ch + 7) of row `row`
+  static __device__ __forceinline__ uint32_t off(uint32_t row, uint32_t ch) {
+    const uint32_t blk = ch / CH, cb = ch % CH;
+    return blk * (QT * SW) + row * SW + ((cb ^ ((row * SW >> 7) & (CH - 1))) << 4);
+  }
+  // wgmma descriptor offset (16-byte units) of head dims 16 ks .. 16 ks + 15 of a K-major tile
+  static __device__ __forceinline__ uint64_t kstep(int ks) { return static_cast<uint64_t>(((ks * 32) / SW * (QT * SW) + (ks * 32) % SW) >> 4); }
+};
+
+// 16-byte cp.async that reads src_bytes (16 or 0) from global memory and zero-fills the rest
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes));
+}
+
+// Copy a 64-row tile of one head (rows s0.. ; row stride `ld` elements; d columns) into the HeadTile<DP> layout; columns d .. DP-1
+// are zero-filled (cp.async reads no bytes for them), so they add nothing to Q K^T.  Rows >= S are clamped to S-1 (their scores
+// are masked / their outputs are never stored).
+template <typename T, int DP>
+__device__ __forceinline__ void load_tile(uint32_t smem_base, const T* __restrict__ gbase, size_t ld, int s0, int S, int d, int tid) {
+  using L = HeadTile<DP>;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int c = tid + i * 128;
-    const int row = c >> 3, ch = c & 7;
-    int s = s0 + row;
+  for (int i = 0; i < L::NCH * QT / 128; ++i) {
+    const uint32_t c = tid + i * 128;  // unsigned: the division and modulo fold to shifts and masks
+    const uint32_t row = c / L::NCH, ch = c % L::NCH;
+    int s = s0 + static_cast<int>(row);
     s = s < S ? s : S - 1;
-    const T* src = gbase + static_cast<size_t>(s) * ld + ch * 8;
-    cp_async16(smem_base + row * 128 + ((ch ^ (row & 7)) << 4), src);
+    const bool in = static_cast<int>(ch * 8) < d;
+    const T* src = gbase + static_cast<size_t>(s) * ld + (in ? ch * 8 : 0);
+    cp_async16_zfill(smem_base + L::off(row, ch), src, in ? 16u : 0u);
   }
 }
 
-template <typename T, typename OutT, bool CAUSAL>
+// Shared memory of a CTA: static up to 48 KB, else dynamic (opted in by attn_launch, 1 KB of slack for the 1024-byte alignment).
+template <int BYTES, bool STATIC = (BYTES <= 48 * 1024)>
+struct AttnSmem {
+  static __device__ __forceinline__ uint8_t* get() {
+    __shared__ __align__(1024) uint8_t smem[BYTES];  // 1024-aligned: the swizzle atoms of the wgmma operands
+    return smem;
+  }
+};
+template <int BYTES>
+struct AttnSmem<BYTES, false> {
+  static __device__ __forceinline__ uint8_t* get() {
+    extern __shared__ uint8_t smem_raw[];
+    return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  }
+};
+
+// Head width d (a multiple of 8, d <= DP); the tiles are padded to DP columns with zeros.  scale_log2 = log2(e) / sqrt(d).
+template <typename T, typename OutT, bool CAUSAL, int DP>
 __global__ void __launch_bounds__(128)
-attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H, float scale_log2, int reverse) {
-  __shared__ __align__(1024) uint8_t smem[QT * 128 + 2 * 2 * KT * 128];  // 1024-aligned: the swizzle atoms of the wgmma operands
+attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H, int d, float scale_log2, int reverse) {
+  using L = HeadTile<DP>;
+  uint8_t* smem = AttnSmem<L::SMEM>::get();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, h = blockIdx.y, b = reverse ? static_cast<int>(gridDim.z) - 1 - static_cast<int>(blockIdx.z) : static_cast<int>(blockIdx.z);
-  const int D = H * HD;
+  const int D = H * d;
   const size_t ld = static_cast<size_t>(3) * D;
-  const T* base = qkv + static_cast<size_t>(b) * S * ld + h * HD;
+  const T* base = qkv + static_cast<size_t>(b) * S * ld + h * d;
   const T* gq = base;
   const T* gk = base + D;
   const T* gv = base + 2 * D;
   const uint32_t sQ = smem_u32(smem);
-  const uint32_t sK0 = sQ + QT * 128;
-  const uint32_t sV0 = sK0 + 2 * KT * 128;
+  const uint32_t sK0 = sQ + L::BYTES;
+  const uint32_t sV0 = sK0 + 2 * L::BYTES;
   const int q0 = qt * QT;
   pdl_launch_dependents();
   pdl_wait();
   int n_kv = (S + KT - 1) / KT;
   if (CAUSAL) n_kv = min(n_kv, qt + 1);
 
-  load_tile<T>(sQ, gq, ld, q0, S, tid);
-  load_tile<T>(sK0, gk, ld, 0, S, tid);
-  load_tile<T>(sV0, gv, ld, 0, S, tid);
+  load_tile<T, DP>(sQ, gq, ld, q0, S, d, tid);
+  load_tile<T, DP>(sK0, gk, ld, 0, S, d, tid);
+  load_tile<T, DP>(sV0, gv, ld, 0, S, d, tid);
   cp_async_commit();
 
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
-  const uint64_t qdesc = make_wgmma_desc_sw128(sQ);
-  float o[8][4];
+  const uint64_t qdesc = make_wgmma_desc<L::SW>(sQ, 16);
+  float o[DP / 8][4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
+  for (int i = 0; i < DP / 8; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
@@ -93,8 +141,8 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
   for (int j = 0; j < n_kv; ++j) {
     const int buf = j & 1;
     if (j + 1 < n_kv) {
-      load_tile<T>(sK0 + (buf ^ 1) * KT * 128, gk, ld, (j + 1) * KT, S, tid);
-      load_tile<T>(sV0 + (buf ^ 1) * KT * 128, gv, ld, (j + 1) * KT, S, tid);
+      load_tile<T, DP>(sK0 + (buf ^ 1) * L::BYTES, gk, ld, (j + 1) * KT, S, d, tid);
+      load_tile<T, DP>(sV0 + (buf ^ 1) * L::BYTES, gv, ld, (j + 1) * KT, S, d, tid);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -102,19 +150,19 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
     }
     fence_proxy_async_smem();  // this thread's cp.async writes -> visible to the tensor cores' (async proxy) reads
     __syncthreads();
-    const uint32_t sK = sK0 + buf * KT * 128, sV = sV0 + buf * KT * 128;
+    const uint32_t sK = sK0 + buf * L::BYTES, sV = sV0 + buf * L::BYTES;
 
     // ---- S = Q K^T (64 x 64 per warpgroup; this warp's 16 rows in the m16n8 accumulator layout, s[n-block][e]) ----
     float s[8][4];
     float (&s_acc)[32] = reinterpret_cast<float (&)[32]>(s);
-    const uint64_t kdesc = make_wgmma_desc_sw128(sK);
+    const uint64_t kdesc = make_wgmma_desc<L::SW>(sK, 16);
 #pragma unroll
     for (int i = 0; i < 32; ++i) s_acc[i] = 0.f;
     wgmma_fence_operands(s_acc);
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks)  // 16 head dims (32 B) per step
-      wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + static_cast<uint64_t>(2 * ks), kdesc + static_cast<uint64_t>(2 * ks), ks != 0 ? 1u : 0u);
+    for (int ks = 0; ks < DP / 16; ++ks)  // 16 head dims (32 B) per step
+      wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + L::kstep(ks), kdesc + L::kstep(ks), ks != 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operands(s_acc);
@@ -159,10 +207,13 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
       s[nt][3] = exp2f(s[nt][3] * scale_log2 - moff[1]);
       l_run[0] += s[nt][0] + s[nt][1];
       l_run[1] += s[nt][2] + s[nt][3];
+    }
+#pragma unroll
+    for (int nt = 0; nt < DP / 8; ++nt) {
       o[nt][0] *= alpha[0]; o[nt][1] *= alpha[0];
       o[nt][2] *= alpha[1]; o[nt][3] *= alpha[1];
     }
-    // ---- O += P V: A = P (keys 16 kk .. 16 kk + 15 of this warp's rows), B = V rows of those keys (MN-major, 2 KB per step) ----
+    // ---- O += P V: A = P (keys 16 kk .. 16 kk + 15 of this warp's rows), B = V rows of those keys (MN-major, 16 rows per step) ----
     uint32_t pf[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
@@ -171,19 +222,19 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
       pf[kk][2] = pack_pair<T>(s[2 * kk + 1][0], s[2 * kk + 1][1]);
       pf[kk][3] = pack_pair<T>(s[2 * kk + 1][2], s[2 * kk + 1][3]);
     }
-    float (&o_acc)[32] = reinterpret_cast<float (&)[32]>(o);
-    const uint64_t vdesc = make_wgmma_desc_sw128(sV);
+    float (&o_acc)[DP / 2] = reinterpret_cast<float (&)[DP / 2]>(o);
+    const uint64_t vdesc = make_wgmma_desc<L::SW>(sV, L::NB > 1 ? QT * L::SW : 16);
     wgmma_fence_operands(o_acc);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<BF16>(o_acc, pf[kk], vdesc + static_cast<uint64_t>(kk * (2048 >> 4)));
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64nNk16_rs<BF16, DP>(o_acc, pf[kk], vdesc + static_cast<uint64_t>(kk * (16 * L::SW >> 4)));
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operands(o_acc);
     __syncthreads();  // everyone done with buf before it is refilled two iterations later
   }
 
-  // ---- finalise: O /= l, store ----
+  // ---- finalise: O /= l, store columns < d ----
   float inv[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -192,33 +243,35 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     inv[r] = 1.0f / l;
   }
-  OutT* obase = out + static_cast<size_t>(b) * S * D + h * HD;
+  OutT* obase = out + static_cast<size_t>(b) * S * D + h * d;
   if constexpr (sizeof(OutT) == 2) {
-    // stage this warp's 16 x 64 tile through its (now free) Q rows so the global stores are 128-byte rows
+    // stage this warp's 16 x DP tile through its (now free) Q rows so the global stores are whole 16-byte chunks of a row
     uint8_t* sq = smem;
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
+    for (int nt = 0; nt < DP / 8; ++nt) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int row = warp * 16 + g + r * 8;
         const int ch = nt;  // 8 columns (16 B) per n-tile
         const uint32_t v = pack_pair<OutT>(o[nt][2 * r] * inv[r], o[nt][2 * r + 1] * inv[r]);
-        *reinterpret_cast<uint32_t*>(sq + row * 128 + ((ch ^ (row & 7)) << 4) + t4 * 4) = v;
+        *reinterpret_cast<uint32_t*>(sq + L::off(row, ch) + t4 * 4) = v;
       }
     }
     __syncwarp();
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int row = warp * 16 + i * 4 + (lane >> 3), ch = lane & 7;
+    for (int i = 0; i < L::NCH / 2; ++i) {  // 16 rows x NCH chunks, 32 per step
+      const uint32_t c = i * 32 + lane;
+      const int row = warp * 16 + static_cast<int>(c / L::NCH), ch = static_cast<int>(c % L::NCH);
       const int srow = q0 + row;
-      if (srow < S) {
-        const uint4 v = *reinterpret_cast<const uint4*>(sq + row * 128 + ((ch ^ (row & 7)) << 4));
+      if (srow < S && ch * 8 < d) {
+        const uint4 v = *reinterpret_cast<const uint4*>(sq + L::off(row, ch));
         *reinterpret_cast<uint4*>(obase + static_cast<size_t>(srow) * D + ch * 8) = v;
       }
     }
   } else {
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
+    for (int nt = 0; nt < DP / 8; ++nt) {
+      if (nt * 8 >= d) break;
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int srow = row_lo + r * 8;
@@ -232,24 +285,57 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
   }
 }
 
-template <typename T, typename OutT>
-static int attn_launch(const void* qkv, void* out, int B, int S, int H, int causal, cudaStream_t stream, int reverse) {
+// The padded widths compiled: d is run at the smallest of them >= d.  16, 32, 64 and 128 are exact for the common head widths; 80
+// serves ViT-H / SigLIP so400m-text widths (80, 72) and 96 widths 88 and 96.  Widths 40-56 run at 64 and 104-120 at 128.
+static int padded_head_dim(int d) { return d <= 16 ? 16 : d <= 32 ? 32 : d <= 64 ? 64 : d <= 80 ? 80 : d <= 96 ? 96 : 128; }
+
+// The softmax scale 1 / sqrt(d) (flax: query / sqrt(depth)) times log2(e), in fp32: 0.125f * log2(e) for d = 64.
+static float attn_scale_log2(int d) { return static_cast<float>(1.0 / std::sqrt(static_cast<double>(d))) * 1.4426950408889634f; }
+
+template <typename T, typename OutT, bool CAUSAL, int DP>
+static int attn_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse) {
+  constexpr int SMEM = HeadTile<DP>::SMEM;
+  constexpr size_t dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
+  if constexpr (dyn > 0) {
+    static DeviceOnce attr_set;
+    if (attr_set.first()) JIMM_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<T, OutT, CAUSAL, DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+  }
   dim3 grid((S + QT - 1) / QT, H, B);
-  const float scale_log2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-  if (causal) JIMM_CUDA_CHECK(launch_k(attention_kernel<T, OutT, true>, grid, dim3(128), 0, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, scale_log2, reverse));
-  else JIMM_CUDA_CHECK(launch_k(attention_kernel<T, OutT, false>, grid, dim3(128), 0, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, scale_log2, reverse));
+  JIMM_CUDA_CHECK(launch_k(attention_kernel<T, OutT, CAUSAL, DP>, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S,
+                           H, d, attn_scale_log2(d), reverse));
   note_launch();
   return 0;
 }
 
-int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, cudaStream_t stream, int reverse) {
+template <typename T, typename OutT, bool CAUSAL>
+static int attn_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse) {
+  switch (padded_head_dim(d)) {
+    case 16: return attn_launch_dp<T, OutT, CAUSAL, 16>(qkv, out, B, S, H, d, stream, reverse);
+    case 32: return attn_launch_dp<T, OutT, CAUSAL, 32>(qkv, out, B, S, H, d, stream, reverse);
+    case 64: return attn_launch_dp<T, OutT, CAUSAL, 64>(qkv, out, B, S, H, d, stream, reverse);
+    case 80: return attn_launch_dp<T, OutT, CAUSAL, 80>(qkv, out, B, S, H, d, stream, reverse);
+    case 96: return attn_launch_dp<T, OutT, CAUSAL, 96>(qkv, out, B, S, H, d, stream, reverse);
+    default: return attn_launch_dp<T, OutT, CAUSAL, 128>(qkv, out, B, S, H, d, stream, reverse);
+  }
+}
+
+template <typename T, typename OutT>
+static int attn_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, int reverse) {
+  if (causal) return attn_launch_causal<T, OutT, true>(qkv, out, B, S, H, d, stream, reverse);
+  return attn_launch_causal<T, OutT, false>(qkv, out, B, S, H, d, stream, reverse);
+}
+
+static bool head_dim_ok(int d) { return d >= 8 && d <= 128 && d % 8 == 0; }
+
+int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream, int reverse) {
+  if (!head_dim_ok(head_dim)) { set_last_error("attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0 || S <= 0) return 0;
   if (B > 65535 || H > 65535) { set_last_error("attention: grid too large (B=%d H=%d)", B, H); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return attn_launch<__half, __half>(qkv, out, B, S, H, causal, stream, reverse);
-  if (io_type == DT_F16 && out_type == DT_F32) return attn_launch<__half, float>(qkv, out, B, S, H, causal, stream, reverse);
-  if (io_type == DT_F16 && out_type == DT_TF32) return attn_launch<__half, tf32_t>(qkv, out, B, S, H, causal, stream, reverse);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return attn_launch<__nv_bfloat16, __nv_bfloat16>(qkv, out, B, S, H, causal, stream, reverse);
-  if (io_type == DT_BF16 && out_type == DT_F32) return attn_launch<__nv_bfloat16, float>(qkv, out, B, S, H, causal, stream, reverse);
+  if (io_type == DT_F16 && out_type == DT_F16) return attn_launch<__half, __half>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
+  if (io_type == DT_F16 && out_type == DT_F32) return attn_launch<__half, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
+  if (io_type == DT_F16 && out_type == DT_TF32) return attn_launch<__half, tf32_t>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
+  if (io_type == DT_BF16 && out_type == DT_BF16) return attn_launch<__nv_bfloat16, __nv_bfloat16>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
+  if (io_type == DT_BF16 && out_type == DT_F32) return attn_launch<__nv_bfloat16, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
   set_last_error("attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
   return -1;
 }
@@ -259,25 +345,25 @@ int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, 
 // ------------------------------------------------------------------------------------------
 template <typename T, typename OutT>
 __global__ void __launch_bounds__(256)
-map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT* __restrict__ out, int S, int H) {
+map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT* __restrict__ out, int S, int H, int d, float qscale) {
   extern __shared__ float sm[];
-  float* sq = sm;             // [64]
-  float* red = sm + 64;       // [8 * 64] cross-group reduction / [8] block reductions
-  float* sc = sm + 64 + 512;  // [S]
+  float* sq = sm;              // [128]
+  float* red = sm + 128;       // [8 * 128] cross-group reduction / [8] block reductions
+  float* sc = sm + 128 + 1024; // [S]
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int D = H * HD;
+  const int D = H * d;
   const size_t ld = static_cast<size_t>(2) * D;
-  const T* kbase = kv + static_cast<size_t>(b) * S * ld + h * HD;
+  const T* kbase = kv + static_cast<size_t>(b) * S * ld + h * d;
   const T* vbase = kbase + D;
-  if (tid < 64) sq[tid] = q[h * HD + tid] * 0.125f;  // query / sqrt(depth)
+  if (tid < d) sq[tid] = q[h * d + tid] * qscale;  // query / sqrt(depth)
   __syncthreads();
   // scores
   float lmax = -INFINITY;
   for (int s = tid; s < S; s += 256) {
     const uint4* kr = reinterpret_cast<const uint4*>(kbase + static_cast<size_t>(s) * ld);
     float acc = 0.f;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
+#pragma unroll 8
+    for (int c = 0; c < d / 8; ++c) {
       const uint4 u = __ldg(kr + c);
       const T* e = reinterpret_cast<const T*>(&u);
 #pragma unroll
@@ -306,43 +392,57 @@ map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT
 #pragma unroll
   for (int w = 0; w < 8; ++w) bsum += red[w];
   __syncthreads();
-  // output: warp = key group, lane = dim pair
-  float a0 = 0.f, a1 = 0.f;
+  // output: warp = key group, lane = dim pairs lane and lane + 32 (columns 2 lane, 2 lane + 1 and 64 more)
+  float a[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
   for (int s = warp; s < S; s += 8) {
     const float p = sc[s];
-    const uint32_t u = __ldg(reinterpret_cast<const uint32_t*>(vbase + static_cast<size_t>(s) * ld) + lane);
-    const T* e = reinterpret_cast<const T*>(&u);
-    a0 = fmaf(p, to_float(e[0]), a0);
-    a1 = fmaf(p, to_float(e[1]), a1);
+    const uint32_t* vr = reinterpret_cast<const uint32_t*>(vbase + static_cast<size_t>(s) * ld);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      if (2 * (lane + 32 * j) < d) {
+        const uint32_t u = __ldg(vr + lane + 32 * j);
+        const T* e = reinterpret_cast<const T*>(&u);
+        a[j][0] = fmaf(p, to_float(e[0]), a[j][0]);
+        a[j][1] = fmaf(p, to_float(e[1]), a[j][1]);
+      }
+    }
   }
-  red[warp * 64 + lane * 2] = a0;
-  red[warp * 64 + lane * 2 + 1] = a1;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int c = 2 * (lane + 32 * j);
+    if (c < d) {
+      red[warp * 128 + c] = a[j][0];
+      red[warp * 128 + c + 1] = a[j][1];
+    }
+  }
   __syncthreads();
-  if (tid < 64) {
+  if (tid < d) {
     float v = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) v += red[w * 64 + tid];
-    out[static_cast<size_t>(b) * D + h * HD + tid] = from_float<OutT>(v / bsum);
+    for (int w = 0; w < 8; ++w) v += red[w * 128 + tid];
+    out[static_cast<size_t>(b) * D + h * d + tid] = from_float<OutT>(v / bsum);
   }
 }
 
 template <typename T, typename OutT>
-static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, cudaStream_t stream) {
+static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream) {
   dim3 grid(H, B);
-  const size_t smem = (64 + 512 + S) * sizeof(float);
-  map_attention_kernel<T, OutT><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H);
+  const size_t smem = (128 + 1024 + S) * sizeof(float);
+  const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(d)));  // 0.125f for d = 64
+  map_attention_kernel<T, OutT><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale);
   JIMM_LAUNCH_CHECK();
   return 0;
 }
 
-int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, cudaStream_t stream) {
+int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream) {
+  if (!head_dim_ok(head_dim)) { set_last_error("map_attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0) return 0;
   if (S > 8192) { set_last_error("map_attention: S=%d too large", S); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, stream);
-  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, stream);
-  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, stream);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, stream);
-  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, stream);
+  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream);
+  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream);
+  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream);
+  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream);
+  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream);
   set_last_error("map_attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
   return -1;
 }

@@ -67,12 +67,14 @@ struct UploadRing {
 };
 int activation_run(const float* x, float* y, size_t n, int act /* 0 none, 1 gelu_tanh, 2 quick_gelu */, cudaStream_t stream);
 
-// Multi-head softmax attention over the fused qkv buffer [B*S, 3D] (q | k | v, heads of 64).  SURVEY 8a row a5.
-//   o[b*S+s, h*64+d] = softmax_k((q/8) k^T  masked) v ; causal: key <= query.  io_type fp16/bf16; out_type fp16/bf16/fp32
-int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, cudaStream_t stream, int reverse = 0);
+// Multi-head softmax attention over the fused qkv buffer [B*S, 3D] (q | k | v, H heads of head_dim d; D = H d).  SURVEY 8a row a5.
+//   o[b*S+s, h*d+j] = softmax_k((q/sqrt(d)) k^T  masked) v ; causal: key <= query.  d a multiple of 8 in [8, 128].
+//   io_type fp16/bf16; out_type fp16/bf16/fp32/tf32
+int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream,
+                  int reverse = 0);
 
 // MAP-head attention with a single (input-independent) probe query (common/vit.py:96-97).
-//   q: fp32 [H*64] (already projected + biased), kv: [B*S, 2D] (k | v) io_type, out [B, D] out_type
-int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, cudaStream_t stream);
+//   q: fp32 [H*d] (already projected + biased), kv: [B*S, 2D] (k | v) io_type, out [B, D] out_type; d as attention_run
+int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream);
 
 }  // namespace jimm

@@ -547,7 +547,7 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   for (BlockW& b : enc->blocks) {
     if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ws.h, m->cdt, c.D, T, c.D, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_qkv, ws.h, c.D, b.qkv, T, s, flip()));
-    JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.causal, s, flip()));
+    JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_out, ws.h, c.D, b.out, T, s, flip()));  // + residual (+ norm2 -> ws.h when fused)
     if (m->simt || !gemm_fuses_ln(&b.p_out, T))
       JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm2.scale, b.norm2.bias, c.eps, ws.h, m->cdt, c.D, T, c.D, s, flip()));
@@ -564,7 +564,7 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s)
   Workspace& ws = m->ws;
   const int D = v.D, T = B * S;
   JIMM_TRY(run_gemm(m, v.p_map_kv, ws.h, D, v.map_kv, T, s));                                        // k | v  [T, 2D]
-  JIMM_TRY(map_attention_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, B, S, v.enc.c.H, s));     // [B, D]
+  JIMM_TRY(map_attention_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, B, S, v.enc.c.H, v.enc.c.D / v.enc.c.H, s));     // [B, D]
   JIMM_TRY(run_gemm(m, v.p_map_out, ws.pooled, D, v.map_out, B, s));                                 // -> feat fp32 [B, D]
   JIMM_TRY(layernorm_run(ws.feat, D, 1, 0, nullptr, v.map_ln.scale, v.map_ln.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
   JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, 4D]
@@ -780,6 +780,17 @@ int jimm_abi_version(void) { return 1; }
 long long jimm_launch_count(void) { return g_launches.load(); }
 long long jimm_graph_replay_count(void) { return g_graph_replays.load(); }
 
+// The attention kernels take head widths (width / heads) that are multiples of 8 from 8 to 128.
+static int check_heads(const char* tower, int width, int heads) {
+  const int hd = heads > 0 ? width / heads : 0;
+  if (heads <= 0 || width % heads != 0 || hd % 8 != 0 || hd < 8 || hd > 128) {
+    set_last_error("%shead_dim: width %d / heads %d = %s%d; supported head widths are multiples of 8 from 8 to 128 (width divisible by heads)", tower,
+                   width, heads, heads > 0 && width % heads == 0 ? "" : "non-integer ", hd);
+    return JIMM_EINVAL;
+  }
+  return 0;
+}
+
 int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) {
   if (!cfg || !out) { set_last_error("jimm_model_create: null argument"); return JIMM_EINVAL; }
   if (cfg->kind < JIMM_VIT || cfg->kind > JIMM_MAPHEAD) { set_last_error("bad kind %d", cfg->kind); return JIMM_EINVAL; }
@@ -788,15 +799,8 @@ int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) 
     set_last_error("pooling_type must be either MAP or CLS.");  // common/vit.py:178
     return JIMM_EINVAL;
   }
-  if (cfg->v_heads <= 0 || cfg->v_width != cfg->v_heads * 64) {
-    set_last_error("vision head_dim must be 64 (width %d, heads %d): the attention kernels are specialised for it", cfg->v_width, cfg->v_heads);
-    return JIMM_EINVAL;
-  }
   const bool dual = cfg->kind == JIMM_CLIP || cfg->kind == JIMM_SIGLIP;
-  if (dual && (cfg->t_heads <= 0 || cfg->t_width != cfg->t_heads * 64)) {
-    set_last_error("text head_dim must be 64 (width %d, heads %d)", cfg->t_width, cfg->t_heads);
-    return JIMM_EINVAL;
-  }
+  if (check_heads(sub ? "" : "vision ", cfg->v_width, cfg->v_heads) || (dual && check_heads("text ", cfg->t_width, cfg->t_heads))) return JIMM_EINVAL;
   if (cfg->compute_dtype < JIMM_F32 || cfg->compute_dtype > JIMM_BF16) { set_last_error("bad compute_dtype"); return JIMM_EINVAL; }
   if (sub && cfg->ctx_len <= 0) { set_last_error("sub-module handle: ctx_len (max tokens per sample) must be positive"); return JIMM_EINVAL; }
   if (!sub && (cfg->patch <= 0 || cfg->img_size < cfg->patch || cfg->in_ch <= 0)) {
@@ -1504,14 +1508,21 @@ int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int3
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream) {
   return jimm_k_layernorm_ex(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, 0, stream);
 }
+int jimm_k_attention_hd(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, int reverse,
+                        void* stream) {
+  return attention_run(qkv, io_type, out, out_type, B, S, H, head_dim, causal, static_cast<cudaStream_t>(stream), reverse);
+}
 int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse, void* stream) {
-  return attention_run(qkv, io_type, out, out_type, B, S, H, causal, static_cast<cudaStream_t>(stream), reverse);
+  return jimm_k_attention_hd(qkv, io_type, out, out_type, B, S, H, 64, causal, reverse, stream);
 }
 int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, void* stream) {
   return jimm_k_attention_ex(qkv, io_type, out, out_type, B, S, H, causal, 0, stream);
 }
+int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, void* stream) {
+  return map_attention_run(q, kv, io_type, out, out_type, B, S, H, head_dim, static_cast<cudaStream_t>(stream));
+}
 int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
-  return map_attention_run(q, kv, io_type, out, out_type, B, S, H, static_cast<cudaStream_t>(stream));
+  return jimm_k_map_attention_hd(q, kv, io_type, out, out_type, B, S, H, 64, stream);
 }
 int jimm_k_patchify_ex(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, int rows_per_sample, int ldk,
                        void* stream) {
