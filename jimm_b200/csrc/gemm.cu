@@ -2,12 +2,16 @@
 //
 //   C[M,N] = epi( A[M,K] . B[N,K]^T ),  A/B K-major fp16 | bf16 | fp32(tf32), fp32 accumulate in registers.
 //
-// CTA = 384 threads (three warpgroups), 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin 128 x 128 tile schedule (n fastest).
-//   warpgroup 0, warp 0 : TMA producer (one lane): 5-stage smem ring of {A 128x128B, B 128x128B} tiles, SWIZZLE_128B
+// CTA = 384 threads (three warpgroups), 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin 128 x 256 tile schedule (n fastest).
+//   warpgroup 0, warp 0 : TMA producer (one lane): 4-stage smem ring of {A 128x128B, B 256x128B} tiles (48 KB), SWIZZLE_128B
 //   warpgroup 0, warps 1-3: idle, or LayerNorm workers of the fused-LayerNorm epilogue
-//   warpgroups 1, 2     : consumers, 64 rows each: wgmma.mma_async m64n128 from shared memory, one wgmma group in flight while the
+//   warpgroups 1, 2     : consumers, 64 rows each: wgmma.mma_async m64n256 from shared memory, one wgmma group in flight while the
 //                         previous stage is released; then the epilogue straight from the accumulator registers.  While they run
 //                         it, the producer is already filling the ring for their next tile.
+// 128 x 256 rather than 128 x 128: a k-slab of 128 B fills (128 + 256) x 128 B of shared memory from L2 for 2 x 128 x 256 x 64 FLOP
+// (fp16), 85 FLOP per byte instead of 64, and the two consumer warpgroups read one B slab per 2 x 64 x 256 instead of 2 x 64 x 128
+// outputs.  The 128 fp32 accumulators per consumer thread do not fit in the 168 registers each of 384 threads starts with, so the
+// warpgroups trade registers with setmaxnreg (PRODUCER_REGS / CONSUMER_REGS below).
 // Two mbarrier arrays: smem full (TMA transaction bytes) / empty (one arrive per consumer warp).
 //
 // Epilogues are compile-time specialised (a run-time branch on dtype / activation inside the unrolled loops costs registers and
@@ -36,9 +40,10 @@
 
 namespace jimm {
 
-static constexpr int BM = 128;  // two consumer warpgroups x 64 rows
-static constexpr int BN = 128;
-static constexpr int STAGES = 5;
+static constexpr int BM = GEMM_TILE_M;  // two consumer warpgroups x 64 rows
+static constexpr int BN = GEMM_TILE_N;  // one m64n256 wgmma per consumer warpgroup and K step
+static_assert(BM == 128 && BN == 256, "the warp roles and the wgmma shape below are written for 128 x 256 tiles");
+static constexpr int STAGES = 4;  // a 48 KB stage is 1024 tensor-core clocks of work (fp16)
 static constexpr int A_STAGE_BYTES = BM * 128;
 static constexpr int B_STAGE_BYTES = BN * 128;
 static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
@@ -48,6 +53,7 @@ static constexpr int EPI_BUF_BYTES = EPI_BOX_ROWS * 128;                  // one
 static constexpr int EPI_BUFS = 2;                                        // per warp: box i + 1 is packed while box i is stored
 static constexpr int EPI_STAGE_BYTES = EPI_WARPS * EPI_BUFS * EPI_BUF_BYTES;  // 32 KB
 static constexpr int NUM_THREADS = 384;
+static constexpr int KERNEL_REGS = 168;  // per thread at launch: 64 K registers / 384 threads, in the allocation unit of 8
 
 enum OutKind : int { OUT_GENERIC = 0, OUT_H16 = 1, OUT_BF16 = 2, OUT_TF32 = 3, OUT_F32_ADD = 4, OUT_F32 = 5 };
 
@@ -101,7 +107,7 @@ __device__ __forceinline__ void store1(const EpiDev& e, int out_row, int col, fl
 }
 
 template <typename T>
-struct Traits;  // KIND: wgmma_m64n128_ss operand kind
+struct Traits;  // KIND: wgmma_m64n256_ss operand kind
 template <>
 struct Traits<__half> {
   static constexpr int KIND = 0;
@@ -131,9 +137,9 @@ struct LnQueue {
 
 template <typename OutT, int NV>
 __device__ __forceinline__ void ln_rows_nv(const EpiDev& e, int row0, int lane) {
-  constexpr int R0 = 12 / NV;
-  constexpr int R = R0 < 1 ? 1 : (R0 > 8 ? 8 : R0);  // rows per batch: <= 12 float4 per lane per buffer
-  constexpr bool DOUBLE = NV <= 9;                   // wider rows: one buffer (a row's loads still go out back to back)
+  constexpr int R0 = 8 / NV;
+  constexpr int R = R0 < 1 ? 1 : R0;  // rows per batch: <= 8 float4 per lane per buffer (the LayerNorm warps hold PRODUCER_REGS)
+  constexpr bool DOUBLE = NV <= 8;    // wider rows: one buffer (a row's loads still go out back to back)
   const float inv_d = 1.0f / static_cast<float>(NV * 128);
   const float4* sc = reinterpret_cast<const float4*>(e.ln_scale);
   const float4* bi = reinterpret_cast<const float4*>(e.ln_bias);
@@ -214,8 +220,6 @@ __device__ __forceinline__ void ln_rows_dispatch(const EpiDev& e, int row0, int 
     case 6: ln_rows_nv<OutT, 6>(e, row0, lane); break;
     case 8: ln_rows_nv<OutT, 8>(e, row0, lane); break;
     case 9: ln_rows_nv<OutT, 9>(e, row0, lane); break;
-    case 10: ln_rows_nv<OutT, 10>(e, row0, lane); break;
-    case 12: ln_rows_nv<OutT, 12>(e, row0, lane); break;
     default: break;
   }
 }
@@ -265,7 +269,7 @@ __device__ __forceinline__ void ln_worker(const EpiDev& e, LnQueue* q, int lane)
 // ---- TMA epilogue of one consumer warp: its 16 rows x BN columns, thread (g = lane / 4, t = lane % 4) holds rows g and g + 8,
 // columns 8 j + 2 t (+1) of the wgmma accumulator.  16-bit outputs: 64 columns per 16 x 128 B box; 32-bit outputs: 32 columns.
 template <int OUT, int ACT>
-__device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const EpiDev& epi, const float (&acc)[64], uint8_t* tbuf0, int lane,
+__device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const EpiDev& epi, const float (&acc)[128], uint8_t* tbuf0, int lane,
                                              int row_base, int n_tile0, uint32_t& box_count) {
   constexpr bool OUT16 = (OUT == OUT_H16 || OUT == OUT_BF16);
   constexpr int ES = OUT16 ? 2 : 4;
@@ -324,7 +328,7 @@ __device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const Epi
 }
 
 // ---- generic LSU epilogue (run-time flags; any N, row remap, row-add, residual read) ---------------------------------
-__device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float (&acc)[64], int lane, int row_base, int n_tile0) {
+__device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float (&acc)[128], int lane, int row_base, int n_tile0) {
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -358,6 +362,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   constexpr int UK = 32 / sizeof(T);   // wgmma K (16 for 16-bit, 8 for tf32)
   constexpr bool FUSE_LN = OUT == OUT_F32_ADD && ACT == ACT_FUSE_LN;  // see "fused LayerNorm" above
   constexpr int EPI_ACT = ACT == ACT_FUSE_LN ? static_cast<int>(ACT_NONE) : ACT;
+  // Registers per thread of the producer warpgroup / of each consumer warpgroup after setmaxnreg.  The consumers hold 128
+  // accumulators; the producer's TMA lane needs few.  The fused LayerNorm's workers live in the producer warpgroup and keep up to 64
+  // registers of row data (ln_rows_nv) plus the scale / bias they load, while its consumers' reduce-add epilogue is the leanest.
+  // Chosen from ptxas -v: splits without spills.  The three warpgroups share the CTA's launch allocation of KERNEL_REGS per thread
+  // (checked at launch).
+  constexpr int PRODUCER_REGS = FUSE_LN ? 152 : 40;
+  constexpr int CONSUMER_REGS = FUSE_LN ? 176 : 232;
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NUM_THREADS * KERNEL_REGS, "register split exceeds the CTA's allocation");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -396,6 +408,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   pdl_wait();  // everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail
 
   if (warp_idx < 4) {
+    setmaxnreg<KERNEL_REGS, PRODUCER_REGS>();
     if (warp_idx == 0) {
       // ===================== TMA producer =====================
       if (lane == 0) {
@@ -418,13 +431,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     }
   } else {
     // ===================== consumers: mainloop + epilogue =====================
+    setmaxnreg<KERNEL_REGS, CONSUMER_REGS>();
     const int wg = (warp_idx - 4) >> 2;  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
     const int wq = warp_idx & 3;         // warp within the warpgroup: rows [16 wq, 16 wq + 16) of those
     uint8_t* tbuf0 = epi_stage + (warp_idx - 4) * EPI_BUFS * EPI_BUF_BYTES;
     int stage = 0;
     uint32_t phase = 0, box_count = 0;
     int ln_rg = -1, ln_cols = 0;  // row group / column count of this warp's previous tile, not yet published (fused LayerNorm)
-    float acc[64];
+    float acc[128];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
       const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
@@ -437,7 +451,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / UK; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
-          wgmma_m64n128_ss<Traits<T>::KIND>(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), (kb | k) != 0 ? 1u : 0u);
+          wgmma_m64n256_ss<Traits<T>::KIND>(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), (kb | k) != 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_fence_operands(acc);
         if (prev >= 0) {
@@ -660,7 +674,16 @@ static EpiDev to_dev(const GemmEpilogue& e, int M, int N) {
 template <typename T, int OUT, int ACT>
 static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
   static DeviceOnce attr_set;
-  if (attr_set.first()) JIMM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<T, OUT, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  if (attr_set.first()) {
+    JIMM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<T, OUT, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    // setmaxnreg moves registers within the launch allocation: with fewer than KERNEL_REGS per thread, an increase would wait forever
+    cudaFuncAttributes fa;
+    JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, gemm_wgmma_kernel<T, OUT, ACT>));
+    if (fa.numRegs != KERNEL_REGS) {
+      set_last_error("gemm: kernel compiled with %d registers per thread, the warpgroup register split assumes %d", fa.numRegs, KERNEL_REGS);
+      return -2;
+    }
+  }
   const int tiles = ((M + BM - 1) / BM) * ((p->N + BN - 1) / BN);
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
   JIMM_CUDA_CHECK(launch_k(gemm_wgmma_kernel<T, OUT, ACT>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, 1, true, p->map_a, p->map_b,
@@ -694,9 +717,9 @@ static int launch_tc(const GemmPlan* p, int M, cudaStream_t stream) {
 // Will gemm_plan_run(p, M) normalise the finished rows itself (GemmEpilogue::ln_*)?  Same predicate as launch_one.
 int gemm_fuses_ln(const GemmPlan* p, int /*M_override: any row count*/) {
   const int nv = p->N >> 7;
-  // ln_rows_dispatch's widths; 2048 (nv = 16) is left to the LayerNorm kernel: its 64-register row buffer does not fit next to the rest
-  // of this kernel without spilling
-  const bool width_ok = p->N % 128 == 0 && (nv <= 4 || nv == 6 || (nv >= 8 && nv <= 10) || nv == 12);
+  // ln_rows_dispatch's widths; 1280, 1536 and 2048 (nv = 10, 12, 16) are left to the LayerNorm kernel: their row buffers do not fit in
+  // the LayerNorm warps' PRODUCER_REGS without spilling
+  const bool width_ok = p->N % 128 == 0 && (nv <= 4 || nv == 6 || nv == 8 || nv == 9);
   // the normalised rows are written in this GEMM's operand type (they are the next GEMM's A operand)
   const int want = p->dtype == DT_F16 ? DT_F16 : p->dtype == DT_BF16 ? DT_BF16 : DT_TF32;
   return p->epi.ln_cnt != nullptr && p->epi.ln_out_type == want && width_ok && p->epi.mode == 2 && p->epi.residual != nullptr && p->epi.tok_pad == 0;

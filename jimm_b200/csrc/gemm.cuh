@@ -20,6 +20,11 @@ enum Act : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_QUICK_GELU = 2 };
 
 inline size_t dtype_size(int dt) { return (dt == DT_F32 || dt == DT_TF32) ? 4 : 2; }
 
+// Output tile of one CTA (M rows x N columns).  A GEMM runs ceil(M / GEMM_TILE_M) x ceil(N / GEMM_TILE_N) tiles on at most one CTA per
+// SM, so its time goes in waves of that many tiles.
+constexpr int GEMM_TILE_M = 128;
+constexpr int GEMM_TILE_N = 256;
+
 struct GemmEpilogue {
   const float* bias = nullptr;      // [N] fp32, added per output column
   int act = ACT_NONE;               // applied after bias

@@ -1209,7 +1209,7 @@ static int ensure_copy_stream(jimm_model* m) {
 }
 
 // Slice schedule of one super-chunk of nb images on the host path.  Two slices: a head slice whose H2D copy is the only exposed
-// one, chosen between nb/head_div and nb/3 so that BOTH slices quantise well into waves of 128 x 128 GEMM tiles (a badly chosen
+// one, chosen between nb/head_div and nb/3 so that BOTH slices quantise well into waves of GEMM tiles (a badly chosen
 // split costs an extra wave in every GEMM).  JIMM_HOST_SLICES (comma separated sizes) overrides it for experiments.
 static void host_slices(const jimm_model* m, int nb, int* sizes, size_t bytes_per_image = 0) {
   for (int i = 0; i < jimm_model::kHostSlices; ++i) sizes[i] = 0;
@@ -1236,8 +1236,8 @@ static void host_slices(const jimm_model* m, int nb, int* sizes, size_t bytes_pe
   const int S = m->vis.S, D = m->vis.D, Mm = m->vis.enc.c.M;
   const int sms = device_sm_count();
   auto cost = [&](int n) {
-    const long mt = (static_cast<long>(n) * S + 127) / 128;
-    auto rounds = [&](int N) { return (mt * ((N + 127) / 128) + sms - 1) / sms; };
+    const long mt = (static_cast<long>(n) * S + GEMM_TILE_M - 1) / GEMM_TILE_M;
+    auto rounds = [&](int N) { return (mt * ((N + GEMM_TILE_N - 1) / GEMM_TILE_N) + sms - 1) / sms; };
     return static_cast<double>(D) * rounds(3 * D) + static_cast<double>(D) * rounds(D) + static_cast<double>(D) * rounds(Mm) +
            static_cast<double>(Mm) * rounds(D);
   };
@@ -1481,7 +1481,7 @@ int jimm_k_gemm_ex(int impl, int dtype, const void* A, int lda, const void* B, i
   GemmPlan p;
   JIMM_TRY(gemm_plan_init(&p, dtype, A, lda, B, ldb, plan_M, N, K, e));
   if (ln_counters && !gemm_fuses_ln(&p, M)) {
-    set_last_error("gemm: this shape does not take the fused LayerNorm path (needs N = 128 x {1,2,3,4,6,8,9,10,12}, aligned operands, "
+    set_last_error("gemm: this shape does not take the fused LayerNorm path (needs N = 128 x {1,2,3,4,6,8,9}, aligned operands, "
                    "LayerNorm output in the operand type)");
     return JIMM_EINVAL;
   }
