@@ -34,7 +34,8 @@ extern "C" {
 typedef struct jimm_model jimm_model_t;
 
 enum jimm_status { JIMM_OK = 0, JIMM_EINVAL = -1, JIMM_ECUDA = -2, JIMM_EDRIVER = -3, JIMM_ESTATE = -4, JIMM_ENOMEM = -5 };
-enum jimm_dtype { JIMM_F32 = 0, JIMM_F16 = 1, JIMM_BF16 = 2, JIMM_I32 = 3 };
+/* JIMM_F8E4M3 is valid only as jimm_config_t.compute_dtype (see there). */
+enum jimm_dtype { JIMM_F32 = 0, JIMM_F16 = 1, JIMM_BF16 = 2, JIMM_I32 = 3, JIMM_F8E4M3 = 4 };
 enum jimm_kind {
   JIMM_VIT = 0, JIMM_CLIP = 1, JIMM_SIGLIP = 2, JIMM_TOWER = 3 /* bare VisionTransformerBase */,
   JIMM_ENCODER = 4 /* bare Transformer / TransformerEncoder stack (common/transformer.py:22-196) */,
@@ -60,8 +61,12 @@ typedef struct jimm_config {
   int t_act, t_causal, t_pool, t_head_bias;
   float t_eps_outer, t_eps_block;
   /* numerics */
-  int compute_dtype;                      /* jimm_dtype of the tensor-core operands: F32 (tf32 MMA) | F16 | BF16;
-                                             accumulation, residual stream, LN statistics, softmax, logits are fp32 */
+  int compute_dtype;                      /* jimm_dtype of the tensor-core operands: F32 (tf32 MMA) | F16 | BF16 | F8E4M3;
+                                             accumulation, residual stream, LN statistics, softmax, logits are fp32.
+                                             F8E4M3: F16 except that the QKV and FC1 GEMMs of every encoder block take float8 e4m3
+                                             operands, scaled by a power of two per token row (from the block LayerNorm) and per
+                                             output channel (from the weight row, at finalize); tower widths must be multiples of 16.
+                                             Not within the 1e-3 parity of the other modes. */
 } jimm_config_t;
 
 JIMM_API const char* jimm_last_error(void);
@@ -185,6 +190,21 @@ JIMM_API int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off
                                  float eps, void* out, int out_type, int ldy, int rows, int D, int reverse, void* stream);
 JIMM_API int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse,
                                  void* stream);
+/* FP8 (e4m3) pieces of the F8E4M3 compute mode.  An e4m3 matrix is one byte per element (row strides in elements = bytes); a scale
+ * vector holds one fp32 power of two per row, s = 2^k with k the smallest integer such that max|row| / s <= 448 (s = 1 for a zero row,
+ * k >= -126); elements are stored as e4m3(x / s), rounded to nearest even.
+ * jimm_k_layernorm_e4m3: the dense per-row LayerNorm of jimm_k_layernorm_ex (group 1, row_off 0) with an e4m3 output [rows, ldy] and
+ *   row_scale fp32 [rows]; the row's scale comes from its fp32 normalised values.
+ * jimm_k_gemm_e4m3: out = act(A . B^T * (a_scale[row] * b_scale[col]) + bias), A e4m3 [M, K], B e4m3 [N, K], a_scale [plan_M],
+ *   b_scale [N] (8-byte aligned); out_type 0 fp32 | 1 fp16 | 2 bf16 | 3 tf32; impl, epi_mode, plan_M, reverse as jimm_k_gemm_ex.
+ * jimm_k_quantize_e4m3: the weight quantiser of finalize: rows of an fp32 [rows, K] matrix (row stride lds) -> e4m3 [rows, ldo]
+ *   and row_scale [rows]; K, lds and ldo multiples of 4. */
+JIMM_API int jimm_k_layernorm_e4m3(const float* x, int ldx, const float* scale, const float* bias, float eps, void* out, int ldy,
+                                   float* row_scale, int rows, int D, int reverse, void* stream);
+JIMM_API int jimm_k_gemm_e4m3(int impl, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* a_scale,
+                              const float* b_scale, const float* bias, int act, void* out, int out_type, int ldo, int epi_mode, int plan_M,
+                              int reverse, void* stream);
+JIMM_API int jimm_k_quantize_e4m3(const float* src, int lds, int rows, int K, void* out, int ldo, float* row_scale, void* stream);
 JIMM_API int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream);
 /* jimm_k_attention_ex / jimm_k_map_attention for heads of head_dim columns (D = H * head_dim; the two are these calls with
  * head_dim = 64).  head_dim: a multiple of 8 from 8 to 128.  Softmax scale 1 / sqrt(head_dim). */

@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libjimm_b200.so")
 
-F32, F16, BF16, I32 = 0, 1, 2, 3
+F32, F16, BF16, I32, F8E4M3 = 0, 1, 2, 3, 4
 PARAM_TRANSPOSED = 1
 KIND_VIT, KIND_CLIP, KIND_SIGLIP, KIND_TOWER, KIND_ENCODER, KIND_MAPHEAD = 0, 1, 2, 3, 4, 5
 POOL_CLS, POOL_MAP = 0, 1
@@ -87,6 +87,9 @@ SIGNATURES = {
     "jimm_k_layernorm_ex": (_i, [_fp, _i, _i, _i, _ip, _fp, _fp, _f, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_attention_ex": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _vp]),
+    "jimm_k_layernorm_e4m3": (_i, [_fp, _i, _fp, _fp, _f, _vp, _i, _fp, _i, _i, _i, _vp]),
+    "jimm_k_gemm_e4m3": (_i, [_i, _vp, _i, _vp, _i, _i, _i, _i, _fp, _fp, _fp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_quantize_e4m3": (_i, [_fp, _i, _i, _i, _vp, _i, _fp, _vp]),
     "jimm_k_attention_hd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention_hd": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),

@@ -159,7 +159,7 @@ class NativeModel:
         return self._vision_host(x, encode)
 
     def _operand_dtype(self) -> torch.dtype:
-        return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16}[self.cfg.compute_dtype]
+        return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16, _lib.F8E4M3: torch.float16}[self.cfg.compute_dtype]
 
     def _vision_host(self, x: torch.Tensor, encode: bool) -> "PendingResult":
         B = x.shape[0]

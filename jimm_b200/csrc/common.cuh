@@ -6,6 +6,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -277,6 +278,17 @@ __device__ __forceinline__ void wgmma_m64n256_ss(float (&d)[128], uint64_t adesc
                  : "l"(adesc), "l"(bdesc), "r"(accumulate));
   }
 }
+// D[64 x 128] (+)= A[64 x 32] . B[128 x 32]^T, e4m3 operands K-major in shared memory, 64 accumulator registers per thread.
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+               "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, "
+               "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+               : JIMM_WGMMA_D8(0), JIMM_WGMMA_D8(8), JIMM_WGMMA_D8(16), JIMM_WGMMA_D8(24), JIMM_WGMMA_D8(32), JIMM_WGMMA_D8(40),
+                 JIMM_WGMMA_D8(48), JIMM_WGMMA_D8(56)
+               : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 #undef JIMM_WGMMA_D128
 #undef JIMM_WGMMA_D8
 #undef JIMM_WGMMA_D128_OPERANDS
@@ -503,6 +515,29 @@ __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { re
 __device__ __forceinline__ float to_float(float v) { return v; }
 __device__ __forceinline__ float to_float(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_float(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_float(__nv_fp8_e4m3 v) { return static_cast<float>(v); }
+
+// ---- FP8 (e4m3) quantisation with power-of-two scales ------------------------------------------------------------------------
+// Scale of a row with absolute maximum a: s = 2^k, k the smallest integer with a / s <= 448 (the largest finite e4m3), s = 1 for
+// a = 0; k is clamped at -126 so that s stays a normal fp32 (rows with a < 2^-117 only).  k comes from the exponent bits (frexpf is
+// exact): a = f 2^E with f in [0.5, 1), and a <= 448 2^k = 0.875 2^(9 + k) holds from k = E - 9 on when f <= 0.875, else from E - 8.
+// x / s is then an exact multiplication by 2^-k, and the dequantised value q s is exact.
+__device__ __forceinline__ int e4m3_scale_exp(float amax) {
+  if (!(amax > 0.f)) return 0;
+  int e;
+  const float f = frexpf(amax, &e);
+  const int k = e - 9 + (f > 0.875f ? 1 : 0);
+  return k < -126 ? -126 : k;
+}
+// two values -> two e4m3 bytes (lo = a, hi = b), round to nearest even, saturating to +-448 (never reached with the scales above)
+__device__ __forceinline__ uint16_t e4m3x2_rn(float a, float b) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
+  return r;
+}
+__device__ __forceinline__ uint32_t e4m3x4_rn(float a, float b, float c, float d) {
+  return static_cast<uint32_t>(e4m3x2_rn(a, b)) | (static_cast<uint32_t>(e4m3x2_rn(c, d)) << 16);
+}
 
 __device__ __forceinline__ uint32_t pack2(float a, float b, int out_type /*1 f16, 2 bf16*/) {
   if (out_type == 1) {

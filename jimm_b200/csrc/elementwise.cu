@@ -13,12 +13,14 @@ namespace jimm {
 
 // ------------------------------------------------------------------------------------------
 // LayerNorm: one warp per row, row kept in registers (D <= 2048), fp32 statistics.
+// OutT = __nv_fp8_e4m3: the normalised fp32 row y is quantised to e4m3 as y / s, s = 2^k from the row's absolute maximum
+// (e4m3_scale_exp), and s goes to row_scale[r] -- the FP8 compute mode's QKV / FC1 A operand with its row scales.
 // ------------------------------------------------------------------------------------------
 template <typename OutT, int MAXV>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, size_t ldx, int group, int row_off, const int* __restrict__ row_index,
                  const float* __restrict__ scale, const float* __restrict__ bias, float eps, OutT* __restrict__ out, size_t ldy,
-                 int rows, int D, int reverse) {
+                 int rows, int D, int reverse, float* __restrict__ row_scale) {
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   pdl_launch_dependents();
@@ -48,6 +50,30 @@ layernorm_kernel(const float* __restrict__ x, size_t ldx, int group, int row_off
   const float4* sc = reinterpret_cast<const float4*>(scale);
   const float4* bi = reinterpret_cast<const float4*>(bias);
   OutT* orow = out + static_cast<size_t>(warp) * ldy;
+  if constexpr (std::is_same<OutT, __nv_fp8_e4m3>::value) {
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int idx = lane + 32 * i;
+      if (idx < nv) {
+        const float4 g = __ldg(sc + idx), b = __ldg(bi + idx);
+        v[i].x = (v[i].x - mean) * rstd * g.x + b.x;
+        v[i].y = (v[i].y - mean) * rstd * g.y + b.y;
+        v[i].z = (v[i].z - mean) * rstd * g.z + b.z;
+        v[i].w = (v[i].w - mean) * rstd * g.w + b.w;
+        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+      }
+    }
+    const int k = e4m3_scale_exp(warp_max(amax));
+    const float inv_s = ldexpf(1.0f, -k);
+    if (lane == 0) row_scale[warp] = ldexpf(1.0f, k);
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int idx = lane + 32 * i;
+      if (idx < nv)
+        reinterpret_cast<uint32_t*>(orow)[idx] = e4m3x4_rn(v[i].x * inv_s, v[i].y * inv_s, v[i].z * inv_s, v[i].w * inv_s);
+    }
+  } else {
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     const int idx = lane + 32 * i;
@@ -62,7 +88,7 @@ layernorm_kernel(const float* __restrict__ x, size_t ldx, int group, int row_off
         reinterpret_cast<float4*>(orow)[idx] = make_float4(round_tf32(y.x), round_tf32(y.y), round_tf32(y.z), round_tf32(y.w));
       } else if constexpr (sizeof(OutT) == 4) {
         reinterpret_cast<float4*>(orow)[idx] = y;
-      } else {
+      } else if constexpr (sizeof(OutT) == 2) {
         uint2 p;
         constexpr int ot = std::is_same<OutT, __half>::value ? 1 : 2;
         p.x = pack2(y.x, y.y, ot);
@@ -71,31 +97,35 @@ layernorm_kernel(const float* __restrict__ x, size_t ldx, int group, int row_off
       }
     }
   }
+  }
 }
 
 template <typename OutT>
 static int ln_launch(const float* x, int ldx, int group, int row_off, const int* row_index, const float* scale, const float* bias,
-                     float eps, void* out, int ldy, int rows, int D, cudaStream_t stream, int reverse) {
+                     float eps, void* out, int ldy, int rows, int D, cudaStream_t stream, int reverse, float* row_scale = nullptr) {
   const int threads = 256, wpb = threads / 32;
   const int grid = (rows + wpb - 1) / wpb;
   const int nv = D / 4;
   if (nv <= 32 * 8)
     JIMM_CUDA_CHECK(launch_k(layernorm_kernel<OutT, 8>, dim3(grid), dim3(threads), 0, stream, 1, true, x, ldx, group, row_off, row_index, scale, bias, eps,
-                             static_cast<OutT*>(out), ldy, rows, D, reverse));
+                             static_cast<OutT*>(out), ldy, rows, D, reverse, row_scale));
   else
     JIMM_CUDA_CHECK(launch_k(layernorm_kernel<OutT, 16>, dim3(grid), dim3(threads), 0, stream, 1, true, x, ldx, group, row_off, row_index, scale, bias, eps,
-                             static_cast<OutT*>(out), ldy, rows, D, reverse));
+                             static_cast<OutT*>(out), ldy, rows, D, reverse, row_scale));
   note_launch();
   return 0;
 }
 
 int layernorm_run(const float* x, int ldx, int group, int row_off, const int* row_index, const float* scale, const float* bias,
-                  float eps, void* out, int out_type, int ldy, int rows, int D, cudaStream_t stream, int reverse) {
+                  float eps, void* out, int out_type, int ldy, int rows, int D, cudaStream_t stream, int reverse, float* row_scale) {
   if (D % 4 != 0 || D > 2048 || ldx % 4 != 0 || ldy % 4 != 0) {
     set_last_error("layernorm: D=%d must be a multiple of 4 and <= 2048 (ldx=%d ldy=%d)", D, ldx, ldy);
     return -1;
   }
+  if (out_type == DT_E4M3 && row_scale == nullptr) { set_last_error("layernorm: e4m3 output needs a row-scale vector"); return -1; }
   if (rows <= 0) return 0;
+  if (out_type == DT_E4M3)
+    return ln_launch<__nv_fp8_e4m3>(x, ldx, group, row_off, row_index, scale, bias, eps, out, ldy, rows, D, stream, reverse, row_scale);
   if (out_type == DT_F32) return ln_launch<float>(x, ldx, group, row_off, row_index, scale, bias, eps, out, ldy, rows, D, stream, reverse);
   if (out_type == DT_TF32) return ln_launch<tf32_t>(x, ldx, group, row_off, row_index, scale, bias, eps, out, ldy, rows, D, stream, reverse);
   if (out_type == DT_F16) return ln_launch<__half>(x, ldx, group, row_off, row_index, scale, bias, eps, out, ldy, rows, D, stream, reverse);
@@ -371,6 +401,38 @@ int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, 
   else if (out_type == DT_TF32) transpose_cast_kernel<tf32_t><<<grid, block, 0, stream>>>(src, K, N, static_cast<tf32_t*>(dst), ldd);
   else if (out_type == DT_F16) transpose_cast_kernel<__half><<<grid, block, 0, stream>>>(src, K, N, static_cast<__half*>(dst), ldd);
   else transpose_cast_kernel<__nv_bfloat16><<<grid, block, 0, stream>>>(src, K, N, static_cast<__nv_bfloat16*>(dst), ldd);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+// FP8 weight quantiser (finalize): one warp per row of K fp32 values; K, lds, ldo multiples of 4.
+__global__ void __launch_bounds__(256)
+quantize_rows_e4m3_kernel(const float* __restrict__ src, size_t lds, int rows, int K4, uint32_t* __restrict__ out, size_t ldo4,
+                          float* __restrict__ row_scale) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= rows) return;
+  const float4* r = reinterpret_cast<const float4*>(src + static_cast<size_t>(warp) * lds);
+  float amax = 0.f;
+  for (int i = lane; i < K4; i += 32) {
+    const float4 v = r[i];
+    amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+  const int k = e4m3_scale_exp(warp_max(amax));
+  const float inv_s = ldexpf(1.0f, -k);
+  if (lane == 0) row_scale[warp] = ldexpf(1.0f, k);
+  uint32_t* o = out + static_cast<size_t>(warp) * ldo4;
+  for (int i = lane; i < K4; i += 32) {
+    const float4 v = r[i];
+    o[i] = e4m3x4_rn(v.x * inv_s, v.y * inv_s, v.z * inv_s, v.w * inv_s);
+  }
+}
+int quantize_rows_e4m3_run(const float* src, int lds, int rows, int K, void* out, int ldo, float* row_scale, cudaStream_t stream) {
+  if (K <= 0 || K % 4 != 0 || lds % 4 != 0 || ldo % 4 != 0 || lds < K || ldo < K) {
+    set_last_error("quantize_rows_e4m3: K=%d, lds=%d and ldo=%d must be multiples of 4 with lds, ldo >= K", K, lds, ldo);
+    return -1;
+  }
+  if (rows <= 0) return 0;
+  quantize_rows_e4m3_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(src, lds, rows, K / 4, static_cast<uint32_t*>(out), ldo / 4, row_scale);
   JIMM_LAUNCH_CHECK();
   return 0;
 }

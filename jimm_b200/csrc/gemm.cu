@@ -1,6 +1,7 @@
 // Persistent, warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
 //   C[M,N] = epi( A[M,K] . B[N,K]^T ),  A/B K-major fp16 | bf16 | fp32(tf32), fp32 accumulate in registers.
+//   e4m3 operands (FP8 compute mode) run gemm_e4m3_kernel below: same structure, 64 x 256 tiles, K-slab promotion, row / column scales.
 //
 // CTA = 384 threads (three warpgroups), 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin 128 x 256 tile schedule (n fastest).
 //   warpgroup 0, warp 0 : TMA producer (one lane): 4-stage smem ring of {A 128x128B, B 256x128B} tiles (48 KB), SWIZZLE_128B
@@ -73,6 +74,8 @@ struct EpiDev {
   int* ln_cnt;
   int ln_out_type, ln_ldo;
   float ln_eps;
+  const float* a_scale;  // e4m3 operands: dequantisation scales (see GemmEpilogue)
+  const float* b_scale;
 };
 
 template <int ACT>
@@ -120,6 +123,8 @@ template <>
 struct Traits<float> {
   static constexpr int KIND = 2;
 };
+template <typename T>
+constexpr bool kScaled = std::is_same<T, __nv_fp8_e4m3>::value;  // the accumulator is multiplied by a_scale[row] * b_scale[col]
 
 // ---- fused LayerNorm of completed 32-row groups (reduce-add epilogue) --------------------------------------------------------------
 // Who normalises: NOT the consumer warps, whose next tile would wait for them.  The consumer warps only PUBLISH (wait for their
@@ -268,16 +273,22 @@ __device__ __forceinline__ void ln_worker(const EpiDev& e, LnQueue* q, int lane)
 
 // ---- TMA epilogue of one consumer warp: its 16 rows x BN columns, thread (g = lane / 4, t = lane % 4) holds rows g and g + 8,
 // columns 8 j + 2 t (+1) of the wgmma accumulator.  16-bit outputs: 64 columns per 16 x 128 B box; 32-bit outputs: 32 columns.
-template <int OUT, int ACT>
-__device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const EpiDev& epi, const float (&acc)[128], uint8_t* tbuf0, int lane,
+// NC: the warp's columns (BN, or 128 in the e4m3 kernel), acc[NC / 2] its accumulators
+template <int OUT, int ACT, bool SCALED, int NC = BN>
+__device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const EpiDev& epi, const float (&acc)[NC / 2], uint8_t* tbuf0, int lane,
                                              int row_base, int n_tile0, uint32_t& box_count) {
   constexpr bool OUT16 = (OUT == OUT_H16 || OUT == OUT_BF16);
   constexpr int ES = OUT16 ? 2 : 4;
   constexpr int COLS_PER_BOX = 128 / ES;
   constexpr int JB = COLS_PER_BOX / 8;  // accumulator n-blocks per box
   const int g = lane >> 2, t = lane & 3;
+  float sa0 = 1.f, sa1 = 1.f;  // row scales of rows g and g + 8 (rows >= M of the last box read row M - 1's: never stored past the box)
+  if constexpr (SCALED) {
+    sa0 = __ldg(epi.a_scale + min(row_base + g, epi.M - 1));
+    sa1 = __ldg(epi.a_scale + min(row_base + g + 8, epi.M - 1));
+  }
 #pragma unroll
-  for (int s = 0; s < BN / COLS_PER_BOX; ++s) {
+  for (int s = 0; s < NC / COLS_PER_BOX; ++s) {
     const int n0 = n_tile0 + s * COLS_PER_BOX;
     if (n0 >= epi.N) break;
     uint8_t* tbuf = tbuf0 + (box_count & (EPI_BUFS - 1)) * EPI_BUF_BYTES;
@@ -290,8 +301,14 @@ __device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const Epi
       const int col = n0 + jj * 8 + 2 * t;
       float2 b2 = make_float2(0.f, 0.f);
       if (epi.bias != nullptr && col < epi.N) b2 = __ldg(reinterpret_cast<const float2*>(epi.bias + col));
-      const float v0 = act_ct<ACT>(acc[4 * j] + b2.x), v1 = act_ct<ACT>(acc[4 * j + 1] + b2.y);
-      const float v2 = act_ct<ACT>(acc[4 * j + 2] + b2.x), v3 = act_ct<ACT>(acc[4 * j + 3] + b2.y);
+      float a0 = acc[4 * j], a1 = acc[4 * j + 1], a2 = acc[4 * j + 2], a3 = acc[4 * j + 3];
+      if constexpr (SCALED) {  // products of two powers of two: exact, in any order
+        float2 s2 = make_float2(0.f, 0.f);
+        if (col < epi.N) s2 = __ldg(reinterpret_cast<const float2*>(epi.b_scale + col));
+        a0 *= sa0 * s2.x; a1 *= sa0 * s2.y; a2 *= sa1 * s2.x; a3 *= sa1 * s2.y;
+      }
+      const float v0 = act_ct<ACT>(a0 + b2.x), v1 = act_ct<ACT>(a1 + b2.y);
+      const float v2 = act_ct<ACT>(a2 + b2.x), v3 = act_ct<ACT>(a3 + b2.y);
       const int byte = (jj * 8 + 2 * t) * ES;
       // 128-byte swizzle: 16-byte chunk c of row r lives at chunk c ^ (r % 8); rows g and g + 8 share r % 8 = g
       const int off = ((((byte >> 4) ^ g)) << 4) + (byte & 15);
@@ -328,7 +345,8 @@ __device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const Epi
 }
 
 // ---- generic LSU epilogue (run-time flags; any N, row remap, row-add, residual read) ---------------------------------
-__device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float (&acc)[128], int lane, int row_base, int n_tile0) {
+template <bool SCALED, int NC = BN>
+__device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float (&acc)[NC / 2], int lane, int row_base, int n_tile0) {
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -336,13 +354,16 @@ __device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float 
     if (row >= epi.M) continue;
     int out_row, add_row;
     remap_row(epi, row, out_row, add_row);
+    float sa = 1.f;
+    if constexpr (SCALED) sa = __ldg(epi.a_scale + row);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
+    for (int j = 0; j < NC / 8; ++j) {
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int col = n_tile0 + 8 * j + 2 * t + q;
         if (col < epi.N) {
           float v = acc[4 * j + 2 * h + q];
+          if constexpr (SCALED) v *= sa * __ldg(epi.b_scale + col);
           if (epi.bias) v += __ldg(epi.bias + col);
           v = apply_act(v, epi.act);
           if (epi.rowadd) v += __ldg(epi.rowadd + static_cast<size_t>(add_row) * epi.N + col);
@@ -468,9 +489,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       const int row_base = m_blk * BM + wg * 64 + wq * 16;
       const int n_tile0 = n_blk * BN;
       if constexpr (OUT == OUT_GENERIC) {
-        epilogue_generic(epi, acc, lane, row_base, n_tile0);
+        epilogue_generic<false>(epi, acc, lane, row_base, n_tile0);
       } else {
-        if (row_base < M) epilogue_tma<OUT, EPI_ACT>(&map_c, epi, acc, tbuf0, lane, row_base, n_tile0, box_count);
+        if (row_base < M) epilogue_tma<OUT, EPI_ACT, false>(&map_c, epi, acc, tbuf0, lane, row_base, n_tile0, box_count);
         if constexpr (FUSE_LN) {
           // Publishing is deferred by one tile: the PREVIOUS tile's reduce-adds were issued a whole mainloop ago, so waiting for them
           // costs nothing.  Both 16-row halves of a 32-row group publish, also a half that lies beyond M.
@@ -485,6 +506,115 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (ln_rg >= 0) ln_publish(epi, lnq, ln_rg, ln_cols);
         __threadfence_block();
         atomicAdd(&lnq->done, 1);
+      }
+    }
+    if constexpr (OUT != OUT_GENERIC) {
+      if (lane == 0) tma_store_wait_all();
+    }
+  }
+}
+
+// ---- e4m3 operands ---------------------------------------------------------------------------------------------------------------
+// The e4m3 wgmma does not accumulate in full fp32: its sums of products lose low-order bits (about 5e-4 of sum |a b| at K = 768..2048
+// on an H100, measured with m64n256k32), which puts an FP8 model at about a third of its whole FP8 error away from an exact-accumulation
+// restatement.  So each 128-deep K slab (four m64n128k32 wgmmas) is accumulated from zero and then added to fp32 registers ("promotion").
+// The 64 promoted sums plus 64 accumulators per thread fit where m64n256 would need 256, so the CTA tile is 64 x 256: both consumer
+// warpgroups take the same 64 A rows, warpgroup wg columns [128 wg, 128 wg + 128) of the B tile.  Same ring, barriers, register split,
+// tile walk and epilogues as gemm_wgmma_kernel (plain stores only).
+static constexpr int BM8 = 64;
+static constexpr int STAGE_BYTES8 = BM8 * 128 + B_STAGE_BYTES;  // bytes one stage's TMA loads bring
+
+template <int OUT, int ACT>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_e4m3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                 const __grid_constant__ CUtensorMap map_c, const EpiDev epi, int K) {
+  constexpr int BK = 128;  // one 128-byte swizzle atom along K per stage
+  constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NUM_THREADS * KERNEL_REGS, "register split exceeds the CTA's allocation");
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+  uint8_t* epi_stage = smem + STAGES * STAGE_BYTES;
+  LnQueue* lnq = reinterpret_cast<LnQueue*>(epi_stage + EPI_STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(lnq + 1);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int M = epi.M, N = epi.N;
+  const int m_tiles = (M + BM8 - 1) / BM8, n_tiles = (N + BN - 1) / BN;
+  const int num_tiles = m_tiles * n_tiles;
+  const int num_kb = (K + BK - 1) / BK;
+
+  pdl_launch_dependents();
+  if (warp_idx == 0 && lane == 0) {
+    tma_prefetch_desc(&map_a);
+    tma_prefetch_desc(&map_b);
+    if constexpr (OUT != OUT_GENERIC) tma_prefetch_desc(&map_c);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], EPI_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp_idx < 4) {
+    setmaxnreg<KERNEL_REGS, PRODUCER_REGS>();
+    if (warp_idx == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
+        const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES8);
+          tma_load_2d(smem_a + stage * A_STAGE_BYTES, &map_a, &full_bar[stage], kb * BK, m_blk * BM8);
+          tma_load_2d(smem_b + stage * B_STAGE_BYTES, &map_b, &full_bar[stage], kb * BK, n_blk * BN);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg<KERNEL_REGS, CONSUMER_REGS>();
+    const int wg = (warp_idx - 4) >> 2;  // consumer warpgroup: columns [128 wg, 128 wg + 128) of the tile
+    const int wq = warp_idx & 3;         // warp within the warpgroup: rows [16 wq, 16 wq + 16)
+    uint8_t* tbuf0 = epi_stage + (warp_idx - 4) * EPI_BUFS * EPI_BUF_BYTES;
+    int stage = 0;
+    uint32_t phase = 0, box_count = 0;
+    float acc[64], sum[64];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
+      const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = make_wgmma_desc_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES));
+        const uint64_t bdesc = make_wgmma_desc_sw128(smem_u32(smem_b + stage * B_STAGE_BYTES + wg * 128 * 128));
+        wgmma_fence_operands(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 32; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
+          wgmma_m64n128k32_e4m3_ss(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      const int row_base = m_blk * BM8 + wq * 16;
+      const int n_tile0 = n_blk * BN + wg * 128;
+      if constexpr (OUT == OUT_GENERIC) {
+        epilogue_generic<true, 128>(epi, sum, lane, row_base, n_tile0);
+      } else {
+        if (row_base < M && n_tile0 < N) epilogue_tma<OUT, ACT, true, 128>(&map_c, epi, sum, tbuf0, lane, row_base, n_tile0, box_count);
       }
     }
     if constexpr (OUT != OUT_GENERIC) {
@@ -516,6 +646,7 @@ __global__ void gemm_simt_kernel(const T* __restrict__ A, int lda, const T* __re
     int out_row, add_row;
     remap_row(epi, row, out_row, add_row);
     float v = acc;
+    if constexpr (kScaled<T>) v *= epi.a_scale[row] * epi.b_scale[col];
     if (epi.bias) v += epi.bias[col];
     v = apply_act(v, epi.act);
     if (epi.rowadd) v += epi.rowadd[static_cast<size_t>(add_row) * epi.N + col];
@@ -553,6 +684,7 @@ static int make_map(CUtensorMap* map, int dtype, const void* ptr, int rows, int 
   if (!enc) return -3;
   const size_t es = dtype_size(dtype);
   CUtensorMapDataType dt = (dtype == DT_F32 || dtype == DT_TF32) ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                           : dtype == DT_E4M3                    ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                            : (dtype == DT_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * es};
@@ -614,10 +746,24 @@ static int check_epi(const GemmEpilogue& e, int N) {
   if (e.ldo < N) { set_last_error("gemm: ldo (%d) < N (%d)", e.ldo, N); return -1; }
   return 0;
 }
+// e4m3 operands take the plain-store epilogues only (bias, activation; modes 0 / 1 / 2) and need both scale vectors
+static int check_e4m3_epi(const GemmEpilogue& e) {
+  if (e.a_scale == nullptr || e.b_scale == nullptr) { set_last_error("gemm: e4m3 operands need row scales for A and B"); return -1; }
+  if ((reinterpret_cast<uintptr_t>(e.b_scale) & 7) != 0) { set_last_error("gemm: the B scales must be 8-byte aligned"); return -1; }
+  if (e.residual || e.rowadd || e.rows_in != 0 || e.tok_pad != 0 || e.ln_cnt) {
+    set_last_error("gemm: e4m3 operands support bias and activation epilogues only (no residual, row-add, row remap, token scatter or "
+                   "fused LayerNorm)");
+    return -1;
+  }
+  return 0;
+}
 int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K,
                    const GemmEpilogue& epi) {
   if (M <= 0 || N <= 0 || K <= 0) { set_last_error("gemm: bad shape %dx%dx%d", M, N, K); return -1; }
   if (int rc = check_epi(epi, N)) return rc;
+  if (dtype == DT_E4M3) {
+    if (int rc = check_e4m3_epi(epi)) return rc;
+  }
   // the token scatter exists only as the TMA reduce-add: every other epilogue would ignore tok_* and write the plain row layout
   if (epi.tok_pad != 0) {
     if (epi.tok_pad < 0 || epi.tok_pad % EPI_BOX_ROWS != 0 || M % epi.tok_pad != 0 || epi.tok_off < 0 || epi.tok_S <= 0) {
@@ -630,7 +776,7 @@ int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void
       return -1;
     }
   }
-  if (int rc = make_map(&plan->map_a, dtype, A, M, K, lda, BM)) return rc;
+  if (int rc = make_map(&plan->map_a, dtype, A, M, K, lda, dtype == DT_E4M3 ? BM8 : BM)) return rc;
   if (int rc = make_map(&plan->map_b, dtype, B, N, K, ldb, BN)) return rc;
   plan->M = M; plan->N = N; plan->K = K; plan->dtype = dtype; plan->epi = epi;
   memset(&plan->map_c, 0, sizeof(plan->map_c));
@@ -668,26 +814,35 @@ static EpiDev to_dev(const GemmEpilogue& e, int M, int N) {
   d.reverse = e.reverse;
   d.ln_scale = e.ln_scale; d.ln_bias = e.ln_bias; d.ln_out = e.ln_out; d.ln_cnt = e.ln_cnt;
   d.ln_out_type = e.ln_out_type; d.ln_ldo = e.ln_ldo; d.ln_eps = e.ln_eps;
+  d.a_scale = e.a_scale; d.b_scale = e.b_scale;
   return d;
 }
 
 template <typename T, int OUT, int ACT>
+static auto kernel_of() {
+  if constexpr (kScaled<T>) return gemm_e4m3_kernel<OUT, ACT>;
+  else return gemm_wgmma_kernel<T, OUT, ACT>;
+}
+
+template <typename T, int OUT, int ACT>
 static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
+  auto* kernel = kernel_of<T, OUT, ACT>();
+  const int bm = kScaled<T> ? BM8 : BM;
   static DeviceOnce attr_set;
   if (attr_set.first()) {
-    JIMM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<T, OUT, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     // setmaxnreg moves registers within the launch allocation: with fewer than KERNEL_REGS per thread, an increase would wait forever
     cudaFuncAttributes fa;
-    JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, gemm_wgmma_kernel<T, OUT, ACT>));
+    JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
     if (fa.numRegs != KERNEL_REGS) {
       set_last_error("gemm: kernel compiled with %d registers per thread, the warpgroup register split assumes %d", fa.numRegs, KERNEL_REGS);
       return -2;
     }
   }
-  const int tiles = ((M + BM - 1) / BM) * ((p->N + BN - 1) / BN);
+  const int tiles = ((M + bm - 1) / bm) * ((p->N + BN - 1) / BN);
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-  JIMM_CUDA_CHECK(launch_k(gemm_wgmma_kernel<T, OUT, ACT>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, 1, true, p->map_a, p->map_b,
-                           p->map_c, to_dev(p->epi, M, p->N), p->K));
+  JIMM_CUDA_CHECK(launch_k(kernel, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, 1, true, p->map_a, p->map_b, p->map_c,
+                           to_dev(p->epi, M, p->N), p->K));
   note_launch();
   return 0;
 }
@@ -705,7 +860,9 @@ template <typename T>
 static int launch_tc(const GemmPlan* p, int M, cudaStream_t stream) {
   const GemmEpilogue& e = p->epi;
   if (e.mode != 2) return launch_one<T, OUT_GENERIC, ACT_NONE>(p, M, stream);
-  if (e.residual) return gemm_fuses_ln(p, M) ? launch_one<T, OUT_F32_ADD, ACT_FUSE_LN>(p, M, stream) : launch_one<T, OUT_F32_ADD, ACT_NONE>(p, M, stream);
+  if constexpr (!kScaled<T>) {  // gemm_plan_init gives e4m3 plans no residual
+    if (e.residual) return gemm_fuses_ln(p, M) ? launch_one<T, OUT_F32_ADD, ACT_FUSE_LN>(p, M, stream) : launch_one<T, OUT_F32_ADD, ACT_NONE>(p, M, stream);
+  }
   switch (e.out_type) {
     case DT_F16: return launch_act<T, OUT_H16>(p, M, stream);
     case DT_BF16: return launch_act<T, OUT_BF16>(p, M, stream);
@@ -739,6 +896,7 @@ int gemm_plan_run(const GemmPlan* p0, int M_override, cudaStream_t stream, int r
     case DT_BF16: return launch_tc<__nv_bfloat16>(p, M, stream);
     case DT_F32:
     case DT_TF32: return launch_tc<float>(p, M, stream);
+    case DT_E4M3: return launch_tc<__nv_fp8_e4m3>(p, M, stream);
   }
   set_last_error("gemm: bad dtype %d", p->dtype);
   return -1;
@@ -747,10 +905,14 @@ int gemm_plan_run(const GemmPlan* p0, int M_override, cudaStream_t stream, int r
 int gemm_simt_run(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmEpilogue& epi,
                   cudaStream_t stream) {
   if (int rc = check_epi(epi, N)) return rc;
+  if (dtype == DT_E4M3) {
+    if (int rc = check_e4m3_epi(epi)) return rc;
+  }
   dim3 block(16, 16), grid((N + 15) / 16, (M + 15) / 16);
   EpiDev d = to_dev(epi, M, N);
   if (dtype == DT_F16) gemm_simt_kernel<__half><<<grid, block, 0, stream>>>(static_cast<const __half*>(A), lda, static_cast<const __half*>(B), ldb, K, d);
   else if (dtype == DT_BF16) gemm_simt_kernel<__nv_bfloat16><<<grid, block, 0, stream>>>(static_cast<const __nv_bfloat16*>(A), lda, static_cast<const __nv_bfloat16*>(B), ldb, K, d);
+  else if (dtype == DT_E4M3) gemm_simt_kernel<__nv_fp8_e4m3><<<grid, block, 0, stream>>>(static_cast<const __nv_fp8_e4m3*>(A), lda, static_cast<const __nv_fp8_e4m3*>(B), ldb, K, d);
   else gemm_simt_kernel<float><<<grid, block, 0, stream>>>(static_cast<const float*>(A), lda, static_cast<const float*>(B), ldb, K, d);
   JIMM_LAUNCH_CHECK();
   return 0;

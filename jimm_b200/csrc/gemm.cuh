@@ -15,10 +15,12 @@ namespace jimm {
 
 // DT_TF32: stored as fp32 with the value rounded (to nearest) to tf32 -- the operand format of the fp32 compute mode, so the
 // tensor core's truncation of the low 13 mantissa bits is exact.  Only ever an internal buffer / operand type.
-enum DType : int { DT_F32 = 0, DT_F16 = 1, DT_BF16 = 2, DT_TF32 = 3 };
+// DT_E4M3: float8 e4m3 (fn) operand with power-of-two scales kept beside it (one per A row, one per B row); the FP8 compute mode's
+// QKV / FC1 operands.
+enum DType : int { DT_F32 = 0, DT_F16 = 1, DT_BF16 = 2, DT_TF32 = 3, DT_E4M3 = 4 };
 enum Act : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_QUICK_GELU = 2 };
 
-inline size_t dtype_size(int dt) { return (dt == DT_F32 || dt == DT_TF32) ? 4 : 2; }
+inline size_t dtype_size(int dt) { return (dt == DT_F32 || dt == DT_TF32) ? 4 : dt == DT_E4M3 ? 1 : 2; }
 
 // Output tile of one CTA (M rows x N columns).  A GEMM runs ceil(M / GEMM_TILE_M) x ceil(N / GEMM_TILE_N) tiles on at most one CTA per
 // SM, so its time goes in waves of that many tiles.
@@ -56,12 +58,17 @@ struct GemmEpilogue {
   int ln_out_type = DT_F16, ln_ldo = 0;
   float ln_eps = 1e-6f;
   int* ln_cnt = nullptr;
+  // DT_E4M3 operands only (required there, ignored otherwise): fp32 dequantisation scales, a_scale [rows of A] and b_scale [N];
+  // the accumulator is multiplied by a_scale[row] * b_scale[col] before the bias.  FP8 plans take the plain stores only (bias,
+  // activation; no residual, row remap, row-add, token scatter or fused LayerNorm).
+  const float* a_scale = nullptr;
+  const float* b_scale = nullptr;
 };
 
 struct GemmPlan {
   CUtensorMap map_a, map_b, map_c;  // map_c: output (mode 2 only)
   int M = 0, N = 0, K = 0;
-  int dtype = DT_F16;  // operand type: DT_F16 / DT_BF16 / DT_F32 (tf32 MMA)
+  int dtype = DT_F16;  // operand type: DT_F16 / DT_BF16 / DT_F32 (tf32 MMA) / DT_E4M3
   GemmEpilogue epi;
 };
 

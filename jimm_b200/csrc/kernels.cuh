@@ -13,8 +13,14 @@ namespace jimm {
 // nnx.LayerNorm (fast variance, fp32 statistics) over fp32 rows.  SURVEY 8a row a3.
 //   src row for output r:  r * group + (row_index ? row_index[r] : row_off)      (row stride ldx elements)
 //   out[r, :] (type out_type, row stride ldy) = (x - mean) * rsqrt(max(0, E[x^2]-mean^2) + eps) * scale + bias
+//   out_type DT_E4M3: out[r, :] = e4m3(y / s_r), row_scale[r] = s_r (power of two from the row's absolute maximum; ldy in bytes)
 int layernorm_run(const float* x, int ldx, int group, int row_off, const int* row_index, const float* scale, const float* bias,
-                  float eps, void* out, int out_type, int ldy, int rows, int D, cudaStream_t stream, int reverse = 0);
+                  float eps, void* out, int out_type, int ldy, int rows, int D, cudaStream_t stream, int reverse = 0,
+                  float* row_scale = nullptr);
+
+// Weight quantiser of the FP8 compute mode: each row of an fp32 [rows, K] matrix (row stride lds) -> e4m3 row of out (row stride ldo
+// bytes) and its scale row_scale[r], by the same rule as the e4m3 LayerNorm.  One warp per row.
+int quantize_rows_e4m3_run(const float* src, int lds, int rows, int K, void* out, int ldo, float* row_scale, cudaStream_t stream);
 
 // Patchify: NHWC image (in_type fp32/fp16/bf16) -> A matrix [B*gh*gw, P*P*C] of out_type, row order (b,gy,gx), column
 // order (ky,kx,c) == the HWIO kernel reshape (common/vit.py:153-165,228-230).  128-bit loads.

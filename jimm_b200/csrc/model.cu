@@ -98,8 +98,9 @@ struct HostParam {
 };
 
 struct LinearW {
-  void* w = nullptr;   // [N, K] compute dtype, K-major
+  void* w = nullptr;   // [N, K] compute dtype, K-major (e4m3 for the FP8 mode's QKV / FC1)
   float* b = nullptr;  // [N] fp32 or null
+  float* ws = nullptr; // [N] fp32 row scales of an e4m3 w, else null
   int N = 0, K = 0;
 };
 struct LNW {
@@ -164,6 +165,8 @@ struct TextWs {
   void* pooled = nullptr; // [Bmax, Dt]
   int* idx = nullptr;     // [Bmax] EOT positions
   int* ln_cnt = nullptr;  // fused-LayerNorm completion counters, one per 32 rows
+  void* h8 = nullptr;     // FP8 mode: e4m3 LayerNorm out [Bmax*T, Dt] ...
+  float* sa = nullptr;    // ... and its row scales [Bmax*T]
 };
 
 struct Workspace {
@@ -180,6 +183,8 @@ struct Workspace {
   float* nrm_t = nullptr;
   void* in_img = nullptr; // host-path staging: image batch (fp32 worst case)
   int* ln_cnt = nullptr;     // fused-LayerNorm completion counters (one per 32 rows of the residual stream), zero between launches
+  void* h8 = nullptr;        // FP8 mode: e4m3 block LayerNorm out [Tmax, Dmax] (the QKV / FC1 A operand) ...
+  float* sa = nullptr;       // ... and its row scales [Tmax]
   uint8_t* in_u8 = nullptr;  // host-path staging of raw uint8 RGB frames (jimm_vit_forward_host_u8); grown on demand
   size_t in_u8_bytes = 0;
   int32_t* in_ids = nullptr;
@@ -198,6 +203,9 @@ struct jimm_model {
   int max_batch = 0;
   int cdt = DT_F16;    // compute dtype of GEMM operands
   int adt = DT_F16;    // dtype of the qkv / MAP-kv buffers consumed by the attention kernels (16-bit even in fp32 mode)
+  // FP8 compute mode (JIMM_F8E4M3): cdt / adt are fp16, except that the QKV and FC1 GEMMs of every encoder block take e4m3 operands
+  // with power-of-two scales per A row (written by the block LayerNorms) and per weight row (computed at finalize)
+  bool f8 = false;
   std::map<std::string, HostParam> host;
   DevPool pool;
   VisionTower vis;
@@ -258,12 +266,25 @@ static size_t cdt_size(const jimm_model* m) { return dtype_size(m->cdt); }
 // zeroed completion counters for the fused LayerNorm of a residual stream of `rows` rows (null when fusion is off)
 static int alloc_ln_counters(jimm_model* m, size_t rows, int** out) {
   *out = nullptr;
-  if (!m->fuse_ln || m->simt || m->epi_mode_res != 2) return 0;
+  // FP8 mode: the block LayerNorms write e4m3 rows with a row scale, which only the LayerNorm kernel computes
+  if (!m->fuse_ln || m->simt || m->epi_mode_res != 2 || m->f8) return 0;
   const size_t n = (rows + 31) / 32 + 1;
   void* p = nullptr;
   if (int rc = m->pool.alloc(&p, n * sizeof(int))) return rc;
   JIMM_CUDA_CHECK(cudaMemset(p, 0, n * sizeof(int)));
   *out = static_cast<int*>(p);
+  return 0;
+}
+
+// FP8 mode: the e4m3 block-LayerNorm output of a residual stream of `rows` x D and its row scales (null otherwise)
+static int alloc_f8_bufs(jimm_model* m, size_t rows, int D, void** h8, float** sa) {
+  *h8 = nullptr;
+  *sa = nullptr;
+  if (!m->f8) return 0;
+  void* p = nullptr;
+  JIMM_TRY(m->pool.alloc(h8, rows * D));
+  JIMM_TRY(m->pool.alloc(&p, rows * sizeof(float)));
+  *sa = static_cast<float*>(p);
   return 0;
 }
 
@@ -274,6 +295,8 @@ struct Packer {
   jimm_model* m;
   UploadRing ring;
   cudaStream_t stream = 0;
+  bool f32_tmp = false;  // pack weights as fp32 into a temporary buffer (the e4m3 quantiser's input), see e4m3()
+  int wtype() const { return f32_tmp ? DT_F32 : m->cdt; }
 
   // one synchronisation for the whole finalize
   void done() {
@@ -354,8 +377,8 @@ struct Packer {
     HostParam* hp = find(name, shape);
     if (!hp) return JIMM_ESTATE;
     if (hp->numel() != static_cast<size_t>(K) * N) { set_last_error("finalize: '%s' numel mismatch", name.c_str()); return JIMM_ESTATE; }
-    uint8_t* dst = static_cast<uint8_t*>(dst_base) + static_cast<size_t>(n0) * ldd * cdt_size(m);
-    if (hp->transposed) return rows_to_device(hp, N, K, dst, m->cdt, ldd);  // already [N, K]: cast-copy
+    uint8_t* dst = static_cast<uint8_t*>(dst_base) + static_cast<size_t>(n0) * ldd * dtype_size(wtype());
+    if (hp->transposed) return rows_to_device(hp, N, K, dst, wtype(), ldd);  // already [N, K]: cast-copy
     const size_t es = hp->esize(), row_bytes = static_cast<size_t>(N) * es;
     if (row_bytes > UploadRing::kCap) { set_last_error("finalize: '%s' row of %zu bytes exceeds the staging slot", name.c_str(), row_bytes); return JIMM_EINVAL; }
     const int per = static_cast<int>(UploadRing::kCap / row_bytes);
@@ -364,14 +387,15 @@ struct Packer {
       const int kc = K - k0 < per ? K - k0 : per;
       void* d = nullptr;
       JIMM_TRY(ring.stage(src + static_cast<size_t>(k0) * row_bytes, static_cast<size_t>(kc) * row_bytes, stream, &d));
-      JIMM_TRY(pack_transpose_run(d, hp->dtype, kc, N, dst, m->cdt, ldd, k0, stream));
+      JIMM_TRY(pack_transpose_run(d, hp->dtype, kc, N, dst, wtype(), ldd, k0, stream));
       JIMM_TRY(ring.commit(stream));
     }
     return 0;
   }
   int alloc_linear(LinearW* lw, int N, int K, bool bias) {
     lw->N = N; lw->K = K;
-    JIMM_TRY(m->pool.alloc(&lw->w, static_cast<size_t>(N) * K * cdt_size(m)));
+    if (f32_tmp) JIMM_CUDA_CHECK(cudaMallocAsync(&lw->w, static_cast<size_t>(N) * K * sizeof(float), stream));  // freed by e4m3()
+    else JIMM_TRY(m->pool.alloc(&lw->w, static_cast<size_t>(N) * K * cdt_size(m)));
     if (bias) {
       void* b = nullptr;
       JIMM_TRY(m->pool.alloc(&b, static_cast<size_t>(N) * sizeof(float)));
@@ -437,6 +461,30 @@ struct Packer {
     v->map_q = static_cast<float*>(dq);
     return 0;
   }
+  // FP8 mode: `pack` (which packs one linear layer through alloc_linear / pack_kernel) runs with fp32 weights into a temporary
+  // buffer, then each [N, K] row is quantised to e4m3 with its power-of-two scale (quantize_rows_e4m3_run) -- the same bytes from a
+  // flax-layout and from a transposed hand-off, since both pack to the same fp32 rows.
+  template <typename F>
+  int e4m3(LinearW* lw, F&& pack) {
+    f32_tmp = true;
+    const int rc = pack();
+    f32_tmp = false;
+    void* f32 = lw->w;
+    lw->w = nullptr;
+    if (rc) {
+      if (f32) cudaFreeAsync(f32, stream);
+      return rc;
+    }
+    void* q = nullptr;
+    void* sc = nullptr;
+    JIMM_TRY(m->pool.alloc(&q, static_cast<size_t>(lw->N) * lw->K));
+    JIMM_TRY(m->pool.alloc(&sc, static_cast<size_t>(lw->N) * sizeof(float)));
+    lw->w = q;
+    lw->ws = static_cast<float*>(sc);
+    JIMM_TRY(quantize_rows_e4m3_run(static_cast<const float*>(f32), lw->K, lw->N, lw->K, q, lw->K, lw->ws, stream));
+    JIMM_CUDA_CHECK(cudaFreeAsync(f32, stream));
+    return 0;
+  }
   int encoder(const std::string& prefix, Encoder* enc) {
     const EncoderCfg& c = enc->c;
     enc->blocks.resize(c.L);
@@ -445,9 +493,11 @@ struct Packer {
       BlockW& b = enc->blocks[i];
       JIMM_TRY(upload_ln(f + "norm1", c.D, &b.norm1));
       JIMM_TRY(upload_ln(f + "norm2", c.D, &b.norm2));
-      JIMM_TRY(fused_proj(f + "attn", {"query", "key", "value"}, c.D, c.H, &b.qkv));
+      auto qkv = [&]() { return fused_proj(f + "attn", {"query", "key", "value"}, c.D, c.H, &b.qkv); };
+      JIMM_TRY(m->f8 ? e4m3(&b.qkv, qkv) : qkv());
       JIMM_TRY(out_proj(f + "attn", c.D, c.H, &b.out));
-      JIMM_TRY(linear(f + "mlp.layers.0", c.D, c.M, true, &b.fc1));
+      auto fc1 = [&]() { return linear(f + "mlp.layers.0", c.D, c.M, true, &b.fc1); };
+      JIMM_TRY(m->f8 ? e4m3(&b.fc1, fc1) : fc1());
       JIMM_TRY(linear(f + "mlp.layers.3", c.M, c.D, true, &b.fc2));
     }
     return 0;
@@ -493,6 +543,8 @@ struct EncBufs {  // the activation buffers one encoder stack works in
   void* h;
   void* big;
   int* ln_cnt;  // completion counters of the fused LayerNorm (one per 32 rows; null = LayerNorm stays a kernel)
+  void* h8;     // FP8 mode: e4m3 block LayerNorm out (QKV / FC1 A operand) and its row scales; null otherwise
+  float* sa;
 };
 
 static int plan_encoder(jimm_model* m, Encoder* enc, int Tmax, EncBufs ws) {
@@ -504,16 +556,23 @@ static int plan_encoder(jimm_model* m, Encoder* enc, int Tmax, EncBufs ws) {
     if (ws.ln_cnt) { e.ln_scale = ln.scale; e.ln_bias = ln.bias; e.ln_out = ws.h; e.ln_out_type = m->cdt; e.ln_ldo = c.D; e.ln_eps = c.eps; e.ln_cnt = ws.ln_cnt; }
     return e;
   };
+  // QKV / FC1 read the block LayerNorm's output: e4m3 with row scales in FP8 mode
+  const int ln_t = m->f8 ? DT_E4M3 : m->cdt;
+  void* ln_h = m->f8 ? ws.h8 : ws.h;
+  auto scaled = [&](GemmEpilogue e, const LinearW& w) {
+    if (m->f8) { e.a_scale = ws.sa; e.b_scale = w.ws; }
+    return e;
+  };
   for (size_t bi = 0; bi < enc->blocks.size(); ++bi) {
     BlockW& b = enc->blocks[bi];
     // QKV: h[T,D] x Wqkv[3D,D]^T + b -> qkv (16-bit) [T,3D]
-    JIMM_TRY(gemm_plan_init(&b.p_qkv, m->cdt, ws.h, c.D, b.qkv.w, c.D, Tmax, 3 * c.D, c.D,
-                            epi_plain(b.qkv, ACT_NONE, ws.big, m->adt, 3 * c.D, m->epi_mode_16)));
+    JIMM_TRY(gemm_plan_init(&b.p_qkv, ln_t, ln_h, c.D, b.qkv.w, c.D, Tmax, 3 * c.D, c.D,
+                            scaled(epi_plain(b.qkv, ACT_NONE, ws.big, m->adt, 3 * c.D, m->epi_mode_16), b.qkv)));
     // out-proj: attn[T,D] x Wo[D,D]^T + bo + x -> x
     JIMM_TRY(gemm_plan_init(&b.p_out, m->cdt, ws.h, c.D, b.out.w, c.D, Tmax, c.D, c.D, with_ln(epi_residual(b.out, ws.x, c.D, m->epi_mode_res), b.norm2)));
     // FC1: h x W1^T + b1 -> act -> mid [T,M]
-    JIMM_TRY(gemm_plan_init(&b.p_fc1, m->cdt, ws.h, c.D, b.fc1.w, c.D, Tmax, c.M, c.D,
-                            epi_plain(b.fc1, act, ws.big, m->cdt, c.M, m->epi_mode_16)));
+    JIMM_TRY(gemm_plan_init(&b.p_fc1, ln_t, ln_h, c.D, b.fc1.w, c.D, Tmax, c.M, c.D,
+                            scaled(epi_plain(b.fc1, act, ws.big, m->cdt, c.M, m->epi_mode_16), b.fc1)));
     // FC2: mid x W2^T + b2 + x -> x
     GemmEpilogue e2 = epi_residual(b.fc2, ws.x, c.D, m->epi_mode_res);
     if (bi + 1 < enc->blocks.size()) e2 = with_ln(e2, enc->blocks[bi + 1].norm1);
@@ -544,14 +603,16 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   int dir = m->l2_alternate ? 1 : 0;  // the patch GEMM / embedding kernels ran forward -> the first LayerNorm runs backward
   auto flip = [&]() { const int d = dir; if (m->l2_alternate) dir ^= 1; return d; };
   bool h_ready = false;  // ws.h already holds norm1(x) of the coming block (written by the previous block's FC2 epilogue)
+  const int ln_t = m->f8 ? DT_E4M3 : m->cdt;  // the block LayerNorms feed QKV / FC1 (see plan_encoder)
+  void* ln_h = m->f8 ? ws.h8 : ws.h;
   for (BlockW& b : enc->blocks) {
-    if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ws.h, m->cdt, c.D, T, c.D, s, flip()));
-    JIMM_TRY(run_gemm(m, b.p_qkv, ws.h, c.D, b.qkv, T, s, flip()));
+    if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
+    JIMM_TRY(run_gemm(m, b.p_qkv, ln_h, c.D, b.qkv, T, s, flip()));
     JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_out, ws.h, c.D, b.out, T, s, flip()));  // + residual (+ norm2 -> ws.h when fused)
     if (m->simt || !gemm_fuses_ln(&b.p_out, T))
-      JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm2.scale, b.norm2.bias, c.eps, ws.h, m->cdt, c.D, T, c.D, s, flip()));
-    JIMM_TRY(run_gemm(m, b.p_fc1, ws.h, c.D, b.fc1, T, s, flip()));
+      JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm2.scale, b.norm2.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
+    JIMM_TRY(run_gemm(m, b.p_fc1, ln_h, c.D, b.fc1, T, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_fc2, ws.big, c.M, b.fc2, T, s, flip()));  // + residual (+ the next block's norm1 -> ws.h when fused)
     h_ready = !m->simt && gemm_fuses_ln(&b.p_fc2, T);
   }
@@ -589,7 +650,7 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, float
     if (v.pooling == JIMM_POOL_CLS) JIMM_TRY(cls_row_run(ws.x, v.cls, v.pos, B, S, D, s));
   }
   if (v.pre_norm) JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, ws.x, DT_F32, D, B * S, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt}));
+  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
   if (v.pooling == JIMM_POOL_CLS) {
     // ln_post is per-row, only row 0 of each sample is consumed (common/vit.py:244-246)
     if (v.head.N > 0) {
@@ -613,7 +674,7 @@ static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out,
   TextTower& t = m->txt;
   TextWs& ws = m->wt;
   JIMM_TRY(embed_run(ids, t.table, t.pos, ws.x, B, T, t.D, t.V, s));
-  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt}));
+  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
   if (t.pool == JIMM_TPOOL_EOT_ARGMAX) {
     JIMM_TRY(argmax_ids_run(ids, ws.idx, B, T, s));
     JIMM_TRY(layernorm_run(ws.x, t.D, T, 0, ws.idx, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
@@ -759,7 +820,8 @@ static int finalize_sub(jimm_model* m, int max_batch) {
   ws.out_dev_elems = Bm * D;
   JIMM_TRY(m->pool.alloc(&p, ws.out_dev_elems * sizeof(float))); ws.out_dev = static_cast<float*>(p);
   JIMM_TRY(alloc_ln_counters(m, Tv, &ws.ln_cnt));
-  if (c.kind == JIMM_ENCODER) JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt}));
+  JIMM_TRY(alloc_f8_bufs(m, Tv, D, &ws.h8, &ws.sa));
+  if (c.kind == JIMM_ENCODER) JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
   else JIMM_TRY(plan_map_head(m, static_cast<int>(Bm), static_cast<int>(Tv)));
   JIMM_CUDA_CHECK(cudaDeviceSynchronize());
   m->graph_max_batch = 0;
@@ -801,7 +863,15 @@ int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) 
   }
   const bool dual = cfg->kind == JIMM_CLIP || cfg->kind == JIMM_SIGLIP;
   if (check_heads(sub ? "" : "vision ", cfg->v_width, cfg->v_heads) || (dual && check_heads("text ", cfg->t_width, cfg->t_heads))) return JIMM_EINVAL;
-  if (cfg->compute_dtype < JIMM_F32 || cfg->compute_dtype > JIMM_BF16) { set_last_error("bad compute_dtype"); return JIMM_EINVAL; }
+  const int cd = cfg->compute_dtype;
+  if (cd != JIMM_F32 && cd != JIMM_F16 && cd != JIMM_BF16 && cd != JIMM_F8E4M3) { set_last_error("bad compute_dtype %d", cd); return JIMM_EINVAL; }
+  // FP8: an e4m3 [T, width] operand's rows are width bytes, and TMA rows are multiples of 16 bytes
+  if (cd == JIMM_F8E4M3 && (cfg->v_width % 16 != 0 || (dual && cfg->t_width % 16 != 0))) {
+    const bool vis = cfg->v_width % 16 != 0;
+    set_last_error("float8_e4m3fn compute: %s width %d must be a multiple of 16 (the e4m3 QKV / FC1 operand rows are width bytes)",
+                   vis ? (sub ? "model" : "vision") : "text", vis ? cfg->v_width : cfg->t_width);
+    return JIMM_EINVAL;
+  }
   if (sub && cfg->ctx_len <= 0) { set_last_error("sub-module handle: ctx_len (max tokens per sample) must be positive"); return JIMM_EINVAL; }
   if (!sub && (cfg->patch <= 0 || cfg->img_size < cfg->patch || cfg->in_ch <= 0)) {
     set_last_error("unsupported patch/img/channels (%d/%d/%d)", cfg->patch, cfg->img_size, cfg->in_ch);
@@ -833,7 +903,9 @@ int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) 
   jimm_model* m = new jimm_model();
   m->cfg = *cfg;
   m->device = device;
-  m->cdt = cfg->compute_dtype == JIMM_F32 ? DT_TF32 : cfg->compute_dtype;  // fp32 mode: operands rounded to tf32 when produced
+  m->f8 = cfg->compute_dtype == JIMM_F8E4M3;
+  // fp32 mode: operands rounded to tf32 when produced; FP8 mode: fp16 outside QKV / FC1
+  m->cdt = cfg->compute_dtype == JIMM_F32 ? DT_TF32 : m->f8 ? DT_F16 : cfg->compute_dtype;
   m->adt = cfg->compute_dtype == JIMM_BF16 ? DT_BF16 : DT_F16;
   const char* env = getenv("JIMM_GEMM_IMPL");
   m->simt = env && strcmp(env, "simt") == 0;
@@ -1015,14 +1087,16 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
     JIMM_TRY(gemm_plan_init(&v.p_patch, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(Bm) * v.n, D, PPC, e));
   }
   JIMM_TRY(alloc_ln_counters(m, Tv, &ws.ln_cnt));
-  JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt}));
+  JIMM_TRY(alloc_f8_bufs(m, Tv, D, &ws.h8, &ws.sa));
+  JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
   if (v.head.N > 0)
     JIMM_TRY(gemm_plan_init(&v.p_head, m->cdt, ws.pooled, D, v.head.w, D, static_cast<int>(Bm), v.head.N, D,
                             epi_plain(v.head, ACT_NONE, ws.out_dev, DT_F32, v.head.N, 0)));
   if (v.pooling == JIMM_POOL_MAP) JIMM_TRY(plan_map_head(m, static_cast<int>(Bm), static_cast<int>(Tv)));
   if (dual) {
     JIMM_TRY(alloc_ln_counters(m, Bm * t.T, &m->wt.ln_cnt));
-    JIMM_TRY(plan_encoder(m, &t.enc, static_cast<int>(Bm) * t.T, EncBufs{m->wt.x, m->wt.h, m->wt.big, m->wt.ln_cnt}));
+    JIMM_TRY(alloc_f8_bufs(m, Bm * t.T, t.D, &m->wt.h8, &m->wt.sa));
+    JIMM_TRY(plan_encoder(m, &t.enc, static_cast<int>(Bm) * t.T, EncBufs{m->wt.x, m->wt.h, m->wt.big, m->wt.ln_cnt, m->wt.h8, m->wt.sa}));
     JIMM_TRY(gemm_plan_init(&t.p_head, m->cdt, m->wt.pooled, t.D, t.head.w, t.D, static_cast<int>(Bm), t.D, t.D,
                             epi_plain(t.head, ACT_NONE, ws.out_dev, DT_F32, t.D, 0)));
   }
@@ -1178,7 +1252,7 @@ int jimm_encoder_forward(jimm_model_t* m, const float* x, int B, int S, float* o
   for (int b0 = 0; b0 < B; b0 += m->max_batch) {
     const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
     JIMM_CUDA_CHECK(cudaMemcpyAsync(m->ws.x, x + b0 * row, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    JIMM_TRY(run_encoder(m, &m->vis.enc, nb, S, s, EncBufs{m->ws.x, m->ws.h, m->ws.big, m->ws.ln_cnt}));
+    JIMM_TRY(run_encoder(m, &m->vis.enc, nb, S, s, EncBufs{m->ws.x, m->ws.h, m->ws.big, m->ws.ln_cnt, m->ws.h8, m->ws.sa}));
     JIMM_CUDA_CHECK(cudaMemcpyAsync(out + b0 * row, m->ws.x, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
   return 0;
@@ -1507,6 +1581,31 @@ int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off, const i
 int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
                      float eps, void* out, int out_type, int ldy, int rows, int D, void* stream) {
   return jimm_k_layernorm_ex(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, 0, stream);
+}
+int jimm_k_layernorm_e4m3(const float* x, int ldx, const float* scale, const float* bias, float eps, void* out, int ldy, float* row_scale,
+                          int rows, int D, int reverse, void* stream) {
+  return layernorm_run(x, ldx, 1, 0, nullptr, scale, bias, eps, out, DT_E4M3, ldy, rows, D, static_cast<cudaStream_t>(stream), reverse,
+                       row_scale);
+}
+int jimm_k_gemm_e4m3(int impl, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* a_scale, const float* b_scale,
+                     const float* bias, int act, void* out, int out_type, int ldo, int epi_mode, int plan_M, int reverse, void* stream) {
+  if (plan_M <= 0) plan_M = M;
+  if (M <= 0 || M > plan_M) { set_last_error("jimm_k_gemm_e4m3: need 0 < M <= plan_M (M=%d plan_M=%d)", M, plan_M); return JIMM_EINVAL; }
+  if (out_type < DT_F32 || out_type > DT_TF32) { set_last_error("jimm_k_gemm_e4m3: bad output type %d", out_type); return JIMM_EINVAL; }
+  GemmEpilogue e;
+  e.bias = bias; e.act = act; e.out = out; e.out_type = out_type; e.ldo = ldo; e.mode = epi_mode;
+  e.a_scale = a_scale; e.b_scale = b_scale;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (impl == 1) {
+    if (plan_M != M || reverse) { set_last_error("jimm_k_gemm_e4m3: the SIMT GEMM has no plan rows or reverse walk"); return JIMM_EINVAL; }
+    return gemm_simt_run(DT_E4M3, A, lda, B, ldb, M, N, K, e, s);
+  }
+  GemmPlan p;
+  JIMM_TRY(gemm_plan_init(&p, DT_E4M3, A, lda, B, ldb, plan_M, N, K, e));
+  return gemm_plan_run(&p, M, s, reverse);
+}
+int jimm_k_quantize_e4m3(const float* src, int lds, int rows, int K, void* out, int ldo, float* row_scale, void* stream) {
+  return quantize_rows_e4m3_run(src, lds, rows, K, out, ldo, row_scale, static_cast<cudaStream_t>(stream));
 }
 int jimm_k_attention_hd(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, int reverse,
                         void* stream) {

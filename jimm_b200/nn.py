@@ -77,20 +77,25 @@ def ones(shape):
     return torch.ones(shape, dtype=torch.float32)
 
 
-_DTYPE_NAMES = {"float32": _lib.F32, "float16": _lib.F16, "bfloat16": _lib.BF16, "half": _lib.F16, "float": _lib.F32}
+_DTYPE_NAMES = {"float32": _lib.F32, "float16": _lib.F16, "bfloat16": _lib.BF16, "half": _lib.F16, "float": _lib.F32,
+                "float8_e4m3fn": _lib.F8E4M3}
 
 
 def compute_dtype_code(dtype) -> int:
-    """Accept torch / numpy / jax.numpy dtypes or strings (the reference's `dtype: DTypeLike`)."""
+    """Accept torch / numpy / jax.numpy dtypes or strings (the reference's `dtype: DTypeLike`).
+
+    float8_e4m3fn selects the FP8 mode: float16 everywhere except the QKV and FC1 GEMMs of each encoder block, which run on e4m3
+    operands with power-of-two scales per token row and per output channel (parameters stay as loaded on the host; the weights are
+    quantised on the GPU).  It is not held to the 1e-3 parity of the other modes."""
     if dtype is None:
         return _lib.F32
-    if isinstance(dtype, int) and dtype in (_lib.F32, _lib.F16, _lib.BF16):
+    if isinstance(dtype, int) and dtype in (_lib.F32, _lib.F16, _lib.BF16, _lib.F8E4M3):
         return dtype
     name = getattr(dtype, "__name__", None) or getattr(dtype, "name", None) or str(dtype)
     name = name.replace("torch.", "").replace("jnp.", "")
     if name in _DTYPE_NAMES:
         return _DTYPE_NAMES[name]
-    raise ValueError(f"Unsupported dtype {dtype!r}: expected float32, float16 or bfloat16")
+    raise ValueError(f"Unsupported dtype {dtype!r}: expected float32, float16, bfloat16 or float8_e4m3fn")
 
 
 class LazyParam:

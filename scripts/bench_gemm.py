@@ -5,8 +5,10 @@
 
 (a) The four GEMMs of one encoder layer of vit_b16, siglip_b16 (vision tower) and vit_l16_map at the benchmark's batch, token count,
     width and operand type, with their epilogues: QKV (operand-type store), FC1 (+ tanh-GELU, operand-type store), and out-projection /
-    FC2 as the fp32 residual reduce-add with the fused LayerNorm (jimm_k_gemm_residual_ln).  CUDA events over --iters launches after a
-    warm-up.  Reported: TFLOP/s, and the bytes the CTAs fill from L2 into shared memory per FLOP with the library's tile shape.
+    FC2 as the fp32 residual reduce-add with the fused LayerNorm (jimm_k_gemm_residual_ln).  QKV and FC1 are also timed as the FP8
+    compute mode runs them (e4m3 operands with row scales, fp16 output; rows "qkv e4m3" / "fc1+gelu e4m3", with their speed-up over the
+    16-bit row).  CUDA events over --iters launches after a warm-up.  Reported: TFLOP/s, and the bytes the CTAs fill from L2 into shared
+    memory per FLOP with the library's tile shape.
 (b) jimm_k_l2_probe: TMA fills of 16 KB stages from an L2-resident buffer on every SM, mode 0 (each CTA its own tiles) and mode 2 with
     2-CTA clusters (each CTA loads half a tile and multicasts it to both).  Reported: bytes landed in shared memory per second.
 
@@ -101,6 +103,24 @@ def gemms(torch, lib, tile, iters: int) -> list:
             rows.append(dict(workload=wl, gemm=name, M=M, N=N, K=K, dtype=dn, us=round(t * 1e6, 1), tflops=round(flop / t / 1e12, 1),
                              l2_fill_bytes_per_flop=round(fill / flop, 5), l2_fill_tb_s=round(fill / t / 1e12, 2)))
             print(json.dumps(rows[-1]), file=sys.stderr, flush=True)
+            if kind in ("store", "gelu"):  # the FP8 mode's form of QKV / FC1: e4m3 operands (128 K elements per stage), fp16 output
+                A8 = torch.randn(M, K, device="cuda", generator=g).to(torch.float8_e4m3fn).view(torch.uint8)
+                W8 = torch.randn(N, K, device="cuda", generator=g).to(torch.float8_e4m3fn).view(torch.uint8)
+                sa, sb = torch.full((M,), 2.0 ** -4, device="cuda"), torch.full((N,), 1.0 / math.sqrt(K), device="cuda")
+                out16 = out if dt == torch.float16 else torch.empty(out.shape, device="cuda", dtype=torch.float16)
+
+                def fn8(N=N, K=K, bias=bias, act=act):
+                    rc = lib.jimm_k_gemm_e4m3(0, vp(A8), K, vp(W8), K, M, N, K, vp(sa), vp(sb), vp(bias), act, vp(out16), 1, out16.stride(0),
+                                              2, M, 0, s)
+                    assert rc == 0, lib.jimm_last_error().decode()
+
+                t8 = time_cuda(torch, fn8, iters)
+                fill8 = math.ceil(M / BM) * math.ceil(N / BN) * math.ceil(K / 128) * (BM + BN) * 128
+                rows.append(dict(workload=wl, gemm=name + " e4m3", M=M, N=N, K=K, dtype="float8_e4m3fn", us=round(t8 * 1e6, 1),
+                                 tflops=round(flop / t8 / 1e12, 1), speedup_vs_16bit=round(t / t8, 3),
+                                 l2_fill_bytes_per_flop=round(fill8 / flop, 5), l2_fill_tb_s=round(fill8 / t8 / 1e12, 2)))
+                print(json.dumps(rows[-1]), file=sys.stderr, flush=True)
+                del A8, W8, out16
         del a_big, x, h, out, cnt
     return rows
 
