@@ -1,14 +1,17 @@
 // Persistent, warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
-//   C[M,N] = epi( A[M,K] . B[N,K]^T ),  A/B K-major fp16 | bf16 | fp32(tf32), fp32 accumulate in registers.
-//   e4m3 operands (FP8 compute mode) run gemm_e4m3_kernel below: same structure, 64 x 256 tiles, K-slab promotion, row / column scales.
+//   C[M,N] = epi( A[M,K] . B[N,K]^T ),  A/B K-major fp16 | bf16 | fp32(tf32) | e4m3, fp32 accumulate in registers.
+//
+// One kernel, gemm_wgmma_kernel<T, OUT, ACT>, with two K-slab bodies: m64n256 wgmmas accumulating straight into registers (16-bit,
+// tf32), and for e4m3 (FP8 compute mode) 64 x 256 tiles whose slabs are summed from zero and promoted into fp32 registers, with row /
+// column scales in the epilogue (see "e4m3 operands" below).
 //
 // CTA = 384 threads (three warpgroups), 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin 128 x 256 tile schedule (n fastest).
 //   warpgroup 0, warp 0 : TMA producer (one lane): 4-stage smem ring of {A 128x128B, B 256x128B} tiles (48 KB), SWIZZLE_128B
 //   warpgroup 0, warps 1-3: idle, or LayerNorm workers of the fused-LayerNorm epilogue
-//   warpgroups 1, 2     : consumers, 64 rows each: wgmma.mma_async m64n256 from shared memory, one wgmma group in flight while the
-//                         previous stage is released; then the epilogue straight from the accumulator registers.  While they run
-//                         it, the producer is already filling the ring for their next tile.
+//   warpgroups 1, 2     : consumers, 64 rows each (e4m3: 128 columns each): wgmma.mma_async from shared memory, one wgmma group in
+//                         flight while the previous stage is released; then the epilogue straight from the accumulator registers.
+//                         While they run it, the producer is already filling the ring for their next tile.
 // 128 x 256 rather than 128 x 128: a k-slab of 128 B fills (128 + 256) x 128 B of shared memory from L2 for 2 x 128 x 256 x 64 FLOP
 // (fp16), 85 FLOP per byte instead of 64, and the two consumer warpgroups read one B slab per 2 x 64 x 256 instead of 2 x 64 x 128
 // outputs.  The 128 fp32 accumulators per consumer thread do not fit in the 168 registers each of 384 threads starts with, so the
@@ -110,21 +113,28 @@ __device__ __forceinline__ void store1(const EpiDev& e, int out_row, int col, fl
 }
 
 template <typename T>
-struct Traits;  // KIND: wgmma_m64n256_ss operand kind
+struct Traits;  // DTYPE: the operand's DType; KIND: wgmma_m64n256_ss operand kind
 template <>
 struct Traits<__half> {
-  static constexpr int KIND = 0;
+  static constexpr int DTYPE = DT_F16, KIND = 0;
 };
 template <>
 struct Traits<__nv_bfloat16> {
-  static constexpr int KIND = 1;
+  static constexpr int DTYPE = DT_BF16, KIND = 1;
 };
 template <>
 struct Traits<float> {
-  static constexpr int KIND = 2;
+  static constexpr int DTYPE = DT_TF32, KIND = 2;
+};
+template <>
+struct Traits<__nv_fp8_e4m3> {
+  static constexpr int DTYPE = DT_E4M3;
 };
 template <typename T>
 constexpr bool kScaled = std::is_same<T, __nv_fp8_e4m3>::value;  // the accumulator is multiplied by a_scale[row] * b_scale[col]
+
+// Rows of one CTA tile: e4m3 tiles are half height (see "e4m3 operands").  The kernel, the grid size and the A tensor map's box read it.
+constexpr int tile_rows(int dtype) { return dtype == DT_E4M3 ? 64 : BM; }
 
 // ---- fused LayerNorm of completed 32-row groups (reduce-add epilogue) --------------------------------------------------------------
 // Who normalises: NOT the consumer warps, whose next tile would wait for them.  The consumer warps only PUBLISH (wait for their
@@ -273,8 +283,8 @@ __device__ __forceinline__ void ln_worker(const EpiDev& e, LnQueue* q, int lane)
 
 // ---- TMA epilogue of one consumer warp: its 16 rows x BN columns, thread (g = lane / 4, t = lane % 4) holds rows g and g + 8,
 // columns 8 j + 2 t (+1) of the wgmma accumulator.  16-bit outputs: 64 columns per 16 x 128 B box; 32-bit outputs: 32 columns.
-// NC: the warp's columns (BN, or 128 in the e4m3 kernel), acc[NC / 2] its accumulators
-template <int OUT, int ACT, bool SCALED, int NC = BN>
+// NC: the warp's columns (BN, or 128 for e4m3), acc[NC / 2] its accumulators
+template <int OUT, int ACT, bool SCALED, int NC>
 __device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const EpiDev& epi, const float (&acc)[NC / 2], uint8_t* tbuf0, int lane,
                                              int row_base, int n_tile0, uint32_t& box_count) {
   constexpr bool OUT16 = (OUT == OUT_H16 || OUT == OUT_BF16);
@@ -345,7 +355,7 @@ __device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const Epi
 }
 
 // ---- generic LSU epilogue (run-time flags; any N, row remap, row-add, residual read) ---------------------------------
-template <bool SCALED, int NC = BN>
+template <bool SCALED, int NC>
 __device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float (&acc)[NC / 2], int lane, int row_base, int n_tile0) {
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
@@ -375,17 +385,35 @@ __device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float 
   }
 }
 
+// ---- e4m3 operands ---------------------------------------------------------------------------------------------------------------
+// The e4m3 wgmma does not accumulate in full fp32: its sums of products lose low-order bits (about 5e-4 of sum |a b| at K = 768..2048
+// on an H100, measured with m64n256k32), which puts an FP8 model at about a third of its whole FP8 error away from an exact-accumulation
+// restatement.  So each 128-deep K slab (four m64n128k32 wgmmas) is accumulated from zero and then added to fp32 registers ("promotion").
+// The 64 promoted sums plus 64 accumulators per thread fit where m64n256 would need 256, so the CTA tile is 64 x 256: both consumer
+// warpgroups take the same 64 A rows, warpgroup wg columns [128 wg, 128 wg + 128) of the B tile.  That is gemm_wgmma_kernel's e4m3
+// slab body and tile split; the ring (A stages keep their 128-row spacing and hold 64 rows), barriers, register split, tile walk and
+// epilogues are shared.  e4m3 plans take the plain-store epilogues only, never the fused LayerNorm.
+
 template <typename T, int OUT, int ACT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                   const __grid_constant__ CUtensorMap map_c, const EpiDev epi, int K) {
+  constexpr bool SCALED = kScaled<T>;  // e4m3: promoted K slabs, scaled epilogue
   constexpr int BK = 128 / sizeof(T);  // one 128-byte swizzle atom along K per stage
-  constexpr int UK = 32 / sizeof(T);   // wgmma K (16 for 16-bit, 8 for tf32)
+  constexpr int UK = 32 / sizeof(T);   // wgmma K (16 for 16-bit, 8 for tf32, 32 for e4m3)
+  constexpr int TM = tile_rows(Traits<T>::DTYPE);
+  constexpr int STAGE_TX = TM * 128 + B_STAGE_BYTES;  // bytes one stage's TMA loads bring
+  // Consumer warpgroup wg's part of the tile starts wg * WG_DM rows and wg * WG_DN columns in: the 16-bit / tf32 tile is split by
+  // rows, the e4m3 tile by columns.  Each consumer warp holds 16 rows x NC columns.
+  constexpr int WG_DM = SCALED ? 0 : 64;
+  constexpr int WG_DN = SCALED ? 128 : 0;
+  constexpr int NC = BN - WG_DN;
   constexpr bool FUSE_LN = OUT == OUT_F32_ADD && ACT == ACT_FUSE_LN;  // see "fused LayerNorm" above
   constexpr int EPI_ACT = ACT == ACT_FUSE_LN ? static_cast<int>(ACT_NONE) : ACT;
   // Registers per thread of the producer warpgroup / of each consumer warpgroup after setmaxnreg.  The consumers hold 128
-  // accumulators; the producer's TMA lane needs few.  The fused LayerNorm's workers live in the producer warpgroup and keep up to 64
-  // registers of row data (ln_rows_nv) plus the scale / bias they load, while its consumers' reduce-add epilogue is the leanest.
+  // accumulators (e4m3: 64 plus 64 promoted sums); the producer's TMA lane needs few.  The fused LayerNorm's workers live in the
+  // producer warpgroup and keep up to 64 registers of row data (ln_rows_nv) plus the scale / bias they load, while its consumers'
+  // reduce-add epilogue is the leanest.
   // Chosen from ptxas -v: splits without spills.  The three warpgroups share the CTA's launch allocation of KERNEL_REGS per thread
   // (checked at launch).
   constexpr int PRODUCER_REGS = FUSE_LN ? 152 : 40;
@@ -404,7 +432,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int M = epi.M, N = epi.N;
-  const int m_tiles = (M + BM - 1) / BM, n_tiles = (N + BN - 1) / BN;
+  const int m_tiles = (M + TM - 1) / TM, n_tiles = (N + BN - 1) / BN;
   const int num_tiles = m_tiles * n_tiles;
   const int num_kb = (K + BK - 1) / BK;
 
@@ -440,8 +468,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
           for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
-            tma_load_2d(smem_a + stage * A_STAGE_BYTES, &map_a, &full_bar[stage], kb * BK, m_blk * BM);
+            mbar_arrive_expect_tx(&full_bar[stage], STAGE_TX);
+            tma_load_2d(smem_a + stage * A_STAGE_BYTES, &map_a, &full_bar[stage], kb * BK, m_blk * TM);
             tma_load_2d(smem_b + stage * B_STAGE_BYTES, &map_b, &full_bar[stage], kb * BK, n_blk * BN);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
@@ -453,45 +481,69 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   } else {
     // ===================== consumers: mainloop + epilogue =====================
     setmaxnreg<KERNEL_REGS, CONSUMER_REGS>();
-    const int wg = (warp_idx - 4) >> 2;  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int wg = (warp_idx - 4) >> 2;  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile (e4m3: 128 columns)
     const int wq = warp_idx & 3;         // warp within the warpgroup: rows [16 wq, 16 wq + 16) of those
     uint8_t* tbuf0 = epi_stage + (warp_idx - 4) * EPI_BUFS * EPI_BUF_BYTES;
     int stage = 0;
     uint32_t phase = 0, box_count = 0;
     int ln_rg = -1, ln_cols = 0;  // row group / column count of this warp's previous tile, not yet published (fused LayerNorm)
-    float acc[128];
+    float acc[NC / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
       const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
       int prev = -1;
+      if constexpr (SCALED) {
+#pragma unroll
+        for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
+      }
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint64_t adesc = make_wgmma_desc_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * 64 * 128));
-        const uint64_t bdesc = make_wgmma_desc_sw128(smem_u32(smem_b + stage * B_STAGE_BYTES));
-        wgmma_fence_operands(acc);
-        wgmma_fence();
+        const uint64_t adesc = make_wgmma_desc_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * WG_DM * 128));
+        const uint64_t bdesc = make_wgmma_desc_sw128(smem_u32(smem_b + stage * B_STAGE_BYTES + wg * WG_DN * 128));
+        if constexpr (SCALED) {
+          // the slab's sum from zero; once its wgmmas have retired, the stage goes back to the producer and the sum is promoted
+          float slab[NC / 2];
+          wgmma_fence_operands(slab);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / UK; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
-          wgmma_m64n256_ss<Traits<T>::KIND>(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_fence_operands(acc);
-        if (prev >= 0) {
-          wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its smem back to the producer
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          for (int k = 0; k < BK / UK; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
+            wgmma_m64n128k32_e4m3_ss(slab, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operands(slab);
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+          for (int i = 0; i < NC / 2; ++i) acc[i] += slab[i];
+        } else {
+          wgmma_fence_operands(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / UK; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
+            wgmma_m64n256_ss<Traits<T>::KIND>(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_fence_operands(acc);
+          if (prev >= 0) {
+            wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its smem back to the producer
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          }
+          prev = stage;
         }
-        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      wgmma_wait<0>();
-      wgmma_fence_operands(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if constexpr (!SCALED) {
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
 
-      const int row_base = m_blk * BM + wg * 64 + wq * 16;
-      const int n_tile0 = n_blk * BN;
+      const int row_base = m_blk * TM + wg * WG_DM + wq * 16;
+      const int n_tile0 = n_blk * BN + wg * WG_DN;
       if constexpr (OUT == OUT_GENERIC) {
-        epilogue_generic<false>(epi, acc, lane, row_base, n_tile0);
+        epilogue_generic<SCALED, NC>(epi, acc, lane, row_base, n_tile0);
       } else {
-        if (row_base < M) epilogue_tma<OUT, EPI_ACT, false>(&map_c, epi, acc, tbuf0, lane, row_base, n_tile0, box_count);
+        // split by columns, a consumer warpgroup's columns can lie wholly past N
+        if (row_base < M && (WG_DN == 0 || n_tile0 < N))
+          epilogue_tma<OUT, EPI_ACT, SCALED, NC>(&map_c, epi, acc, tbuf0, lane, row_base, n_tile0, box_count);
         if constexpr (FUSE_LN) {
           // Publishing is deferred by one tile: the PREVIOUS tile's reduce-adds were issued a whole mainloop ago, so waiting for them
           // costs nothing.  Both 16-row halves of a 32-row group publish, also a half that lies beyond M.
@@ -506,115 +558,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (ln_rg >= 0) ln_publish(epi, lnq, ln_rg, ln_cols);
         __threadfence_block();
         atomicAdd(&lnq->done, 1);
-      }
-    }
-    if constexpr (OUT != OUT_GENERIC) {
-      if (lane == 0) tma_store_wait_all();
-    }
-  }
-}
-
-// ---- e4m3 operands ---------------------------------------------------------------------------------------------------------------
-// The e4m3 wgmma does not accumulate in full fp32: its sums of products lose low-order bits (about 5e-4 of sum |a b| at K = 768..2048
-// on an H100, measured with m64n256k32), which puts an FP8 model at about a third of its whole FP8 error away from an exact-accumulation
-// restatement.  So each 128-deep K slab (four m64n128k32 wgmmas) is accumulated from zero and then added to fp32 registers ("promotion").
-// The 64 promoted sums plus 64 accumulators per thread fit where m64n256 would need 256, so the CTA tile is 64 x 256: both consumer
-// warpgroups take the same 64 A rows, warpgroup wg columns [128 wg, 128 wg + 128) of the B tile.  Same ring, barriers, register split,
-// tile walk and epilogues as gemm_wgmma_kernel (plain stores only).
-static constexpr int BM8 = 64;
-static constexpr int STAGE_BYTES8 = BM8 * 128 + B_STAGE_BYTES;  // bytes one stage's TMA loads bring
-
-template <int OUT, int ACT>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_e4m3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_c, const EpiDev epi, int K) {
-  constexpr int BK = 128;  // one 128-byte swizzle atom along K per stage
-  constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
-  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NUM_THREADS * KERNEL_REGS, "register split exceeds the CTA's allocation");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint8_t* epi_stage = smem + STAGES * STAGE_BYTES;
-  LnQueue* lnq = reinterpret_cast<LnQueue*>(epi_stage + EPI_STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(lnq + 1);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int M = epi.M, N = epi.N;
-  const int m_tiles = (M + BM8 - 1) / BM8, n_tiles = (N + BN - 1) / BN;
-  const int num_tiles = m_tiles * n_tiles;
-  const int num_kb = (K + BK - 1) / BK;
-
-  pdl_launch_dependents();
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
-    if constexpr (OUT != OUT_GENERIC) tma_prefetch_desc(&map_c);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_wait();
-
-  if (warp_idx < 4) {
-    setmaxnreg<KERNEL_REGS, PRODUCER_REGS>();
-    if (warp_idx == 0 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
-        const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES8);
-          tma_load_2d(smem_a + stage * A_STAGE_BYTES, &map_a, &full_bar[stage], kb * BK, m_blk * BM8);
-          tma_load_2d(smem_b + stage * B_STAGE_BYTES, &map_b, &full_bar[stage], kb * BK, n_blk * BN);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    setmaxnreg<KERNEL_REGS, CONSUMER_REGS>();
-    const int wg = (warp_idx - 4) >> 2;  // consumer warpgroup: columns [128 wg, 128 wg + 128) of the tile
-    const int wq = warp_idx & 3;         // warp within the warpgroup: rows [16 wq, 16 wq + 16)
-    uint8_t* tbuf0 = epi_stage + (warp_idx - 4) * EPI_BUFS * EPI_BUF_BYTES;
-    int stage = 0;
-    uint32_t phase = 0, box_count = 0;
-    float acc[64], sum[64];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int tv = epi.reverse ? num_tiles - 1 - tile : tile;
-      const int m_blk = tv / n_tiles, n_blk = tv - m_blk * n_tiles;
-#pragma unroll
-      for (int i = 0; i < 64; ++i) sum[i] = 0.f;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint64_t adesc = make_wgmma_desc_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES));
-        const uint64_t bdesc = make_wgmma_desc_sw128(smem_u32(smem_b + stage * B_STAGE_BYTES + wg * 128 * 128));
-        wgmma_fence_operands(acc);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 32; ++k)  // descriptors advance by 32 bytes (>> 4) per wgmma K step
-          wgmma_m64n128k32_e4m3_ss(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), k != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_operands(acc);
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);
-#pragma unroll
-        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      const int row_base = m_blk * BM8 + wq * 16;
-      const int n_tile0 = n_blk * BN + wg * 128;
-      if constexpr (OUT == OUT_GENERIC) {
-        epilogue_generic<true, 128>(epi, sum, lane, row_base, n_tile0);
-      } else {
-        if (row_base < M && n_tile0 < N) epilogue_tma<OUT, ACT, true, 128>(&map_c, epi, sum, tbuf0, lane, row_base, n_tile0, box_count);
       }
     }
     if constexpr (OUT != OUT_GENERIC) {
@@ -678,15 +621,23 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// 2-D K-major tensor map: dims {K, rows}, box {128 B worth of K, box_rows}, SWIZZLE_128B, zero OOB fill.
-static int make_map(CUtensorMap* map, int dtype, const void* ptr, int rows, int K, int ld, int box_rows) {
+static CUtensorMapDataType tensor_map_dtype(int dtype) {
+  switch (dtype) {
+    case DT_F32:
+    case DT_TF32: return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    case DT_F16: return CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    case DT_E4M3: return CU_TENSOR_MAP_DATA_TYPE_UINT8;
+    default: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  }
+}
+
+// 2-D tensor map over a row-major [rows, cols] matrix (K-major operands: cols = K): dims {cols, rows}, box {128 B worth of columns,
+// box_rows}, SWIZZLE_128B, zero OOB fill.
+int make_tensor_map_2d(CUtensorMap* map, int dtype, const void* ptr, int rows, int cols, int ld, int box_rows) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return -3;
   const size_t es = dtype_size(dtype);
-  CUtensorMapDataType dt = (dtype == DT_F32 || dtype == DT_TF32) ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                           : dtype == DT_E4M3                    ? CU_TENSOR_MAP_DATA_TYPE_UINT8
-                                           : (dtype == DT_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
+  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * es};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / es), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
@@ -694,10 +645,10 @@ static int make_map(CUtensorMap* map, int dtype, const void* ptr, int rows, int 
     set_last_error("gemm: operand pointer/stride must be 16-byte aligned (ptr=%p, ld=%d)", ptr, ld);
     return -1;
   }
-  CUresult r = enc(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(map, tensor_map_dtype(dtype), 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed: CUresult %d (rows=%d K=%d ld=%d)", static_cast<int>(r), rows, K, ld);
+    set_last_error("cuTensorMapEncodeTiled failed: CUresult %d (rows=%d cols=%d ld=%d)", static_cast<int>(r), rows, cols, ld);
     return -3;
   }
   return 0;
@@ -705,25 +656,18 @@ static int make_map(CUtensorMap* map, int dtype, const void* ptr, int rows, int 
 
 // 3-D tensor map over out[B, S, N] (dims {N, S, B}), box {128 B of columns, 16 rows, 1}, SWIZZLE_128B: rows >= S are clipped,
 // so a 16-row box never spills into the next sample.
-int make_tensor_map_3d(CUtensorMap* map, int dtype, const void* ptr, int B, int S, int N, int ld) {
+static int make_tensor_map_3d(CUtensorMap* map, int dtype, const void* ptr, int B, int S, int N, int ld) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return -3;
   const size_t es = dtype_size(dtype);
-  CUtensorMapDataType dt = (dtype == DT_F32 || dtype == DT_TF32) ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                           : (dtype == DT_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
   cuuint64_t dims[3] = {static_cast<cuuint64_t>(N), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(B)};
   cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * es, static_cast<cuuint64_t>(S) * ld * es};
   cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / es), EPI_BOX_ROWS, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, dt, 3, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(map, tensor_map_dtype(dtype), 3, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled(3d) failed: CUresult %d", static_cast<int>(r)); return -3; }
   return 0;
-}
-static int make_map_3d_f32(CUtensorMap* map, const void* ptr, int B, int S, int N, int ld) { return make_tensor_map_3d(map, DT_F32, ptr, B, S, N, ld); }
-
-int make_tensor_map_2d(CUtensorMap* map, int dtype, const void* ptr, int rows, int cols, int ld, int box_rows) {
-  return make_map(map, dtype, ptr, rows, cols, ld, box_rows);
 }
 
 int device_sm_count() {  // of the CURRENT device (cached per device: a process may drive several GPUs)
@@ -776,8 +720,8 @@ int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void
       return -1;
     }
   }
-  if (int rc = make_map(&plan->map_a, dtype, A, M, K, lda, dtype == DT_E4M3 ? BM8 : BM)) return rc;
-  if (int rc = make_map(&plan->map_b, dtype, B, N, K, ldb, BN)) return rc;
+  if (int rc = make_tensor_map_2d(&plan->map_a, dtype, A, M, K, lda, tile_rows(dtype))) return rc;
+  if (int rc = make_tensor_map_2d(&plan->map_b, dtype, B, N, K, ldb, BN)) return rc;
   plan->M = M; plan->N = N; plan->K = K; plan->dtype = dtype; plan->epi = epi;
   memset(&plan->map_c, 0, sizeof(plan->map_c));
   if (plan->epi.mode == 2) {
@@ -790,9 +734,9 @@ int gemm_plan_init(GemmPlan* plan, int dtype, const void* A, int lda, const void
                     (epi.bias == nullptr || ((reinterpret_cast<uintptr_t>(epi.bias) & 15) == 0 && N % 4 == 0)) &&
                     !(epi.residual && epi.act != ACT_NONE);
     if (ok && epi.tok_pad > 0) {
-      if (int rc = make_map_3d_f32(&plan->map_c, epi.out, M / epi.tok_pad, epi.tok_S, N, epi.ldo)) return rc;
+      if (int rc = make_tensor_map_3d(&plan->map_c, DT_F32, epi.out, M / epi.tok_pad, epi.tok_S, N, epi.ldo)) return rc;
     } else if (ok) {
-      if (int rc = make_map(&plan->map_c, epi.out_type, epi.out, M, N, epi.ldo, EPI_BOX_ROWS)) return rc;
+      if (int rc = make_tensor_map_2d(&plan->map_c, epi.out_type, epi.out, M, N, epi.ldo, EPI_BOX_ROWS)) return rc;
     } else {
       plan->epi.mode = 0;
     }
@@ -819,15 +763,9 @@ static EpiDev to_dev(const GemmEpilogue& e, int M, int N) {
 }
 
 template <typename T, int OUT, int ACT>
-static auto kernel_of() {
-  if constexpr (kScaled<T>) return gemm_e4m3_kernel<OUT, ACT>;
-  else return gemm_wgmma_kernel<T, OUT, ACT>;
-}
-
-template <typename T, int OUT, int ACT>
 static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
-  auto* kernel = kernel_of<T, OUT, ACT>();
-  const int bm = kScaled<T> ? BM8 : BM;
+  auto* kernel = gemm_wgmma_kernel<T, OUT, ACT>;
+  constexpr int TM = tile_rows(Traits<T>::DTYPE);
   static DeviceOnce attr_set;
   if (attr_set.first()) {
     JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -839,7 +777,7 @@ static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
       return -2;
     }
   }
-  const int tiles = ((M + bm - 1) / bm) * ((p->N + BN - 1) / BN);
+  const int tiles = ((M + TM - 1) / TM) * ((p->N + BN - 1) / BN);
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
   JIMM_CUDA_CHECK(launch_k(kernel, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, 1, true, p->map_a, p->map_b, p->map_c,
                            to_dev(p->epi, M, p->N), p->K));

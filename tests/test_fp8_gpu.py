@@ -216,7 +216,7 @@ def test_gemm_e4m3_refuses_other_epilogues(lib):
 def test_fp8_accumulation_error(lib, K):
     """fp32 output of the e4m3 GEMM against fp64 on the same (exactly representable) operands: the MMA's accumulation error alone.
     Recorded per K; the bound is about 3x the worst value measured on an H100 (6.8e-5 at K = 768, 4.0e-5 at K = 2048, with the K-slab
-    promotion of gemm_e4m3_kernel; without it the e4m3 wgmma gave 4.3e-4 to 5.2e-4)."""
+    promotion of gemm_wgmma_kernel; without it the e4m3 wgmma gave 4.3e-4 to 5.2e-4)."""
     M, N = 2048, 2304
     ops, Ad, Bd = _mk8(M, N, K, seed=K)
     out = torch.empty(M, N, device=DEV)
