@@ -92,6 +92,14 @@ JIMM_API int jimm_model_set_param_ref(jimm_model_t* m, const char* flax_path, co
  * `max_batch` samples per call.  Fails (JIMM_ESTATE) naming the first missing / unexpected / mis-shaped parameter --
  * the analogue of the reference's strict visit checks (models/vit.py:229-232,259-268). */
 JIMM_API int jimm_model_finalize(jimm_model_t* m, int max_batch);
+/* Token budget of the vision workspace for the *_hw entry points, called before finalize: the workspace then holds
+ * max_batch x max(tokens_per_sample, the native count (img_size / patch)^2 (+1)) tokens (a token is a patch, or the CLS token), and
+ * any one image of up to that many tokens fits it.  Without this call the budget is max_batch x the native count, and an image of
+ * another size may need more room than its token count says (its padded patch rows).  Vision models only. */
+JIMM_API int jimm_model_set_max_tokens(jimm_model_t* m, int tokens_per_sample);
+/* Images of H x W that one chunk of a *_hw call runs on this handle: max_batch on the trained patch grid, otherwise as many as the
+ * workspace holds, up to max_batch; 0 when one image does not fit (the *_hw call then returns JIMM_EINVAL). */
+JIMM_API int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images);
 JIMM_API int jimm_model_destroy(jimm_model_t* m);
 /* Introspection used by the Python mirror. */
 JIMM_API int jimm_model_output_dim(const jimm_model_t* m, int* vision_out, int* text_out);
@@ -116,6 +124,18 @@ JIMM_API int jimm_dual_encode(jimm_model_t* m, const void* img, int in_dtype, in
 /* CLIP.__call__ / SigLIP.__call__ (models/clip.py:169-188, models/siglip.py:155-174) on one GPU. */
 JIMM_API int jimm_dual_forward(jimm_model_t* m, const void* img, int in_dtype, int Bi, const int32_t* ids, int Bt, int T, float* logits,
                       void* stream);
+/* The four calls above for images of any size H x W >= patch (HF's interpolate_pos_encoding=True): img is device NHWC [B,H,W,in_ch].
+ * The patch grid is (H / patch) x (W / patch), trailing pixels that do not fill a patch dropped (the VALID conv).  On a grid other
+ * than the trained g x g, the patch rows of the position table are resampled bicubically to it (torch.nn.functional.interpolate,
+ * mode="bicubic", align_corners=False), the CLS row kept, tokens row-major over the grid.  At H == W == img_size each call is its
+ * twin above.  Other sizes run eagerly (no CUDA-graph replay) in chunks of min(max_batch, budget / tokens) images, the budget being
+ * the workspace's max_batch x tokens-per-sample (jimm_model_set_max_tokens); an image that alone does not fit is JIMM_EINVAL. */
+JIMM_API int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream);
+JIMM_API int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream);
+JIMM_API int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T,
+                                 float* img_e, float* txt_e, void* stream);
+JIMM_API int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T,
+                                  float* logits, void* stream);
 
 /* -- forward of a bare sub-module (kinds JIMM_ENCODER / JIMM_MAPHEAD; config fields used: v_width, v_heads, v_mlp, v_layers, v_act,
  *    v_eps_block, v_eps_outer, t_causal (attn_mask = tril), ctx_len = max tokens per sample, compute_dtype; parameters keyed
@@ -219,6 +239,10 @@ JIMM_API int jimm_k_patchify_ex(const void* img, int in_type, int B, int H, int 
                                 int ldk, void* stream);
 /* y = act(x) elementwise on device fp32 (act: 1 tanh-GELU == nnx.gelu, 2 QuickGELU == common/transformer.py:12-19). */
 JIMM_API int jimm_k_activation(const float* x, float* y, long long n, int act, void* stream);
+/* Initial residual stream of a tower on a gh x gw patch grid, for a position table trained on a g x g grid: x fp32 [B, (1 +) gh*gw, D];
+ * row 0 = cls + pos[0] when cls (fp32 [D]) is not NULL, the patch rows the bicubic resampling of pos's g x g patch rows described at
+ * jimm_vit_forward_hw (pos fp32 [(1 +) g*g, D]); D a multiple of 4.  (gh, gw) == (g, g) gives the table itself, bit for bit. */
+JIMM_API int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream);
 JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream);
 JIMM_API int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream);
 JIMM_API int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,

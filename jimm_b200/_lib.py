@@ -57,6 +57,8 @@ SIGNATURES = {
     "jimm_model_set_param": (_i, [_vp, C.c_char_p, _vp, C.POINTER(C.c_int64), _i, _i]),
     "jimm_model_set_param_ref": (_i, [_vp, C.c_char_p, _vp, C.POINTER(C.c_int64), _i, _i, _i]),
     "jimm_model_finalize": (_i, [_vp, _i]),
+    "jimm_model_set_max_tokens": (_i, [_vp, _i]),
+    "jimm_model_images_per_call": (_i, [_vp, _i, _i, C.POINTER(_i)]),
     "jimm_model_destroy": (_i, [_vp]),
     "jimm_model_output_dim": (_i, [_vp, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_model_max_batch": (_i, [_vp]),
@@ -66,6 +68,10 @@ SIGNATURES = {
     "jimm_contrastive_logits": (_i, [_vp, _fp, _i, _fp, _i, _fp, _vp]),
     "jimm_dual_encode": (_i, [_vp, _vp, _i, _i, _ip, _i, _i, _fp, _fp, _vp]),
     "jimm_dual_forward": (_i, [_vp, _vp, _i, _i, _ip, _i, _i, _fp, _vp]),
+    "jimm_vit_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _fp, _vp]),
+    "jimm_encode_image_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _fp, _vp]),
+    "jimm_dual_encode_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _i, _i, _fp, _fp, _vp]),
+    "jimm_dual_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _i, _i, _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -95,6 +101,7 @@ SIGNATURES = {
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),
+    "jimm_k_tokens_init_interp": (_i, [_fp, _fp, _i, _i, _fp, _i, _i, _i, _vp]),
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),
     "jimm_k_logits": (_i, [_fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),

@@ -49,7 +49,8 @@ class PendingResult:
 class NativeModel:
     """One opaque jimm_model_t on one GPU."""
 
-    def __init__(self, cfg: _lib.Config, params: Dict[str, torch.Tensor], max_batch: int, device: Optional[int] = None):
+    def __init__(self, cfg: _lib.Config, params: Dict[str, torch.Tensor], max_batch: int, device: Optional[int] = None,
+                 max_tokens: int = 0):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.JimmError("jimm_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -75,6 +76,8 @@ class NativeModel:
                 shape = (C.c_int64 * max(len(shape_t), 1))(*shape_t)
                 _lib.check(self.lib.jimm_model_set_param_ref(self.handle, name.encode(), C.c_void_p(t.data_ptr()), shape, len(shape_t),
                                                               _TORCH_TO_CODE[t.dtype], flags))
+            if max_tokens > 0:
+                _lib.check(self.lib.jimm_model_set_max_tokens(self.handle, int(max_tokens)))
             _lib.check(self.lib.jimm_model_finalize(self.handle, int(max_batch)))
         except Exception:
             self.lib.jimm_model_destroy(self.handle)
@@ -86,6 +89,12 @@ class NativeModel:
         self.vision_out, self.text_out = vo.value, to.value
         self._comm = None
         self.preproc = None  # ImagePreprocessor for uint8 inputs (set by the owning model's set_preprocessor)
+
+    def images_per_call(self, height: int, width: int) -> int:
+        """Images of height x width one chunk of an interpolate_pos_encoding call runs on this handle (0: one does not fit)."""
+        n = C.c_int()
+        _lib.check(self.lib.jimm_model_images_per_call(self.handle, int(height), int(width), C.byref(n)))
+        return n.value
 
     def side_stream(self) -> torch.cuda.Stream:
         """Copy stream for host inputs of the multi-GPU dual path."""
@@ -105,7 +114,8 @@ class NativeModel:
             pass
 
     # ---- input normalisation ----
-    def _prep_images(self, x) -> torch.Tensor:
+    def _prep_images(self, x, interpolate: bool = False) -> torch.Tensor:
+        """interpolate: HF's interpolate_pos_encoding -- any image size of at least one patch is accepted."""
         x = _as_tensor(x, "image")
         if x.ndim != 4:
             raise ValueError(f"expected images of shape [batch, height, width, channels], got {tuple(x.shape)}")
@@ -118,14 +128,37 @@ class NativeModel:
             if x.shape[3] != 3:
                 raise ValueError(f"expected uint8 RGB frames [B,H,W,3], got {tuple(x.shape)}")
             oh, ow = self.preproc.output_size(x.shape[1], x.shape[2])
-            if (oh, ow) != (c.img_size, c.img_size):
+            if interpolate:
+                self._check_grid(oh, ow)
+            elif (oh, ow) != (c.img_size, c.img_size):
                 raise ValueError(f"the image front-end maps {x.shape[1]}x{x.shape[2]} frames to {oh}x{ow}, the model takes {c.img_size}x{c.img_size}")
             return x.contiguous()
-        if x.shape[1] != c.img_size or x.shape[2] != c.img_size or x.shape[3] != c.in_ch:
+        if interpolate:
+            if x.shape[3] != c.in_ch:
+                raise ValueError(f"expected NHWC images [B,H,W,{c.in_ch}], got {tuple(x.shape)}")
+            self._check_grid(x.shape[1], x.shape[2])
+        elif x.shape[1] != c.img_size or x.shape[2] != c.img_size or x.shape[3] != c.in_ch:
             raise ValueError(f"expected NHWC images [B,{c.img_size},{c.img_size},{c.in_ch}], got {tuple(x.shape)}")
         if x.dtype not in _TORCH_TO_CODE:
             x = x.to(torch.float32)
         return x.contiguous()
+
+    def _check_grid(self, h: int, w: int):
+        P = self.cfg.patch
+        if h < P or w < P:
+            raise ValueError(f"interpolate_pos_encoding: a {h}x{w} image is smaller than one {P}x{P} patch")
+
+    def _off_grid(self, x: torch.Tensor, interpolate: bool) -> bool:
+        """True when an interpolate_pos_encoding call's (prepared) images are not the native size: the *_hw entry points run it."""
+        if not interpolate:
+            return False
+        hw = self.preproc.output_size(x.shape[1], x.shape[2]) if x.dtype == torch.uint8 else (x.shape[1], x.shape[2])
+        return tuple(hw) != (self.cfg.img_size, self.cfg.img_size)
+
+    def _device_images(self, x: torch.Tensor) -> torch.Tensor:
+        """Prepared images on this GPU in a tower input type (uint8 frames through the image front-end)."""
+        xd = x.to(self.device, non_blocking=True)
+        return self.preproc(xd, dtype=self._operand_dtype()) if xd.dtype == torch.uint8 else xd
 
     def _prep_ids(self, t) -> torch.Tensor:
         t = _as_tensor(t, "text")
@@ -134,9 +167,12 @@ class NativeModel:
         return t.to(torch.int32).contiguous()
 
     # ---- forward ----
-    def vision(self, x, encode: bool = False) -> torch.Tensor:
-        """VisionTransformer.__call__ / encode_image.  CUDA input -> async CUDA output; host input -> host output."""
-        x = self._prep_images(x)
+    def vision(self, x, encode: bool = False, interpolate: bool = False) -> torch.Tensor:
+        """VisionTransformer.__call__ / encode_image.  CUDA input -> async CUDA output; host input -> host output.
+        interpolate: HF's interpolate_pos_encoding (images of any size; see jimm_vit_forward_hw)."""
+        x = self._prep_images(x, interpolate)
+        if self._off_grid(x, interpolate):
+            return self._vision_hw(x, encode)
         B = x.shape[0]
         fn_dev = self.lib.jimm_encode_image if encode else self.lib.jimm_vit_forward
         if x.is_cuda:
@@ -149,14 +185,26 @@ class NativeModel:
             return out
         return self._vision_host(x, encode).result()
 
-    def vision_async(self, x, encode: bool = False) -> "PendingResult":
+    def vision_async(self, x, encode: bool = False, interpolate: bool = False) -> "PendingResult":
         """Host input: enqueue H2D + forward + D2H and return without synchronising (JAX-style asynchronous dispatch);
         `.result()` waits for this call only.  Back-to-back calls pipeline: the copies of call k+1 run under the towers of
-        call k.  The caller keeps `x` alive and unmodified until the result is taken."""
-        x = self._prep_images(x)
-        if x.is_cuda:
-            return PendingResult(self.vision(x, encode), None)
+        call k.  The caller keeps `x` alive and unmodified until the result is taken.  Host images off the native size
+        (interpolate=True) run synchronously."""
+        x = self._prep_images(x, interpolate)
+        if x.is_cuda or self._off_grid(x, interpolate):
+            return PendingResult(self.vision(x, encode, interpolate), None)
         return self._vision_host(x, encode)
+
+    def _vision_hw(self, x: torch.Tensor, encode: bool) -> torch.Tensor:
+        """A vision call at a size other than the native one: host images are copied to the GPU here and the result back."""
+        B = x.shape[0]
+        fn = self.lib.jimm_encode_image_hw if encode else self.lib.jimm_vit_forward_hw
+        with torch.cuda.device(self.device):
+            xd = self._device_images(x)
+            out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
+            _lib.check(fn(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], B, xd.shape[1], xd.shape[2],
+                          C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
+        return out if x.is_cuda else out.cpu()
 
     def _operand_dtype(self) -> torch.dtype:
         return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16, _lib.F8E4M3: torch.float16}[self.cfg.compute_dtype]
@@ -210,8 +258,10 @@ class NativeModel:
                 x = self.preproc(x, dtype=self._operand_dtype())
             ie = torch.empty((Bi, self.vision_out), dtype=torch.float32, device=self.device)
             te = torch.empty((Bt, self.text_out), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.jimm_dual_encode(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], Bi, C.c_void_p(ids.data_ptr()), Bt, T,
-                                                 C.c_void_p(ie.data_ptr()), C.c_void_p(te.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
+            # images of the native size run exactly as jimm_dual_encode; others only reach here with interpolate_pos_encoding
+            _lib.check(self.lib.jimm_dual_encode_hw(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], Bi, x.shape[1], x.shape[2],
+                                                    C.c_void_p(ids.data_ptr()), Bt, T, C.c_void_p(ie.data_ptr()), C.c_void_p(te.data_ptr()),
+                                                    C.c_void_p(_stream_ptr(self.device))))
         return ie, te
 
     def logits(self, img_e: torch.Tensor, txt_e: torch.Tensor) -> torch.Tensor:
@@ -224,12 +274,19 @@ class NativeModel:
                                                         C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
         return out
 
-    def dual(self, image, text) -> torch.Tensor:
+    def dual(self, image, text, interpolate: bool = False) -> torch.Tensor:
         """CLIP.__call__ / SigLIP.__call__ on one GPU."""
-        x = self._prep_images(image)
+        x = self._prep_images(image, interpolate)
         ids = self._prep_ids(text)
         Bi, (Bt, T) = x.shape[0], ids.shape
         with torch.cuda.device(self.device):
+            if self._off_grid(x, interpolate):
+                xd, idd = self._device_images(x), ids.to(self.device, non_blocking=True)
+                out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
+                _lib.check(self.lib.jimm_dual_forward_hw(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], Bi, xd.shape[1],
+                                                         xd.shape[2], C.c_void_p(idd.data_ptr()), Bt, T, C.c_void_p(out.data_ptr()),
+                                                         C.c_void_p(_stream_ptr(self.device))))
+                return out if (x.is_cuda or ids.is_cuda) else out.cpu()
             if x.dtype == torch.uint8:
                 # raw RGB frames (model.set_preprocessor): bytes over PCIe, the image front-end on the GPU, then both towers concurrently
                 host_in = not x.is_cuda and not ids.is_cuda
@@ -331,6 +388,11 @@ def activation(x, act: int) -> torch.Tensor:
         y = torch.empty_like(xd)
         _lib.check(lib.jimm_k_activation(C.c_void_p(xd.data_ptr()), C.c_void_p(y.data_ptr()), xd.numel(), int(act), C.c_void_p(_stream_ptr(x.device))))
     return y
+
+
+def grid_tokens(cfg: _lib.Config, height: int, width: int) -> int:
+    """Tokens per image of a vision tower on height x width images: the patches (trailing pixels dropped) and the CLS token."""
+    return (int(height) // cfg.patch) * (int(width) // cfg.patch) + (1 if cfg.pooling == _lib.POOL_CLS else 0)
 
 
 def default_max_batch() -> int:

@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _lib, nn
-from .._runtime import NativeModel, default_max_batch
+from .._runtime import NativeModel, default_max_batch, grid_tokens
 from .transformer import Transformer, _SubModuleRunner, g_wrap
 
 
@@ -58,6 +58,7 @@ class _NativeOwner:
         object.__setattr__(self, "_preproc", None)
         object.__setattr__(self, "_compute_dtype", nn.compute_dtype_code(dtype))
         object.__setattr__(self, "_max_batch", default_max_batch())
+        object.__setattr__(self, "_max_tokens", 0)  # vision tokens per sample of the workspace (0: the native count)
 
     @staticmethod
     def _release_native(n):
@@ -81,19 +82,54 @@ class _NativeOwner:
     def _native_config(self) -> _lib.Config:
         raise NotImplementedError
 
-    def native(self, batch: int = 1, require: bool = False) -> NativeModel:
+    def native(self, batch: int = 1, require: bool = False, hw=None) -> NativeModel:
         """Native handle whose workspace holds `max_batch` samples per call; larger vision / text batches are chunked by
-        the library, the contrastive head needs the whole batch resident (`require=True`)."""
+        the library, the contrastive head needs the whole batch resident (`require=True`).  hw: the (height, width) of the images of
+        an interpolate_pos_encoding call; the handle is rebuilt with a larger token budget only when the library reports that one
+        such image does not fit (a call whose images merely fit fewer at a time runs in smaller chunks).  A raised budget is kept
+        for later rebuilds."""
         n = self._native
-        if n is not None and (not require or batch <= n.max_batch):
+        if n is not None and (not require or batch <= n.max_batch) and (hw is None or n.images_per_call(*hw) > 0):
             return n
         if n is not None:
             self._release_native(n)
         mb = max(self._max_batch, int(batch) if require else 1)
-        n = NativeModel(self._native_config(), self.flat_params(raw=True), mb)
+        cfg = self._native_config()
+        # any jimm_model_set_max_tokens budget of at least ceil(tokens / max_batch) holds one image of that many tokens
+        need = -(-grid_tokens(cfg, *hw) // mb) if hw is not None else 0
+        if need > max(self._max_tokens, grid_tokens(cfg, cfg.img_size, cfg.img_size)):  # more tokens than the workspace rows
+            object.__setattr__(self, "_max_tokens", need)
+        n = self._build_native(mb)
+        if hw is not None and n.images_per_call(*hw) == 0:  # enough rows, but not the bytes of its padded patch rows
+            self._release_native(n)
+            object.__setattr__(self, "_max_tokens", max(self._max_tokens, need))
+            n = self._build_native(mb)
+        return n
+
+    def _build_native(self, mb: int) -> NativeModel:
+        n = NativeModel(self._native_config(), self.flat_params(raw=True), mb, max_tokens=self._max_tokens)
         n.preproc = self._preproc
         object.__setattr__(self, "_native", n)
         return n
+
+    def _call_hw(self, img, interpolate_pos_encoding: bool):
+        """(height, width) the tower sees for the images of an interpolate_pos_encoding call, else None (sizes below a patch are
+        refused later)."""
+        if not interpolate_pos_encoding or getattr(img, "ndim", 0) != 4:
+            return None
+        h, w = int(img.shape[1]), int(img.shape[2])
+        if str(img.dtype).endswith("uint8") and self._preproc is not None:
+            h, w = self._preproc.output_size(h, w)
+        P = self._native_config().patch
+        return (h, w) if h >= P and w >= P else None
+
+    def set_max_image_size(self, height: int, width: int):
+        """Size the vision workspace for interpolate_pos_encoding calls on images up to height x width: `max_batch` such images run
+        in one chunk, and no call on them rebuilds the handle.  The default holds `max_batch` images of the native size (larger
+        images then run fewer at a time)."""
+        object.__setattr__(self, "_max_tokens", grid_tokens(self._native_config(), height, width))
+        self._invalidate()
+        return self
 
     def set_preprocessor(self, preprocessor):
         """Attach a `jimm_b200.preprocess.ImagePreprocessor`: the model then also accepts raw uint8 RGB frames [B,H,W,3] (host or
@@ -166,12 +202,15 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
         cfg.compute_dtype = self._compute_dtype
         return cfg
 
-    def __call__(self, img) -> torch.Tensor:
-        """[batch, height, width, channels] -> [batch, hidden_size] (CLS token or MAP head output)."""
+    def __call__(self, img, interpolate_pos_encoding: bool = False) -> torch.Tensor:
+        """[batch, height, width, channels] -> [batch, hidden_size] (CLS token or MAP head output).  interpolate_pos_encoding
+        (HuggingFace's keyword): images of any size of at least one patch, the position embeddings resampled bicubically to the
+        patch grid."""
         B = img.shape[0]
-        return self.native(B).vision(img)
+        return self.native(B, hw=self._call_hw(img, interpolate_pos_encoding)).vision(img, interpolate=interpolate_pos_encoding)
 
-    def forward_async(self, img):
+    def forward_async(self, img, interpolate_pos_encoding: bool = False):
         """Asynchronous dispatch for host inputs (the reference's calls return before the device finishes, examples/vit_inference.py:54
         only blocks when it reads the logits): returns a `PendingResult`; back-to-back calls overlap their copies with compute."""
-        return self.native(img.shape[0]).vision_async(img)
+        n = self.native(img.shape[0], hw=self._call_hw(img, interpolate_pos_encoding))
+        return n.vision_async(img, interpolate=interpolate_pos_encoding)

@@ -277,6 +277,84 @@ int tokens_init_run(float* x, const float* cls, const float* pos, int B, int S, 
 }
 
 // ------------------------------------------------------------------------------------------
+// Bicubic resampling of the position table (torch.nn.functional.interpolate(mode="bicubic", align_corners=False), the operation
+// HF's interpolate_pos_encoding applies): source index and Keys' cubic weights (A = -0.75) of output index `dst` along an axis
+// of `in` -> `out` samples, with PyTorch's float operations in PyTorch's order.  The _rn intrinsics keep nvcc from contracting them
+// into FMAs.  At out == in the weights are exactly (0, 1, 0, 0).
+__device__ __forceinline__ void bicubic_taps(int in, int out, int dst, int (&idx)[4], float (&w)[4]) {
+  const float scale = static_cast<float>(in) / static_cast<float>(out);
+  const float real = __fsub_rn(__fmul_rn(scale, __fadd_rn(static_cast<float>(dst), 0.5f)), 0.5f);
+  const int i0 = min(static_cast<int>(floorf(real)), in - 1);
+  const float t = fminf(fmaxf(__fsub_rn(real, static_cast<float>(i0)), 0.f), 1.f);
+  constexpr float A = -0.75f;
+  auto cc1 = [](float x) { return __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2.f, x), A + 3.f), x), x), 1.f); };
+  auto cc2 = [](float x) {
+    return __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, x), 5.f * A), x), 8.f * A), x), 4.f * A);
+  };
+  const float u = __fsub_rn(1.f, t);
+  w[0] = cc2(__fadd_rn(t, 1.f));
+  w[1] = cc1(t);
+  w[2] = cc1(u);
+  w[3] = cc2(__fadd_rn(u, 1.f));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) idx[k] = max(min(i0 - 1 + k, in - 1), 0);
+}
+
+// One thread per (token r, 4 columns): the value is the same for every sample, so it is computed once and stored B times.
+__global__ void __launch_bounds__(256)
+tokens_init_interp_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int B,
+                          int gh, int gw, int S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S * D4) return;
+  const int r = i / D4, c = i - r * D4;
+  const int off = cls != nullptr ? 1 : 0;
+  float4 v;
+  if (r < off) {
+    const float4 a = __ldg(pos + c), b = __ldg(cls + c);
+    v = make_float4(b.x + a.x, b.y + a.y, b.z + a.z, b.w + a.w);
+  } else {
+    const int q = r - off, gy = q / gw, gx = q - gy * gw;
+    int iy[4], ix[4];
+    float wy[4], wx[4];
+    bicubic_taps(g, gh, gy, iy, wy);
+    bicubic_taps(g, gw, gx, ix, wx);
+    const float4* src = pos + static_cast<size_t>(off) * D4 + c;
+    // sum over rows of (sum over columns of tap * wx) * wy, each sum in tap order: PyTorch's separable accumulation
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const float4* row = src + static_cast<size_t>(iy[a]) * g * D4;
+      float4 h = __ldg(row + static_cast<size_t>(ix[0]) * D4);
+      h = make_float4(__fmul_rn(h.x, wx[0]), __fmul_rn(h.y, wx[0]), __fmul_rn(h.z, wx[0]), __fmul_rn(h.w, wx[0]));
+#pragma unroll
+      for (int b = 1; b < 4; ++b) {
+        const float4 p = __ldg(row + static_cast<size_t>(ix[b]) * D4);
+        h.x = __fadd_rn(h.x, __fmul_rn(p.x, wx[b])); h.y = __fadd_rn(h.y, __fmul_rn(p.y, wx[b]));
+        h.z = __fadd_rn(h.z, __fmul_rn(p.z, wx[b])); h.w = __fadd_rn(h.w, __fmul_rn(p.w, wx[b]));
+      }
+      if (a == 0) {
+        v = make_float4(__fmul_rn(h.x, wy[0]), __fmul_rn(h.y, wy[0]), __fmul_rn(h.z, wy[0]), __fmul_rn(h.w, wy[0]));
+      } else {
+        v.x = __fadd_rn(v.x, __fmul_rn(h.x, wy[a])); v.y = __fadd_rn(v.y, __fmul_rn(h.y, wy[a]));
+        v.z = __fadd_rn(v.z, __fmul_rn(h.z, wy[a])); v.w = __fadd_rn(v.w, __fmul_rn(h.w, wy[a]));
+      }
+    }
+  }
+  const size_t SD4 = static_cast<size_t>(S) * D4;
+  for (int b = 0; b < B; ++b) x[b * SD4 + i] = v;
+}
+int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream) {
+  if (B <= 0) return 0;
+  if (D % 4 != 0) { set_last_error("tokens_init_interp: D must be a multiple of 4"); return -1; }
+  if (g <= 0 || gh <= 0 || gw <= 0) { set_last_error("tokens_init_interp: empty grid (g=%d, output %dx%d)", g, gh, gw); return -1; }
+  const int S = gh * gw + (cls != nullptr ? 1 : 0), D4 = D / 4;
+  const int n = S * D4;
+  tokens_init_interp_kernel<<<(n + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls),
+                                                                  reinterpret_cast<const float4*>(pos), g, D4, B, gh, gw, S);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 __global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos, int B, size_t SD, int D) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * D) return;

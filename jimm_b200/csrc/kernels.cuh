@@ -32,6 +32,11 @@ int patchify_run(const void* img, int in_type, int B, int H, int W, int C, int P
 // patch embeddings into rows tok_off.. (common/vit.py:231-236)
 int tokens_init_run(float* x, const float* cls, const float* pos, int B, int S, int D, cudaStream_t stream);
 
+// tokens_init_run on a gh x gw patch grid for a table trained on a g x g grid: x[b, 0, :] = cls + pos[0] (cls != null), and the patch
+// rows (row-major over (gh, gw)) are the bicubic resampling of pos's g x g patch rows (F.interpolate, align_corners=False), computed
+// on the fly from 16 table rows each.  x: fp32 [B, gh*gw (+1), D]; at (gh, gw) == (g, g) the same bits as tokens_init_run.
+int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream);
+
 // x[b, 0, :] = cls + pos[0]   (common/vit.py:231-236), fp32 residual stream [B, S, D]
 int cls_row_run(float* x, const float* cls, const float* pos, int B, int S, int D, cudaStream_t stream);
 

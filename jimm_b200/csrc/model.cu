@@ -16,6 +16,7 @@
 #include <map>
 #include <tuple>
 #include <memory>
+#include <utility>
 #include <string>
 #include <vector>
 
@@ -192,6 +193,13 @@ struct Workspace {
   size_t out_dev_elems = 0;
 };
 
+// A vision forward on a patch grid other than the trained one (jimm_vit_forward_hw & co.): gh x gw patches, S tokens per image, the
+// patch GEMM for this grid and the most images the workspace holds at once.  Host-side state only (tensor maps into the workspace).
+struct PatchGrid {
+  int gh = 0, gw = 0, n = 0, n_pad = 0, S = 0, chunk = 0;
+  GemmPlan patch;
+};
+
 }  // namespace jimm
 
 using namespace jimm;
@@ -201,6 +209,11 @@ struct jimm_model {
   int device = 0;
   bool finalized = false;
   int max_batch = 0;
+  int max_tokens = 0;        // jimm_model_set_max_tokens: vision tokens per sample the workspace holds (the native count when lower)
+  size_t ws_rows = 0;        // residual-stream rows of the vision workspace (x, h, ln_cnt, h8 / sa, the encoder plans' M)
+  size_t ws_big = 0;         // bytes of ws.big
+  static constexpr size_t kMaxGrids = 16;
+  std::map<std::pair<int, int>, PatchGrid> grids;  // off-grid plans by (gh, gw), built on first use
   int cdt = DT_F16;    // compute dtype of GEMM operands
   int adt = DT_F16;    // dtype of the qkv / MAP-kv buffers consumed by the attention kernels (16-bit even in fp32 mode)
   // FP8 compute mode (JIMM_F8E4M3): cdt / adt are fp16, except that the QKV and FC1 GEMMs of every encoder block take e4m3 operands
@@ -634,20 +647,28 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s)
   return run_gemm(m, p, ws.mid2, 4 * D, v.map_fc2, B, s);
 }
 
-// VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  out: fp32 [B, out_dim]
-static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, float* out, cudaStream_t s) {
+// VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  img: [B, H, W, C]; grid: null for the trained patch
+// grid, else the grid of H x W (position table resampled).  out: fp32 [B, out_dim]
+static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, const PatchGrid* grid, float* out, cudaStream_t s) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
-  const int D = v.D, S = v.S, n = v.n;
+  const int D = v.D, S = grid ? grid->S : v.S, n = v.n;
+  const float* cls = v.pooling == JIMM_POOL_CLS ? v.cls : nullptr;
   // patch embed + pos (+cls)
-  if (v.patch_scatter) {
-    JIMM_TRY(tokens_init_run(ws.x, v.pooling == JIMM_POOL_CLS ? v.cls : nullptr, v.pos, B, S, D, s));
-    JIMM_TRY(patchify_run(img, in_dtype, B, v.img, v.img, v.C, v.P, ws.big, m->cdt, s, v.n_pad, v.Kp));
+  if (grid) {
+    // resampled pos (+cls) first; the patch GEMM adds onto it (token scatter, or a residual-reading epilogue with row remap)
+    JIMM_TRY(tokens_init_interp_run(ws.x, cls, v.pos, v.img / v.P, D, B, grid->gh, grid->gw, s));
+    const int rows = v.patch_scatter ? grid->n_pad : grid->n;
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, v.patch_scatter ? grid->n_pad : 0, v.Kp));
+    JIMM_TRY(run_gemm(m, grid->patch, ws.big, v.patch.K, v.patch, B * rows, s));
+  } else if (v.patch_scatter) {
+    JIMM_TRY(tokens_init_run(ws.x, cls, v.pos, B, S, D, s));
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, v.n_pad, v.Kp));
     JIMM_TRY(run_gemm(m, v.p_patch, ws.big, v.patch.K, v.patch, B * v.n_pad, s));
   } else {
-    JIMM_TRY(patchify_run(img, in_dtype, B, v.img, v.img, v.C, v.P, ws.big, m->cdt, s, 0, v.Kp));
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, 0, v.Kp));
     JIMM_TRY(run_gemm(m, v.p_patch, ws.big, v.patch.K, v.patch, B * n, s));
-    if (v.pooling == JIMM_POOL_CLS) JIMM_TRY(cls_row_run(ws.x, v.cls, v.pos, B, S, D, s));
+    if (cls) JIMM_TRY(cls_row_run(ws.x, v.cls, v.pos, B, S, D, s));
   }
   if (v.pre_norm) JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, ws.x, DT_F32, D, B * S, D, s));
   JIMM_TRY(run_encoder(m, &v.enc, B, S, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
@@ -765,13 +786,14 @@ static int run_graphed(jimm_model* m, std::tuple<int, int, int> key, cudaStream_
 
 // Vision tower of one chunk.  Small chunks go through the graph: input staged into ws.in_img, result from m->graph_out.
 static int exec_vision(jimm_model* m, const void* img, int in_dtype, int n, float* out, cudaStream_t s) {
-  if (n <= 0 || n > m->graph_max_batch || !m->graph_out) return run_vision(m, img, in_dtype, n, out, s);
+  const int px = m->vis.img;
+  if (n <= 0 || n > m->graph_max_batch || !m->graph_out) return run_vision(m, img, in_dtype, n, px, px, nullptr, out, s);
   const size_t bytes = static_cast<size_t>(n) * m->vis.img * m->vis.img * m->vis.C * dtype_size(in_dtype);
   if (img != m->ws.in_img) {
     m->host_chain = false;  // the staging buffer is written outside the host path's slot protocol
     JIMM_CUDA_CHECK(cudaMemcpyAsync(m->ws.in_img, img, bytes, cudaMemcpyDeviceToDevice, s));
   }
-  JIMM_TRY(run_graphed(m, std::make_tuple(0, n, in_dtype), s, [&](cudaStream_t cs) { return run_vision(m, m->ws.in_img, in_dtype, n, m->graph_out, cs); }));
+  JIMM_TRY(run_graphed(m, std::make_tuple(0, n, in_dtype), s, [&](cudaStream_t cs) { return run_vision(m, m->ws.in_img, in_dtype, n, px, px, nullptr, m->graph_out, cs); }));
   JIMM_CUDA_CHECK(cudaMemcpyAsync(out, m->graph_out, static_cast<size_t>(n) * vision_out_dim(m) * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return 0;
 }
@@ -1030,9 +1052,12 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   Workspace& ws = m->ws;
   const size_t cs = cdt_size(m);
   const size_t Bm = max_batch;
-  size_t Tv = Bm * v.S, Dmax = D, x_elems = Tv * D, big_bytes = 0;
+  // token budget: max_batch x the native token count, or x jimm_model_set_max_tokens when that is larger
+  const size_t St = m->max_tokens > v.S ? m->max_tokens : v.S;
+  size_t Tv = Bm * St, Dmax = D, x_elems = Tv * D, big_bytes = 0;
   auto upd = [&](size_t b) { if (b > big_bytes) big_bytes = b; };
   upd(Bm * v.n_pad * PPC * cs);          // patches (rows per sample padded to a multiple of 32)
+  if (m->max_tokens > 0) upd((Tv + 31) / 32 * 32 * PPC * cs);  // the padded patch rows of one image of up to Tv tokens
   upd(Tv * 3 * D * 2);                   // qkv (16-bit)
   upd(Tv * static_cast<size_t>(c.v_mlp) * cs);  // MLP hidden
   if (v.pooling == JIMM_POOL_MAP) upd(Tv * 2 * D * 2);
@@ -1102,7 +1127,21 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   }
   JIMM_CUDA_CHECK(cudaDeviceSynchronize());
   m->max_batch = max_batch;
+  m->ws_rows = Tv;
+  m->ws_big = big_bytes;
   m->finalized = true;
+  return 0;
+}
+
+int jimm_model_set_max_tokens(jimm_model_t* m, int tokens_per_sample) {
+  if (!m) { set_last_error("null model"); return JIMM_EINVAL; }
+  if (m->finalized) { set_last_error("jimm_model_set_max_tokens: call it before jimm_model_finalize"); return JIMM_ESTATE; }
+  if (m->cfg.kind == JIMM_ENCODER || m->cfg.kind == JIMM_MAPHEAD) {
+    set_last_error("jimm_model_set_max_tokens: sub-module handles take their token count from ctx_len");
+    return JIMM_EINVAL;
+  }
+  if (tokens_per_sample <= 0) { set_last_error("jimm_model_set_max_tokens: tokens_per_sample must be positive (got %d)", tokens_per_sample); return JIMM_EINVAL; }
+  m->max_tokens = tokens_per_sample;
   return 0;
 }
 
@@ -1146,6 +1185,83 @@ static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, fl
   }
   return 0;
 }
+// How many images of a gh x gw patch grid one chunk of an off-grid call runs: max_batch, or fewer when the token-sized buffers (x, h,
+// ln_cnt, h8 / sa: ws_rows rows; ws.big: patches | qkv | MLP hidden | MAP k,v, counted in bytes) hold fewer.  0: one image does not fit.
+static size_t grid_chunk(const jimm_model* m, int gh, int gw) {
+  const VisionTower& v = m->vis;
+  const size_t n = static_cast<size_t>(gh) * gw, S = n + (v.pooling == JIMM_POOL_CLS ? 1 : 0), n_pad = (n + 31) / 32 * 32;
+  const size_t cs = cdt_size(m), D = v.D, Mlp = v.enc.c.M;
+  size_t per_big = (v.patch_scatter ? n_pad : n) * v.Kp * cs;
+  auto upd = [&](size_t b) { if (b > per_big) per_big = b; };
+  upd(S * 3 * D * 2);
+  upd(S * Mlp * cs);
+  if (v.pooling == JIMM_POOL_MAP) upd(S * 2 * D * 2);
+  size_t chunk = m->max_batch;
+  if (m->ws_rows / S < chunk) chunk = m->ws_rows / S;
+  if (m->ws_big / per_big < chunk) chunk = m->ws_big / per_big;
+  return chunk;
+}
+
+// The off-grid state for H x W images: the patch grid, how many images a chunk runs (grid_chunk) and the patch GEMM plan for that many.
+// The plan is host-side tensor maps only, so the cache is simply dropped when full.
+static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
+  const VisionTower& v = m->vis;
+  const int gh = H / v.P, gw = W / v.P, off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  auto it = m->grids.find(std::make_pair(gh, gw));
+  if (it != m->grids.end()) { *out = &it->second; return 0; }
+  const size_t n = static_cast<size_t>(gh) * gw, S = n + off, n_pad = (n + 31) / 32 * 32;
+  const size_t chunk = grid_chunk(m, gh, gw);
+  if (chunk == 0) {
+    set_last_error("a %dx%d image needs %zu tokens (%dx%d patches%s), more than fit this handle's vision workspace (%zu tokens in all); "
+                   "raise the budget with jimm_model_set_max_tokens before jimm_model_finalize", H, W, S, gh, gw, off ? " + CLS" : "",
+                   m->ws_rows);
+    return JIMM_EINVAL;
+  }
+  PatchGrid g;
+  g.gh = gh; g.gw = gw; g.n = static_cast<int>(n); g.n_pad = static_cast<int>(n_pad); g.S = static_cast<int>(S); g.chunk = static_cast<int>(chunk);
+  GemmEpilogue e;
+  e.bias = v.patch.b; e.residual = m->ws.x; e.ldr = v.D; e.out = m->ws.x; e.out_type = DT_F32; e.ldo = v.D;
+  int rows = g.n;
+  if (v.patch_scatter) {
+    e.mode = 2; e.tok_pad = g.n_pad; e.tok_off = off; e.tok_S = g.S;
+    rows = g.n_pad;
+  } else {
+    e.mode = 0; e.rows_in = g.n; e.rows_out = g.S; e.row_off = off;  // adds onto the resampled table already in x
+  }
+  JIMM_TRY(gemm_plan_init(&g.patch, m->cdt, m->ws.big, v.Kp, v.patch.w, v.Kp, g.chunk * rows, v.D, v.Kp, e));
+  if (v.patch_scatter && g.patch.epi.mode != 2) { set_last_error("patch GEMM: token-scatter epilogue unavailable"); return JIMM_EINVAL; }
+  if (m->grids.size() >= jimm_model::kMaxGrids) m->grids.clear();
+  *out = &(m->grids[std::make_pair(gh, gw)] = g);
+  return 0;
+}
+
+// Vision forward of B images of H x W.  The native size goes through vision_chunks (graphs, staging); other sizes run eagerly.
+static int vision_chunks_hw(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s) {
+  const VisionTower& v = m->vis;
+  if (H < v.P || W < v.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, v.P, v.P); return JIMM_EINVAL; }
+  if (H == v.img && W == v.img) return vision_chunks(m, img, in_dtype, B, out, s);
+  PatchGrid* grid = nullptr;  // null: the trained grid (the trailing pixels differ only)
+  if (H / v.P != v.img / v.P || W / v.P != v.img / v.P) JIMM_TRY(get_grid(m, H, W, &grid));
+  const int chunk = grid ? grid->chunk : m->max_batch;
+  const size_t img_bytes = static_cast<size_t>(H) * W * v.C * dtype_size(in_dtype);
+  const int od = vision_out_dim(m);
+  for (int b0 = 0; b0 < B; b0 += chunk) {
+    const int nb = B - b0 < chunk ? B - b0 : chunk;
+    JIMM_TRY(run_vision(m, static_cast<const uint8_t*>(img) + b0 * img_bytes, in_dtype, nb, H, W, grid, out + static_cast<size_t>(b0) * od, s));
+  }
+  return 0;
+}
+
+int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images) {
+  JIMM_TRY(check_ready(m, 0));
+  if (!m->vis.present || !images) { set_last_error("jimm_model_images_per_call: %s", images ? "model has no vision tower" : "null argument"); return JIMM_EINVAL; }
+  const VisionTower& v = m->vis;
+  if (H < v.P || W < v.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, v.P, v.P); return JIMM_EINVAL; }
+  const bool trained = H / v.P == v.img / v.P && W / v.P == v.img / v.P;
+  *images = trained ? m->max_batch : static_cast<int>(grid_chunk(m, H / v.P, W / v.P));
+  return 0;
+}
+
 static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
   for (int b0 = 0; b0 < B; b0 += m->max_batch) {
     const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
@@ -1167,6 +1283,22 @@ int jimm_encode_image(jimm_model_t* m, const void* img, int in_dtype, int B, flo
   if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   return vision_chunks(m, img, in_dtype, B, out, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
+  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_hw on a dual-tower model; use jimm_encode_image_hw"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  return vision_chunks_hw(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
+  if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  return vision_chunks_hw(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {
@@ -1214,26 +1346,39 @@ static int join_text(jimm_model* m, cudaStream_t s, cudaStream_t ts) {
 }
 
 // encode_image + encode_text of one call, the two towers running concurrently (device inputs); img_e fp32 [Bi,E], txt_e fp32 [Bt,E].
-int jimm_dual_encode(jimm_model_t* m, const void* img, int in_dtype, int Bi, const int32_t* ids, int Bt, int T, float* img_e, float* txt_e,
-                     void* stream) {
+int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T, float* img_e,
+                        float* txt_e, void* stream) {
   JIMM_TRY(check_ready(m, Bi));
   if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
   if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
   if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
+  if (H < m->vis.P || W < m->vis.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, m->vis.P, m->vis.P); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   cudaStream_t s = static_cast<cudaStream_t>(stream), ts = s;
   JIMM_TRY(fork_text(m, s, &ts));
   JIMM_TRY(text_chunks(m, ids, Bt, T, txt_e, ts));
-  JIMM_TRY(vision_chunks(m, img, in_dtype, Bi, img_e, s));
+  JIMM_TRY(vision_chunks_hw(m, img, in_dtype, Bi, H, W, img_e, s));
   return join_text(m, s, ts);
+}
+
+int jimm_dual_encode(jimm_model_t* m, const void* img, int in_dtype, int Bi, const int32_t* ids, int Bt, int T, float* img_e, float* txt_e,
+                     void* stream) {
+  JIMM_TRY(check_ready(m, Bi));
+  return jimm_dual_encode_hw(m, img, in_dtype, Bi, m->vis.img, m->vis.img, ids, Bt, T, img_e, txt_e, stream);
+}
+
+int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T, float* logits,
+                         void* stream) {
+  JIMM_TRY(check_ready(m, Bi));
+  if (Bi > m->max_batch || Bt > m->max_batch) { set_last_error("dual_forward: batch (%d,%d) exceeds max_batch %d", Bi, Bt, m->max_batch); return JIMM_EINVAL; }
+  JIMM_TRY(jimm_dual_encode_hw(m, img, in_dtype, Bi, H, W, ids, Bt, T, m->ws.emb_i, m->ws.emb_t, stream));
+  return jimm_contrastive_logits(m, m->ws.emb_i, Bi, m->ws.emb_t, Bt, logits, stream);
 }
 
 int jimm_dual_forward(jimm_model_t* m, const void* img, int in_dtype, int Bi, const int32_t* ids, int Bt, int T, float* logits,
                       void* stream) {
   JIMM_TRY(check_ready(m, Bi));
-  if (Bi > m->max_batch || Bt > m->max_batch) { set_last_error("dual_forward: batch (%d,%d) exceeds max_batch %d", Bi, Bt, m->max_batch); return JIMM_EINVAL; }
-  JIMM_TRY(jimm_dual_encode(m, img, in_dtype, Bi, ids, Bt, T, m->ws.emb_i, m->ws.emb_t, stream));
-  return jimm_contrastive_logits(m, m->ws.emb_i, Bi, m->ws.emb_t, Bt, logits, stream);
+  return jimm_dual_forward_hw(m, img, in_dtype, Bi, m->vis.img, m->vis.img, ids, Bt, T, logits, stream);
 }
 
 // ---- forward of a bare sub-module (device buffers) ----
@@ -1633,6 +1778,9 @@ int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, in
 int jimm_k_activation(const float* x, float* y, long long n, int act, void* stream) {
   if (n < 0 || (n > 0 && (!x || !y))) { set_last_error("jimm_k_activation: bad arguments"); return JIMM_EINVAL; }
   return activation_run(x, y, static_cast<size_t>(n), act, static_cast<cudaStream_t>(stream));
+}
+int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream) {
+  return tokens_init_interp_run(x, cls, pos, g, D, B, gh, gw, static_cast<cudaStream_t>(stream));
 }
 int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream) {
   return embed_run(ids, table, pos, x, B, T, D, vocab, static_cast<cudaStream_t>(stream));

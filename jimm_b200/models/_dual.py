@@ -35,21 +35,26 @@ class DualTower(_NativeOwner, nn.Module):
         return cfg
 
     # ---- reference API ----
-    def encode_image(self, image) -> torch.Tensor:
-        return self.native(image.shape[0]).vision(image, encode=True)
+    def encode_image(self, image, interpolate_pos_encoding: bool = False) -> torch.Tensor:
+        """interpolate_pos_encoding (HuggingFace's keyword): images of any size of at least one patch, the position embeddings
+        resampled bicubically to the patch grid."""
+        n = self.native(image.shape[0], hw=self._call_hw(image, interpolate_pos_encoding))
+        return n.vision(image, encode=True, interpolate=interpolate_pos_encoding)
 
     def encode_text(self, text) -> torch.Tensor:
         return self.native(text.shape[0]).text(text)
 
-    def __call__(self, image, text) -> torch.Tensor:
+    def __call__(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """Similarity logits.  Single process: [B_img, B_txt].  Under torch.distributed (one process per GPU, batch sharded
         over ranks like the reference's P("batch") inputs, examples/clip_inference.py:41-42): this rank's row block
-        [B_local, world*B_local], embeddings exchanged over NVLink peer memory inside the fused logits kernel."""
+        [B_local, world*B_local], embeddings exchanged over NVLink peer memory inside the fused logits kernel.
+        interpolate_pos_encoding: as in encode_image."""
         import torch.distributed as dist
 
         if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and self._comm_mode != "off":
-            return self._call_distributed(image, text)
-        return self.native(max(image.shape[0], text.shape[0]), require=True).dual(image, text)
+            return self._call_distributed(image, text, interpolate_pos_encoding)
+        n = self.native(max(image.shape[0], text.shape[0]), require=True, hw=self._call_hw(image, interpolate_pos_encoding))
+        return n.dual(image, text, interpolate=interpolate_pos_encoding)
 
     def set_comm(self, mode: str):
         """'peer' (default, fused NVLink peer-store kernel) | 'nccl' (torch.distributed all_gather baseline) | 'off'."""
@@ -58,12 +63,12 @@ class DualTower(_NativeOwner, nn.Module):
         object.__setattr__(self, "_comm_mode", mode)
         return self
 
-    def _call_distributed(self, image, text) -> torch.Tensor:
+    def _call_distributed(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         import torch.distributed as dist
 
         B = image.shape[0]
-        n = self.native(B, require=True)
-        x, ids = n._prep_images(image), n._prep_ids(text)
+        n = self.native(B, require=True, hw=self._call_hw(image, interpolate_pos_encoding))
+        x, ids = n._prep_images(image, interpolate_pos_encoding), n._prep_ids(text)
         host_in = not x.is_cuda and not ids.is_cuda
         with torch.cuda.device(n.device):
             cur = torch.cuda.current_stream(n.device)
@@ -88,7 +93,7 @@ class DualTower(_NativeOwner, nn.Module):
                 te = n.text(ids_d)
                 cur.wait_stream(side)
                 x_d.record_stream(cur)
-                ie = n.vision(x_d, encode=True)
+                ie = n.vision(x_d, encode=True, interpolate=interpolate_pos_encoding)
             out = self._distributed_logits(n, ie, te, B)
             if not host_in:
                 return out

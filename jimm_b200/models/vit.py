@@ -43,16 +43,18 @@ class VisionTransformer(_NativeOwner, nn.Module):
         cfg.compute_dtype = self._compute_dtype
         return cfg
 
-    def __call__(self, x) -> torch.Tensor:
+    def __call__(self, x, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """[batch, height, width, channels] -> logits [batch, num_classes] (models/vit.py:91-103).
 
-        Inference semantics (dropout is the identity), like the reference after `.eval()`."""
-        return self.native(x.shape[0]).vision(x)
+        Inference semantics (dropout is the identity), like the reference after `.eval()`.  interpolate_pos_encoding (HuggingFace's
+        keyword): images of any size of at least one patch, the position embeddings resampled bicubically to the patch grid."""
+        return self.native(x.shape[0], hw=self._call_hw(x, interpolate_pos_encoding)).vision(x, interpolate=interpolate_pos_encoding)
 
-    def forward_async(self, x):
+    def forward_async(self, x, interpolate_pos_encoding: bool = False):
         """Asynchronous dispatch for host inputs (JAX dispatches asynchronously; examples/vit_inference.py:54-58 only blocks when
         it reads the logits): returns a `PendingResult`; back-to-back calls overlap their H2D copies with the previous forward."""
-        return self.native(x.shape[0]).vision_async(x)
+        n = self.native(x.shape[0], hw=self._call_hw(x, interpolate_pos_encoding))
+        return n.vision_async(x, interpolate=interpolate_pos_encoding)
 
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "VisionTransformer":
