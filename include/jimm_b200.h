@@ -136,6 +136,14 @@ JIMM_API int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype,
                                  float* img_e, float* txt_e, void* stream);
 JIMM_API int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T,
                                   float* logits, void* stream);
+/* B images of different sizes in one call.  imgs: host array of B device pointers, image i NHWC [H[i], W[i], in_ch], contiguous;
+ * H, W: host int arrays, read during the call; out: device fp32 [B, out_dim].  Image i's row equals the *_hw call on that image alone.
+ * The tokens of consecutive images are packed into one stream (variable-length attention): the images are walked in order, and a new
+ * chunk starts when the next image would pass max_batch images, the token budget or the workspace bytes (counted as for the *_hw
+ * calls).  An image that alone does not fit is JIMM_EINVAL with the *_hw message, before anything is enqueued.  Packed calls run
+ * eagerly and return without synchronising; back-to-back calls on one stream are safe. */
+JIMM_API int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
+JIMM_API int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
 
 /* -- forward of a bare sub-module (kinds JIMM_ENCODER / JIMM_MAPHEAD; config fields used: v_width, v_heads, v_mlp, v_layers, v_act,
  *    v_eps_block, v_eps_outer, t_causal (attn_mask = tril), ctx_len = max tokens per sample, compute_dtype; parameters keyed
@@ -232,6 +240,13 @@ JIMM_API int jimm_k_attention_hd(const void* qkv, int io_type, void* out, int ou
                                  int reverse, void* stream);
 JIMM_API int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim,
                                      void* stream);
+/* Packed forms of the two above (non-causal): seq_off device int32 [B + 1], sample b = rows seq_off[b] .. seq_off[b+1]-1 of the packed
+ * [rows, 3D] qkv / [rows, 2D] kv (and of out [rows, D] for attention; out [B, D] for MAP), every length >= 1 and <= max_S.  Each
+ * sample's result is the bits of the _hd call on that sample alone; rows outside every sample are not written. */
+JIMM_API int jimm_k_attention_packed(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H,
+                                     int head_dim, int reverse, void* stream);
+JIMM_API int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B,
+                                         int max_S, int H, int head_dim, void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
 /* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left
  * untouched) and ldk (row stride in elements, 0 = P*P*C; more = pad columns, written as zeros). */

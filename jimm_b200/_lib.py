@@ -72,6 +72,8 @@ SIGNATURES = {
     "jimm_encode_image_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _fp, _vp]),
     "jimm_dual_encode_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _i, _i, _fp, _fp, _vp]),
     "jimm_dual_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _i, _i, _fp, _vp]),
+    "jimm_vit_forward_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
+    "jimm_encode_image_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -98,6 +100,8 @@ SIGNATURES = {
     "jimm_k_quantize_e4m3": (_i, [_fp, _i, _i, _i, _vp, _i, _fp, _vp]),
     "jimm_k_attention_hd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention_hd": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_attention_packed": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_map_attention_packed": (_i, [_fp, _vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),

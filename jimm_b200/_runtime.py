@@ -206,6 +206,63 @@ class NativeModel:
                           C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
         return out if x.is_cuda else out.cpu()
 
+    # ---- packed lists of images of different sizes (jimm_vit_forward_packed) ----
+    def _prep_image_list(self, images, interpolate: bool):
+        """Each element of a list / tuple as one prepared image [H, W, C] (a leading batch dimension of 1 is dropped), all of one
+        dtype and on one device; the checks of _prep_images, per image."""
+        xs = []
+        for i, x in enumerate(images):
+            x = _as_tensor(x, "image")
+            if x.ndim == 4 and x.shape[0] == 1:
+                x = x[0]
+            if x.ndim != 3:
+                raise ValueError(f"image {i} of the list: expected [height, width, channels] or [1, height, width, channels], got {tuple(x.shape)}")
+            xs.append(x)
+        if len({x.dtype for x in xs}) > 1:
+            raise ValueError(f"the images of a list must share one dtype, got {sorted({str(x.dtype) for x in xs})}")
+        if len({x.device for x in xs}) > 1:
+            raise ValueError(f"the images of a list must be on one device, got {sorted({str(x.device) for x in xs})}")
+        return [self._prep_images(x[None], interpolate)[0] for x in xs]
+
+    def _vision_packed_dev(self, images, encode: bool, interpolate: bool):
+        """The rows of a list of images on this GPU (fp32 [len, out_dim]) and whether the inputs were host memory."""
+        xs = self._prep_image_list(images, interpolate)
+        B = len(xs)
+        host = B > 0 and not xs[0].is_cuda
+        with torch.cuda.device(self.device):
+            out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
+            if B == 0:
+                return out, True
+            # uint8 frames go through the image front-end one at a time (their output sizes differ)
+            xd = [self._device_images(x[None])[0].contiguous() for x in xs]
+            ptrs = (C.c_void_p * B)(*[x.data_ptr() for x in xd])
+            hs = (C.c_int * B)(*[x.shape[0] for x in xd])
+            ws = (C.c_int * B)(*[x.shape[1] for x in xd])
+            fn = self.lib.jimm_encode_image_packed if encode else self.lib.jimm_vit_forward_packed
+            _lib.check(fn(self.handle, ptrs, _TORCH_TO_CODE[xd[0].dtype], B, hs, ws, C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
+            if not host:
+                cur = torch.cuda.current_stream(self.device)
+                for x in xd:  # freshly made device copies are freed only after the call's work
+                    x.record_stream(cur)
+        return out, host
+
+    def vision_packed(self, images, encode: bool = False, interpolate: bool = False) -> torch.Tensor:
+        """A list / tuple of images of different sizes in one call: their tokens packed into one stream (variable-length
+        attention).  Row i is the result of the call on images[i] alone.  CUDA inputs -> CUDA output without a host synchronisation;
+        host inputs -> host output."""
+        out, host = self._vision_packed_dev(images, encode, interpolate)
+        return out.cpu() if host else out
+
+    def dual_packed(self, images, text, interpolate: bool = False) -> torch.Tensor:
+        """CLIP.__call__ / SigLIP.__call__ on a list of images of different sizes."""
+        ids = self._prep_ids(text)
+        ie, host = self._vision_packed_dev(images, True, interpolate)
+        host = host and not ids.is_cuda
+        with torch.cuda.device(self.device):
+            te = self.text(ids.to(self.device, non_blocking=True))
+            out = self.logits(ie, te)
+        return out.cpu() if host else out
+
     def _operand_dtype(self) -> torch.dtype:
         return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16, _lib.F8E4M3: torch.float16}[self.cfg.compute_dtype]
 

@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _lib, nn
-from .._runtime import NativeModel, default_max_batch, grid_tokens
+from .._runtime import NativeModel, PendingResult, default_max_batch, grid_tokens
 from .transformer import Transformer, _SubModuleRunner, g_wrap
 
 
@@ -123,6 +123,22 @@ class _NativeOwner:
         P = self._native_config().patch
         return (h, w) if h >= P and w >= P else None
 
+    def _list_hw(self, images, interpolate_pos_encoding: bool):
+        """The (height, width) with the most tokens among a list's images (what the tower sees: uint8 frames after the front-end), for
+        native(hw=...): the handle is rebuilt only when that image alone does not fit.  None for an empty list or without
+        interpolate_pos_encoding."""
+        best, cfg = None, self._native_config()
+        for img in images:
+            hw = self._call_hw(img[None] if getattr(img, "ndim", 0) == 3 else img, interpolate_pos_encoding)
+            if hw is not None and (best is None or grid_tokens(cfg, *hw) > grid_tokens(cfg, *best)):
+                best = hw
+        return best
+
+    def _vision_list(self, images, interpolate_pos_encoding: bool, encode: bool = False) -> torch.Tensor:
+        """A list / tuple of images of different sizes in one packed call (NativeModel.vision_packed)."""
+        return self.native(max(len(images), 1), hw=self._list_hw(images, interpolate_pos_encoding)).vision_packed(
+            images, encode=encode, interpolate=interpolate_pos_encoding)
+
     def set_max_image_size(self, height: int, width: int):
         """Size the vision workspace for interpolate_pos_encoding calls on images up to height x width: `max_batch` such images run
         in one chunk, and no call on them rebuilds the handle.  The default holds `max_batch` images of the native size (larger
@@ -205,12 +221,18 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
     def __call__(self, img, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """[batch, height, width, channels] -> [batch, hidden_size] (CLS token or MAP head output).  interpolate_pos_encoding
         (HuggingFace's keyword): images of any size of at least one patch, the position embeddings resampled bicubically to the
-        patch grid."""
+        patch grid.  A list / tuple of images [H_i, W_i, C] (or [1, H_i, W_i, C]) of different sizes runs in one packed call; row i
+        is the result of images[i] alone."""
+        if isinstance(img, (list, tuple)):
+            return self._vision_list(img, interpolate_pos_encoding)
         B = img.shape[0]
         return self.native(B, hw=self._call_hw(img, interpolate_pos_encoding)).vision(img, interpolate=interpolate_pos_encoding)
 
     def forward_async(self, img, interpolate_pos_encoding: bool = False):
         """Asynchronous dispatch for host inputs (the reference's calls return before the device finishes, examples/vit_inference.py:54
-        only blocks when it reads the logits): returns a `PendingResult`; back-to-back calls overlap their copies with compute."""
+        only blocks when it reads the logits): returns a `PendingResult`; back-to-back calls overlap their copies with compute.  A
+        list of images runs as in __call__, synchronously for host images."""
+        if isinstance(img, (list, tuple)):
+            return PendingResult(self._vision_list(img, interpolate_pos_encoding), None)
         n = self.native(img.shape[0], hw=self._call_hw(img, interpolate_pos_encoding))
         return n.vision_async(img, interpolate=interpolate_pos_encoding)

@@ -100,16 +100,27 @@ struct AttnSmem<BYTES, false> {
 };
 
 // Head width d (a multiple of 8, d <= DP); the tiles are padded to DP columns with zeros.  scale_log2 = log2(e) / sqrt(d).
-template <typename T, typename OutT, bool CAUSAL, int DP>
+// PACKED: sample b is rows seq_off[b] .. seq_off[b + 1] - 1 of qkv / out (S_arg unused); query tiles past a sample's end exit at once.
+template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED = false>
 __global__ void __launch_bounds__(128)
-attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H, int d, float scale_log2, int reverse) {
+attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, int H, int d, float scale_log2, int reverse,
+                 const int* __restrict__ seq_off) {
   using L = HeadTile<DP>;
   uint8_t* smem = AttnSmem<L::SMEM>::get();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, h = blockIdx.y, b = reverse ? static_cast<int>(gridDim.z) - 1 - static_cast<int>(blockIdx.z) : static_cast<int>(blockIdx.z);
   const int D = H * d;
   const size_t ld = static_cast<size_t>(3) * D;
-  const T* base = qkv + static_cast<size_t>(b) * S * ld + h * d;
+  int S = S_arg;
+  size_t row0 = static_cast<size_t>(b) * S_arg;
+  if constexpr (PACKED) {
+    pdl_launch_dependents();
+    pdl_wait();  // the offsets may come from the previous kernel
+    row0 = static_cast<size_t>(seq_off[b]);
+    S = seq_off[b + 1] - seq_off[b];
+    if (qt * QT >= S) return;
+  }
+  const T* base = qkv + row0 * ld + h * d;
   const T* gq = base;
   const T* gk = base + D;
   const T* gv = base + 2 * D;
@@ -117,8 +128,10 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
   const uint32_t sK0 = sQ + L::BYTES;
   const uint32_t sV0 = sK0 + 2 * L::BYTES;
   const int q0 = qt * QT;
-  pdl_launch_dependents();
-  pdl_wait();
+  if constexpr (!PACKED) {
+    pdl_launch_dependents();
+    pdl_wait();
+  }
   int n_kv = (S + KT - 1) / KT;
   if (CAUSAL) n_kv = min(n_kv, qt + 1);
 
@@ -243,7 +256,7 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S, int H
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     inv[r] = 1.0f / l;
   }
-  OutT* obase = out + static_cast<size_t>(b) * S * D + h * d;
+  OutT* obase = out + row0 * D + h * d;
   if constexpr (sizeof(OutT) == 2) {
     // stage this warp's 16 x DP tile through its (now free) Q rows so the global stores are whole 16-byte chunks of a row
     uint8_t* sq = smem;
@@ -292,60 +305,77 @@ static int padded_head_dim(int d) { return d <= 16 ? 16 : d <= 32 ? 32 : d <= 64
 // The softmax scale 1 / sqrt(d) (flax: query / sqrt(depth)) times log2(e), in fp32: 0.125f * log2(e) for d = 64.
 static float attn_scale_log2(int d) { return static_cast<float>(1.0 / std::sqrt(static_cast<double>(d))) * 1.4426950408889634f; }
 
-template <typename T, typename OutT, bool CAUSAL, int DP>
-static int attn_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse) {
+// seq_off null: B samples of S rows each; else the packed form (S = the longest sample, sample b = rows seq_off[b] .. seq_off[b + 1] - 1)
+template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED>
+static int attn_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse, const int* seq_off) {
   constexpr int SMEM = HeadTile<DP>::SMEM;
   constexpr size_t dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
+  auto* kernel = attention_kernel<T, OutT, CAUSAL, DP, PACKED>;
   if constexpr (dyn > 0) {
     static DeviceOnce attr_set;
-    if (attr_set.first()) JIMM_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<T, OutT, CAUSAL, DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+    if (attr_set.first()) JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
   }
   dim3 grid((S + QT - 1) / QT, H, B);
-  JIMM_CUDA_CHECK(launch_k(attention_kernel<T, OutT, CAUSAL, DP>, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S,
-                           H, d, attn_scale_log2(d), reverse));
+  JIMM_CUDA_CHECK(launch_k(kernel, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d,
+                           attn_scale_log2(d), reverse, seq_off));
   note_launch();
   return 0;
 }
 
-template <typename T, typename OutT, bool CAUSAL>
-static int attn_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse) {
+template <typename T, typename OutT, bool CAUSAL, bool PACKED>
+static int attn_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse, const int* seq_off) {
   switch (padded_head_dim(d)) {
-    case 16: return attn_launch_dp<T, OutT, CAUSAL, 16>(qkv, out, B, S, H, d, stream, reverse);
-    case 32: return attn_launch_dp<T, OutT, CAUSAL, 32>(qkv, out, B, S, H, d, stream, reverse);
-    case 64: return attn_launch_dp<T, OutT, CAUSAL, 64>(qkv, out, B, S, H, d, stream, reverse);
-    case 80: return attn_launch_dp<T, OutT, CAUSAL, 80>(qkv, out, B, S, H, d, stream, reverse);
-    case 96: return attn_launch_dp<T, OutT, CAUSAL, 96>(qkv, out, B, S, H, d, stream, reverse);
-    default: return attn_launch_dp<T, OutT, CAUSAL, 128>(qkv, out, B, S, H, d, stream, reverse);
+    case 16: return attn_launch_dp<T, OutT, CAUSAL, 16, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+    case 32: return attn_launch_dp<T, OutT, CAUSAL, 32, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+    case 64: return attn_launch_dp<T, OutT, CAUSAL, 64, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+    case 80: return attn_launch_dp<T, OutT, CAUSAL, 80, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+    case 96: return attn_launch_dp<T, OutT, CAUSAL, 96, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+    default: return attn_launch_dp<T, OutT, CAUSAL, 128, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
   }
 }
 
+// the packed form is non-causal only
 template <typename T, typename OutT>
-static int attn_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, int reverse) {
-  if (causal) return attn_launch_causal<T, OutT, true>(qkv, out, B, S, H, d, stream, reverse);
-  return attn_launch_causal<T, OutT, false>(qkv, out, B, S, H, d, stream, reverse);
+static int attn_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, int reverse, const int* seq_off) {
+  if (seq_off) return attn_launch_causal<T, OutT, false, true>(qkv, out, B, S, H, d, stream, reverse, seq_off);
+  if (causal) return attn_launch_causal<T, OutT, true, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
+  return attn_launch_causal<T, OutT, false, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
 }
 
 static bool head_dim_ok(int d) { return d >= 8 && d <= 128 && d % 8 == 0; }
 
-int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream, int reverse) {
+static int attn_dispatch(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream,
+                         int reverse, const int* seq_off) {
   if (!head_dim_ok(head_dim)) { set_last_error("attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0 || S <= 0) return 0;
   if (B > 65535 || H > 65535) { set_last_error("attention: grid too large (B=%d H=%d)", B, H); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return attn_launch<__half, __half>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
-  if (io_type == DT_F16 && out_type == DT_F32) return attn_launch<__half, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
-  if (io_type == DT_F16 && out_type == DT_TF32) return attn_launch<__half, tf32_t>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return attn_launch<__nv_bfloat16, __nv_bfloat16>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
-  if (io_type == DT_BF16 && out_type == DT_F32) return attn_launch<__nv_bfloat16, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse);
+  if (io_type == DT_F16 && out_type == DT_F16) return attn_launch<__half, __half>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
+  if (io_type == DT_F16 && out_type == DT_F32) return attn_launch<__half, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
+  if (io_type == DT_F16 && out_type == DT_TF32) return attn_launch<__half, tf32_t>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
+  if (io_type == DT_BF16 && out_type == DT_BF16) return attn_launch<__nv_bfloat16, __nv_bfloat16>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
+  if (io_type == DT_BF16 && out_type == DT_F32) return attn_launch<__nv_bfloat16, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
   set_last_error("attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
   return -1;
+}
+
+int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream, int reverse) {
+  return attn_dispatch(qkv, io_type, out, out_type, B, S, H, head_dim, causal, stream, reverse, nullptr);
+}
+
+int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H, int head_dim,
+                         cudaStream_t stream, int reverse) {
+  if (!seq_off) { set_last_error("attention_packed: null seq_off"); return -1; }
+  return attn_dispatch(qkv, io_type, out, out_type, B, max_S, H, head_dim, 0, stream, reverse, seq_off);
 }
 
 // ------------------------------------------------------------------------------------------
 // MAP-head attention: one CTA (256 threads) per (sample, head); scores in smem; HBM-bound on K/V.
 // ------------------------------------------------------------------------------------------
-template <typename T, typename OutT>
+// PACKED: sample b is rows seq_off[b] .. seq_off[b + 1] - 1 of kv (S_arg: the longest sample, which the scores' smem is sized for)
+template <typename T, typename OutT, bool PACKED = false>
 __global__ void __launch_bounds__(256)
-map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT* __restrict__ out, int S, int H, int d, float qscale) {
+map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT* __restrict__ out, int S_arg, int H, int d, float qscale,
+                     const int* __restrict__ seq_off) {
   extern __shared__ float sm[];
   float* sq = sm;              // [128]
   float* red = sm + 128;       // [8 * 128] cross-group reduction / [8] block reductions
@@ -353,7 +383,13 @@ map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int D = H * d;
   const size_t ld = static_cast<size_t>(2) * D;
-  const T* kbase = kv + static_cast<size_t>(b) * S * ld + h * d;
+  int S = S_arg;
+  size_t row0 = static_cast<size_t>(b) * S_arg;
+  if constexpr (PACKED) {
+    row0 = static_cast<size_t>(seq_off[b]);
+    S = seq_off[b + 1] - seq_off[b];
+  }
+  const T* kbase = kv + row0 * ld + h * d;
   const T* vbase = kbase + D;
   if (tid < d) sq[tid] = q[h * d + tid] * qscale;  // query / sqrt(depth)
   __syncthreads();
@@ -425,26 +461,38 @@ map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT
 }
 
 template <typename T, typename OutT>
-static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream) {
+static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
   dim3 grid(H, B);
   const size_t smem = (128 + 1024 + S) * sizeof(float);
   const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(d)));  // 0.125f for d = 64
-  map_attention_kernel<T, OutT><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale);
+  if (seq_off) map_attention_kernel<T, OutT, true><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off);
+  else map_attention_kernel<T, OutT><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, nullptr);
   JIMM_LAUNCH_CHECK();
   return 0;
 }
 
-int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream) {
+static int map_dispatch(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
+                        const int* seq_off) {
   if (!head_dim_ok(head_dim)) { set_last_error("map_attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0) return 0;
   if (S > 8192) { set_last_error("map_attention: S=%d too large", S); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream);
-  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream);
-  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream);
-  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream);
+  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream, seq_off);
+  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream, seq_off);
+  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream, seq_off);
+  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream, seq_off);
+  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream, seq_off);
   set_last_error("map_attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
   return -1;
+}
+
+int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream) {
+  return map_dispatch(q, kv, io_type, out, out_type, B, S, H, head_dim, stream, nullptr);
+}
+
+int map_attention_packed_run(const float* q, const void* kv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H,
+                             int head_dim, cudaStream_t stream) {
+  if (!seq_off) { set_last_error("map_attention_packed: null seq_off"); return -1; }
+  return map_dispatch(q, kv, io_type, out, out_type, B, max_S, H, head_dim, stream, seq_off);
 }
 
 }  // namespace jimm

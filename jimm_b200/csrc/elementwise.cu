@@ -300,13 +300,10 @@ __device__ __forceinline__ void bicubic_taps(int in, int out, int dst, int (&idx
   for (int k = 0; k < 4; ++k) idx[k] = max(min(i0 - 1 + k, in - 1), 0);
 }
 
-// One thread per (token r, 4 columns): the value is the same for every sample, so it is computed once and stored B times.
-__global__ void __launch_bounds__(256)
-tokens_init_interp_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int B,
-                          int gh, int gw, int S) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= S * D4) return;
-  const int r = i / D4, c = i - r * D4;
+// Row r of the initial residual stream of a gh x gw grid, columns 4 c .. 4 c + 3: cls + pos[0] for the CLS row (cls != null), else
+// the bicubic resampling of pos's g x g patch rows.
+__device__ __forceinline__ float4 interp_token(const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int gh, int gw, int r,
+                                               int c) {
   const int off = cls != nullptr ? 1 : 0;
   float4 v;
   if (r < off) {
@@ -339,9 +336,52 @@ tokens_init_interp_kernel(float4* __restrict__ x, const float4* __restrict__ cls
       }
     }
   }
+  return v;
+}
+
+// One thread per (token r, 4 columns): the value is the same for every sample, so it is computed once and stored B times.
+__global__ void __launch_bounds__(256)
+tokens_init_interp_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int B,
+                          int gh, int gw, int S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S * D4) return;
+  const int r = i / D4, c = i - r * D4;
+  const float4 v = interp_token(cls, pos, g, D4, gh, gw, r, c);
   const size_t SD4 = static_cast<size_t>(S) * D4;
   for (int b = 0; b < B; ++b) x[b * SD4 + i] = v;
 }
+
+// blockIdx.y = image; one thread per (token r of the image, 4 columns)
+__global__ void __launch_bounds__(256)
+tokens_add_interp_packed_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4,
+                                const int* __restrict__ seq_off, const int* __restrict__ gw_of) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int row0 = seq_off[b], S = seq_off[b + 1] - row0;
+  if (i >= S * D4) return;
+  const int r = i / D4, c = i - r * D4;
+  const int gw = gw_of[b], gh = (S - (cls != nullptr ? 1 : 0)) / gw;
+  const float4 v = interp_token(cls, pos, g, D4, gh, gw, r, c);
+  float4* dst = x + static_cast<size_t>(row0) * D4 + i;
+  if (cls != nullptr && r == 0) {
+    *dst = v;
+  } else {  // table + embedding: the per-image path reduce-adds the embedding onto the table, and fp32 addition commutes
+    const float4 e = *dst;
+    *dst = make_float4(v.x + e.x, v.y + e.y, v.z + e.z, v.w + e.w);
+  }
+}
+
+int tokens_add_interp_packed_run(float* x, const float* cls, const float* pos, int g, int D, const int* seq_off, const int* gw, int B, int max_S,
+                                 cudaStream_t stream) {
+  if (B <= 0) return 0;
+  if (D % 4 != 0) { set_last_error("tokens_add_interp_packed: D must be a multiple of 4"); return -1; }
+  if (B > 65535) { set_last_error("tokens_add_interp_packed: %d images exceed the grid", B); return -1; }
+  const int D4 = D / 4, n = max_S * D4;
+  tokens_add_interp_packed_kernel<<<dim3((n + 255) / 256, B), 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls),
+                                                                                reinterpret_cast<const float4*>(pos), g, D4, seq_off, gw);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
 int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream) {
   if (B <= 0) return 0;
   if (D % 4 != 0) { set_last_error("tokens_init_interp: D must be a multiple of 4"); return -1; }

@@ -37,6 +37,13 @@ int tokens_init_run(float* x, const float* cls, const float* pos, int B, int S, 
 // on the fly from 16 table rows each.  x: fp32 [B, gh*gw (+1), D]; at (gh, gw) == (g, g) the same bits as tokens_init_run.
 int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream);
 
+// Packed form of tokens_init_interp_run for B images of different grids, after the patch GEMM: image b is rows seq_off[b] ..
+// seq_off[b + 1] - 1 of x (device int32 [B + 1]), its grid is (n_b / gw[b]) x gw[b] (gw: device int32 [B]).  Its CLS row (cls != null) is
+// set to cls + pos[0]; every patch row, which holds that patch's embedding, gets the resampled table row added -- the bits the
+// per-image path gives by reduce-adding the embedding onto the table.  max_S: the longest image's rows.
+int tokens_add_interp_packed_run(float* x, const float* cls, const float* pos, int g, int D, const int* seq_off, const int* gw, int B, int max_S,
+                                 cudaStream_t stream);
+
 // x[b, 0, :] = cls + pos[0]   (common/vit.py:231-236), fp32 residual stream [B, S, D]
 int cls_row_run(float* x, const float* cls, const float* pos, int B, int S, int D, cudaStream_t stream);
 
@@ -84,8 +91,17 @@ int activation_run(const float* x, float* y, size_t n, int act /* 0 none, 1 gelu
 int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream,
                   int reverse = 0);
 
+// attention_run over B samples of different lengths packed into one [rows, 3D] qkv / [rows, D] out: sample b is rows seq_off[b] ..
+// seq_off[b + 1] - 1 (seq_off: device int32 [B + 1]), max_S >= every length.  Non-causal; each sample's rows are the bits
+// attention_run gives on that sample alone.
+int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H, int head_dim,
+                         cudaStream_t stream, int reverse = 0);
+
 // MAP-head attention with a single (input-independent) probe query (common/vit.py:96-97).
 //   q: fp32 [H*d] (already projected + biased), kv: [B*S, 2D] (k | v) io_type, out [B, D] out_type; d as attention_run
 int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream);
+// map_attention_run on samples packed as in attention_packed_run (kv: [rows, 2D]); out [B, D]
+int map_attention_packed_run(const float* q, const void* kv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H,
+                             int head_dim, cudaStream_t stream);
 
 }  // namespace jimm

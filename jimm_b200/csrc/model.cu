@@ -11,6 +11,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <map>
@@ -142,6 +143,9 @@ struct VisionTower {
   // head after pooling (classifier / visual_projection); N == 0 -> none
   LinearW head;
   GemmPlan p_patch, p_head, p_map_kv, p_map_out, p_map_fc1, p_map_fc2;
+  // packed calls (jimm_vit_forward_packed): plain fp32 acc + bias over patch rows laid out like the tokens they become (a CLS row's
+  // A row is never written and its output is overwritten), straight into the residual stream
+  GemmPlan p_patch_packed;
 };
 
 struct TextTower {
@@ -191,6 +195,7 @@ struct Workspace {
   int32_t* in_ids = nullptr;
   float* out_dev = nullptr;  // host-path staging for results
   size_t out_dev_elems = 0;
+  int* pk_meta = nullptr;    // packed calls: int32 token offsets [Bmax + 1] and grid widths [Bmax] of the images of a chunk
 };
 
 // A vision forward on a patch grid other than the trained one (jimm_vit_forward_hw & co.): gh x gw patches, S tokens per image, the
@@ -607,10 +612,16 @@ static int plan_map_head(jimm_model* m, int Bm, int Tv) {
   return 0;
 }
 
-// x: fp32 [B*S, D] residual stream in ws.x.  TransformerEncoder.__call__ x L (common/transformer.py:116-132,190-196).
-static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, EncBufs ws) {
+// B samples of different lengths packed into T rows: sample b is rows seq_off[b] .. seq_off[b + 1] - 1 (device), max_S the longest
+struct PackedRows {
+  const int* seq_off;
+  int T, max_S;
+};
+
+// x: fp32 [B*S, D] residual stream in ws.x (pk: the packed rows instead).  TransformerEncoder.__call__ x L (common/transformer.py:116-132,190-196).
+static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, EncBufs ws, const PackedRows* pk = nullptr) {
   const EncoderCfg& c = enc->c;
-  const int T = B * S;
+  const int T = pk ? pk->T : B * S;
   // Boustrophedon schedule: every kernel walks its rows / tiles / items in the direction opposite to its producer, so it
   // starts on the data written last -- the part of the 77-310 MB activation still resident in the 50 MB L2.
   int dir = m->l2_alternate ? 1 : 0;  // the patch GEMM / embedding kernels ran forward -> the first LayerNorm runs backward
@@ -621,7 +632,8 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   for (BlockW& b : enc->blocks) {
     if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
     JIMM_TRY(run_gemm(m, b.p_qkv, ln_h, c.D, b.qkv, T, s, flip()));
-    JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
+    if (pk) JIMM_TRY(attention_packed_run(ws.big, m->adt, ws.h, m->cdt, pk->seq_off, B, pk->max_S, c.H, c.D / c.H, s, flip()));
+    else JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_out, ws.h, c.D, b.out, T, s, flip()));  // + residual (+ norm2 -> ws.h when fused)
     if (m->simt || !gemm_fuses_ln(&b.p_out, T))
       JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm2.scale, b.norm2.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
@@ -632,13 +644,15 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   return 0;
 }
 
-// MultiHeadAttentionPoolingHead.__call__ (common/vit.py:87-101) on the tokens in ws.h (compute dtype, [B*S, D]); out fp32 [B, D]
-static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s) {
+// MultiHeadAttentionPoolingHead.__call__ (common/vit.py:87-101) on the tokens in ws.h (compute dtype, [B*S, D], or the packed rows pk);
+// out fp32 [B, D]
+static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
-  const int D = v.D, T = B * S;
+  const int D = v.D, T = pk ? pk->T : B * S, H = v.enc.c.H, d = v.enc.c.D / v.enc.c.H;
   JIMM_TRY(run_gemm(m, v.p_map_kv, ws.h, D, v.map_kv, T, s));                                        // k | v  [T, 2D]
-  JIMM_TRY(map_attention_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, B, S, v.enc.c.H, v.enc.c.D / v.enc.c.H, s));     // [B, D]
+  if (pk) JIMM_TRY(map_attention_packed_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, pk->seq_off, B, pk->max_S, H, d, s));
+  else JIMM_TRY(map_attention_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s));     // [B, D]
   JIMM_TRY(run_gemm(m, v.p_map_out, ws.pooled, D, v.map_out, B, s));                                 // -> feat fp32 [B, D]
   JIMM_TRY(layernorm_run(ws.feat, D, 1, 0, nullptr, v.map_ln.scale, v.map_ln.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
   JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, 4D]
@@ -688,6 +702,42 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H
   const int T = B * S;
   JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.h, m->cdt, D, T, D, s));
   return run_map_head(m, B, S, out, s);
+}
+
+// run_vision on B images of different sizes packed into one token stream: image b (imgs[b], NHWC H[b] x W[b]) is token rows tok[b] ..
+// tok[b + 1] - 1 (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets,
+// image by image, so row b of out is the bits run_vision gives on image b alone.
+static int run_vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, const int* tok, int max_S,
+                             float* out, cudaStream_t s) {
+  VisionTower& v = m->vis;
+  Workspace& ws = m->ws;
+  const int D = v.D, T = tok[B], off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  const float* cls = off ? v.cls : nullptr;
+  // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
+  // on this stream has read its own offsets before this copy lands.
+  std::vector<int> meta(2 * static_cast<size_t>(B) + 1);
+  for (int b = 0; b <= B; ++b) meta[b] = tok[b];
+  for (int b = 0; b < B; ++b) meta[B + 1 + b] = W[b] / v.P;
+  JIMM_CUDA_CHECK(cudaMemcpyAsync(ws.pk_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  const PackedRows pk{ws.pk_meta, T, max_S};
+  const size_t row_bytes = static_cast<size_t>(v.Kp) * cdt_size(m);
+  for (int b = 0; b < B; ++b)
+    JIMM_TRY(patchify_run(imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.big) + (tok[b] + off) * row_bytes, m->cdt, s, 0, v.Kp));
+  JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.big, v.Kp, v.patch, T, s));
+  JIMM_TRY(tokens_add_interp_packed_run(ws.x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, s));
+  if (v.pre_norm) JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, ws.x, DT_F32, D, T, D, s));
+  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}, &pk));
+  if (v.pooling == JIMM_POOL_CLS) {  // ln_post of each image's first row: the offsets are the row index (group 0)
+    if (v.head.N > 0) {
+      JIMM_TRY(layernorm_run(ws.x, D, 0, 0, pk.seq_off, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
+      GemmPlan p = v.p_head;
+      p.epi.out = out;
+      return run_gemm(m, p, ws.pooled, D, v.head, B, s);
+    }
+    return layernorm_run(ws.x, D, 0, 0, pk.seq_off, v.ln_post.scale, v.ln_post.bias, v.eps_outer, out, DT_F32, D, B, D, s);
+  }
+  JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.h, m->cdt, D, T, D, s));
+  return run_map_head(m, B, 0, out, s, &pk);
 }
 
 // CLIP.encode_text (models/clip.py:148-167) / SigLIP.encode_text (models/siglip.py:135-153).  out fp32 [B, Dt]
@@ -1086,6 +1136,7 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.nrm_i = static_cast<float*>(p);
   if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.nrm_t = static_cast<float*>(p);
   if ((rc = m->pool.alloc(&ws.in_img, Bm * v.img * v.img * v.C * sizeof(float)))) return rc;
+  if ((rc = m->pool.alloc(&p, (2 * Bm + 1) * sizeof(int)))) return rc; ws.pk_meta = static_cast<int*>(p);
   if (dual) { if ((rc = m->pool.alloc(&p, Bm * t.T * sizeof(int32_t)))) return rc; ws.in_ids = static_cast<int32_t*>(p); }
   ws.out_dev_elems = dual ? Bm * Bm : Bm * vision_out_dim(m);
   if (ws.out_dev_elems < Bm * E) ws.out_dev_elems = Bm * E;
@@ -1110,6 +1161,10 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
     e.bias = v.patch.b; e.rowadd = v.pos; e.out = ws.x; e.out_type = DT_F32; e.ldo = D;
     e.rows_in = v.n; e.rows_out = v.S; e.row_off = v.pooling == JIMM_POOL_CLS ? 1 : 0; e.mode = 0;
     JIMM_TRY(gemm_plan_init(&v.p_patch, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(Bm) * v.n, D, PPC, e));
+  }
+  {  // as many patch rows as the token budget and ws.big hold (packed_fit keeps a chunk's rows within both)
+    const size_t rows = std::min(Tv, big_bytes / (static_cast<size_t>(PPC) * cs));
+    JIMM_TRY(gemm_plan_init(&v.p_patch_packed, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(rows), D, PPC, epi_plain(v.patch, ACT_NONE, ws.x, DT_F32, D, 2)));
   }
   JIMM_TRY(alloc_ln_counters(m, Tv, &ws.ln_cnt));
   JIMM_TRY(alloc_f8_bufs(m, Tv, D, &ws.h8, &ws.sa));
@@ -1202,6 +1257,16 @@ static size_t grid_chunk(const jimm_model* m, int gh, int gw) {
   return chunk;
 }
 
+// JIMM_EINVAL for an H x W image that alone does not fit the vision workspace
+static int image_too_large(const jimm_model* m, int H, int W) {
+  const VisionTower& v = m->vis;
+  const int gh = H / v.P, gw = W / v.P, off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  set_last_error("a %dx%d image needs %zu tokens (%dx%d patches%s), more than fit this handle's vision workspace (%zu tokens in all); "
+                 "raise the budget with jimm_model_set_max_tokens before jimm_model_finalize", H, W, static_cast<size_t>(gh) * gw + off, gh, gw,
+                 off ? " + CLS" : "", m->ws_rows);
+  return JIMM_EINVAL;
+}
+
 // The off-grid state for H x W images: the patch grid, how many images a chunk runs (grid_chunk) and the patch GEMM plan for that many.
 // The plan is host-side tensor maps only, so the cache is simply dropped when full.
 static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
@@ -1211,12 +1276,7 @@ static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
   if (it != m->grids.end()) { *out = &it->second; return 0; }
   const size_t n = static_cast<size_t>(gh) * gw, S = n + off, n_pad = (n + 31) / 32 * 32;
   const size_t chunk = grid_chunk(m, gh, gw);
-  if (chunk == 0) {
-    set_last_error("a %dx%d image needs %zu tokens (%dx%d patches%s), more than fit this handle's vision workspace (%zu tokens in all); "
-                   "raise the budget with jimm_model_set_max_tokens before jimm_model_finalize", H, W, S, gh, gw, off ? " + CLS" : "",
-                   m->ws_rows);
-    return JIMM_EINVAL;
-  }
+  if (chunk == 0) return image_too_large(m, H, W);
   PatchGrid g;
   g.gh = gh; g.gw = gw; g.n = static_cast<int>(n); g.n_pad = static_cast<int>(n_pad); g.S = static_cast<int>(S); g.chunk = static_cast<int>(chunk);
   GemmEpilogue e;
@@ -1262,6 +1322,47 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
   return 0;
 }
 
+// Does a chunk of T packed tokens fit the vision workspace?  The token-sized buffers hold ws_rows rows, and ws.big holds, one phase at a
+// time, T rows of each of: patch-GEMM operand (laid out by token), qkv, MLP hidden and MAP k | v -- the terms of grid_chunk.  One image
+// fits whenever grid_chunk says so, except where its token-layout patch rows (S rather than the padded n_pad) outgrow every other term
+// of a handle without a set_max_tokens budget.
+static bool packed_fit(const jimm_model* m, size_t T) {
+  const VisionTower& v = m->vis;
+  const size_t cs = cdt_size(m), D = v.D;
+  size_t per_tok = static_cast<size_t>(v.Kp) * cs;
+  per_tok = std::max(per_tok, 3 * D * 2);
+  per_tok = std::max(per_tok, static_cast<size_t>(v.enc.c.M) * cs);
+  if (v.pooling == JIMM_POOL_MAP) per_tok = std::max(per_tok, 2 * D * 2);
+  return T <= m->ws_rows && T * per_tok <= m->ws_big;
+}
+
+// B images of different sizes: chunks of consecutive images, each as many as fit (packed_fit, at most max_batch), run packed.
+static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s) {
+  const VisionTower& v = m->vis;
+  const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
+    if (!imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
+    if (H[b] < v.P || W[b] < v.P) { set_last_error("image %d: %dx%d is smaller than one %dx%d patch", b, H[b], W[b], v.P, v.P); return JIMM_EINVAL; }
+    if (!packed_fit(m, static_cast<size_t>(H[b] / v.P) * (W[b] / v.P) + off)) return image_too_large(m, H[b], W[b]);
+  }
+  const int od = vision_out_dim(m);
+  std::vector<int> tok;
+  for (int b0 = 0; b0 < B;) {
+    tok.assign(1, 0);
+    int b1 = b0, max_S = 0;
+    while (b1 < B && b1 - b0 < m->max_batch) {
+      const int S = (H[b1] / v.P) * (W[b1] / v.P) + off;
+      if (!packed_fit(m, static_cast<size_t>(tok.back()) + S)) break;
+      tok.push_back(tok.back() + S);
+      max_S = std::max(max_S, S);
+      ++b1;
+    }
+    JIMM_TRY(run_vision_packed(m, imgs + b0, in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, out + static_cast<size_t>(b0) * od, s));
+    b0 = b1;
+  }
+  return 0;
+}
+
 static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
   for (int b0 = 0; b0 < B; b0 += m->max_batch) {
     const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
@@ -1299,6 +1400,27 @@ int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, 
   if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   return vision_chunks_hw(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+}
+
+static int check_packed_args(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out) {
+  JIMM_TRY(check_ready(m, B));
+  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
+  if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
+  if (B > 0 && (!imgs || !H || !W || !out)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
+  return 0;
+}
+
+int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
+  JIMM_TRY(check_packed_args(m, imgs, in_dtype, B, H, W, out));
+  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_packed on a dual-tower model; use jimm_encode_image_packed"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
+  JIMM_TRY(check_packed_args(m, imgs, in_dtype, B, H, W, out));
+  JIMM_TRY(set_device(m));
+  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {
@@ -1764,6 +1886,14 @@ int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int 
 }
 int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, void* stream) {
   return map_attention_run(q, kv, io_type, out, out_type, B, S, H, head_dim, static_cast<cudaStream_t>(stream));
+}
+int jimm_k_attention_packed(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H, int head_dim,
+                            int reverse, void* stream) {
+  return attention_packed_run(qkv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream), reverse);
+}
+int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S,
+                                int H, int head_dim, void* stream) {
+  return map_attention_packed_run(q, kv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream));
 }
 int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
   return jimm_k_map_attention_hd(q, kv, io_type, out, out_type, B, S, H, 64, stream);

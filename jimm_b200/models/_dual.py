@@ -37,7 +37,10 @@ class DualTower(_NativeOwner, nn.Module):
     # ---- reference API ----
     def encode_image(self, image, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """interpolate_pos_encoding (HuggingFace's keyword): images of any size of at least one patch, the position embeddings
-        resampled bicubically to the patch grid."""
+        resampled bicubically to the patch grid.  A list / tuple of images of different sizes runs in one packed call; row i is the
+        embedding of image[i] alone."""
+        if isinstance(image, (list, tuple)):
+            return self._vision_list(image, interpolate_pos_encoding, encode=True)
         n = self.native(image.shape[0], hw=self._call_hw(image, interpolate_pos_encoding))
         return n.vision(image, encode=True, interpolate=interpolate_pos_encoding)
 
@@ -48,11 +51,16 @@ class DualTower(_NativeOwner, nn.Module):
         """Similarity logits.  Single process: [B_img, B_txt].  Under torch.distributed (one process per GPU, batch sharded
         over ranks like the reference's P("batch") inputs, examples/clip_inference.py:41-42): this rank's row block
         [B_local, world*B_local], embeddings exchanged over NVLink peer memory inside the fused logits kernel.
-        interpolate_pos_encoding: as in encode_image."""
+        interpolate_pos_encoding: as in encode_image.  `image` may be a list of images of different sizes (single process only)."""
         import torch.distributed as dist
 
         if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and self._comm_mode != "off":
+            if isinstance(image, (list, tuple)):
+                raise ValueError("a list of images is not supported by the multi-GPU contrastive call; pass one [B, H, W, C] tensor per rank")
             return self._call_distributed(image, text, interpolate_pos_encoding)
+        if isinstance(image, (list, tuple)):
+            n = self.native(max(len(image), text.shape[0]), require=True, hw=self._list_hw(image, interpolate_pos_encoding))
+            return n.dual_packed(image, text, interpolate=interpolate_pos_encoding)
         n = self.native(max(image.shape[0], text.shape[0]), require=True, hw=self._call_hw(image, interpolate_pos_encoding))
         return n.dual(image, text, interpolate=interpolate_pos_encoding)
 
