@@ -262,6 +262,18 @@ JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* p
 JIMM_API int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream);
 JIMM_API int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
                   int E, int ldl, void* stream);
+/* Checkpoint ingestion as jimm_model_finalize runs it: host memory of src_type (0 fp32 | 1 fp16 | 2 bf16) is streamed through a
+ * pinned staging ring in chunks of at most 32 MiB, cast on the device to out_type (0 fp32 | 1 fp16 | 2 bf16 round to nearest even |
+ * 3 tf32 round to nearest, ties away) and written to device memory dst.  The ring belongs to the call, which returns once its last
+ * chunk has been written.
+ * jimm_k_upload_rows: rows of K elements, row-major -> dst[r * ldd + k] (ldd >= K); a single row longer than a chunk (rows = 1,
+ *   ldd = K) is split along K.
+ * jimm_k_upload_kernel: a kernel's (K, N) view -> rows n0 .. n0 + N - 1 of the K-major operand dst [*, ldd] (ldd >= K):
+ *   dst[(n0 + n) * ldd + k] = value (k, n).  host holds the (K, N) matrix row-major (flax layout, transposed = 0) or its [N, K]
+ *   transpose (a HuggingFace (out, in) weight, transposed = 1).  Columns K .. ldd - 1 and other rows are not written. */
+JIMM_API int jimm_k_upload_rows(const void* host, int src_type, long long rows, long long K, void* dst, int out_type, long long ldd, void* stream);
+JIMM_API int jimm_k_upload_kernel(const void* host, int src_type, int K, int N, int transposed, void* dst, int out_type, long long ldd, int n0,
+                                  void* stream);
 /* ---- image front-end (SURVEY.md 8f.1): the HuggingFace image processor the reference's examples run on the host ----
  * Replaces `processor(images=..., return_tensors="np")["pixel_values"]` + the NCHW->NHWC transpose of
  * examples/vit_inference.py:27-37, examples/clip_inference.py:35-38 (transformers 4.53.0 slow processors on Pillow 11.3.0,

@@ -109,6 +109,8 @@ SIGNATURES = {
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),
     "jimm_k_logits": (_i, [_fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
+    "jimm_k_upload_rows": (_i, [_vp, _i, C.c_longlong, C.c_longlong, _vp, _i, C.c_longlong, _vp]),
+    "jimm_k_upload_kernel": (_i, [_vp, _i, _i, _i, _i, _vp, _i, C.c_longlong, _i, _vp]),
     "jimm_k_l2_probe": (_i, [_vp, _i, _i, _i, _i, C.POINTER(C.c_float), _vp]),
     "jimm_postprocess": (_i, [_fp, _i, _i, _i, _i, _fp, _i, _ip, _ip, _vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),

@@ -313,7 +313,11 @@ static int attn_launch_dp(const void* qkv, void* out, int B, int S, int H, int d
   auto* kernel = attention_kernel<T, OutT, CAUSAL, DP, PACKED>;
   if constexpr (dyn > 0) {
     static DeviceOnce attr_set;
-    if (attr_set.first()) JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+    if (int rc = attr_set.run([&]() -> int {
+          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+          return 0;
+        }))
+      return rc;
   }
   dim3 grid((S + QT - 1) / QT, H, B);
   JIMM_CUDA_CHECK(launch_k(kernel, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d,

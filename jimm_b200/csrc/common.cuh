@@ -10,6 +10,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <mutex>
+#include <string>
+
 namespace jimm {
 
 // ----------------------------------------------------------------------------
@@ -63,19 +67,33 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// Per-device one-shot flag: function attributes (cudaFuncSetAttribute) and device properties are PER DEVICE, while a process may
+// Per-device once-guard: function attributes (cudaFuncSetAttribute) and device properties are PER DEVICE, while a process may
 // hold models on several GPUs (jimm_model_create takes a device index); a process-wide `static bool` would leave the second GPU's
-// kernels without their > 48 KB dynamic shared memory opt-in.
+// kernels without their > 48 KB dynamic shared memory opt-in.  Distinct handles may be driven from distinct threads, so `run`
+// is a real once: the first caller on a device runs `setup` under the lock, every concurrent caller waits for it, and every
+// later caller gets the first caller's status (and its message) -- a failed check is never skipped by a later launch.
+const char* last_error_message();
 struct DeviceOnce {
   static constexpr int kMaxDevices = 64;
-  bool done[kMaxDevices] = {};
-  bool first() {
+  std::mutex mu;
+  std::atomic<bool> done[kMaxDevices] = {};
+  int rc[kMaxDevices] = {};
+  std::string msg[kMaxDevices];
+  template <typename F>
+  int run(F&& setup) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices) return true;
-    if (done[dev]) return false;
-    done[dev] = true;
-    return true;
+    if (dev < 0 || dev >= kMaxDevices) dev = 0;
+    if (done[dev].load(std::memory_order_acquire) && rc[dev] == 0) return 0;
+    std::lock_guard<std::mutex> lock(mu);
+    if (!done[dev].load(std::memory_order_relaxed)) {
+      rc[dev] = setup();
+      if (rc[dev] != 0) msg[dev] = last_error_message();
+      done[dev].store(true, std::memory_order_release);
+    } else if (rc[dev] != 0) {
+      set_last_error("%s", msg[dev].c_str());
+    }
+    return rc[dev];
   }
 };
 

@@ -608,8 +608,8 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 static PFN_encodeTiled get_encode_fn() {
-  static PFN_encodeTiled fn = nullptr;
-  if (fn) return fn;
+  static std::atomic<PFN_encodeTiled> fn{nullptr};  // handles finalized in several threads may resolve it at once (same pointer)
+  if (PFN_encodeTiled f = fn.load(std::memory_order_acquire)) return f;
   void* p = nullptr;
   cudaDriverEntryPointQueryResult qres;
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres);
@@ -617,8 +617,8 @@ static PFN_encodeTiled get_encode_fn() {
     set_last_error("cudaGetDriverEntryPoint(cuTensorMapEncodeTiled) failed: %s", cudaGetErrorString(e));
     return nullptr;
   }
-  fn = reinterpret_cast<PFN_encodeTiled>(p);
-  return fn;
+  fn.store(reinterpret_cast<PFN_encodeTiled>(p), std::memory_order_release);
+  return reinterpret_cast<PFN_encodeTiled>(p);
 }
 
 static CUtensorMapDataType tensor_map_dtype(int dtype) {
@@ -671,18 +671,19 @@ static int make_tensor_map_3d(CUtensorMap* map, int dtype, const void* ptr, int 
 }
 
 int device_sm_count() {  // of the CURRENT device (cached per device: a process may drive several GPUs)
-  static int sms[DeviceOnce::kMaxDevices] = {};
+  // threads driving distinct handles may fill an entry at once: they compute the same value, and the atomic makes that defined
+  static std::atomic<int> sms[DeviceOnce::kMaxDevices] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= DeviceOnce::kMaxDevices) dev = 0;
-  if (sms[dev] == 0) {
-    int n = 0;
+  int n = sms[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     const char* env = getenv("JIMM_NUM_SMS");
     if (env && atoi(env) > 0) n = atoi(env);
-    sms[dev] = n;
+    sms[dev].store(n, std::memory_order_relaxed);
   }
-  return sms[dev];
+  return n;
 }
 
 static int check_epi(const GemmEpilogue& e, int N) {
@@ -767,16 +768,18 @@ static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
   auto* kernel = gemm_wgmma_kernel<T, OUT, ACT>;
   constexpr int TM = tile_rows(Traits<T>::DTYPE);
   static DeviceOnce attr_set;
-  if (attr_set.first()) {
-    JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    // setmaxnreg moves registers within the launch allocation: with fewer than KERNEL_REGS per thread, an increase would wait forever
-    cudaFuncAttributes fa;
-    JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
-    if (fa.numRegs != KERNEL_REGS) {
-      set_last_error("gemm: kernel compiled with %d registers per thread, the warpgroup register split assumes %d", fa.numRegs, KERNEL_REGS);
-      return -2;
-    }
-  }
+  if (int rc = attr_set.run([&]() -> int {
+        JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        // setmaxnreg moves registers within the launch allocation: with fewer than KERNEL_REGS per thread, an increase would wait forever
+        cudaFuncAttributes fa;
+        JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
+        if (fa.numRegs != KERNEL_REGS) {
+          set_last_error("gemm: kernel compiled with %d registers per thread, the warpgroup register split assumes %d", fa.numRegs, KERNEL_REGS);
+          return -2;
+        }
+        return 0;
+      }))
+    return rc;
   const int tiles = ((M + TM - 1) / TM) * ((p->N + BN - 1) / BN);
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
   JIMM_CUDA_CHECK(launch_k(kernel, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, 1, true, p->map_a, p->map_b, p->map_c,

@@ -83,6 +83,14 @@ struct UploadRing {
   int stage(const void* src, size_t bytes, cudaStream_t s, void** dptr);  // host -> pinned slot -> device slot (async); *dptr = device slot
   int commit(cudaStream_t s);                                              // after the consuming kernel has been enqueued
 };
+// The chunked host -> device loops of finalize, through `ring` on stream s (a chunk is at most one ring slot):
+//   upload_rows: rows of K src_type elements (row-major host memory) -> dst[r * ldd + k] of out_type; a single row longer than a slot
+//     (rows == 1, ldd == K) is split along K.
+//   upload_kernel: a kernel's (K, N) view -- host memory holding it row-major (the flax layout) or, transposed, its [N, K] transpose --
+//     into rows n0 .. n0 + N - 1 of the K-major operand dst [*, ldd] of out_type; columns K .. ldd - 1 are not written.
+int upload_rows(UploadRing& ring, const void* host, int src_type, size_t rows, size_t K, void* dst, int out_type, size_t ldd, cudaStream_t s);
+int upload_kernel(UploadRing& ring, const void* host, int src_type, int K, int N, bool transposed, void* dst, int out_type, size_t ldd, int n0,
+                  cudaStream_t s);
 int activation_run(const float* x, float* y, size_t n, int act /* 0 none, 1 gelu_tanh, 2 quick_gelu */, cudaStream_t stream);
 
 // Multi-head softmax attention over the fused qkv buffer [B*S, 3D] (q | k | v, H heads of head_dim d; D = H d).  SURVEY 8a row a5.

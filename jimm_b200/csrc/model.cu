@@ -39,12 +39,22 @@ void set_last_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
+const char* last_error_message() { return g_err; }
 static std::atomic<long long> g_launches{0};
 static std::atomic<long long> g_graph_replays{0};
-void note_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+// Small-batch forwards are captured in cudaStreamCaptureModeRelaxed, so CUDA does not stop another thread's potentially unsafe calls
+// (cudaMalloc / cudaFree / cudaHostAlloc / cudaFreeHost / device or legacy-stream synchronisation) while a capture is open, and their
+// effect on it is undefined.  Distinct handles may live in distinct threads: the library's own such phases -- finalize, destroy, the
+// growth of a host-path staging buffer -- hold this lock, and a capture only starts when it can take it (otherwise that call runs
+// eagerly and a later one captures).
+static std::mutex g_capture_mu;
+static thread_local long long t_launches = 0;  // launches of the calling thread (what a capture on it recorded)
+void note_launch() {
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  ++t_launches;
+}
 int pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* env = getenv("JIMM_PDL"); v = env ? atoi(env) : 1; }
+  static const int v = [] { const char* env = getenv("JIMM_PDL"); return env ? atoi(env) : 1; }();  // thread-safe static init
   return v;
 }
 
@@ -343,31 +353,7 @@ struct Packer {
 
   // `rows` rows of K stored elements -> dst[r * ldd + k] of out_type, streamed through the ring in row chunks
   int rows_to_device(const HostParam* hp, size_t rows, size_t K, void* dst, int out_type, size_t ldd) {
-    const size_t es = hp->esize(), row_bytes = K * es;
-    if (row_bytes == 0 || rows == 0) return 0;
-    const uint8_t* src = static_cast<const uint8_t*>(hp->ptr());
-    const size_t out_es = dtype_size(out_type);
-    if (row_bytes > UploadRing::kCap) {  // a single very long row (flat vectors): split it into pieces
-      if (rows != 1 || ldd != K) { set_last_error("finalize: row of %zu bytes exceeds the staging slot", row_bytes); return JIMM_EINVAL; }
-      const size_t per = UploadRing::kCap / es;
-      for (size_t k0 = 0; k0 < K; k0 += per) {
-        const size_t kc = K - k0 < per ? K - k0 : per;
-        void* d = nullptr;
-        JIMM_TRY(ring.stage(src + k0 * es, kc * es, stream, &d));
-        JIMM_TRY(pack_rows_run(d, hp->dtype, 1, kc, static_cast<uint8_t*>(dst) + k0 * out_es, out_type, kc, stream));
-        JIMM_TRY(ring.commit(stream));
-      }
-      return 0;
-    }
-    const size_t per = UploadRing::kCap / row_bytes;
-    for (size_t r0 = 0; r0 < rows; r0 += per) {
-      const size_t rc = rows - r0 < per ? rows - r0 : per;
-      void* d = nullptr;
-      JIMM_TRY(ring.stage(src + r0 * row_bytes, rc * row_bytes, stream, &d));
-      JIMM_TRY(pack_rows_run(d, hp->dtype, rc, K, static_cast<uint8_t*>(dst) + r0 * ldd * out_es, out_type, ldd, stream));
-      JIMM_TRY(ring.commit(stream));
-    }
-    return 0;
+    return upload_rows(ring, hp->ptr(), hp->dtype, rows, K, dst, out_type, ldd, stream);
   }
 
   // fp32 vector / tensor uploaded element for element (biases, LayerNorm, cls, pos, embedding table, scalars)
@@ -395,20 +381,7 @@ struct Packer {
     HostParam* hp = find(name, shape);
     if (!hp) return JIMM_ESTATE;
     if (hp->numel() != static_cast<size_t>(K) * N) { set_last_error("finalize: '%s' numel mismatch", name.c_str()); return JIMM_ESTATE; }
-    uint8_t* dst = static_cast<uint8_t*>(dst_base) + static_cast<size_t>(n0) * ldd * dtype_size(wtype());
-    if (hp->transposed) return rows_to_device(hp, N, K, dst, wtype(), ldd);  // already [N, K]: cast-copy
-    const size_t es = hp->esize(), row_bytes = static_cast<size_t>(N) * es;
-    if (row_bytes > UploadRing::kCap) { set_last_error("finalize: '%s' row of %zu bytes exceeds the staging slot", name.c_str(), row_bytes); return JIMM_EINVAL; }
-    const int per = static_cast<int>(UploadRing::kCap / row_bytes);
-    const uint8_t* src = static_cast<const uint8_t*>(hp->ptr());
-    for (int k0 = 0; k0 < K; k0 += per) {
-      const int kc = K - k0 < per ? K - k0 : per;
-      void* d = nullptr;
-      JIMM_TRY(ring.stage(src + static_cast<size_t>(k0) * row_bytes, static_cast<size_t>(kc) * row_bytes, stream, &d));
-      JIMM_TRY(pack_transpose_run(d, hp->dtype, kc, N, dst, wtype(), ldd, k0, stream));
-      JIMM_TRY(ring.commit(stream));
-    }
-    return 0;
+    return upload_kernel(ring, hp->ptr(), hp->dtype, K, N, hp->transposed, dst_base, wtype(), ldd, n0, stream);
   }
   int alloc_linear(LinearW* lw, int N, int K, bool bias) {
     lw->N = N; lw->K = K;
@@ -799,6 +772,9 @@ static int run_graphed(jimm_model* m, std::tuple<int, int, int> key, cudaStream_
     return 0;
   }
   if (e.seen++ == 0) return body(s);
+  // another thread is in finalize / destroy (see g_capture_mu): run eagerly now, capture on a later call
+  std::unique_lock<std::mutex> capture_lock(g_capture_mu, std::try_to_lock);
+  if (!capture_lock.owns_lock()) return body(s);
   // Capture on a private stream: the caller's stream may be the legacy default stream, which cannot be captured; nothing
   // executes during capture, and the instantiated graph is launched on the caller's stream.
   if (!m->capture_stream && cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking) != cudaSuccess) {
@@ -806,7 +782,7 @@ static int run_graphed(jimm_model* m, std::tuple<int, int, int> key, cudaStream_
     m->graph_max_batch = 0;
     return body(s);
   }
-  const long long l0 = g_launches.load();
+  const long long l0 = t_launches;
   if (cudaStreamBeginCapture(m->capture_stream, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
     cudaGetLastError();
     m->graph_max_batch = 0;
@@ -815,7 +791,7 @@ static int run_graphed(jimm_model* m, std::tuple<int, int, int> key, cudaStream_
   const int rc = body(m->capture_stream);
   cudaGraph_t g = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(m->capture_stream, &g);
-  const long long captured = g_launches.load() - l0;
+  const long long captured = t_launches - l0;  // this thread's launches only: other threads' eager launches did run
   g_launches.fetch_sub(captured, std::memory_order_relaxed);  // captured launches have not run
   cudaGraphExec_t exec = nullptr;
   if (rc == 0 && ce == cudaSuccess && g && cudaGraphInstantiate(&exec, g, 0) == cudaSuccess) {
@@ -1034,6 +1010,7 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   if (!m) { set_last_error("null model"); return JIMM_EINVAL; }
   if (m->finalized) { set_last_error("model already finalized"); return JIMM_ESTATE; }
   if (max_batch <= 0) { set_last_error("max_batch must be positive"); return JIMM_EINVAL; }
+  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // allocations, pinned staging and synchronisation follow
   JIMM_TRY(set_device(m));
   const jimm_config_t& c = m->cfg;
   if (c.kind == JIMM_ENCODER || c.kind == JIMM_MAPHEAD) return finalize_sub(m, max_batch);
@@ -1202,6 +1179,7 @@ int jimm_model_set_max_tokens(jimm_model_t* m, int tokens_per_sample) {
 
 int jimm_model_destroy(jimm_model_t* m) {
   if (!m) return 0;
+  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // device synchronisation and frees follow
   cudaSetDevice(m->device);
   cudaDeviceSynchronize();
   comm_destroy(&m->comm);
@@ -1572,8 +1550,7 @@ static void host_slices(const jimm_model* m, int nb, int* sizes, size_t bytes_pe
   // Slicing hides all but the first slice's copy but costs GEMM waves and launches: only worth it when the whole copy is long.  Raw
   // uint8 frames (38 MB for 256 x 224 x 224 x 3) go in one piece.
   if (bytes_per_image && static_cast<size_t>(nb) * bytes_per_image < (static_cast<size_t>(64) << 20)) return;
-  static int head_div = -1;
-  if (head_div < 0) { const char* env = getenv("JIMM_HOST_HEAD_DIV"); head_div = (env && atoi(env) > 0) ? atoi(env) : 4; }
+  static const int head_div = [] { const char* env = getenv("JIMM_HOST_HEAD_DIV"); return (env && atoi(env) > 0) ? atoi(env) : 4; }();
   const int S = m->vis.S, D = m->vis.D, Mm = m->vis.enc.c.M;
   const int sms = device_sm_count();
   auto cost = [&](int n) {
@@ -1606,6 +1583,7 @@ static int vit_forward_host_impl(jimm_model_t* m, const void* img_host, int in_d
   if (pre) {
     const size_t need = static_cast<size_t>(m->max_batch) * src_bytes;
     if (need > m->ws.in_u8_bytes) {  // first call (or larger frames): grow the byte staging buffer
+      std::lock_guard<std::mutex> no_capture(g_capture_mu);
       JIMM_CUDA_CHECK(cudaDeviceSynchronize());
       if (m->ws.in_u8) cudaFree(m->ws.in_u8);
       m->ws.in_u8 = nullptr; m->ws.in_u8_bytes = 0;
@@ -1921,6 +1899,36 @@ int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void*
 int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
                   int E, int ldl, void* stream) {
   return logits_run(img, txt, logit_scale, logit_bias, logits, Bi, Bt, E, ldl, static_cast<cudaStream_t>(stream));
+}
+
+// checkpoint ingestion as finalize runs it, through a staging ring of this call's own (freed, its last chunk done, before returning)
+static int check_upload_types(const char* fn, const void* host, void* dst, int src_type, int out_type) {
+  if (!host || !dst) { set_last_error("%s: null pointer", fn); return JIMM_EINVAL; }
+  if (src_type < DT_F32 || src_type > DT_BF16 || out_type < DT_F32 || out_type > DT_TF32) {
+    set_last_error("%s: bad type codes (src %d, out %d)", fn, src_type, out_type);
+    return JIMM_EINVAL;
+  }
+  return 0;
+}
+int jimm_k_upload_rows(const void* host, int src_type, long long rows, long long K, void* dst, int out_type, long long ldd, void* stream) {
+  JIMM_TRY(check_upload_types("jimm_k_upload_rows", host, dst, src_type, out_type));
+  if (rows < 0 || K < 0 || ldd < K) { set_last_error("jimm_k_upload_rows: bad shape (rows %lld, K %lld, ldd %lld)", rows, K, ldd); return JIMM_EINVAL; }
+  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // pinned staging ring
+  UploadRing ring;
+  const int rc = upload_rows(ring, host, src_type, static_cast<size_t>(rows), static_cast<size_t>(K), dst, out_type, static_cast<size_t>(ldd),
+                             static_cast<cudaStream_t>(stream));
+  ring.destroy();
+  return rc;
+}
+int jimm_k_upload_kernel(const void* host, int src_type, int K, int N, int transposed, void* dst, int out_type, long long ldd, int n0, void* stream) {
+  JIMM_TRY(check_upload_types("jimm_k_upload_kernel", host, dst, src_type, out_type));
+  if (K < 0 || N < 0 || n0 < 0 || ldd < K) { set_last_error("jimm_k_upload_kernel: bad shape (K %d, N %d, ldd %lld, n0 %d)", K, N, ldd, n0); return JIMM_EINVAL; }
+  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // pinned staging ring
+  UploadRing ring;
+  const int rc = upload_kernel(ring, host, src_type, K, N, transposed != 0, dst, out_type, static_cast<size_t>(ldd), n0,
+                               static_cast<cudaStream_t>(stream));
+  ring.destroy();
+  return rc;
 }
 
 }  // extern "C"

@@ -118,4 +118,53 @@ int UploadRing::commit(cudaStream_t s) {
   return 0;
 }
 
+// ---- host -> device packing through the ring (finalize, and the jimm_k_upload_* test entry points) ------------------------------
+int upload_rows(UploadRing& ring, const void* host, int src_type, size_t rows, size_t K, void* dst, int out_type, size_t ldd, cudaStream_t s) {
+  const size_t es = dtype_size(src_type), row_bytes = K * es;
+  if (row_bytes == 0 || rows == 0) return 0;
+  const uint8_t* src = static_cast<const uint8_t*>(host);
+  const size_t out_es = dtype_size(out_type);
+  if (row_bytes > UploadRing::kCap) {  // a single very long row (flat vectors): split it into pieces
+    if (rows != 1 || ldd != K) { set_last_error("upload: row of %zu bytes exceeds the staging slot", row_bytes); return -1; }
+    const size_t per = UploadRing::kCap / es;
+    for (size_t k0 = 0; k0 < K; k0 += per) {
+      const size_t kc = K - k0 < per ? K - k0 : per;
+      void* d = nullptr;
+      JIMM_TRY_RC(ring.stage(src + k0 * es, kc * es, s, &d));
+      JIMM_TRY_RC(pack_rows_run(d, src_type, 1, kc, static_cast<uint8_t*>(dst) + k0 * out_es, out_type, kc, s));
+      JIMM_TRY_RC(ring.commit(s));
+    }
+    return 0;
+  }
+  const size_t per = UploadRing::kCap / row_bytes;
+  for (size_t r0 = 0; r0 < rows; r0 += per) {
+    const size_t rc = rows - r0 < per ? rows - r0 : per;
+    void* d = nullptr;
+    JIMM_TRY_RC(ring.stage(src + r0 * row_bytes, rc * row_bytes, s, &d));
+    JIMM_TRY_RC(pack_rows_run(d, src_type, rc, K, static_cast<uint8_t*>(dst) + r0 * ldd * out_es, out_type, ldd, s));
+    JIMM_TRY_RC(ring.commit(s));
+  }
+  return 0;
+}
+
+int upload_kernel(UploadRing& ring, const void* host, int src_type, int K, int N, bool transposed, void* dst_base, int out_type, size_t ldd,
+                  int n0, cudaStream_t s) {
+  if (K <= 0 || N <= 0) return 0;
+  uint8_t* dst = static_cast<uint8_t*>(dst_base) + static_cast<size_t>(n0) * ldd * dtype_size(out_type);
+  if (transposed) return upload_rows(ring, host, src_type, N, K, dst, out_type, ldd, s);  // already [N, K]: cast-copy
+  const size_t row_bytes = static_cast<size_t>(N) * dtype_size(src_type);
+  if (row_bytes > UploadRing::kCap) { set_last_error("upload: kernel row of %zu bytes exceeds the staging slot", row_bytes); return -1; }
+  // K is split into chunks of whole (K, N) rows; a chunk starts at row k0 of the kernel (not a multiple of the kernel's 32-row tile)
+  const int per = static_cast<int>(UploadRing::kCap / row_bytes);
+  const uint8_t* src = static_cast<const uint8_t*>(host);
+  for (int k0 = 0; k0 < K; k0 += per) {
+    const int kc = K - k0 < per ? K - k0 : per;
+    void* d = nullptr;
+    JIMM_TRY_RC(ring.stage(src + static_cast<size_t>(k0) * row_bytes, static_cast<size_t>(kc) * row_bytes, s, &d));
+    JIMM_TRY_RC(pack_transpose_run(d, src_type, kc, N, dst, out_type, ldd, k0, s));
+    JIMM_TRY_RC(ring.commit(s));
+  }
+  return 0;
+}
+
 }  // namespace jimm

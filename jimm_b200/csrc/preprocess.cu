@@ -366,9 +366,11 @@ int get_plan(jimm_preproc* p, int H, int W, SizePlan** out) {
 template <typename OUT>
 int launch(const KernelArgs& a, const SizePlan& s, int B, cudaStream_t stream) {
   static DeviceOnce attr_set;
-  if (attr_set.first()) {
-    JIMM_CUDA_CHECK(cudaFuncSetAttribute(preprocess_kernel<OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  }
+  if (int rc = attr_set.run([]() -> int {
+        JIMM_CUDA_CHECK(cudaFuncSetAttribute(preprocess_kernel<OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        return 0;
+      }))
+    return rc;
   const dim3 grid((s.oh + s.TY - 1) / s.TY, B);
   JIMM_CUDA_CHECK(launch_k(preprocess_kernel<OUT>, grid, dim3(kThreads), s.smem, stream, 1, false, a));
   note_launch();

@@ -23,6 +23,7 @@ def test_abi_exports_every_declared_symbol(lib):
     declared = set(re.findall(r"\b(jimm_[a-z0-9_]+)\s*\(", header))
     declared -= {"jimm_model", "jimm_config"}
     assert declared, "no declarations parsed"
+    assert {"jimm_k_upload_rows", "jimm_k_upload_kernel"} <= declared  # the ingestion entry points of tests/test_ingestion_gpu.py
     assert declared == set(_lib.SIGNATURES), (declared ^ set(_lib.SIGNATURES))
     for name in declared:
         assert hasattr(lib, name), name
