@@ -98,7 +98,10 @@ JIMM_API int jimm_model_finalize(jimm_model_t* m, int max_batch);
  * another size may need more room than its token count says (its padded patch rows).  Vision models only. */
 JIMM_API int jimm_model_set_max_tokens(jimm_model_t* m, int tokens_per_sample);
 /* Images of H x W that one chunk of a *_hw call runs on this handle: max_batch on the trained patch grid, otherwise as many as the
- * workspace holds, up to max_batch; 0 when one image does not fit (the *_hw call then returns JIMM_EINVAL). */
+ * workspace holds, up to max_batch; 0 when one image does not fit (the *_hw call then returns JIMM_EINVAL; a larger
+ * jimm_model_set_max_tokens budget would fit it).  JIMM_EINVAL itself, with a message naming the tokens and the limit, for an image
+ * of a MAP-pooled tower with more patches than the MAP head's attention pools: it holds one score per token in shared memory, so a
+ * device with 227 KB of opt-in shared memory per block (H100) takes at most 56960 tokens, and no budget lifts that. */
 JIMM_API int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images);
 JIMM_API int jimm_model_destroy(jimm_model_t* m);
 /* Introspection used by the Python mirror. */
@@ -129,7 +132,8 @@ JIMM_API int jimm_dual_forward(jimm_model_t* m, const void* img, int in_dtype, i
  * than the trained g x g, the patch rows of the position table are resampled bicubically to it (torch.nn.functional.interpolate,
  * mode="bicubic", align_corners=False), the CLS row kept, tokens row-major over the grid.  At H == W == img_size each call is its
  * twin above.  Other sizes run eagerly (no CUDA-graph replay) in chunks of min(max_batch, budget / tokens) images, the budget being
- * the workspace's max_batch x tokens-per-sample (jimm_model_set_max_tokens); an image that alone does not fit is JIMM_EINVAL. */
+ * the workspace's max_batch x tokens-per-sample (jimm_model_set_max_tokens); an image that alone does not fit, or that is past the MAP
+ * head's sequence limit (jimm_model_images_per_call), is JIMM_EINVAL before anything is enqueued. */
 JIMM_API int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream);
 JIMM_API int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream);
 JIMM_API int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T,
@@ -140,7 +144,8 @@ JIMM_API int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype
  * H, W: host int arrays, read during the call; out: device fp32 [B, out_dim].  Image i's row equals the *_hw call on that image alone.
  * The tokens of consecutive images are packed into one stream (variable-length attention): the images are walked in order, and a new
  * chunk starts when the next image would pass max_batch images, the token budget or the workspace bytes (counted as for the *_hw
- * calls).  An image that alone does not fit is JIMM_EINVAL with the *_hw message, before anything is enqueued.  Packed calls run
+ * calls).  An image that alone does not fit, or that is past the MAP head's sequence limit, is JIMM_EINVAL with the *_hw message,
+ * before anything is enqueued.  Packed calls run
  * eagerly and return without synchronising; back-to-back calls on one stream are safe. */
 JIMM_API int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
 JIMM_API int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
@@ -150,7 +155,9 @@ JIMM_API int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, 
  *    "blocks.layers.{i}.<...>" resp. "probe", "attn.<...>", "layernorm.<...>", "mlp.layers.{0,2}.<...>") ---------------------------- */
 /* Transformer.__call__ / TransformerEncoder.__call__ (common/transformer.py:116-132,190-196): x, out device fp32 [B,S,D]. */
 JIMM_API int jimm_encoder_forward(jimm_model_t* m, const float* x, int B, int S, float* out, void* stream);
-/* MultiHeadAttentionPoolingHead.__call__ (common/vit.py:87-101): x device fp32 [B,S,D] -> out device fp32 [B,D]. */
+/* MultiHeadAttentionPoolingHead.__call__ (common/vit.py:87-101): x device fp32 [B,S,D] -> out device fp32 [B,D].  A ctx_len past the
+ * MAP head's sequence limit (jimm_model_images_per_call) is JIMM_EINVAL at jimm_model_finalize; so is a MAP-pooled tower whose
+ * trained image size is. */
 JIMM_API int jimm_map_head_forward(jimm_model_t* m, const float* x, int B, int S, float* out, void* stream);
 
 /* -- forward: HOST buffers (the reference-facing call: host->device copy, forward, device->host copy, all enqueued on

@@ -53,8 +53,8 @@ class _SubModuleRunner:
         B, S = int(x.shape[0]), int(x.shape[1])
         sub = self._sub
         if sub is None or S > sub.max_seq:
-            if sub is not None:
-                sub.close()
+            if sub is not None:  # dropped first: a refused rebuild (a sequence past the MAP head's limit) leaves no closed handle behind
+                self._invalidate()
             # workspace for `rows` tokens: batches beyond that are chunked by the library
             mb = max(1, min(default_max_batch(), max(1, 65536 // S)))
             sub = NativeSubModule(self._sub_config(S), self._sub_params(), mb)

@@ -87,7 +87,8 @@ class _NativeOwner:
         the library, the contrastive head needs the whole batch resident (`require=True`).  hw: the (height, width) of the images of
         an interpolate_pos_encoding call; the handle is rebuilt with a larger token budget only when the library reports that one
         such image does not fit (a call whose images merely fit fewer at a time runs in smaller chunks).  A raised budget is kept
-        for later rebuilds."""
+        for later rebuilds.  An image past a limit no budget lifts (the MAP head's sequence limit) raises ValueError from
+        images_per_call: an existing handle is kept as it is, and a handle built for this call is dropped with its budget."""
         n = self._native
         if n is not None and (not require or batch <= n.max_batch) and (hw is None or n.images_per_call(*hw) > 0):
             return n
@@ -97,10 +98,17 @@ class _NativeOwner:
         cfg = self._native_config()
         # any jimm_model_set_max_tokens budget of at least ceil(tokens / max_batch) holds one image of that many tokens
         need = -(-grid_tokens(cfg, *hw) // mb) if hw is not None else 0
+        budget = self._max_tokens
         if need > max(self._max_tokens, grid_tokens(cfg, cfg.img_size, cfg.img_size)):  # more tokens than the workspace rows
             object.__setattr__(self, "_max_tokens", need)
         n = self._build_native(mb)
-        if hw is not None and n.images_per_call(*hw) == 0:  # enough rows, but not the bytes of its padded patch rows
+        try:
+            fits = hw is None or n.images_per_call(*hw) > 0
+        except ValueError:
+            object.__setattr__(self, "_max_tokens", budget)
+            self._invalidate()
+            raise
+        if not fits:  # enough rows, but not the bytes of its padded patch rows
             self._release_native(n)
             object.__setattr__(self, "_max_tokens", max(self._max_tokens, need))
             n = self._build_native(mb)

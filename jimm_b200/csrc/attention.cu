@@ -464,22 +464,51 @@ map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT
   }
 }
 
-template <typename T, typename OutT>
-static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
-  dim3 grid(H, B);
-  const size_t smem = (128 + 1024 + S) * sizeof(float);
+// The scores of a sample sit in shared memory after 128 + 1024 floats of probe and reductions: the longest sequence is what the
+// device's opt-in shared memory per block holds (56960 tokens at the 227 KB of an H100).
+static constexpr int kMapSmemFloats = 128 + 1024;
+int map_attention_max_seq(int device, int* max_S) {
+  int optin = 0;
+  JIMM_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  *max_S = optin / static_cast<int>(sizeof(float)) - kMapSmemFloats;
+  return 0;
+}
+
+template <typename T, typename OutT, bool PACKED>
+static int map_launch_k(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
+  auto* kernel = map_attention_kernel<T, OutT, PACKED>;
+  const size_t smem = (kMapSmemFloats + S) * sizeof(float);
+  if (smem > 48 * 1024) {  // opt in once per device to all the shared memory map_attention_max_seq counts on
+    static DeviceOnce attr_set;
+    if (int rc = attr_set.run([&]() -> int {
+          int dev = 0, max_S = 0;
+          JIMM_CUDA_CHECK(cudaGetDevice(&dev));
+          if (int rc = map_attention_max_seq(dev, &max_S)) return rc;
+          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>((kMapSmemFloats + max_S) * sizeof(float))));
+          return 0;
+        }))
+      return rc;
+  }
   const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(d)));  // 0.125f for d = 64
-  if (seq_off) map_attention_kernel<T, OutT, true><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off);
-  else map_attention_kernel<T, OutT><<<grid, 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, nullptr);
+  kernel<<<dim3(H, B), 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off);
   JIMM_LAUNCH_CHECK();
   return 0;
+}
+
+template <typename T, typename OutT>
+static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
+  if (seq_off) return map_launch_k<T, OutT, true>(q, kv, out, B, S, H, d, stream, seq_off);
+  return map_launch_k<T, OutT, false>(q, kv, out, B, S, H, d, stream, nullptr);
 }
 
 static int map_dispatch(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
                         const int* seq_off) {
   if (!head_dim_ok(head_dim)) { set_last_error("map_attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0) return 0;
-  if (S > 8192) { set_last_error("map_attention: S=%d too large", S); return -1; }
+  int dev = 0, max_S = 0;
+  JIMM_CUDA_CHECK(cudaGetDevice(&dev));
+  if (int rc = map_attention_max_seq(dev, &max_S)) return rc;
+  if (S > max_S) { set_last_error("map_attention: S=%d too large (the scores of a sample live in shared memory: at most %d tokens on device %d)", S, max_S, dev); return -1; }
   if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream, seq_off);
   if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream, seq_off);
   if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream, seq_off);

@@ -111,5 +111,7 @@ int map_attention_run(const float* q, const void* kv, int io_type, void* out, in
 // map_attention_run on samples packed as in attention_packed_run (kv: [rows, 2D]); out [B, D]
 int map_attention_packed_run(const float* q, const void* kv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H,
                              int head_dim, cudaStream_t stream);
+// The longest sequence the MAP-head attention takes on `device` (its scores live in shared memory): into *max_S; 0 or an error code.
+int map_attention_max_seq(int device, int* max_S);
 
 }  // namespace jimm

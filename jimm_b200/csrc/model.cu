@@ -832,12 +832,24 @@ static int exec_text(jimm_model* m, const int32_t* ids, int n, int T, float* out
   return 0;
 }
 
+// JIMM_EINVAL when samples of S tokens are more than the MAP head's attention pools on the handle's device (map_attention_max_seq): it
+// keeps one score per token in shared memory, so no token budget lifts this limit.  `what` names the sample in the message.
+static int map_seq_fits(const jimm_model* m, size_t S, const char* what) {
+  int max_S = 0;
+  JIMM_TRY(map_attention_max_seq(m->device, &max_S));
+  if (S <= static_cast<size_t>(max_S)) return 0;
+  set_last_error("%s: %zu tokens, more than the MAP head's attention pools on device %d (at most %d tokens per sample: one score per "
+                 "token in shared memory)", what, S, m->device, max_S);
+  return JIMM_EINVAL;
+}
+
 // Handle of a bare sub-module (kind JIMM_ENCODER: Transformer, parameters "blocks.layers.{i}.*", common/transformer.py:135-196;
 // kind JIMM_MAPHEAD: MultiHeadAttentionPoolingHead, parameters "probe", "attn.*", "layernorm.*", "mlp.layers.{0,2}.*",
 // common/vit.py:12-101).  cfg: v_width / v_heads / v_mlp / v_layers / v_act / v_eps_block (block LN) / v_eps_outer (MAP LN) / t_causal,
 // ctx_len = max tokens per sample.  The same kernels and orchestration as inside a tower (run_encoder / run_map_head).
 static int finalize_sub(jimm_model* m, int max_batch) {
   const jimm_config_t& c = m->cfg;
+  if (c.kind == JIMM_MAPHEAD) JIMM_TRY(map_seq_fits(m, static_cast<size_t>(c.ctx_len), "MAP head ctx_len"));
   Packer pk{m};
   int rc = 0;
   VisionTower& v = m->vis;
@@ -1014,6 +1026,10 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   JIMM_TRY(set_device(m));
   const jimm_config_t& c = m->cfg;
   if (c.kind == JIMM_ENCODER || c.kind == JIMM_MAPHEAD) return finalize_sub(m, max_batch);
+  if (c.pooling == JIMM_POOL_MAP) {
+    const size_t g = static_cast<size_t>(c.img_size / c.patch);
+    JIMM_TRY(map_seq_fits(m, g * g, "the trained image size"));
+  }
   const bool dual = c.kind == JIMM_CLIP || c.kind == JIMM_SIGLIP;
   const std::string vp = c.kind == JIMM_VIT ? "encoder." : (dual ? "vision_model." : "");
   Packer pk{m};
@@ -1245,6 +1261,15 @@ static int image_too_large(const jimm_model* m, int H, int W) {
   return JIMM_EINVAL;
 }
 
+// JIMM_EINVAL for an H x W image past the MAP head's sequence limit (map_seq_fits); 0 for a CLS tower
+static int image_map_fits(const jimm_model* m, int H, int W) {
+  const VisionTower& v = m->vis;
+  if (v.pooling != JIMM_POOL_MAP) return 0;
+  char what[64];
+  snprintf(what, sizeof what, "a %dx%d image (%dx%d patches)", H, W, H / v.P, W / v.P);
+  return map_seq_fits(m, static_cast<size_t>(H / v.P) * (W / v.P), what);
+}
+
 // The off-grid state for H x W images: the patch grid, how many images a chunk runs (grid_chunk) and the patch GEMM plan for that many.
 // The plan is host-side tensor maps only, so the cache is simply dropped when full.
 static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
@@ -1253,6 +1278,7 @@ static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
   auto it = m->grids.find(std::make_pair(gh, gw));
   if (it != m->grids.end()) { *out = &it->second; return 0; }
   const size_t n = static_cast<size_t>(gh) * gw, S = n + off, n_pad = (n + 31) / 32 * 32;
+  JIMM_TRY(image_map_fits(m, H, W));
   const size_t chunk = grid_chunk(m, gh, gw);
   if (chunk == 0) return image_too_large(m, H, W);
   PatchGrid g;
@@ -1296,6 +1322,7 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
   const VisionTower& v = m->vis;
   if (H < v.P || W < v.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, v.P, v.P); return JIMM_EINVAL; }
   const bool trained = H / v.P == v.img / v.P && W / v.P == v.img / v.P;
+  if (!trained) JIMM_TRY(image_map_fits(m, H, W));
   *images = trained ? m->max_batch : static_cast<int>(grid_chunk(m, H / v.P, W / v.P));
   return 0;
 }
@@ -1321,6 +1348,7 @@ static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, i
   for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
     if (!imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
     if (H[b] < v.P || W[b] < v.P) { set_last_error("image %d: %dx%d is smaller than one %dx%d patch", b, H[b], W[b], v.P, v.P); return JIMM_EINVAL; }
+    JIMM_TRY(image_map_fits(m, H[b], W[b]));
     if (!packed_fit(m, static_cast<size_t>(H[b] / v.P) * (W[b] / v.P) + off)) return image_too_large(m, H[b], W[b]);
   }
   const int od = vision_out_dim(m);
@@ -1454,6 +1482,10 @@ int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, 
   if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
   if (H < m->vis.P || W < m->vis.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, m->vis.P, m->vis.P); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
+  if (H / m->vis.P != m->vis.img / m->vis.P || W / m->vis.P != m->vis.img / m->vis.P) {  // refuse an image that does not fit before the text tower runs
+    PatchGrid* grid = nullptr;
+    JIMM_TRY(get_grid(m, H, W, &grid));
+  }
   cudaStream_t s = static_cast<cudaStream_t>(stream), ts = s;
   JIMM_TRY(fork_text(m, s, &ts));
   JIMM_TRY(text_chunks(m, ids, Bt, T, txt_e, ts));
