@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libjimm_b200.so")
-SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "pack.cu", "comm.cu", "preprocess.cu", "postprocess.cu", "probe.cu", "model.cu"]
+SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "pack.cu", "comm.cu", "preprocess.cu", "postprocess.cu", "probe.cu", "model.cu", "kernel_api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

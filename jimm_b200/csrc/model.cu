@@ -46,8 +46,8 @@ static std::atomic<long long> g_graph_replays{0};
 // (cudaMalloc / cudaFree / cudaHostAlloc / cudaFreeHost / device or legacy-stream synchronisation) while a capture is open, and their
 // effect on it is undefined.  Distinct handles may live in distinct threads: the library's own such phases -- finalize, destroy, the
 // growth of a host-path staging buffer -- hold this lock, and a capture only starts when it can take it (otherwise that call runs
-// eagerly and a later one captures).
-static std::mutex g_capture_mu;
+// eagerly and a later one captures).  The ingestion test entry points (kernel_api.cu) take it too.
+std::mutex g_capture_mu;
 static thread_local long long t_launches = 0;  // launches of the calling thread (what a capture on it recorded)
 void note_launch() {
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -81,6 +81,13 @@ struct DevPool {
     ptrs.push_back(p);
     bytes += n;
     *out = p;
+    return 0;
+  }
+  template <typename T>
+  int alloc(T** out, size_t n) {
+    void* p = nullptr;
+    JIMM_TRY(alloc(&p, n));
+    *out = static_cast<T*>(p);
     return 0;
   }
   void release() {
@@ -170,36 +177,34 @@ struct TextTower {
   GemmPlan p_head;
 };
 
+struct EncBufs {  // the activation buffers one encoder stack works in, for `rows` rows of width D (alloc_stack)
+  float* x = nullptr;     // fp32 residual stream [rows, D]
+  void* h = nullptr;      // LN out / attention out (compute dtype) [rows, D]
+  void* big = nullptr;    // qkv | mlp hidden, and in the vision tower patches | MAP k,v (aliased; disjoint lifetimes; big_bytes)
+  int* ln_cnt = nullptr;  // completion counters of the fused LayerNorm (one per 32 rows, zero between launches; null = LayerNorm stays a kernel)
+  void* h8 = nullptr;     // FP8 mode: e4m3 block LayerNorm out [rows, D] (QKV / FC1 A operand) and its row scales [rows]; null otherwise
+  float* sa = nullptr;
+};
+
 // The text tower has its own residual stream / activation buffers so that the two towers of CLIP / SigLIP can run CONCURRENTLY on two
 // streams (they are independent until the contrastive head): the tail rounds of one tower's persistent GEMMs and its small kernels are
 // filled by the other tower's CTAs instead of leaving SMs idle.
 struct TextWs {
-  float* x = nullptr;     // fp32 residual stream [Bmax*T, Dt]
-  void* h = nullptr;      // LN out / attention out
-  void* big = nullptr;    // qkv | mlp hidden
+  EncBufs enc;            // [Bmax*T, Dt]
   void* pooled = nullptr; // [Bmax, Dt]
   int* idx = nullptr;     // [Bmax] EOT positions
-  int* ln_cnt = nullptr;  // fused-LayerNorm completion counters, one per 32 rows
-  void* h8 = nullptr;     // FP8 mode: e4m3 LayerNorm out [Bmax*T, Dt] ...
-  float* sa = nullptr;    // ... and its row scales [Bmax*T]
 };
 
 struct Workspace {
-  float* x = nullptr;     // fp32 residual stream [Tmax, Dmax]
-  void* h = nullptr;      // LN out / attention out (compute dtype) [Tmax, Dmax]
-  void* big = nullptr;    // patches | qkv | mlp hidden | MAP kv (aliased; disjoint lifetimes)
-  void* pooled = nullptr; // [Bmax, Dmax] compute dtype
-  float* feat = nullptr;  // [Bmax, Dmax] fp32 (MAP attention out-proj / residual)
-  void* mid2 = nullptr;   // [Bmax, 4*Dmax] compute dtype (MAP MLP hidden)
-  int* idx = nullptr;     // [Bmax]
+  EncBufs enc;            // [Tmax, D] (ws_rows x D), ws.big ws_big bytes
+  void* pooled = nullptr; // [Bmax, D] compute dtype
+  float* feat = nullptr;  // [Bmax, D] fp32 (MAP attention out-proj / residual)
+  void* mid2 = nullptr;   // [Bmax, 4*D] compute dtype (MAP MLP hidden)
   float* emb_i = nullptr; // [Bmax, E] fp32 encoder outputs
   float* emb_t = nullptr;
   float* nrm_i = nullptr; // normalised
   float* nrm_t = nullptr;
   void* in_img = nullptr; // host-path staging: image batch (fp32 worst case)
-  int* ln_cnt = nullptr;     // fused-LayerNorm completion counters (one per 32 rows of the residual stream), zero between launches
-  void* h8 = nullptr;        // FP8 mode: e4m3 block LayerNorm out [Tmax, Dmax] (the QKV / FC1 A operand) ...
-  float* sa = nullptr;       // ... and its row scales [Tmax]
   uint8_t* in_u8 = nullptr;  // host-path staging of raw uint8 RGB frames (jimm_vit_forward_host_u8); grown on demand
   size_t in_u8_bytes = 0;
   int32_t* in_ids = nullptr;
@@ -291,29 +296,35 @@ namespace jimm {
 
 static size_t cdt_size(const jimm_model* m) { return dtype_size(m->cdt); }
 
-// zeroed completion counters for the fused LayerNorm of a residual stream of `rows` rows (null when fusion is off)
-static int alloc_ln_counters(jimm_model* m, size_t rows, int** out) {
-  *out = nullptr;
-  // FP8 mode: the block LayerNorms write e4m3 rows with a row scale, which only the LayerNorm kernel computes
-  if (!m->fuse_ln || m->simt || m->epi_mode_res != 2 || m->f8) return 0;
-  const size_t n = (rows + 31) / 32 + 1;
-  void* p = nullptr;
-  if (int rc = m->pool.alloc(&p, n * sizeof(int))) return rc;
-  JIMM_CUDA_CHECK(cudaMemset(p, 0, n * sizeof(int)));
-  *out = static_cast<int*>(p);
+// The buffers of an encoder stack over `rows` rows of width D, with `big` bytes of b->big.
+static int alloc_stack(jimm_model* m, size_t rows, size_t D, size_t big, EncBufs* b) {
+  *b = EncBufs{};
+  JIMM_TRY(m->pool.alloc(&b->x, rows * D * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&b->h, rows * D * cdt_size(m)));
+  JIMM_TRY(m->pool.alloc(&b->big, big));
+  // zeroed completion counters of the fused LayerNorm; not in FP8 mode, where the block LayerNorms write e4m3 rows with a row scale,
+  // which only the LayerNorm kernel computes
+  if (m->fuse_ln && !m->simt && m->epi_mode_res == 2 && !m->f8) {
+    const size_t n = (rows + 31) / 32 + 1;
+    JIMM_TRY(m->pool.alloc(&b->ln_cnt, n * sizeof(int)));
+    JIMM_CUDA_CHECK(cudaMemset(b->ln_cnt, 0, n * sizeof(int)));
+  }
+  if (m->f8) {
+    JIMM_TRY(m->pool.alloc(&b->h8, rows * D));
+    JIMM_TRY(m->pool.alloc(&b->sa, rows * sizeof(float)));
+  }
   return 0;
 }
 
-// FP8 mode: the e4m3 block-LayerNorm output of a residual stream of `rows` x D and its row scales (null otherwise)
-static int alloc_f8_bufs(jimm_model* m, size_t rows, int D, void** h8, float** sa) {
-  *h8 = nullptr;
-  *sa = nullptr;
-  if (!m->f8) return 0;
-  void* p = nullptr;
-  JIMM_TRY(m->pool.alloc(h8, rows * D));
-  JIMM_TRY(m->pool.alloc(&p, rows * sizeof(float)));
-  *sa = static_cast<float*>(p);
-  return 0;
+// Bytes of the vision tower's ws.big for a chunk of T tokens whose patch-GEMM operand has patch_rows rows.  The buffer holds one phase
+// at a time: the patch operand, the 16-bit qkv, the MLP hidden layer or the MAP head's 16-bit k | v.  Finalize sizes ws.big with it and
+// every chunk is admitted by it (grid_chunk, packed_fit), so no chunk outgrows the allocation.
+static size_t big_bytes(const jimm_model* m, size_t T, size_t patch_rows) {
+  const VisionTower& v = m->vis;
+  const size_t cs = cdt_size(m), D = v.D;
+  size_t b = std::max({patch_rows * v.Kp * cs, T * 3 * D * 2, T * v.enc.c.M * cs});
+  if (v.pooling == JIMM_POOL_MAP) b = std::max(b, T * 2 * D * 2);
+  return b;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -529,16 +540,7 @@ static GemmEpilogue epi_residual(const LinearW& w, float* x, int ld, int mode) {
   return e;
 }
 
-struct EncBufs {  // the activation buffers one encoder stack works in
-  float* x;
-  void* h;
-  void* big;
-  int* ln_cnt;  // completion counters of the fused LayerNorm (one per 32 rows; null = LayerNorm stays a kernel)
-  void* h8;     // FP8 mode: e4m3 block LayerNorm out (QKV / FC1 A operand) and its row scales; null otherwise
-  float* sa;
-};
-
-static int plan_encoder(jimm_model* m, Encoder* enc, int Tmax, EncBufs ws) {
+static int plan_encoder(jimm_model* m, Encoder* enc, int Tmax, const EncBufs& ws) {
   const EncoderCfg& c = enc->c;
   const int act = c.act == JIMM_QUICK_GELU ? ACT_QUICK_GELU : ACT_GELU_TANH;
   // x + attn(norm1(x)) is followed by norm2, x + mlp(norm2(x)) by the NEXT block's norm1 (common/transformer.py:130-131): the residual
@@ -576,12 +578,33 @@ static int plan_map_head(jimm_model* m, int Bm, int Tv) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
   const int D = v.D;
-  JIMM_TRY(gemm_plan_init(&v.p_map_kv, m->cdt, ws.h, D, v.map_kv.w, D, Tv, 2 * D, D, epi_plain(v.map_kv, ACT_NONE, ws.big, m->adt, 2 * D, m->epi_mode_16)));
+  JIMM_TRY(gemm_plan_init(&v.p_map_kv, m->cdt, ws.enc.h, D, v.map_kv.w, D, Tv, 2 * D, D, epi_plain(v.map_kv, ACT_NONE, ws.enc.big, m->adt, 2 * D, m->epi_mode_16)));
   JIMM_TRY(gemm_plan_init(&v.p_map_out, m->cdt, ws.pooled, D, v.map_out.w, D, Bm, D, D, epi_plain(v.map_out, ACT_NONE, ws.feat, DT_F32, D, 0)));
   JIMM_TRY(gemm_plan_init(&v.p_map_fc1, m->cdt, ws.pooled, D, v.map_fc1.w, D, Bm, 4 * D, D, epi_plain(v.map_fc1, ACT_GELU_TANH, ws.mid2, m->cdt, 4 * D, 0)));
   GemmEpilogue e = epi_plain(v.map_fc2, ACT_NONE, ws.out_dev, DT_F32, D, 0);
   e.residual = ws.feat; e.ldr = D;
   JIMM_TRY(gemm_plan_init(&v.p_map_fc2, m->cdt, ws.mid2, 4 * D, v.map_fc2.w, 4 * D, Bm, D, 4 * D, e));
+  return 0;
+}
+
+// The patch GEMM of up to `images` images of n patches (n_pad when padded to 32 rows) and S tokens, writing the residual stream ws.x.
+// Token scatter: it reduce-adds each patch row into its token row, onto the position rows already there.  Otherwise it maps patch rows
+// to token rows (leaving the CLS row) and adds `pos` (the trained table) or, when pos is null, the resampled table already in ws.x.
+static int plan_patch(jimm_model* m, int n, int n_pad, int S, int images, const float* pos, GemmPlan* p) {
+  const VisionTower& v = m->vis;
+  float* x = m->ws.enc.x;
+  const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  GemmEpilogue e;
+  e.bias = v.patch.b; e.out = x; e.out_type = DT_F32; e.ldo = v.D;
+  if (v.patch_scatter) {
+    e.residual = x; e.ldr = v.D; e.mode = 2; e.tok_pad = n_pad; e.tok_off = off; e.tok_S = S;
+  } else {
+    if (pos) e.rowadd = pos;
+    else { e.residual = x; e.ldr = v.D; }
+    e.mode = 0; e.rows_in = n; e.rows_out = S; e.row_off = off;
+  }
+  JIMM_TRY(gemm_plan_init(p, m->cdt, m->ws.enc.big, v.Kp, v.patch.w, v.Kp, images * (v.patch_scatter ? n_pad : n), v.D, v.Kp, e));
+  if (v.patch_scatter && p->epi.mode != 2) { set_last_error("patch GEMM: token-scatter epilogue unavailable"); return JIMM_EINVAL; }
   return 0;
 }
 
@@ -592,7 +615,7 @@ struct PackedRows {
 };
 
 // x: fp32 [B*S, D] residual stream in ws.x (pk: the packed rows instead).  TransformerEncoder.__call__ x L (common/transformer.py:116-132,190-196).
-static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, EncBufs ws, const PackedRows* pk = nullptr) {
+static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, const EncBufs& ws, const PackedRows* pk = nullptr) {
   const EncoderCfg& c = enc->c;
   const int T = pk ? pk->T : B * S;
   // Boustrophedon schedule: every kernel walks its rows / tiles / items in the direction opposite to its producer, so it
@@ -623,9 +646,9 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s,
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
   const int D = v.D, T = pk ? pk->T : B * S, H = v.enc.c.H, d = v.enc.c.D / v.enc.c.H;
-  JIMM_TRY(run_gemm(m, v.p_map_kv, ws.h, D, v.map_kv, T, s));                                        // k | v  [T, 2D]
-  if (pk) JIMM_TRY(map_attention_packed_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, pk->seq_off, B, pk->max_S, H, d, s));
-  else JIMM_TRY(map_attention_run(v.map_q, ws.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s));     // [B, D]
+  JIMM_TRY(run_gemm(m, v.p_map_kv, ws.enc.h, D, v.map_kv, T, s));                                    // k | v  [T, 2D]
+  if (pk) JIMM_TRY(map_attention_packed_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, pk->seq_off, B, pk->max_S, H, d, s));
+  else JIMM_TRY(map_attention_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s)); // [B, D]
   JIMM_TRY(run_gemm(m, v.p_map_out, ws.pooled, D, v.map_out, B, s));                                 // -> feat fp32 [B, D]
   JIMM_TRY(layernorm_run(ws.feat, D, 1, 0, nullptr, v.map_ln.scale, v.map_ln.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
   JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, 4D]
@@ -634,47 +657,53 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s,
   return run_gemm(m, p, ws.mid2, 4 * D, v.map_fc2, B, s);
 }
 
+// ln_post + the pooling head of B samples of S tokens (pk: the packed rows instead) in ws.x.  CLS: ln_post is per-row and only row 0 of
+// each sample is consumed (common/vit.py:244-246): every S-th row, or the packed offsets as row index (group 0).  MAP: ln_post of every
+// row, then the MAP head (common/vit.py:87-101).  out: fp32 [B, out_dim]
+static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr) {
+  VisionTower& v = m->vis;
+  Workspace& ws = m->ws;
+  const int D = v.D;
+  if (v.pooling == JIMM_POOL_MAP) {
+    JIMM_TRY(layernorm_run(ws.enc.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.enc.h, m->cdt, D, pk ? pk->T : B * S, D, s));
+    return run_map_head(m, B, S, out, s, pk);
+  }
+  const int group = pk ? 0 : S;
+  const int* row_index = pk ? pk->seq_off : nullptr;
+  if (v.head.N == 0) return layernorm_run(ws.enc.x, D, group, 0, row_index, v.ln_post.scale, v.ln_post.bias, v.eps_outer, out, DT_F32, D, B, D, s);
+  JIMM_TRY(layernorm_run(ws.enc.x, D, group, 0, row_index, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
+  GemmPlan p = v.p_head;
+  p.epi.out = out;
+  return run_gemm(m, p, ws.pooled, D, v.head, B, s);
+}
+
 // VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  img: [B, H, W, C]; grid: null for the trained patch
 // grid, else the grid of H x W (position table resampled).  out: fp32 [B, out_dim]
 static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, const PatchGrid* grid, float* out, cudaStream_t s) {
   VisionTower& v = m->vis;
-  Workspace& ws = m->ws;
+  float* x = m->ws.enc.x;
+  void* big = m->ws.enc.big;
   const int D = v.D, S = grid ? grid->S : v.S, n = v.n;
   const float* cls = v.pooling == JIMM_POOL_CLS ? v.cls : nullptr;
   // patch embed + pos (+cls)
   if (grid) {
     // resampled pos (+cls) first; the patch GEMM adds onto it (token scatter, or a residual-reading epilogue with row remap)
-    JIMM_TRY(tokens_init_interp_run(ws.x, cls, v.pos, v.img / v.P, D, B, grid->gh, grid->gw, s));
+    JIMM_TRY(tokens_init_interp_run(x, cls, v.pos, v.img / v.P, D, B, grid->gh, grid->gw, s));
     const int rows = v.patch_scatter ? grid->n_pad : grid->n;
-    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, v.patch_scatter ? grid->n_pad : 0, v.Kp));
-    JIMM_TRY(run_gemm(m, grid->patch, ws.big, v.patch.K, v.patch, B * rows, s));
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, big, m->cdt, s, v.patch_scatter ? grid->n_pad : 0, v.Kp));
+    JIMM_TRY(run_gemm(m, grid->patch, big, v.patch.K, v.patch, B * rows, s));
   } else if (v.patch_scatter) {
-    JIMM_TRY(tokens_init_run(ws.x, cls, v.pos, B, S, D, s));
-    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, v.n_pad, v.Kp));
-    JIMM_TRY(run_gemm(m, v.p_patch, ws.big, v.patch.K, v.patch, B * v.n_pad, s));
+    JIMM_TRY(tokens_init_run(x, cls, v.pos, B, S, D, s));
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, big, m->cdt, s, v.n_pad, v.Kp));
+    JIMM_TRY(run_gemm(m, v.p_patch, big, v.patch.K, v.patch, B * v.n_pad, s));
   } else {
-    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, ws.big, m->cdt, s, 0, v.Kp));
-    JIMM_TRY(run_gemm(m, v.p_patch, ws.big, v.patch.K, v.patch, B * n, s));
-    if (cls) JIMM_TRY(cls_row_run(ws.x, v.cls, v.pos, B, S, D, s));
+    JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, big, m->cdt, s, 0, v.Kp));
+    JIMM_TRY(run_gemm(m, v.p_patch, big, v.patch.K, v.patch, B * n, s));
+    if (cls) JIMM_TRY(cls_row_run(x, v.cls, v.pos, B, S, D, s));
   }
-  if (v.pre_norm) JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, ws.x, DT_F32, D, B * S, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
-  if (v.pooling == JIMM_POOL_CLS) {
-    // ln_post is per-row, only row 0 of each sample is consumed (common/vit.py:244-246)
-    if (v.head.N > 0) {
-      JIMM_TRY(layernorm_run(ws.x, D, S, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
-      GemmPlan p = v.p_head;
-      p.epi.out = out;
-      JIMM_TRY(run_gemm(m, p, ws.pooled, D, v.head, B, s));
-    } else {
-      JIMM_TRY(layernorm_run(ws.x, D, S, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, out, DT_F32, D, B, D, s));
-    }
-    return 0;
-  }
-  // MAP head (common/vit.py:87-101)
-  const int T = B * S;
-  JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.h, m->cdt, D, T, D, s));
-  return run_map_head(m, B, S, out, s);
+  if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, B * S, D, s));
+  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc));
+  return run_pool(m, B, S, out, s);
 }
 
 // run_vision on B images of different sizes packed into one token stream: image b (imgs[b], NHWC H[b] x W[b]) is token rows tok[b] ..
@@ -684,6 +713,7 @@ static int run_vision_packed(jimm_model* m, const void* const* imgs, int in_dtyp
                              float* out, cudaStream_t s) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
+  float* x = ws.enc.x;
   const int D = v.D, T = tok[B], off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
   const float* cls = off ? v.cls : nullptr;
   // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
@@ -695,35 +725,26 @@ static int run_vision_packed(jimm_model* m, const void* const* imgs, int in_dtyp
   const PackedRows pk{ws.pk_meta, T, max_S};
   const size_t row_bytes = static_cast<size_t>(v.Kp) * cdt_size(m);
   for (int b = 0; b < B; ++b)
-    JIMM_TRY(patchify_run(imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.big) + (tok[b] + off) * row_bytes, m->cdt, s, 0, v.Kp));
-  JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.big, v.Kp, v.patch, T, s));
-  JIMM_TRY(tokens_add_interp_packed_run(ws.x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, s));
-  if (v.pre_norm) JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, ws.x, DT_F32, D, T, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}, &pk));
-  if (v.pooling == JIMM_POOL_CLS) {  // ln_post of each image's first row: the offsets are the row index (group 0)
-    if (v.head.N > 0) {
-      JIMM_TRY(layernorm_run(ws.x, D, 0, 0, pk.seq_off, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
-      GemmPlan p = v.p_head;
-      p.epi.out = out;
-      return run_gemm(m, p, ws.pooled, D, v.head, B, s);
-    }
-    return layernorm_run(ws.x, D, 0, 0, pk.seq_off, v.ln_post.scale, v.ln_post.bias, v.eps_outer, out, DT_F32, D, B, D, s);
-  }
-  JIMM_TRY(layernorm_run(ws.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.h, m->cdt, D, T, D, s));
-  return run_map_head(m, B, 0, out, s, &pk);
+    JIMM_TRY(patchify_run(imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.enc.big) + (tok[b] + off) * row_bytes, m->cdt, s, 0,
+                          v.Kp));
+  JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.enc.big, v.Kp, v.patch, T, s));
+  JIMM_TRY(tokens_add_interp_packed_run(x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, s));
+  if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, T, D, s));
+  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, ws.enc, &pk));
+  return run_pool(m, B, 0, out, s, &pk);
 }
 
 // CLIP.encode_text (models/clip.py:148-167) / SigLIP.encode_text (models/siglip.py:135-153).  out fp32 [B, Dt]
 static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
   TextTower& t = m->txt;
   TextWs& ws = m->wt;
-  JIMM_TRY(embed_run(ids, t.table, t.pos, ws.x, B, T, t.D, t.V, s));
-  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
+  JIMM_TRY(embed_run(ids, t.table, t.pos, ws.enc.x, B, T, t.D, t.V, s));
+  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, ws.enc));
   if (t.pool == JIMM_TPOOL_EOT_ARGMAX) {
     JIMM_TRY(argmax_ids_run(ids, ws.idx, B, T, s));
-    JIMM_TRY(layernorm_run(ws.x, t.D, T, 0, ws.idx, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
+    JIMM_TRY(layernorm_run(ws.enc.x, t.D, T, 0, ws.idx, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
   } else {
-    JIMM_TRY(layernorm_run(ws.x, t.D, T, T - 1, nullptr, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
+    JIMM_TRY(layernorm_run(ws.enc.x, t.D, T, T - 1, nullptr, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
   }
   GemmPlan p = t.p_head;
   p.epi.out = out;
@@ -739,6 +760,40 @@ static int check_ready(const jimm_model* m, int B) {
 }
 static int set_device(const jimm_model* m) {
   JIMM_CUDA_CHECK(cudaSetDevice(m->device));
+  return 0;
+}
+
+// argument checks shared by the entry points
+static int check_image_dtype(int in_dtype) {
+  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
+  return 0;
+}
+// a vision tower and, for a jimm_vit_forward* call (vit_fn names it), a ViT-only model
+static int check_vision(const jimm_model* m, const char* vit_fn) {
+  if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
+  if (vit_fn && m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) {
+    set_last_error("%s on a dual-tower model; use the jimm_encode_image* / jimm_dual_* calls", vit_fn);
+    return JIMM_EINVAL;
+  }
+  return 0;
+}
+static int check_text(const jimm_model* m) {
+  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
+  return 0;
+}
+static int check_text_len(const jimm_model* m, int T) {
+  if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
+  return 0;
+}
+static int check_patch(const jimm_model* m, int H, int W) {
+  if (H < m->vis.P || W < m->vis.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, m->vis.P, m->vis.P); return JIMM_EINVAL; }
+  return 0;
+}
+
+// fn(b0, nb) on consecutive chunks [b0, b0 + nb) of B items, at most `chunk` each
+template <typename F>
+static int for_chunks(int B, int chunk, F&& fn) {
+  for (int b0 = 0; b0 < B; b0 += chunk) JIMM_TRY(fn(b0, std::min(chunk, B - b0)));
   return 0;
 }
 
@@ -843,6 +898,34 @@ static int map_seq_fits(const jimm_model* m, size_t S, const char* what) {
   return JIMM_EINVAL;
 }
 
+// After packing: every parameter that was set must have been used (`what` names the handle in the message).  Drops the host copies.
+static int check_all_used(jimm_model* m, const char* what) {
+  for (auto& kv : m->host) {
+    if (!kv.second.used) {
+      set_last_error("finalize: unexpected parameter '%s' was set but is not part of this %s", kv.first.c_str(), what);
+      return JIMM_ESTATE;
+    }
+  }
+  m->host.clear();
+  return 0;
+}
+
+// The vision workspace, or a bare sub-module's: the encoder stack over Tv rows with `big` bytes of ws.big, the pooled rows and MAP head
+// buffers of Bm samples, and the result staging of out_elems floats.
+static int alloc_workspace(jimm_model* m, size_t Bm, size_t Tv, size_t big, size_t out_elems) {
+  Workspace& ws = m->ws;
+  const size_t D = m->vis.D, cs = cdt_size(m);
+  JIMM_TRY(alloc_stack(m, Tv, D, big, &ws.enc));
+  JIMM_TRY(m->pool.alloc(&ws.pooled, Bm * D * cs));
+  JIMM_TRY(m->pool.alloc(&ws.feat, Bm * D * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.mid2, Bm * 4 * D * cs));
+  ws.out_dev_elems = out_elems;
+  JIMM_TRY(m->pool.alloc(&ws.out_dev, out_elems * sizeof(float)));
+  m->ws_rows = Tv;
+  m->ws_big = big;
+  return 0;
+}
+
 // Handle of a bare sub-module (kind JIMM_ENCODER: Transformer, parameters "blocks.layers.{i}.*", common/transformer.py:135-196;
 // kind JIMM_MAPHEAD: MultiHeadAttentionPoolingHead, parameters "probe", "attn.*", "layernorm.*", "mlp.layers.{0,2}.*",
 // common/vit.py:12-101).  cfg: v_width / v_heads / v_mlp / v_layers / v_act / v_eps_block (block LN) / v_eps_outer (MAP LN) / t_causal,
@@ -850,43 +933,56 @@ static int map_seq_fits(const jimm_model* m, size_t S, const char* what) {
 static int finalize_sub(jimm_model* m, int max_batch) {
   const jimm_config_t& c = m->cfg;
   if (c.kind == JIMM_MAPHEAD) JIMM_TRY(map_seq_fits(m, static_cast<size_t>(c.ctx_len), "MAP head ctx_len"));
-  Packer pk{m};
-  int rc = 0;
   VisionTower& v = m->vis;
   v.present = false;
   v.D = c.v_width; v.S = c.ctx_len; v.n = v.S; v.pooling = JIMM_POOL_MAP; v.eps_outer = c.v_eps_outer;
   v.enc.c.D = c.v_width; v.enc.c.H = c.v_heads; v.enc.c.M = c.v_mlp; v.enc.c.L = c.kind == JIMM_ENCODER ? c.v_layers : 0;
   v.enc.c.act = c.v_act; v.enc.c.causal = c.t_causal; v.enc.c.eps = c.v_eps_block;
-  const int D = v.D;
-  if (c.kind == JIMM_ENCODER) rc = pk.encoder("", &v.enc);
-  else rc = pk.map_head("", D, c.v_heads, &v);
+  Packer pk{m};
+  const int rc = c.kind == JIMM_ENCODER ? pk.encoder("", &v.enc) : pk.map_head("", v.D, c.v_heads, &v);
   pk.done();
-  if (rc) return rc;
-  for (auto& kv : m->host) {
-    if (!kv.second.used) { set_last_error("finalize: unexpected parameter '%s' was set but is not part of this module", kv.first.c_str()); return JIMM_ESTATE; }
-  }
-  m->host.clear();
-  Workspace& ws = m->ws;
-  const size_t cs = cdt_size(m), Bm = max_batch, Tv = Bm * v.S;
-  size_t big = Tv * 3 * D * 2;
-  if (Tv * static_cast<size_t>(c.v_mlp) * cs > big) big = Tv * static_cast<size_t>(c.v_mlp) * cs;
-  void* p = nullptr;
-  JIMM_TRY(m->pool.alloc(&p, Tv * D * sizeof(float))); ws.x = static_cast<float*>(p);
-  JIMM_TRY(m->pool.alloc(&ws.h, Tv * D * cs));
-  JIMM_TRY(m->pool.alloc(&ws.big, big));
-  JIMM_TRY(m->pool.alloc(&ws.pooled, Bm * D * cs));
-  JIMM_TRY(m->pool.alloc(&p, Bm * D * sizeof(float))); ws.feat = static_cast<float*>(p);
-  JIMM_TRY(m->pool.alloc(&ws.mid2, Bm * 4 * D * cs));
-  ws.out_dev_elems = Bm * D;
-  JIMM_TRY(m->pool.alloc(&p, ws.out_dev_elems * sizeof(float))); ws.out_dev = static_cast<float*>(p);
-  JIMM_TRY(alloc_ln_counters(m, Tv, &ws.ln_cnt));
-  JIMM_TRY(alloc_f8_bufs(m, Tv, D, &ws.h8, &ws.sa));
-  if (c.kind == JIMM_ENCODER) JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
+  JIMM_TRY(rc);
+  JIMM_TRY(check_all_used(m, "module"));
+  const size_t Bm = max_batch, Tv = Bm * v.S;
+  JIMM_TRY(alloc_workspace(m, Bm, Tv, big_bytes(m, Tv, 0), Bm * v.D));
+  if (c.kind == JIMM_ENCODER) JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), m->ws.enc));
   else JIMM_TRY(plan_map_head(m, static_cast<int>(Bm), static_cast<int>(Tv)));
   JIMM_CUDA_CHECK(cudaDeviceSynchronize());
   m->graph_max_batch = 0;
   m->max_batch = max_batch;
   m->finalized = true;
+  return 0;
+}
+
+// Uploads and packs every parameter of a ViT / tower / CLIP / SigLIP handle whose towers finalize has configured.  The caller runs
+// pk.done() whatever the result.
+static int pack_model(jimm_model* m, Packer& pk) {
+  const jimm_config_t& c = m->cfg;
+  const bool dual = c.kind == JIMM_CLIP || c.kind == JIMM_SIGLIP;
+  const std::string vp = c.kind == JIMM_VIT ? "encoder." : (dual ? "vision_model." : "");
+  VisionTower& v = m->vis;
+  const int D = v.D, PPC0 = c.patch * c.patch * c.in_ch;
+  JIMM_TRY(pk.alloc_linear(&v.patch, D, v.Kp, c.patch_bias != 0));
+  if (v.Kp != PPC0) JIMM_CUDA_CHECK(cudaMemsetAsync(v.patch.w, 0, static_cast<size_t>(D) * v.Kp * cdt_size(m), pk.stream));
+  JIMM_TRY(pk.pack_kernel(vp + "patch_embeddings.kernel", {c.patch, c.patch, c.in_ch, D}, PPC0, D, v.patch.w, 0, v.Kp));
+  if (c.patch_bias) JIMM_TRY(pk.upload_bias_at(vp + "patch_embeddings.bias", {D}, v.patch.b, D));
+  if (v.pooling == JIMM_POOL_CLS) JIMM_TRY(pk.upload_f32(vp + "cls_token", {1, 1, D}, &v.cls));
+  JIMM_TRY(pk.upload_f32(vp + "position_embeddings", {1, v.S, D}, &v.pos));
+  if (c.pre_norm) JIMM_TRY(pk.upload_ln(vp + "ln_pre", D, &v.ln_pre));
+  JIMM_TRY(pk.upload_ln(vp + "ln_post", D, &v.ln_post));
+  JIMM_TRY(pk.encoder(vp + "transformer.", &v.enc));
+  if (v.pooling == JIMM_POOL_MAP) JIMM_TRY(pk.map_head(vp + "MAPHead.", D, c.v_heads, &v));
+  if (c.kind == JIMM_VIT && c.num_classes > 0) JIMM_TRY(pk.linear("classifier", D, c.num_classes, true, &v.head));
+  else if (c.kind == JIMM_CLIP) JIMM_TRY(pk.linear("visual_projection", D, c.t_width, false, &v.head));
+  if (!dual) return 0;
+  TextTower& t = m->txt;
+  JIMM_TRY(pk.upload_f32("token_embedding.embedding", {t.V, t.D}, &t.table));
+  JIMM_TRY(pk.upload_f32("positional_embedding", {t.T, t.D}, &t.pos));
+  JIMM_TRY(pk.upload_ln("ln_final", t.D, &t.ln_final));
+  JIMM_TRY(pk.encoder("text_model.", &t.enc));
+  JIMM_TRY(pk.linear("text_projection", t.D, t.D, c.t_head_bias != 0, &t.head));
+  JIMM_TRY(pk.upload_f32("logit_scale", {}, &m->logit_scale));
+  if (c.kind == JIMM_SIGLIP) JIMM_TRY(pk.upload_f32("logit_bias", {}, &m->logit_bias));
   return 0;
 }
 
@@ -979,43 +1075,38 @@ int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) 
   return 0;
 }
 
-static int make_host_param(const int64_t* shape, int ndim, HostParam* hp) {
-  size_t n = 1;
+// jimm_model_set_param (fn; an owned copy, ref null) and jimm_model_set_param_ref (a borrowed host pointer, ref = host)
+static int add_param(jimm_model_t* m, const char* fn, const char* flax_path, const void* host, const void* ref, const int64_t* shape, int ndim,
+                     int dtype, bool transposed) {
+  if (!m || !flax_path || !host || (ndim > 0 && !shape)) { set_last_error("jimm_model_%s: null argument", fn); return JIMM_EINVAL; }
+  if (m->finalized) { set_last_error("model already finalized"); return JIMM_ESTATE; }
+  if (dtype < JIMM_F32 || dtype > JIMM_BF16) { set_last_error("%s: unsupported dtype %d", fn, dtype); return JIMM_EINVAL; }
+  HostParam hp;
+  hp.n = 1;
   for (int i = 0; i < ndim; ++i) {
     if (shape[i] < 0) { set_last_error("negative dim"); return JIMM_EINVAL; }
-    hp->shape.push_back(shape[i]);
-    n *= static_cast<size_t>(shape[i]);
+    hp.shape.push_back(shape[i]);
+    hp.n *= static_cast<size_t>(shape[i]);
   }
-  hp->n = n;
+  hp.dtype = dtype;  // kept in the caller's element type: the cast happens on the GPU at finalize
+  hp.ref = ref;
+  hp.transposed = transposed;
+  if (transposed && ndim < 2) { set_last_error("%s: '%s': only kernels (ndim >= 2) can be handed over transposed", fn, flax_path); return JIMM_EINVAL; }
+  if (!ref) {
+    const size_t bytes = hp.n * hp.esize();
+    hp.data.resize((bytes + 3) / 4);
+    memcpy(hp.data.data(), host, bytes);
+  }
+  m->host[flax_path] = std::move(hp);
   return 0;
 }
 
 int jimm_model_set_param(jimm_model_t* m, const char* flax_path, const void* host, const int64_t* shape, int ndim, int dtype) {
-  if (!m || !flax_path || !host || (ndim > 0 && !shape)) { set_last_error("jimm_model_set_param: null argument"); return JIMM_EINVAL; }
-  if (m->finalized) { set_last_error("model already finalized"); return JIMM_ESTATE; }
-  if (dtype < JIMM_F32 || dtype > JIMM_BF16) { set_last_error("set_param: unsupported dtype %d", dtype); return JIMM_EINVAL; }
-  HostParam hp;
-  JIMM_TRY(make_host_param(shape, ndim, &hp));
-  hp.dtype = dtype;  // kept in the caller's element type: the cast happens on the GPU at finalize
-  const size_t bytes = hp.n * hp.esize();
-  hp.data.resize((bytes + 3) / 4);
-  memcpy(hp.data.data(), host, bytes);
-  m->host[flax_path] = std::move(hp);
-  return 0;
+  return add_param(m, "set_param", flax_path, host, nullptr, shape, ndim, dtype, false);
 }
 
 int jimm_model_set_param_ref(jimm_model_t* m, const char* flax_path, const void* host, const int64_t* shape, int ndim, int dtype, int flags) {
-  if (!m || !flax_path || !host || (ndim > 0 && !shape)) { set_last_error("jimm_model_set_param_ref: null argument"); return JIMM_EINVAL; }
-  if (m->finalized) { set_last_error("model already finalized"); return JIMM_ESTATE; }
-  if (dtype < JIMM_F32 || dtype > JIMM_BF16) { set_last_error("set_param_ref: unsupported dtype %d", dtype); return JIMM_EINVAL; }
-  HostParam hp;
-  JIMM_TRY(make_host_param(shape, ndim, &hp));
-  hp.dtype = dtype;
-  hp.ref = host;
-  hp.transposed = (flags & JIMM_PARAM_TRANSPOSED) != 0;
-  if (hp.transposed && ndim < 2) { set_last_error("set_param_ref: '%s': only kernels (ndim >= 2) can be handed over transposed", flax_path); return JIMM_EINVAL; }
-  m->host[flax_path] = std::move(hp);
-  return 0;
+  return add_param(m, "set_param_ref", flax_path, host, host, shape, ndim, dtype, (flags & JIMM_PARAM_TRANSPOSED) != 0);
 }
 
 int jimm_model_finalize(jimm_model_t* m, int max_batch) {
@@ -1031,12 +1122,8 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
     JIMM_TRY(map_seq_fits(m, g * g, "the trained image size"));
   }
   const bool dual = c.kind == JIMM_CLIP || c.kind == JIMM_SIGLIP;
-  const std::string vp = c.kind == JIMM_VIT ? "encoder." : (dual ? "vision_model." : "");
-  Packer pk{m};
-  int rc = 0;
-  auto fail = [&](int code) { pk.done(); return code; };
 
-  // ---- vision tower ----
+  // ---- towers ----
   VisionTower& v = m->vis;
   v.present = true;
   v.img = c.img_size; v.P = c.patch; v.C = c.in_ch; v.D = c.v_width;
@@ -1045,138 +1132,73 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   v.S = v.n + (v.pooling == JIMM_POOL_CLS ? 1 : 0);
   v.n_pad = ((v.n + 31) / 32) * 32;
   v.patch_scatter = !m->simt && m->epi_mode_res == 2;
+  v.Kp = (c.patch * c.patch * c.in_ch + 7) / 8 * 8;  // K of the patch GEMM, zero-padded (patch 14: 588 -> 592)
   v.enc.c.D = c.v_width; v.enc.c.H = c.v_heads; v.enc.c.M = c.v_mlp; v.enc.c.L = c.v_layers;
   v.enc.c.act = c.v_act; v.enc.c.causal = 0; v.enc.c.eps = c.v_eps_block;
-  const int D = v.D, PPC0 = c.patch * c.patch * c.in_ch;
-  const int PPC = (PPC0 + 7) / 8 * 8;  // K of the patch GEMM, zero-padded (patch 14: 588 -> 592)
-  v.Kp = PPC;
-  if ((rc = pk.alloc_linear(&v.patch, D, PPC, c.patch_bias != 0))) return fail(rc);
-  if (PPC != PPC0) JIMM_CUDA_CHECK(cudaMemsetAsync(v.patch.w, 0, static_cast<size_t>(D) * PPC * cdt_size(m), pk.stream));
-  if ((rc = pk.pack_kernel(vp + "patch_embeddings.kernel", {c.patch, c.patch, c.in_ch, D}, PPC0, D, v.patch.w, 0, PPC))) return fail(rc);
-  if (c.patch_bias && (rc = pk.upload_bias_at(vp + "patch_embeddings.bias", {D}, v.patch.b, D))) return fail(rc);
-  if (v.pooling == JIMM_POOL_CLS && (rc = pk.upload_f32(vp + "cls_token", {1, 1, D}, &v.cls))) return fail(rc);
-  if ((rc = pk.upload_f32(vp + "position_embeddings", {1, v.S, D}, &v.pos))) return fail(rc);
-  if (c.pre_norm && (rc = pk.upload_ln(vp + "ln_pre", D, &v.ln_pre))) return fail(rc);
-  if ((rc = pk.upload_ln(vp + "ln_post", D, &v.ln_post))) return fail(rc);
-  if ((rc = pk.encoder(vp + "transformer.", &v.enc))) return fail(rc);
-  if (v.pooling == JIMM_POOL_MAP && (rc = pk.map_head(vp + "MAPHead.", D, c.v_heads, &v))) return fail(rc);
-  if (c.kind == JIMM_VIT && c.num_classes > 0) {
-    if ((rc = pk.linear("classifier", D, c.num_classes, true, &v.head))) return fail(rc);
-  } else if (c.kind == JIMM_CLIP) {
-    if ((rc = pk.linear("visual_projection", D, c.t_width, false, &v.head))) return fail(rc);
-  }
-
-  // ---- text tower ----
   TextTower& t = m->txt;
   if (dual) {
     t.present = true;
     t.T = c.ctx_len; t.V = c.vocab; t.D = c.t_width; t.pool = c.t_pool; t.eps_outer = c.t_eps_outer;
     t.enc.c.D = c.t_width; t.enc.c.H = c.t_heads; t.enc.c.M = c.t_mlp; t.enc.c.L = c.t_layers;
     t.enc.c.act = c.t_act; t.enc.c.causal = c.t_causal; t.enc.c.eps = c.t_eps_block;
-    if (t.D % 8 != 0 || c.t_mlp % 8 != 0) { set_last_error("text dims must be multiples of 8"); return fail(JIMM_EINVAL); }
-    if ((rc = pk.upload_f32("token_embedding.embedding", {t.V, t.D}, &t.table))) return fail(rc);
-    if ((rc = pk.upload_f32("positional_embedding", {t.T, t.D}, &t.pos))) return fail(rc);
-    if ((rc = pk.upload_ln("ln_final", t.D, &t.ln_final))) return fail(rc);
-    if ((rc = pk.encoder("text_model.", &t.enc))) return fail(rc);
-    if ((rc = pk.linear("text_projection", t.D, t.D, c.t_head_bias != 0, &t.head))) return fail(rc);
-    if ((rc = pk.upload_f32("logit_scale", {}, &m->logit_scale))) return fail(rc);
-    if (c.kind == JIMM_SIGLIP && (rc = pk.upload_f32("logit_bias", {}, &m->logit_bias))) return fail(rc);
   }
-  pk.done();
-  for (auto& kv : m->host) {
-    if (!kv.second.used) {
-      set_last_error("finalize: unexpected parameter '%s' was set but is not part of this model", kv.first.c_str());
-      return JIMM_ESTATE;
-    }
-  }
-  m->host.clear();
+  Packer pk{m};
+  const int rc = pack_model(m, pk);
+  pk.done();  // one synchronisation for the whole upload, whatever its result
+  JIMM_TRY(rc);
+  JIMM_TRY(check_all_used(m, "model"));
 
   // ---- workspace ----
   Workspace& ws = m->ws;
-  const size_t cs = cdt_size(m);
-  const size_t Bm = max_batch;
+  const int D = v.D;
+  const size_t cs = cdt_size(m), Bm = max_batch;
   // token budget: max_batch x the native token count, or x jimm_model_set_max_tokens when that is larger
-  const size_t St = m->max_tokens > v.S ? m->max_tokens : v.S;
-  size_t Tv = Bm * St, Dmax = D, x_elems = Tv * D, big_bytes = 0;
-  auto upd = [&](size_t b) { if (b > big_bytes) big_bytes = b; };
-  upd(Bm * v.n_pad * PPC * cs);          // patches (rows per sample padded to a multiple of 32)
-  if (m->max_tokens > 0) upd((Tv + 31) / 32 * 32 * PPC * cs);  // the padded patch rows of one image of up to Tv tokens
-  upd(Tv * 3 * D * 2);                   // qkv (16-bit)
-  upd(Tv * static_cast<size_t>(c.v_mlp) * cs);  // MLP hidden
-  if (v.pooling == JIMM_POOL_MAP) upd(Tv * 2 * D * 2);
+  const size_t Tv = Bm * std::max(m->max_tokens, v.S);
+  // patch rows: max_batch images of the trained grid (rows padded to a multiple of 32 per image) or, under a token budget, the padded
+  // rows of one image of up to Tv tokens
+  size_t patch_rows = Bm * v.n_pad;
+  if (m->max_tokens > 0) patch_rows = std::max(patch_rows, (Tv + 31) / 32 * 32);
+  const size_t E = dual ? t.D : vision_out_dim(m);
+  JIMM_TRY(alloc_workspace(m, Bm, Tv, big_bytes(m, Tv, patch_rows), std::max(dual ? Bm * Bm : Bm * vision_out_dim(m), Bm * E)));
   if (dual) {  // the text tower's own buffers (it runs concurrently with the vision tower)
     const size_t Tt = Bm * t.T;
-    size_t tb = Tt * 3 * t.D * 2;
-    if (Tt * static_cast<size_t>(c.t_mlp) * cs > tb) tb = Tt * static_cast<size_t>(c.t_mlp) * cs;
-    void* q = nullptr;
-    if ((rc = m->pool.alloc(&q, Tt * t.D * sizeof(float)))) return rc; m->wt.x = static_cast<float*>(q);
-    if ((rc = m->pool.alloc(&m->wt.h, Tt * t.D * cs))) return rc;
-    if ((rc = m->pool.alloc(&m->wt.big, tb))) return rc;
-    if ((rc = m->pool.alloc(&m->wt.pooled, Bm * t.D * cs))) return rc;
-    if ((rc = m->pool.alloc(&q, Bm * sizeof(int)))) return rc; m->wt.idx = static_cast<int*>(q);
+    JIMM_TRY(alloc_stack(m, Tt, t.D, std::max(Tt * 3 * t.D * 2, Tt * t.enc.c.M * cs), &m->wt.enc));
+    JIMM_TRY(m->pool.alloc(&m->wt.pooled, Bm * t.D * cs));
+    JIMM_TRY(m->pool.alloc(&m->wt.idx, Bm * sizeof(int)));
+    JIMM_TRY(m->pool.alloc(&ws.in_ids, Bm * t.T * sizeof(int32_t)));
   }
-  const size_t E = dual ? t.D : vision_out_dim(m);
-  void* p = nullptr;
-  if ((rc = m->pool.alloc(&p, x_elems * sizeof(float)))) return rc; ws.x = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&ws.h, x_elems * cs))) return rc;
-  if ((rc = m->pool.alloc(&ws.big, big_bytes))) return rc;
-  if ((rc = m->pool.alloc(&ws.pooled, Bm * Dmax * cs))) return rc;
-  if ((rc = m->pool.alloc(&p, Bm * Dmax * sizeof(float)))) return rc; ws.feat = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&ws.mid2, Bm * 4 * Dmax * cs))) return rc;
-  if ((rc = m->pool.alloc(&p, Bm * sizeof(int)))) return rc; ws.idx = static_cast<int*>(p);
-  if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.emb_i = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.emb_t = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.nrm_i = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&p, Bm * E * sizeof(float)))) return rc; ws.nrm_t = static_cast<float*>(p);
-  if ((rc = m->pool.alloc(&ws.in_img, Bm * v.img * v.img * v.C * sizeof(float)))) return rc;
-  if ((rc = m->pool.alloc(&p, (2 * Bm + 1) * sizeof(int)))) return rc; ws.pk_meta = static_cast<int*>(p);
-  if (dual) { if ((rc = m->pool.alloc(&p, Bm * t.T * sizeof(int32_t)))) return rc; ws.in_ids = static_cast<int32_t*>(p); }
-  ws.out_dev_elems = dual ? Bm * Bm : Bm * vision_out_dim(m);
-  if (ws.out_dev_elems < Bm * E) ws.out_dev_elems = Bm * E;
-  if ((rc = m->pool.alloc(&p, ws.out_dev_elems * sizeof(float)))) return rc; ws.out_dev = static_cast<float*>(p);
+  JIMM_TRY(m->pool.alloc(&ws.emb_i, Bm * E * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.emb_t, Bm * E * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.nrm_i, Bm * E * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.nrm_t, Bm * E * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.in_img, Bm * v.img * v.img * v.C * sizeof(float)));
+  JIMM_TRY(m->pool.alloc(&ws.pk_meta, (2 * Bm + 1) * sizeof(int)));
   if (m->graph_max_batch > 0) {
-    const size_t gw = static_cast<size_t>(vision_out_dim(m)) > E ? vision_out_dim(m) : E;
-    const size_t gb = static_cast<size_t>(m->graph_max_batch) < Bm ? m->graph_max_batch : Bm;
-    if ((rc = m->pool.alloc(&p, gb * gw * sizeof(float)))) return rc;
-    m->graph_out = static_cast<float*>(p);
-    if (dual) { if ((rc = m->pool.alloc(&p, gb * gw * sizeof(float)))) return rc; m->graph_out_t = static_cast<float*>(p); }
+    const size_t gw = std::max(static_cast<size_t>(vision_out_dim(m)), E);
+    const size_t gb = std::min(static_cast<size_t>(m->graph_max_batch), Bm);
+    JIMM_TRY(m->pool.alloc(&m->graph_out, gb * gw * sizeof(float)));
+    if (dual) JIMM_TRY(m->pool.alloc(&m->graph_out_t, gb * gw * sizeof(float)));
   }
 
   // ---- GEMM plans (TMA descriptors bound to the fixed workspace / weight buffers) ----
-  if (v.patch_scatter) {
-    GemmEpilogue e;
-    e.bias = v.patch.b; e.residual = ws.x; e.ldr = D; e.out = ws.x; e.out_type = DT_F32; e.ldo = D; e.mode = 2;
-    e.tok_pad = v.n_pad; e.tok_off = v.pooling == JIMM_POOL_CLS ? 1 : 0; e.tok_S = v.S;
-    JIMM_TRY(gemm_plan_init(&v.p_patch, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(Bm) * v.n_pad, D, PPC, e));
-    if (v.p_patch.epi.mode != 2) { set_last_error("patch GEMM: token-scatter epilogue unavailable"); return JIMM_EINVAL; }
-  } else {
-    GemmEpilogue e;
-    e.bias = v.patch.b; e.rowadd = v.pos; e.out = ws.x; e.out_type = DT_F32; e.ldo = D;
-    e.rows_in = v.n; e.rows_out = v.S; e.row_off = v.pooling == JIMM_POOL_CLS ? 1 : 0; e.mode = 0;
-    JIMM_TRY(gemm_plan_init(&v.p_patch, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(Bm) * v.n, D, PPC, e));
-  }
+  JIMM_TRY(plan_patch(m, v.n, v.n_pad, v.S, max_batch, v.pos, &v.p_patch));
   {  // as many patch rows as the token budget and ws.big hold (packed_fit keeps a chunk's rows within both)
-    const size_t rows = std::min(Tv, big_bytes / (static_cast<size_t>(PPC) * cs));
-    JIMM_TRY(gemm_plan_init(&v.p_patch_packed, m->cdt, ws.big, PPC, v.patch.w, PPC, static_cast<int>(rows), D, PPC, epi_plain(v.patch, ACT_NONE, ws.x, DT_F32, D, 2)));
+    const size_t rows = std::min(Tv, m->ws_big / (static_cast<size_t>(v.Kp) * cs));
+    JIMM_TRY(gemm_plan_init(&v.p_patch_packed, m->cdt, ws.enc.big, v.Kp, v.patch.w, v.Kp, static_cast<int>(rows), D, v.Kp,
+                            epi_plain(v.patch, ACT_NONE, ws.enc.x, DT_F32, D, 2)));
   }
-  JIMM_TRY(alloc_ln_counters(m, Tv, &ws.ln_cnt));
-  JIMM_TRY(alloc_f8_bufs(m, Tv, D, &ws.h8, &ws.sa));
-  JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), EncBufs{ws.x, ws.h, ws.big, ws.ln_cnt, ws.h8, ws.sa}));
+  JIMM_TRY(plan_encoder(m, &v.enc, static_cast<int>(Tv), ws.enc));
   if (v.head.N > 0)
     JIMM_TRY(gemm_plan_init(&v.p_head, m->cdt, ws.pooled, D, v.head.w, D, static_cast<int>(Bm), v.head.N, D,
                             epi_plain(v.head, ACT_NONE, ws.out_dev, DT_F32, v.head.N, 0)));
   if (v.pooling == JIMM_POOL_MAP) JIMM_TRY(plan_map_head(m, static_cast<int>(Bm), static_cast<int>(Tv)));
   if (dual) {
-    JIMM_TRY(alloc_ln_counters(m, Bm * t.T, &m->wt.ln_cnt));
-    JIMM_TRY(alloc_f8_bufs(m, Bm * t.T, t.D, &m->wt.h8, &m->wt.sa));
-    JIMM_TRY(plan_encoder(m, &t.enc, static_cast<int>(Bm) * t.T, EncBufs{m->wt.x, m->wt.h, m->wt.big, m->wt.ln_cnt, m->wt.h8, m->wt.sa}));
+    JIMM_TRY(plan_encoder(m, &t.enc, static_cast<int>(Bm) * t.T, m->wt.enc));
     JIMM_TRY(gemm_plan_init(&t.p_head, m->cdt, m->wt.pooled, t.D, t.head.w, t.D, static_cast<int>(Bm), t.D, t.D,
                             epi_plain(t.head, ACT_NONE, ws.out_dev, DT_F32, t.D, 0)));
   }
   JIMM_CUDA_CHECK(cudaDeviceSynchronize());
   m->max_batch = max_batch;
-  m->ws_rows = Tv;
-  m->ws_big = big_bytes;
   m->finalized = true;
   return 0;
 }
@@ -1224,31 +1246,12 @@ int jimm_model_output_dim(const jimm_model_t* m, int* vision_out, int* text_out)
 int jimm_model_max_batch(const jimm_model_t* m) { return m ? m->max_batch : 0; }
 
 // ---- forward, device buffers ----
-static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, float* out, cudaStream_t s) {
-  const size_t img_elems = static_cast<size_t>(m->vis.img) * m->vis.img * m->vis.C;
-  const size_t in_es = dtype_size(in_dtype);
-  const int od = vision_out_dim(m);
-  for (int b0 = 0; b0 < B; b0 += m->max_batch) {
-    const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
-    JIMM_TRY(exec_vision(m, static_cast<const uint8_t*>(img) + b0 * img_elems * in_es, in_dtype, nb, out + static_cast<size_t>(b0) * od, s));
-  }
-  return 0;
-}
 // How many images of a gh x gw patch grid one chunk of an off-grid call runs: max_batch, or fewer when the token-sized buffers (x, h,
-// ln_cnt, h8 / sa: ws_rows rows; ws.big: patches | qkv | MLP hidden | MAP k,v, counted in bytes) hold fewer.  0: one image does not fit.
+// ln_cnt, h8 / sa: ws_rows rows) or ws.big (big_bytes) hold fewer.  0: one image does not fit.
 static size_t grid_chunk(const jimm_model* m, int gh, int gw) {
   const VisionTower& v = m->vis;
   const size_t n = static_cast<size_t>(gh) * gw, S = n + (v.pooling == JIMM_POOL_CLS ? 1 : 0), n_pad = (n + 31) / 32 * 32;
-  const size_t cs = cdt_size(m), D = v.D, Mlp = v.enc.c.M;
-  size_t per_big = (v.patch_scatter ? n_pad : n) * v.Kp * cs;
-  auto upd = [&](size_t b) { if (b > per_big) per_big = b; };
-  upd(S * 3 * D * 2);
-  upd(S * Mlp * cs);
-  if (v.pooling == JIMM_POOL_MAP) upd(S * 2 * D * 2);
-  size_t chunk = m->max_batch;
-  if (m->ws_rows / S < chunk) chunk = m->ws_rows / S;
-  if (m->ws_big / per_big < chunk) chunk = m->ws_big / per_big;
-  return chunk;
+  return std::min({static_cast<size_t>(m->max_batch), m->ws_rows / S, m->ws_big / big_bytes(m, S, v.patch_scatter ? n_pad : n)});
 }
 
 // JIMM_EINVAL for an H x W image that alone does not fit the vision workspace
@@ -1270,76 +1273,60 @@ static int image_map_fits(const jimm_model* m, int H, int W) {
   return map_seq_fits(m, static_cast<size_t>(H / v.P) * (W / v.P), what);
 }
 
+// H x W images cut into the trained patch grid (they differ from the trained size in the trailing pixels at most)
+static bool trained_grid(const VisionTower& v, int H, int W) { return H / v.P == v.img / v.P && W / v.P == v.img / v.P; }
+
 // The off-grid state for H x W images: the patch grid, how many images a chunk runs (grid_chunk) and the patch GEMM plan for that many.
 // The plan is host-side tensor maps only, so the cache is simply dropped when full.
 static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
   const VisionTower& v = m->vis;
-  const int gh = H / v.P, gw = W / v.P, off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  const int gh = H / v.P, gw = W / v.P;
   auto it = m->grids.find(std::make_pair(gh, gw));
   if (it != m->grids.end()) { *out = &it->second; return 0; }
-  const size_t n = static_cast<size_t>(gh) * gw, S = n + off, n_pad = (n + 31) / 32 * 32;
   JIMM_TRY(image_map_fits(m, H, W));
   const size_t chunk = grid_chunk(m, gh, gw);
   if (chunk == 0) return image_too_large(m, H, W);
   PatchGrid g;
-  g.gh = gh; g.gw = gw; g.n = static_cast<int>(n); g.n_pad = static_cast<int>(n_pad); g.S = static_cast<int>(S); g.chunk = static_cast<int>(chunk);
-  GemmEpilogue e;
-  e.bias = v.patch.b; e.residual = m->ws.x; e.ldr = v.D; e.out = m->ws.x; e.out_type = DT_F32; e.ldo = v.D;
-  int rows = g.n;
-  if (v.patch_scatter) {
-    e.mode = 2; e.tok_pad = g.n_pad; e.tok_off = off; e.tok_S = g.S;
-    rows = g.n_pad;
-  } else {
-    e.mode = 0; e.rows_in = g.n; e.rows_out = g.S; e.row_off = off;  // adds onto the resampled table already in x
-  }
-  JIMM_TRY(gemm_plan_init(&g.patch, m->cdt, m->ws.big, v.Kp, v.patch.w, v.Kp, g.chunk * rows, v.D, v.Kp, e));
-  if (v.patch_scatter && g.patch.epi.mode != 2) { set_last_error("patch GEMM: token-scatter epilogue unavailable"); return JIMM_EINVAL; }
+  g.gh = gh; g.gw = gw; g.n = gh * gw; g.n_pad = (g.n + 31) / 32 * 32; g.S = g.n + (v.pooling == JIMM_POOL_CLS ? 1 : 0);
+  g.chunk = static_cast<int>(chunk);
+  JIMM_TRY(plan_patch(m, g.n, g.n_pad, g.S, g.chunk, nullptr, &g.patch));  // adds onto the resampled table already in x
   if (m->grids.size() >= jimm_model::kMaxGrids) m->grids.clear();
   *out = &(m->grids[std::make_pair(gh, gw)] = g);
   return 0;
 }
 
-// Vision forward of B images of H x W.  The native size goes through vision_chunks (graphs, staging); other sizes run eagerly.
-static int vision_chunks_hw(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s) {
+// Vision forward of B images of H x W.  The native size goes through exec_vision (graphs, staging); other sizes run eagerly.
+static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s) {
   const VisionTower& v = m->vis;
-  if (H < v.P || W < v.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, v.P, v.P); return JIMM_EINVAL; }
-  if (H == v.img && W == v.img) return vision_chunks(m, img, in_dtype, B, out, s);
-  PatchGrid* grid = nullptr;  // null: the trained grid (the trailing pixels differ only)
-  if (H / v.P != v.img / v.P || W / v.P != v.img / v.P) JIMM_TRY(get_grid(m, H, W, &grid));
-  const int chunk = grid ? grid->chunk : m->max_batch;
+  JIMM_TRY(check_patch(m, H, W));
+  const bool native = H == v.img && W == v.img;
+  PatchGrid* grid = nullptr;  // null: the trained grid
+  if (!trained_grid(v, H, W)) JIMM_TRY(get_grid(m, H, W, &grid));
   const size_t img_bytes = static_cast<size_t>(H) * W * v.C * dtype_size(in_dtype);
   const int od = vision_out_dim(m);
-  for (int b0 = 0; b0 < B; b0 += chunk) {
-    const int nb = B - b0 < chunk ? B - b0 : chunk;
-    JIMM_TRY(run_vision(m, static_cast<const uint8_t*>(img) + b0 * img_bytes, in_dtype, nb, H, W, grid, out + static_cast<size_t>(b0) * od, s));
-  }
-  return 0;
+  return for_chunks(B, grid ? grid->chunk : m->max_batch, [&](int b0, int nb) {
+    const void* src = static_cast<const uint8_t*>(img) + b0 * img_bytes;
+    float* dst = out + static_cast<size_t>(b0) * od;
+    return native ? exec_vision(m, src, in_dtype, nb, dst, s) : run_vision(m, src, in_dtype, nb, H, W, grid, dst, s);
+  });
 }
 
 int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images) {
   JIMM_TRY(check_ready(m, 0));
-  if (!m->vis.present || !images) { set_last_error("jimm_model_images_per_call: %s", images ? "model has no vision tower" : "null argument"); return JIMM_EINVAL; }
+  if (!images) { set_last_error("jimm_model_images_per_call: null argument"); return JIMM_EINVAL; }
+  JIMM_TRY(check_vision(m, nullptr));
+  JIMM_TRY(check_patch(m, H, W));
   const VisionTower& v = m->vis;
-  if (H < v.P || W < v.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, v.P, v.P); return JIMM_EINVAL; }
-  const bool trained = H / v.P == v.img / v.P && W / v.P == v.img / v.P;
+  const bool trained = trained_grid(v, H, W);
   if (!trained) JIMM_TRY(image_map_fits(m, H, W));
   *images = trained ? m->max_batch : static_cast<int>(grid_chunk(m, H / v.P, W / v.P));
   return 0;
 }
 
-// Does a chunk of T packed tokens fit the vision workspace?  The token-sized buffers hold ws_rows rows, and ws.big holds, one phase at a
-// time, T rows of each of: patch-GEMM operand (laid out by token), qkv, MLP hidden and MAP k | v -- the terms of grid_chunk.  One image
-// fits whenever grid_chunk says so, except where its token-layout patch rows (S rather than the padded n_pad) outgrow every other term
-// of a handle without a set_max_tokens budget.
-static bool packed_fit(const jimm_model* m, size_t T) {
-  const VisionTower& v = m->vis;
-  const size_t cs = cdt_size(m), D = v.D;
-  size_t per_tok = static_cast<size_t>(v.Kp) * cs;
-  per_tok = std::max(per_tok, 3 * D * 2);
-  per_tok = std::max(per_tok, static_cast<size_t>(v.enc.c.M) * cs);
-  if (v.pooling == JIMM_POOL_MAP) per_tok = std::max(per_tok, 2 * D * 2);
-  return T <= m->ws_rows && T * per_tok <= m->ws_big;
-}
+// Does a chunk of T packed tokens fit the vision workspace?  The token-sized buffers hold ws_rows rows, and ws.big the chunk's phases
+// (big_bytes), with the patch-GEMM operand laid out by token: T rows.  One image fits whenever grid_chunk says so, except where its
+// token-layout patch rows (S rather than the padded n_pad) outgrow every other term of a handle without a set_max_tokens budget.
+static bool packed_fit(const jimm_model* m, size_t T) { return T <= m->ws_rows && big_bytes(m, T, T) <= m->ws_big; }
 
 // B images of different sizes: chunks of consecutive images, each as many as fit (packed_fit, at most max_batch), run packed.
 static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s) {
@@ -1370,76 +1357,68 @@ static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, i
 }
 
 static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
-  for (int b0 = 0; b0 < B; b0 += m->max_batch) {
-    const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
-    JIMM_TRY(exec_text(m, ids + static_cast<size_t>(b0) * T, nb, T, out + static_cast<size_t>(b0) * m->txt.D, s));
-  }
-  return 0;
+  return for_chunks(B, m->max_batch, [&](int b0, int nb) {
+    return exec_text(m, ids + static_cast<size_t>(b0) * T, nb, T, out + static_cast<size_t>(b0) * m->txt.D, s);
+  });
+}
+
+// The jimm_vit_forward* (vit_fn: its name) and jimm_encode_image* calls on device images
+static int encode_images(jimm_model* m, const char* vit_fn, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_vision(m, vit_fn));
+  JIMM_TRY(set_device(m));
+  return vision_chunks(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_vit_forward(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
   JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward on a dual-tower model; use jimm_encode_image"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return vision_chunks(m, img, in_dtype, B, out, static_cast<cudaStream_t>(stream));
+  return encode_images(m, "jimm_vit_forward", img, in_dtype, B, m->vis.img, m->vis.img, out, stream);
 }
 
 int jimm_encode_image(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
   JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return vision_chunks(m, img, in_dtype, B, out, static_cast<cudaStream_t>(stream));
+  return encode_images(m, nullptr, img, in_dtype, B, m->vis.img, m->vis.img, out, stream);
 }
 
 int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_hw on a dual-tower model; use jimm_encode_image_hw"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return vision_chunks_hw(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+  return encode_images(m, "jimm_vit_forward_hw", img, in_dtype, B, H, W, out, stream);
 }
 
 int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return vision_chunks_hw(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+  return encode_images(m, nullptr, img, in_dtype, B, H, W, out, stream);
 }
 
-static int check_packed_args(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out) {
+// The jimm_vit_forward_packed (vit_fn: its name) and jimm_encode_image_packed calls
+static int encode_packed(jimm_model* m, const char* vit_fn, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out,
+                         void* stream) {
   JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (!m->vis.present) { set_last_error("model has no vision tower"); return JIMM_EINVAL; }
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_vision(m, vit_fn));
   if (B > 0 && (!imgs || !H || !W || !out)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
-  return 0;
+  JIMM_TRY(set_device(m));
+  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
-  JIMM_TRY(check_packed_args(m, imgs, in_dtype, B, H, W, out));
-  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_packed on a dual-tower model; use jimm_encode_image_packed"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+  return encode_packed(m, "jimm_vit_forward_packed", imgs, in_dtype, B, H, W, out, stream);
 }
 
 int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
-  JIMM_TRY(check_packed_args(m, imgs, in_dtype, B, H, W, out));
-  JIMM_TRY(set_device(m));
-  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+  return encode_packed(m, nullptr, imgs, in_dtype, B, H, W, out, stream);
 }
 
 int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {
   JIMM_TRY(check_ready(m, B));
-  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
-  if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
+  JIMM_TRY(check_text(m));
+  JIMM_TRY(check_text_len(m, T));
   JIMM_TRY(set_device(m));
   return text_chunks(m, ids, B, T, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const float* txt_e, int Bt, float* logits, void* stream) {
   JIMM_TRY(check_ready(m, Bi));
-  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
+  JIMM_TRY(check_text(m));
   if (Bi > m->max_batch || Bt > m->max_batch) { set_last_error("contrastive_logits: batch (%d,%d) exceeds max_batch %d", Bi, Bt, m->max_batch); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1477,19 +1456,19 @@ static int join_text(jimm_model* m, cudaStream_t s, cudaStream_t ts) {
 int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, int H, int W, const int32_t* ids, int Bt, int T, float* img_e,
                         float* txt_e, void* stream) {
   JIMM_TRY(check_ready(m, Bi));
-  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
-  if (H < m->vis.P || W < m->vis.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, m->vis.P, m->vis.P); return JIMM_EINVAL; }
+  JIMM_TRY(check_text(m));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_text_len(m, T));
+  JIMM_TRY(check_patch(m, H, W));
   JIMM_TRY(set_device(m));
-  if (H / m->vis.P != m->vis.img / m->vis.P || W / m->vis.P != m->vis.img / m->vis.P) {  // refuse an image that does not fit before the text tower runs
+  if (!trained_grid(m->vis, H, W)) {  // refuse an image that does not fit before the text tower runs
     PatchGrid* grid = nullptr;
     JIMM_TRY(get_grid(m, H, W, &grid));
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream), ts = s;
   JIMM_TRY(fork_text(m, s, &ts));
   JIMM_TRY(text_chunks(m, ids, Bt, T, txt_e, ts));
-  JIMM_TRY(vision_chunks_hw(m, img, in_dtype, Bi, H, W, img_e, s));
+  JIMM_TRY(vision_chunks(m, img, in_dtype, Bi, H, W, img_e, s));
   return join_text(m, s, ts);
 }
 
@@ -1526,25 +1505,22 @@ int jimm_encoder_forward(jimm_model_t* m, const float* x, int B, int S, float* o
   JIMM_TRY(check_sub(m, JIMM_ENCODER, B, S, x, out));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t row = static_cast<size_t>(S) * m->vis.D;
-  for (int b0 = 0; b0 < B; b0 += m->max_batch) {
-    const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
-    JIMM_CUDA_CHECK(cudaMemcpyAsync(m->ws.x, x + b0 * row, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    JIMM_TRY(run_encoder(m, &m->vis.enc, nb, S, s, EncBufs{m->ws.x, m->ws.h, m->ws.big, m->ws.ln_cnt, m->ws.h8, m->ws.sa}));
-    JIMM_CUDA_CHECK(cudaMemcpyAsync(out + b0 * row, m->ws.x, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  }
-  return 0;
+  return for_chunks(B, m->max_batch, [&](int b0, int nb) {
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(m->ws.enc.x, x + b0 * row, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    JIMM_TRY(run_encoder(m, &m->vis.enc, nb, S, s, m->ws.enc));
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(out + b0 * row, m->ws.enc.x, nb * row * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return 0;
+  });
 }
 
 int jimm_map_head_forward(jimm_model_t* m, const float* x, int B, int S, float* out, void* stream) {
   JIMM_TRY(check_sub(m, JIMM_MAPHEAD, B, S, x, out));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t row = static_cast<size_t>(S) * m->vis.D;
-  for (int b0 = 0; b0 < B; b0 += m->max_batch) {
-    const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
-    JIMM_TRY(cast_run(x + b0 * row, m->ws.h, m->cdt, nb * row, s));  // the head's inputs are GEMM operands: compute dtype
-    JIMM_TRY(run_map_head(m, nb, S, out + static_cast<size_t>(b0) * m->vis.D, s));
-  }
-  return 0;
+  return for_chunks(B, m->max_batch, [&](int b0, int nb) {
+    JIMM_TRY(cast_run(x + b0 * row, m->ws.enc.h, m->cdt, nb * row, s));  // the head's inputs are GEMM operands: compute dtype
+    return run_map_head(m, nb, S, out + static_cast<size_t>(b0) * m->vis.D, s);
+  });
 }
 
 // ---- forward, host buffers ----
@@ -1627,8 +1603,7 @@ static int vit_forward_host_impl(jimm_model_t* m, const void* img_host, int in_d
   // Sliced pipeline per super-chunk of <= max_batch images: slice i+1 is copied on the side stream while slice i is in the
   // tower, and the next super-chunk's first copy overlaps this one's last forward.  The slices partition the staging buffer
   // (max_batch images), one event pair each; one D2H of the super-chunk's result at its end.
-  for (int b0 = 0; b0 < B; b0 += m->max_batch) {
-    const int nb = B - b0 < m->max_batch ? B - b0 : m->max_batch;
+  return for_chunks(B, m->max_batch, [&](int b0, int nb) {
     int sizes[jimm_model::kHostSlices];
     host_slices(m, nb, sizes, src_bytes);
     bool same_layout = m->host_chain && m->host_chain_stream == s && m->host_chain_kind == kind;
@@ -1672,14 +1647,14 @@ static int vit_forward_host_impl(jimm_model_t* m, const void* img_host, int in_d
     }
     JIMM_CUDA_CHECK(cudaMemcpyAsync(out_host + static_cast<size_t>(b0) * od, m->ws.out_dev, static_cast<size_t>(nb) * od * sizeof(float),
                                     cudaMemcpyDeviceToHost, s));
-  }
-  return 0;
+    return 0;
+  });
 }
 
 int jimm_vit_forward_host(jimm_model_t* m, const void* img_host, int in_dtype, int B, float* out_host, void* stream) {
   JIMM_TRY(check_ready(m, B));
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_host on a dual-tower model"); return JIMM_EINVAL; }
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_vision(m, "jimm_vit_forward_host"));
   JIMM_TRY(set_device(m));
   return vit_forward_host_impl(m, img_host, in_dtype, B, out_host, static_cast<cudaStream_t>(stream), nullptr, 0, 0);
 }
@@ -1687,7 +1662,7 @@ int jimm_vit_forward_host(jimm_model_t* m, const void* img_host, int in_dtype, i
 int jimm_vit_forward_host_u8(jimm_model_t* m, jimm_preproc_t* pre, const uint8_t* img_host, int B, int H, int W, float* out_host, void* stream) {
   JIMM_TRY(check_ready(m, B));
   if (!pre || !img_host || !out_host) { set_last_error("jimm_vit_forward_host_u8: null argument"); return JIMM_EINVAL; }
-  if (m->cfg.kind != JIMM_VIT && m->cfg.kind != JIMM_TOWER) { set_last_error("jimm_vit_forward_host_u8 on a dual-tower model"); return JIMM_EINVAL; }
+  JIMM_TRY(check_vision(m, "jimm_vit_forward_host_u8"));
   if (m->vis.C != 3) { set_last_error("the image front-end produces 3-channel images; the model takes %d", m->vis.C); return JIMM_EINVAL; }
   int oh = 0, ow = 0;
   if (int rc = jimm_preproc_output_size(pre, H, W, &oh, &ow)) return rc;
@@ -1702,10 +1677,10 @@ int jimm_vit_forward_host_u8(jimm_model_t* m, jimm_preproc_t* pre, const uint8_t
 int jimm_dual_forward_host(jimm_model_t* m, const void* img_host, int in_dtype, int Bi, const int32_t* ids_host, int Bt, int T,
                            float* logits_host, void* stream) {
   JIMM_TRY(check_ready(m, Bi));
-  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
+  JIMM_TRY(check_text(m));
   if (Bi > m->max_batch || Bt > m->max_batch) { set_last_error("dual_forward_host: batch (%d,%d) exceeds max_batch %d", Bi, Bt, m->max_batch); return JIMM_EINVAL; }
-  if (in_dtype < JIMM_F32 || in_dtype > JIMM_BF16) { set_last_error("bad image dtype %d", in_dtype); return JIMM_EINVAL; }
-  if (T <= 0 || T > m->txt.T) { set_last_error("sequence length %d outside (0, context_length=%d]", T, m->txt.T); return JIMM_EINVAL; }
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_text_len(m, T));
   JIMM_TRY(set_device(m));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   JIMM_TRY(ensure_copy_stream(m));
@@ -1755,7 +1730,7 @@ int jimm_dual_forward_host(jimm_model_t* m, const void* img_host, int in_dtype, 
 // ---- multi-GPU contrastive head ----
 int jimm_comm_init(jimm_model_t* m, int rank, int world, int max_rows_per_rank, unsigned char* handle_out) {
   JIMM_TRY(check_ready(m, 0));
-  if (!m->txt.present) { set_last_error("model has no text tower"); return JIMM_EINVAL; }
+  JIMM_TRY(check_text(m));
   JIMM_TRY(set_device(m));
   return comm_init(&m->comm, rank, world, max_rows_per_rank, m->txt.D, handle_out);
 }
@@ -1804,163 +1779,6 @@ int jimm_profile_end(jimm_model_t* m, double* gemm_ms, double* gemm_flops, long 
   if (gemm_launches) *gemm_launches = m->prof_launches;
   m->prof_used = 0;
   return 0;
-}
-
-// ---- per-kernel entry points ----
-int jimm_k_gemm_ex(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
-                   const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
-                   int row_off, int epi_mode, int plan_M, int reverse, int tok_pad, int tok_off, int tok_S, const float* ln_scale,
-                   const float* ln_bias, float ln_eps, void* ln_out, int ln_out_type, int ln_ldo, int* ln_counters, void* stream) {
-  if (plan_M <= 0) plan_M = M;
-  if (M <= 0 || M > plan_M) { set_last_error("jimm_k_gemm_ex: need 0 < M <= plan_M (M=%d plan_M=%d)", M, plan_M); return JIMM_EINVAL; }
-  GemmEpilogue e;
-  e.bias = bias; e.act = act; e.rowadd = rowadd; e.residual = residual; e.ldr = ldr; e.out = out; e.out_type = out_type; e.ldo = ldo;
-  e.rows_in = rows_in; e.rows_out = rows_out; e.row_off = row_off; e.mode = epi_mode;
-  e.tok_pad = tok_pad; e.tok_off = tok_off; e.tok_S = tok_S;
-  if (ln_counters) {  // fp32 operands: the normalised rows are the next GEMM's tf32 operand
-    e.ln_scale = ln_scale; e.ln_bias = ln_bias; e.ln_out = ln_out; e.ln_out_type = ln_out_type == JIMM_F32 ? DT_TF32 : ln_out_type; e.ln_ldo = ln_ldo;
-    e.ln_eps = ln_eps; e.ln_cnt = ln_counters;
-  }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (impl == 1) {
-    if (plan_M != M || reverse || tok_pad || ln_counters) {
-      set_last_error("jimm_k_gemm_ex: the SIMT GEMM has no plan rows, reverse walk, token scatter or fused LayerNorm");
-      return JIMM_EINVAL;
-    }
-    return gemm_simt_run(dtype, A, lda, B, ldb, M, N, K, e, s);
-  }
-  GemmPlan p;
-  JIMM_TRY(gemm_plan_init(&p, dtype, A, lda, B, ldb, plan_M, N, K, e));
-  if (ln_counters && !gemm_fuses_ln(&p, M)) {
-    set_last_error("gemm: this shape does not take the fused LayerNorm path (needs N = 128 x {1,2,3,4,6,8,9}, aligned operands, "
-                   "LayerNorm output in the operand type)");
-    return JIMM_EINVAL;
-  }
-  return gemm_plan_run(&p, M, s, reverse);
-}
-int jimm_k_gemm(int impl, int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, int act,
-                const float* rowadd, const float* residual, int ldr, void* out, int out_type, int ldo, int rows_in, int rows_out,
-                int row_off, int epi_mode, void* stream) {
-  return jimm_k_gemm_ex(impl, dtype, A, lda, B, ldb, M, N, K, bias, act, rowadd, residual, ldr, out, out_type, ldo, rows_in, rows_out, row_off,
-                        epi_mode, M, 0, 0, 0, 0, nullptr, nullptr, 0.f, nullptr, 0, 0, nullptr, stream);
-}
-int jimm_k_gemm_residual_ln(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* bias, float* x, int ldx,
-                            const float* ln_scale, const float* ln_bias, float eps, void* ln_out, int ln_out_type, int ln_ldo, int* counters,
-                            void* stream) {
-  if (!counters) { set_last_error("jimm_k_gemm_residual_ln: null counters"); return JIMM_EINVAL; }
-  return jimm_k_gemm_ex(0, dtype, A, lda, B, ldb, M, N, K, bias, 0, nullptr, x, ldx, x, JIMM_F32, ldx, 0, 0, 0, 2, M, 0, 0, 0, 0, ln_scale,
-                        ln_bias, eps, ln_out, ln_out_type, ln_ldo, counters, stream);
-}
-int jimm_k_layernorm_ex(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
-                        float eps, void* out, int out_type, int ldy, int rows, int D, int reverse, void* stream) {
-  return layernorm_run(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, static_cast<cudaStream_t>(stream), reverse);
-}
-int jimm_k_layernorm(const float* x, int ldx, int group, int row_off, const int32_t* row_index, const float* scale, const float* bias,
-                     float eps, void* out, int out_type, int ldy, int rows, int D, void* stream) {
-  return jimm_k_layernorm_ex(x, ldx, group, row_off, row_index, scale, bias, eps, out, out_type, ldy, rows, D, 0, stream);
-}
-int jimm_k_layernorm_e4m3(const float* x, int ldx, const float* scale, const float* bias, float eps, void* out, int ldy, float* row_scale,
-                          int rows, int D, int reverse, void* stream) {
-  return layernorm_run(x, ldx, 1, 0, nullptr, scale, bias, eps, out, DT_E4M3, ldy, rows, D, static_cast<cudaStream_t>(stream), reverse,
-                       row_scale);
-}
-int jimm_k_gemm_e4m3(int impl, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const float* a_scale, const float* b_scale,
-                     const float* bias, int act, void* out, int out_type, int ldo, int epi_mode, int plan_M, int reverse, void* stream) {
-  if (plan_M <= 0) plan_M = M;
-  if (M <= 0 || M > plan_M) { set_last_error("jimm_k_gemm_e4m3: need 0 < M <= plan_M (M=%d plan_M=%d)", M, plan_M); return JIMM_EINVAL; }
-  if (out_type < DT_F32 || out_type > DT_TF32) { set_last_error("jimm_k_gemm_e4m3: bad output type %d", out_type); return JIMM_EINVAL; }
-  GemmEpilogue e;
-  e.bias = bias; e.act = act; e.out = out; e.out_type = out_type; e.ldo = ldo; e.mode = epi_mode;
-  e.a_scale = a_scale; e.b_scale = b_scale;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (impl == 1) {
-    if (plan_M != M || reverse) { set_last_error("jimm_k_gemm_e4m3: the SIMT GEMM has no plan rows or reverse walk"); return JIMM_EINVAL; }
-    return gemm_simt_run(DT_E4M3, A, lda, B, ldb, M, N, K, e, s);
-  }
-  GemmPlan p;
-  JIMM_TRY(gemm_plan_init(&p, DT_E4M3, A, lda, B, ldb, plan_M, N, K, e));
-  return gemm_plan_run(&p, M, s, reverse);
-}
-int jimm_k_quantize_e4m3(const float* src, int lds, int rows, int K, void* out, int ldo, float* row_scale, void* stream) {
-  return quantize_rows_e4m3_run(src, lds, rows, K, out, ldo, row_scale, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_attention_hd(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, int reverse,
-                        void* stream) {
-  return attention_run(qkv, io_type, out, out_type, B, S, H, head_dim, causal, static_cast<cudaStream_t>(stream), reverse);
-}
-int jimm_k_attention_ex(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, int reverse, void* stream) {
-  return jimm_k_attention_hd(qkv, io_type, out, out_type, B, S, H, 64, causal, reverse, stream);
-}
-int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int causal, void* stream) {
-  return jimm_k_attention_ex(qkv, io_type, out, out_type, B, S, H, causal, 0, stream);
-}
-int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, void* stream) {
-  return map_attention_run(q, kv, io_type, out, out_type, B, S, H, head_dim, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_attention_packed(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H, int head_dim,
-                            int reverse, void* stream) {
-  return attention_packed_run(qkv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream), reverse);
-}
-int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S,
-                                int H, int head_dim, void* stream) {
-  return map_attention_packed_run(q, kv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
-  return jimm_k_map_attention_hd(q, kv, io_type, out, out_type, B, S, H, 64, stream);
-}
-int jimm_k_patchify_ex(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, int rows_per_sample, int ldk,
-                       void* stream) {
-  return patchify_run(img, in_type, B, H, W, C, P, out, out_type, static_cast<cudaStream_t>(stream), rows_per_sample, ldk);
-}
-int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream) {
-  return jimm_k_patchify_ex(img, in_type, B, H, W, C, P, out, out_type, 0, 0, stream);
-}
-int jimm_k_activation(const float* x, float* y, long long n, int act, void* stream) {
-  if (n < 0 || (n > 0 && (!x || !y))) { set_last_error("jimm_k_activation: bad arguments"); return JIMM_EINVAL; }
-  return activation_run(x, y, static_cast<size_t>(n), act, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream) {
-  return tokens_init_interp_run(x, cls, pos, g, D, B, gh, gw, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream) {
-  return embed_run(ids, table, pos, x, B, T, D, vocab, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream) {
-  return l2_normalize_run(x, out, ldo, B, E, static_cast<cudaStream_t>(stream));
-}
-int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
-                  int E, int ldl, void* stream) {
-  return logits_run(img, txt, logit_scale, logit_bias, logits, Bi, Bt, E, ldl, static_cast<cudaStream_t>(stream));
-}
-
-// checkpoint ingestion as finalize runs it, through a staging ring of this call's own (freed, its last chunk done, before returning)
-static int check_upload_types(const char* fn, const void* host, void* dst, int src_type, int out_type) {
-  if (!host || !dst) { set_last_error("%s: null pointer", fn); return JIMM_EINVAL; }
-  if (src_type < DT_F32 || src_type > DT_BF16 || out_type < DT_F32 || out_type > DT_TF32) {
-    set_last_error("%s: bad type codes (src %d, out %d)", fn, src_type, out_type);
-    return JIMM_EINVAL;
-  }
-  return 0;
-}
-int jimm_k_upload_rows(const void* host, int src_type, long long rows, long long K, void* dst, int out_type, long long ldd, void* stream) {
-  JIMM_TRY(check_upload_types("jimm_k_upload_rows", host, dst, src_type, out_type));
-  if (rows < 0 || K < 0 || ldd < K) { set_last_error("jimm_k_upload_rows: bad shape (rows %lld, K %lld, ldd %lld)", rows, K, ldd); return JIMM_EINVAL; }
-  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // pinned staging ring
-  UploadRing ring;
-  const int rc = upload_rows(ring, host, src_type, static_cast<size_t>(rows), static_cast<size_t>(K), dst, out_type, static_cast<size_t>(ldd),
-                             static_cast<cudaStream_t>(stream));
-  ring.destroy();
-  return rc;
-}
-int jimm_k_upload_kernel(const void* host, int src_type, int K, int N, int transposed, void* dst, int out_type, long long ldd, int n0, void* stream) {
-  JIMM_TRY(check_upload_types("jimm_k_upload_kernel", host, dst, src_type, out_type));
-  if (K < 0 || N < 0 || n0 < 0 || ldd < K) { set_last_error("jimm_k_upload_kernel: bad shape (K %d, N %d, ldd %lld, n0 %d)", K, N, ldd, n0); return JIMM_EINVAL; }
-  std::lock_guard<std::mutex> no_capture(g_capture_mu);  // pinned staging ring
-  UploadRing ring;
-  const int rc = upload_kernel(ring, host, src_type, K, N, transposed != 0, dst, out_type, static_cast<size_t>(ldd), n0,
-                               static_cast<cudaStream_t>(stream));
-  ring.destroy();
-  return rc;
 }
 
 }  // extern "C"
