@@ -5,7 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, Optional
+from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -16,11 +16,7 @@ from .nn import LazyParam
 _TORCH_TO_CODE = {torch.float32: _lib.F32, torch.float16: _lib.F16, torch.bfloat16: _lib.BF16}
 
 
-def _stream_ptr(device: torch.device) -> int:
-    return torch.cuda.current_stream(device).cuda_stream
-
-
-def _as_tensor(x, what: str) -> torch.Tensor:
+def _as_tensor(x) -> torch.Tensor:
     if isinstance(x, torch.Tensor):
         return x
     if isinstance(x, np.ndarray):
@@ -28,6 +24,79 @@ def _as_tensor(x, what: str) -> torch.Tensor:
     if hasattr(x, "__dlpack__"):
         return torch.from_dlpack(x)
     return torch.as_tensor(np.asarray(x))
+
+
+def _call(lib, device: torch.device, name: str, *args):
+    """Library entry point `name` on `args` and the current stream of `device`, with `device` current: tensors are passed as their
+    data pointers, torch dtypes as dtype codes."""
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else _TORCH_TO_CODE[a] if isinstance(a, torch.dtype) else a for a in args]
+    with torch.cuda.device(device):
+        _lib.check(getattr(lib, name)(*args, torch.cuda.current_stream(device).cuda_stream))
+
+
+class Images(NamedTuple):
+    """The images of one vision call, checked and prepared once (prep_images)."""
+
+    x: Union[torch.Tensor, List[torch.Tensor]]  # [B, H, W, C], or a list of [H, W, C]
+    host: bool  # host memory: the result goes back to the host
+    u8: bool  # raw RGB frames for the image front-end
+    hw: Optional[Tuple[int, int]]  # the (height, width) the tower sees; for a list the one with the most tokens (None: empty list)
+    trained: bool  # hw is the trained size
+
+
+def _prep_batch(x, cfg: _lib.Config, preproc, interpolate: bool):
+    """One [B, H, W, C] batch, checked and made contiguous, and the (height, width) the tower sees."""
+    x = _as_tensor(x)
+    if x.ndim != 4:
+        raise ValueError(f"expected images of shape [batch, height, width, channels], got {tuple(x.shape)}")
+    _, h, w, ch = x.shape
+    S = cfg.img_size
+    if x.dtype == torch.uint8:
+        # raw RGB frames: need the attached image front-end (model.set_preprocessor); any frame size it maps to the model's input
+        if preproc is None:
+            raise ValueError("uint8 images need an image front-end: call model.set_preprocessor(ImagePreprocessor...) first, "
+                             "or pass normalised float pixel values")
+        if ch != 3:
+            raise ValueError(f"expected uint8 RGB frames [B,H,W,3], got {tuple(x.shape)}")
+        hw = preproc.output_size(h, w)
+        if not interpolate and hw != (S, S):
+            raise ValueError(f"the image front-end maps {h}x{w} frames to {hw[0]}x{hw[1]}, the model takes {S}x{S}")
+    else:
+        if interpolate and ch != cfg.in_ch:
+            raise ValueError(f"expected NHWC images [B,H,W,{cfg.in_ch}], got {tuple(x.shape)}")
+        if not interpolate and (h != S or w != S or ch != cfg.in_ch):
+            raise ValueError(f"expected NHWC images [B,{S},{S},{cfg.in_ch}], got {tuple(x.shape)}")
+        hw = (h, w)
+        if x.dtype not in _TORCH_TO_CODE:
+            x = x.to(torch.float32)
+    if interpolate and min(hw) < cfg.patch:
+        raise ValueError(f"interpolate_pos_encoding: a {hw[0]}x{hw[1]} image is smaller than one {cfg.patch}x{cfg.patch} patch")
+    return x.contiguous(), hw
+
+
+def prep_images(images, cfg: _lib.Config, preproc, interpolate: bool) -> Images:
+    """The input step of every vision call: a [B, H, W, C] batch, or a list / tuple of [H, W, C] (or [1, H, W, C]) images of one dtype
+    on one device, checked against the model and the image front-end `preproc`.  interpolate: HF's interpolate_pos_encoding -- any
+    image size of at least one patch is accepted."""
+    if not isinstance(images, (list, tuple)):
+        x, hw = _prep_batch(images, cfg, preproc, interpolate)
+        return Images(x, not x.is_cuda, x.dtype == torch.uint8, hw, hw == (cfg.img_size, cfg.img_size))
+    xs = []
+    for i, x in enumerate(images):
+        x = _as_tensor(x)
+        if x.ndim == 4 and x.shape[0] == 1:
+            x = x[0]
+        if x.ndim != 3:
+            raise ValueError(f"image {i} of the list: expected [height, width, channels] or [1, height, width, channels], got {tuple(x.shape)}")
+        xs.append(x)
+    if len({x.dtype for x in xs}) > 1:
+        raise ValueError(f"the images of a list must share one dtype, got {sorted({str(x.dtype) for x in xs})}")
+    if len({x.device for x in xs}) > 1:
+        raise ValueError(f"the images of a list must be on one device, got {sorted({str(x.device) for x in xs})}")
+    prepped = [_prep_batch(x[None], cfg, preproc, interpolate) for x in xs]
+    hw = max((hw for _, hw in prepped), key=lambda s: grid_tokens(cfg, *s), default=None)
+    xs = [x[0] for x, _ in prepped]
+    return Images(xs, not xs or not xs[0].is_cuda, bool(xs) and xs[0].dtype == torch.uint8, hw, hw == (cfg.img_size, cfg.img_size))
 
 
 class PendingResult:
@@ -113,276 +182,139 @@ class NativeModel:
         except Exception:
             pass
 
-    # ---- input normalisation ----
-    def _prep_images(self, x, interpolate: bool = False) -> torch.Tensor:
-        """interpolate: HF's interpolate_pos_encoding -- any image size of at least one patch is accepted."""
-        x = _as_tensor(x, "image")
-        if x.ndim != 4:
-            raise ValueError(f"expected images of shape [batch, height, width, channels], got {tuple(x.shape)}")
-        c = self.cfg
-        if x.dtype == torch.uint8:
-            # raw RGB frames: need the attached image front-end (model.set_preprocessor); any frame size it maps to the model's input
-            if self.preproc is None:
-                raise ValueError("uint8 images need an image front-end: call model.set_preprocessor(ImagePreprocessor...) first, "
-                                 "or pass normalised float pixel values")
-            if x.shape[3] != 3:
-                raise ValueError(f"expected uint8 RGB frames [B,H,W,3], got {tuple(x.shape)}")
-            oh, ow = self.preproc.output_size(x.shape[1], x.shape[2])
-            if interpolate:
-                self._check_grid(oh, ow)
-            elif (oh, ow) != (c.img_size, c.img_size):
-                raise ValueError(f"the image front-end maps {x.shape[1]}x{x.shape[2]} frames to {oh}x{ow}, the model takes {c.img_size}x{c.img_size}")
-            return x.contiguous()
-        if interpolate:
-            if x.shape[3] != c.in_ch:
-                raise ValueError(f"expected NHWC images [B,H,W,{c.in_ch}], got {tuple(x.shape)}")
-            self._check_grid(x.shape[1], x.shape[2])
-        elif x.shape[1] != c.img_size or x.shape[2] != c.img_size or x.shape[3] != c.in_ch:
-            raise ValueError(f"expected NHWC images [B,{c.img_size},{c.img_size},{c.in_ch}], got {tuple(x.shape)}")
-        if x.dtype not in _TORCH_TO_CODE:
-            x = x.to(torch.float32)
-        return x.contiguous()
-
-    def _check_grid(self, h: int, w: int):
-        P = self.cfg.patch
-        if h < P or w < P:
-            raise ValueError(f"interpolate_pos_encoding: a {h}x{w} image is smaller than one {P}x{P} patch")
-
-    def _off_grid(self, x: torch.Tensor, interpolate: bool) -> bool:
-        """True when an interpolate_pos_encoding call's (prepared) images are not the native size: the *_hw entry points run it."""
-        if not interpolate:
-            return False
-        hw = self.preproc.output_size(x.shape[1], x.shape[2]) if x.dtype == torch.uint8 else (x.shape[1], x.shape[2])
-        return tuple(hw) != (self.cfg.img_size, self.cfg.img_size)
-
-    def _device_images(self, x: torch.Tensor) -> torch.Tensor:
-        """Prepared images on this GPU in a tower input type (uint8 frames through the image front-end)."""
+    def _device_images(self, x):
+        """Prepared images on this GPU in a tower input type: host images copied over, uint8 frames through the image front-end (one
+        at a time for a list; their output sizes differ)."""
+        if isinstance(x, list):
+            return [self._device_images(t[None])[0].contiguous() for t in x]
         xd = x.to(self.device, non_blocking=True)
         return self.preproc(xd, dtype=self._operand_dtype()) if xd.dtype == torch.uint8 else xd
-
-    def _prep_ids(self, t) -> torch.Tensor:
-        t = _as_tensor(t, "text")
-        if t.ndim != 2:
-            raise ValueError(f"expected token ids of shape [batch, context_length], got {tuple(t.shape)}")
-        return t.to(torch.int32).contiguous()
-
-    # ---- forward ----
-    def vision(self, x, encode: bool = False, interpolate: bool = False) -> torch.Tensor:
-        """VisionTransformer.__call__ / encode_image.  CUDA input -> async CUDA output; host input -> host output.
-        interpolate: HF's interpolate_pos_encoding (images of any size; see jimm_vit_forward_hw)."""
-        x = self._prep_images(x, interpolate)
-        if self._off_grid(x, interpolate):
-            return self._vision_hw(x, encode)
-        B = x.shape[0]
-        fn_dev = self.lib.jimm_encode_image if encode else self.lib.jimm_vit_forward
-        if x.is_cuda:
-            if x.dtype == torch.uint8:  # device frames: front-end kernel, then the tower, on the current stream
-                x = self.preproc(x, dtype=self._operand_dtype())
-            with torch.cuda.device(self.device):
-                out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-                _lib.check(fn_dev(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], B, C.c_void_p(out.data_ptr()),
-                                  C.c_void_p(_stream_ptr(self.device))))
-            return out
-        return self._vision_host(x, encode).result()
-
-    def vision_async(self, x, encode: bool = False, interpolate: bool = False) -> "PendingResult":
-        """Host input: enqueue H2D + forward + D2H and return without synchronising (JAX-style asynchronous dispatch);
-        `.result()` waits for this call only.  Back-to-back calls pipeline: the copies of call k+1 run under the towers of
-        call k.  The caller keeps `x` alive and unmodified until the result is taken.  Host images off the native size
-        (interpolate=True) run synchronously."""
-        x = self._prep_images(x, interpolate)
-        if x.is_cuda or self._off_grid(x, interpolate):
-            return PendingResult(self.vision(x, encode, interpolate), None)
-        return self._vision_host(x, encode)
-
-    def _vision_hw(self, x: torch.Tensor, encode: bool) -> torch.Tensor:
-        """A vision call at a size other than the native one: host images are copied to the GPU here and the result back."""
-        B = x.shape[0]
-        fn = self.lib.jimm_encode_image_hw if encode else self.lib.jimm_vit_forward_hw
-        with torch.cuda.device(self.device):
-            xd = self._device_images(x)
-            out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-            _lib.check(fn(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], B, xd.shape[1], xd.shape[2],
-                          C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
-        return out if x.is_cuda else out.cpu()
-
-    # ---- packed lists of images of different sizes (jimm_vit_forward_packed) ----
-    def _prep_image_list(self, images, interpolate: bool):
-        """Each element of a list / tuple as one prepared image [H, W, C] (a leading batch dimension of 1 is dropped), all of one
-        dtype and on one device; the checks of _prep_images, per image."""
-        xs = []
-        for i, x in enumerate(images):
-            x = _as_tensor(x, "image")
-            if x.ndim == 4 and x.shape[0] == 1:
-                x = x[0]
-            if x.ndim != 3:
-                raise ValueError(f"image {i} of the list: expected [height, width, channels] or [1, height, width, channels], got {tuple(x.shape)}")
-            xs.append(x)
-        if len({x.dtype for x in xs}) > 1:
-            raise ValueError(f"the images of a list must share one dtype, got {sorted({str(x.dtype) for x in xs})}")
-        if len({x.device for x in xs}) > 1:
-            raise ValueError(f"the images of a list must be on one device, got {sorted({str(x.device) for x in xs})}")
-        return [self._prep_images(x[None], interpolate)[0] for x in xs]
-
-    def _vision_packed_dev(self, images, encode: bool, interpolate: bool):
-        """The rows of a list of images on this GPU (fp32 [len, out_dim]) and whether the inputs were host memory."""
-        xs = self._prep_image_list(images, interpolate)
-        B = len(xs)
-        host = B > 0 and not xs[0].is_cuda
-        with torch.cuda.device(self.device):
-            out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-            if B == 0:
-                return out, True
-            # uint8 frames go through the image front-end one at a time (their output sizes differ)
-            xd = [self._device_images(x[None])[0].contiguous() for x in xs]
-            ptrs = (C.c_void_p * B)(*[x.data_ptr() for x in xd])
-            hs = (C.c_int * B)(*[x.shape[0] for x in xd])
-            ws = (C.c_int * B)(*[x.shape[1] for x in xd])
-            fn = self.lib.jimm_encode_image_packed if encode else self.lib.jimm_vit_forward_packed
-            _lib.check(fn(self.handle, ptrs, _TORCH_TO_CODE[xd[0].dtype], B, hs, ws, C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
-            if not host:
-                cur = torch.cuda.current_stream(self.device)
-                for x in xd:  # freshly made device copies are freed only after the call's work
-                    x.record_stream(cur)
-        return out, host
-
-    def vision_packed(self, images, encode: bool = False, interpolate: bool = False) -> torch.Tensor:
-        """A list / tuple of images of different sizes in one call: their tokens packed into one stream (variable-length
-        attention).  Row i is the result of the call on images[i] alone.  CUDA inputs -> CUDA output without a host synchronisation;
-        host inputs -> host output."""
-        out, host = self._vision_packed_dev(images, encode, interpolate)
-        return out.cpu() if host else out
-
-    def dual_packed(self, images, text, interpolate: bool = False) -> torch.Tensor:
-        """CLIP.__call__ / SigLIP.__call__ on a list of images of different sizes."""
-        ids = self._prep_ids(text)
-        ie, host = self._vision_packed_dev(images, True, interpolate)
-        host = host and not ids.is_cuda
-        with torch.cuda.device(self.device):
-            te = self.text(ids.to(self.device, non_blocking=True))
-            out = self.logits(ie, te)
-        return out.cpu() if host else out
 
     def _operand_dtype(self) -> torch.dtype:
         return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16, _lib.F8E4M3: torch.float16}[self.cfg.compute_dtype]
 
-    def _vision_host(self, x: torch.Tensor, encode: bool) -> "PendingResult":
-        B = x.shape[0]
-        fn_dev = self.lib.jimm_encode_image if encode else self.lib.jimm_vit_forward
-        # host path: H2D + forward + D2H enqueued by the library on the current stream
-        with torch.cuda.device(self.device):
-            # fresh pinned result (torch's caching host allocator makes this cheap); no CPU-side tensor op on this path: an
+    def _prep_ids(self, t) -> torch.Tensor:
+        t = _as_tensor(t)
+        if t.ndim != 2:
+            raise ValueError(f"expected token ids of shape [batch, context_length], got {tuple(t.shape)}")
+        return t.to(torch.int32).contiguous()
+
+    def _run(self, name: str, *args):
+        """Entry point `name` on this handle (see _call)."""
+        _call(self.lib, self.device, name, self.handle, *args)
+
+    def _back(self, out: torch.Tensor, host: bool, keep=None) -> PendingResult:
+        """A call's result as its caller gets it: `out` as it is for device inputs; for host inputs a pinned host tensor (`out` itself
+        when the library wrote it there, else a copy queued behind the call) and the event that marks it filled.  `keep` stays
+        referenced until the result is taken."""
+        if not host:
+            return PendingResult(out, None)
+        if out.is_cuda:
+            # fresh pinned result (torch's caching host allocator makes this cheap); no CPU-side tensor op on the host path: an
             # intra-op OpenMP team on a CPU-quota-limited box costs milliseconds
+            out = torch.empty(out.shape, dtype=out.dtype, pin_memory=True).copy_(out, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        return PendingResult(out, ev, keep)
+
+    # ---- forward ----
+    def vision(self, x, encode: bool = False, interpolate: bool = False, wait: bool = True):
+        """VisionTransformer.__call__ / encode_image on Images, or on a tensor / list prepared here.  CUDA input -> async CUDA output;
+        host input -> host output.  interpolate: HF's interpolate_pos_encoding (images of any size; see jimm_vit_forward_hw); a list
+        runs in one packed call (jimm_vit_forward_packed).  wait=False returns a PendingResult: host images of the trained size are
+        left in flight (JAX-style asynchronous dispatch: back-to-back calls pipeline, the copies of call k+1 run under the towers of
+        call k, and the caller keeps the images alive and unmodified until the result is taken); any other input comes back
+        finished."""
+        im = x if isinstance(x, Images) else prep_images(x, self.cfg, self.preproc, interpolate)
+        if im.host and im.trained and not encode and not isinstance(im.x, list):
+            # host path: H2D + forward + D2H enqueued by the library on the current stream, into a pinned result (uint8 frames: bytes
+            # over PCIe, front-end + tower in the library's sliced copy/compute pipeline)
+            B = len(im.x)
             out = torch.empty((B, self.vision_out), dtype=torch.float32, pin_memory=True)
-            cur = torch.cuda.current_stream(self.device)
-            if x.dtype == torch.uint8 and not encode:
-                # raw frames: bytes over PCIe, front-end + tower in the library's sliced copy/compute pipeline
-                _lib.check(self.lib.jimm_vit_forward_host_u8(self.handle, self.preproc.handle, C.c_void_p(x.data_ptr()), B, x.shape[1], x.shape[2],
-                                                             C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
-            elif encode:
-                xd = x.to(self.device, non_blocking=True)
-                if xd.dtype == torch.uint8:
-                    xd = self.preproc(xd, dtype=self._operand_dtype())
-                od = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-                _lib.check(fn_dev(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], B, C.c_void_p(od.data_ptr()),
-                                  C.c_void_p(_stream_ptr(self.device))))
-                out.copy_(od, non_blocking=True)
+            if im.u8:
+                self._run("jimm_vit_forward_host_u8", self.preproc.handle, im.x, B, im.x.shape[1], im.x.shape[2], out)
             else:
-                _lib.check(self.lib.jimm_vit_forward_host(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], B,
-                                                          C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
-            ev = torch.cuda.Event()
-            ev.record(cur)
-        return PendingResult(out, ev, keep=x)
+                self._run("jimm_vit_forward_host", im.x, im.x.dtype, B, out)
+            res = self._back(out, True, keep=im.x)
+            return res if not wait else res.result()
+        res = self._back(self._vision_dev(im, encode), im.host, keep=im.x).result()
+        return res if wait else PendingResult(res, None)
+
+    def _vision_dev(self, im: Images, encode: bool) -> torch.Tensor:
+        """The vision call on the images on this GPU (host images copied over): fp32 [B, out_dim] on this GPU."""
+        xd = self._device_images(im.x)
+        B = len(xd)
+        out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
+        if isinstance(xd, list):
+            if B:
+                self._run("jimm_encode_image_packed" if encode else "jimm_vit_forward_packed", (C.c_void_p * B)(*[t.data_ptr() for t in xd]),
+                          xd[0].dtype, B, (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]), out)
+                if not im.host:
+                    for t in xd:  # freshly made device copies are freed only after the call's work
+                        t.record_stream(torch.cuda.current_stream(self.device))
+        elif im.trained:
+            self._run("jimm_encode_image" if encode else "jimm_vit_forward", xd, xd.dtype, B, out)
+        else:
+            self._run("jimm_encode_image_hw" if encode else "jimm_vit_forward_hw", xd, xd.dtype, B, xd.shape[1], xd.shape[2], out)
+        return out
 
     def text(self, ids) -> torch.Tensor:
         ids = self._prep_ids(ids)
-        host = not ids.is_cuda
         B, T = ids.shape
-        with torch.cuda.device(self.device):
-            idd = ids.to(self.device, non_blocking=True)
-            out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.jimm_encode_text(self.handle, C.c_void_p(idd.data_ptr()), B, T, C.c_void_p(out.data_ptr()),
-                                                 C.c_void_p(_stream_ptr(self.device))))
-            if host:
-                out = out.cpu()
-        return out
+        out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
+        self._run("jimm_encode_text", ids.to(self.device, non_blocking=True), B, T, out)
+        return self._back(out, not ids.is_cuda).result()
 
     def dual_encode(self, x: torch.Tensor, ids: torch.Tensor):
         """encode_image + encode_text of device-resident inputs with the two towers running concurrently (jimm_dual_encode)."""
+        x = self._device_images(x)
         Bi, (Bt, T) = x.shape[0], ids.shape
-        with torch.cuda.device(self.device):
-            if x.dtype == torch.uint8:  # raw frames: the image front-end first (model.set_preprocessor)
-                x = self.preproc(x, dtype=self._operand_dtype())
-            ie = torch.empty((Bi, self.vision_out), dtype=torch.float32, device=self.device)
-            te = torch.empty((Bt, self.text_out), dtype=torch.float32, device=self.device)
-            # images of the native size run exactly as jimm_dual_encode; others only reach here with interpolate_pos_encoding
-            _lib.check(self.lib.jimm_dual_encode_hw(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], Bi, x.shape[1], x.shape[2],
-                                                    C.c_void_p(ids.data_ptr()), Bt, T, C.c_void_p(ie.data_ptr()), C.c_void_p(te.data_ptr()),
-                                                    C.c_void_p(_stream_ptr(self.device))))
+        ie = torch.empty((Bi, self.vision_out), dtype=torch.float32, device=self.device)
+        te = torch.empty((Bt, self.text_out), dtype=torch.float32, device=self.device)
+        # images of the native size run exactly as jimm_dual_encode; others only reach here with interpolate_pos_encoding
+        self._run("jimm_dual_encode_hw", x, x.dtype, Bi, x.shape[1], x.shape[2], ids, Bt, T, ie, te)
         return ie, te
 
     def logits(self, img_e: torch.Tensor, txt_e: torch.Tensor) -> torch.Tensor:
-        with torch.cuda.device(self.device):
-            img_e = img_e.to(self.device, torch.float32).contiguous()
-            txt_e = txt_e.to(self.device, torch.float32).contiguous()
-            Bi, Bt = img_e.shape[0], txt_e.shape[0]
-            out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.jimm_contrastive_logits(self.handle, C.c_void_p(img_e.data_ptr()), Bi, C.c_void_p(txt_e.data_ptr()), Bt,
-                                                        C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
+        img_e = img_e.to(self.device, torch.float32).contiguous()
+        txt_e = txt_e.to(self.device, torch.float32).contiguous()
+        Bi, Bt = img_e.shape[0], txt_e.shape[0]
+        out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
+        self._run("jimm_contrastive_logits", img_e, Bi, txt_e, Bt, out)
         return out
 
-    def dual(self, image, text, interpolate: bool = False) -> torch.Tensor:
-        """CLIP.__call__ / SigLIP.__call__ on one GPU."""
-        x = self._prep_images(image, interpolate)
+    def dual(self, images, text, interpolate: bool = False) -> torch.Tensor:
+        """CLIP.__call__ / SigLIP.__call__ on one GPU, on Images or on a tensor / list prepared here.  The result is on the host
+        when the images and the ids were."""
+        im = images if isinstance(images, Images) else prep_images(images, self.cfg, self.preproc, interpolate)
         ids = self._prep_ids(text)
-        Bi, (Bt, T) = x.shape[0], ids.shape
-        with torch.cuda.device(self.device):
-            if self._off_grid(x, interpolate):
-                xd, idd = self._device_images(x), ids.to(self.device, non_blocking=True)
-                out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
-                _lib.check(self.lib.jimm_dual_forward_hw(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], Bi, xd.shape[1],
-                                                         xd.shape[2], C.c_void_p(idd.data_ptr()), Bt, T, C.c_void_p(out.data_ptr()),
-                                                         C.c_void_p(_stream_ptr(self.device))))
-                return out if (x.is_cuda or ids.is_cuda) else out.cpu()
-            if x.dtype == torch.uint8:
-                # raw RGB frames (model.set_preprocessor): bytes over PCIe, the image front-end on the GPU, then both towers concurrently
-                host_in = not x.is_cuda and not ids.is_cuda
-                xd = self.preproc(x.to(self.device, non_blocking=True), dtype=self._operand_dtype())
-                idd = ids.to(self.device, non_blocking=True)
-                out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
-                _lib.check(self.lib.jimm_dual_forward(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], Bi,
-                                                      C.c_void_p(idd.data_ptr()), Bt, T, C.c_void_p(out.data_ptr()),
-                                                      C.c_void_p(_stream_ptr(self.device))))
-                if not host_in:
-                    return out
-                out_h = torch.empty((Bi, Bt), dtype=torch.float32, pin_memory=True)
-                out_h.copy_(out, non_blocking=True)
-                torch.cuda.current_stream(self.device).synchronize()
-                return out_h
-            if not x.is_cuda and not ids.is_cuda:
-                out = torch.empty((Bi, Bt), dtype=torch.float32, pin_memory=True)
-                _lib.check(self.lib.jimm_dual_forward_host(self.handle, C.c_void_p(x.data_ptr()), _TORCH_TO_CODE[x.dtype], Bi,
-                                                           C.c_void_p(ids.data_ptr()), Bt, T, C.c_void_p(out.data_ptr()),
-                                                           C.c_void_p(_stream_ptr(self.device))))
-                torch.cuda.current_stream(self.device).synchronize()
-                return out
-            xd, idd = x.to(self.device, non_blocking=True), ids.to(self.device, non_blocking=True)
+        host = im.host and not ids.is_cuda
+        Bi, (Bt, T) = len(im.x), ids.shape
+        if isinstance(im.x, list):
+            out = self.logits(self._vision_dev(im, True), self.text(ids.to(self.device, non_blocking=True)))
+        elif host and im.trained and not im.u8:
+            # float pixels and ids: the library's pipeline copies both in and the logits out
+            out = torch.empty((Bi, Bt), dtype=torch.float32, pin_memory=True)
+            self._run("jimm_dual_forward_host", im.x, im.x.dtype, Bi, ids, Bt, T, out)
+        else:
+            xd, idd = self._device_images(im.x), ids.to(self.device, non_blocking=True)
             out = torch.empty((Bi, Bt), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.jimm_dual_forward(self.handle, C.c_void_p(xd.data_ptr()), _TORCH_TO_CODE[xd.dtype], Bi,
-                                                  C.c_void_p(idd.data_ptr()), Bt, T, C.c_void_p(out.data_ptr()),
-                                                  C.c_void_p(_stream_ptr(self.device))))
-        return out
+            if im.trained:
+                self._run("jimm_dual_forward", xd, xd.dtype, Bi, idd, Bt, T, out)
+            else:
+                self._run("jimm_dual_forward_hw", xd, xd.dtype, Bi, xd.shape[1], xd.shape[2], idd, Bt, T, out)
+        return self._back(out, host).result()
 
     # ---- multi-GPU contrastive head (one process per GPU; torch.distributed is the control plane) ----
     def comm_setup(self, max_rows_per_rank: int, group=None):
         import torch.distributed as dist
 
+        from .dist import exchange_handles
+
         rank, world = dist.get_rank(group), dist.get_world_size(group)
         handle = C.create_string_buffer(64)
         _lib.check(self.lib.jimm_comm_init(self.handle, rank, world, int(max_rows_per_rank), handle))
-        handles = [None] * world
-        dist.all_gather_object(handles, bytes(handle.raw), group=group)
-        _lib.check(self.lib.jimm_comm_connect(self.handle, b"".join(handles)))
+        _lib.check(self.lib.jimm_comm_connect(self.handle, exchange_handles(handle.raw, group)))
         dist.barrier(group)
         self._comm = (rank, world, int(max_rows_per_rank))
 
@@ -391,15 +323,13 @@ class NativeModel:
         if self._comm is None:
             raise _lib.JimmError("comm_setup() has not been called")
         rank, world, _ = self._comm
-        with torch.cuda.device(self.device):
-            img_e = img_e.to(self.device, torch.float32).contiguous()
-            txt_e = txt_e.to(self.device, torch.float32).contiguous()
-            B = img_e.shape[0]
-            if txt_e.shape[0] != B:
-                raise ValueError("multi-GPU contrastive head needs equal image/text batch per rank")
-            out = torch.empty((B, world * B), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.jimm_comm_contrastive_logits(self.handle, C.c_void_p(img_e.data_ptr()), C.c_void_p(txt_e.data_ptr()), B,
-                                                             C.c_void_p(out.data_ptr()), C.c_void_p(_stream_ptr(self.device))))
+        img_e = img_e.to(self.device, torch.float32).contiguous()
+        txt_e = txt_e.to(self.device, torch.float32).contiguous()
+        B = img_e.shape[0]
+        if txt_e.shape[0] != B:
+            raise ValueError("multi-GPU contrastive head needs equal image/text batch per rank")
+        out = torch.empty((B, world * B), dtype=torch.float32, device=self.device)
+        self._run("jimm_comm_contrastive_logits", img_e, txt_e, B, out)
         return out
 
 
@@ -416,34 +346,29 @@ class NativeSubModule:
 
     def __call__(self, x) -> torch.Tensor:
         n = self.native
-        x = _as_tensor(x, "activations")
+        x = _as_tensor(x)
         if x.ndim != 3 or x.shape[2] != self.D:
             raise ValueError(f"expected activations of shape [batch, seq, {self.D}], got {tuple(x.shape)}")
-        host = not x.is_cuda
         B, S, D = x.shape
-        with torch.cuda.device(n.device):
-            xd = x.to(n.device, torch.float32, non_blocking=True).contiguous()
-            st = C.c_void_p(_stream_ptr(n.device))
-            if self.kind == _lib.KIND_ENCODER:
-                out = torch.empty((B, S, D), dtype=torch.float32, device=n.device)
-                _lib.check(n.lib.jimm_encoder_forward(n.handle, C.c_void_p(xd.data_ptr()), B, S, C.c_void_p(out.data_ptr()), st))
-            else:
-                out = torch.empty((B, D), dtype=torch.float32, device=n.device)
-                _lib.check(n.lib.jimm_map_head_forward(n.handle, C.c_void_p(xd.data_ptr()), B, S, C.c_void_p(out.data_ptr()), st))
-            xd.record_stream(torch.cuda.current_stream(n.device))
-        return out.cpu() if host else out
+        xd = x.to(n.device, torch.float32, non_blocking=True).contiguous()
+        if self.kind == _lib.KIND_ENCODER:
+            out = torch.empty((B, S, D), dtype=torch.float32, device=n.device)
+            n._run("jimm_encoder_forward", xd, B, S, out)
+        else:
+            out = torch.empty((B, D), dtype=torch.float32, device=n.device)
+            n._run("jimm_map_head_forward", xd, B, S, out)
+        xd.record_stream(torch.cuda.current_stream(n.device))
+        return n._back(out, not x.is_cuda).result()
 
 
 def activation(x, act: int) -> torch.Tensor:
     """Elementwise activation kernel (1 tanh-GELU, 2 QuickGELU) on a CUDA tensor; fp32 result."""
-    x = _as_tensor(x, "x")
+    x = _as_tensor(x)
     if not x.is_cuda:
         raise _lib.JimmError("jimm_b200 runs on CUDA tensors only (there is no CPU fallback)")
-    lib = _lib.load()
-    with torch.cuda.device(x.device):
-        xd = x.to(torch.float32).contiguous()
-        y = torch.empty_like(xd)
-        _lib.check(lib.jimm_k_activation(C.c_void_p(xd.data_ptr()), C.c_void_p(y.data_ptr()), xd.numel(), int(act), C.c_void_p(_stream_ptr(x.device))))
+    xd = x.to(torch.float32).contiguous()
+    y = torch.empty_like(xd)
+    _call(_lib.load(), x.device, "jimm_k_activation", xd, y, xd.numel(), int(act))
     return y
 
 

@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _lib, nn
-from .._runtime import NativeModel, PendingResult, default_max_batch, grid_tokens
+from .._runtime import Images, NativeModel, default_max_batch, grid_tokens, prep_images
 from .transformer import Transformer, _SubModuleRunner, g_wrap
 
 
@@ -120,32 +120,16 @@ class _NativeOwner:
         object.__setattr__(self, "_native", n)
         return n
 
-    def _call_hw(self, img, interpolate_pos_encoding: bool):
-        """(height, width) the tower sees for the images of an interpolate_pos_encoding call, else None (sizes below a patch are
-        refused later)."""
-        if not interpolate_pos_encoding or getattr(img, "ndim", 0) != 4:
-            return None
-        h, w = int(img.shape[1]), int(img.shape[2])
-        if str(img.dtype).endswith("uint8") and self._preproc is not None:
-            h, w = self._preproc.output_size(h, w)
-        P = self._native_config().patch
-        return (h, w) if h >= P and w >= P else None
+    def _images(self, images, interpolate_pos_encoding: bool) -> Images:
+        """The image-input step (prep_images) on this model's config and image front-end, before any handle is built."""
+        n = self._native
+        return prep_images(images, n.cfg if n is not None else self._native_config(), self._preproc, interpolate_pos_encoding)
 
-    def _list_hw(self, images, interpolate_pos_encoding: bool):
-        """The (height, width) with the most tokens among a list's images (what the tower sees: uint8 frames after the front-end), for
-        native(hw=...): the handle is rebuilt only when that image alone does not fit.  None for an empty list or without
-        interpolate_pos_encoding."""
-        best, cfg = None, self._native_config()
-        for img in images:
-            hw = self._call_hw(img[None] if getattr(img, "ndim", 0) == 3 else img, interpolate_pos_encoding)
-            if hw is not None and (best is None or grid_tokens(cfg, *hw) > grid_tokens(cfg, *best)):
-                best = hw
-        return best
-
-    def _vision_list(self, images, interpolate_pos_encoding: bool, encode: bool = False) -> torch.Tensor:
-        """A list / tuple of images of different sizes in one packed call (NativeModel.vision_packed)."""
-        return self.native(max(len(images), 1), hw=self._list_hw(images, interpolate_pos_encoding)).vision_packed(
-            images, encode=encode, interpolate=interpolate_pos_encoding)
+    def _vision(self, images, interpolate_pos_encoding: bool, encode: bool = False, wait: bool = True):
+        """A vision call (NativeModel.vision) on a [B, H, W, C] batch or a list / tuple of images of different sizes (one packed
+        call).  The handle is rebuilt only when the largest image of an interpolate_pos_encoding call does not fit it."""
+        im = self._images(images, interpolate_pos_encoding)
+        return self.native(hw=im.hw if interpolate_pos_encoding else None).vision(im, encode=encode, wait=wait)
 
     def set_max_image_size(self, height: int, width: int):
         """Size the vision workspace for interpolate_pos_encoding calls on images up to height x width: `max_batch` such images run
@@ -231,16 +215,10 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
         (HuggingFace's keyword): images of any size of at least one patch, the position embeddings resampled bicubically to the
         patch grid.  A list / tuple of images [H_i, W_i, C] (or [1, H_i, W_i, C]) of different sizes runs in one packed call; row i
         is the result of images[i] alone."""
-        if isinstance(img, (list, tuple)):
-            return self._vision_list(img, interpolate_pos_encoding)
-        B = img.shape[0]
-        return self.native(B, hw=self._call_hw(img, interpolate_pos_encoding)).vision(img, interpolate=interpolate_pos_encoding)
+        return self._vision(img, interpolate_pos_encoding)
 
     def forward_async(self, img, interpolate_pos_encoding: bool = False):
         """Asynchronous dispatch for host inputs (the reference's calls return before the device finishes, examples/vit_inference.py:54
         only blocks when it reads the logits): returns a `PendingResult`; back-to-back calls overlap their copies with compute.  A
         list of images runs as in __call__, synchronously for host images."""
-        if isinstance(img, (list, tuple)):
-            return PendingResult(self._vision_list(img, interpolate_pos_encoding), None)
-        n = self.native(img.shape[0], hw=self._call_hw(img, interpolate_pos_encoding))
-        return n.vision_async(img, interpolate=interpolate_pos_encoding)
+        return self._vision(img, interpolate_pos_encoding, wait=False)

@@ -5,6 +5,7 @@ from __future__ import annotations
 import torch
 
 from .. import _lib, nn
+from .._runtime import _call
 from ..common.transformer import Transformer, g_wrap
 from ..common.vit import _NativeOwner, tower_config_fields
 
@@ -39,10 +40,7 @@ class DualTower(_NativeOwner, nn.Module):
         """interpolate_pos_encoding (HuggingFace's keyword): images of any size of at least one patch, the position embeddings
         resampled bicubically to the patch grid.  A list / tuple of images of different sizes runs in one packed call; row i is the
         embedding of image[i] alone."""
-        if isinstance(image, (list, tuple)):
-            return self._vision_list(image, interpolate_pos_encoding, encode=True)
-        n = self.native(image.shape[0], hw=self._call_hw(image, interpolate_pos_encoding))
-        return n.vision(image, encode=True, interpolate=interpolate_pos_encoding)
+        return self._vision(image, interpolate_pos_encoding, encode=True)
 
     def encode_text(self, text) -> torch.Tensor:
         return self.native(text.shape[0]).text(text)
@@ -58,11 +56,9 @@ class DualTower(_NativeOwner, nn.Module):
             if isinstance(image, (list, tuple)):
                 raise ValueError("a list of images is not supported by the multi-GPU contrastive call; pass one [B, H, W, C] tensor per rank")
             return self._call_distributed(image, text, interpolate_pos_encoding)
-        if isinstance(image, (list, tuple)):
-            n = self.native(max(len(image), text.shape[0]), require=True, hw=self._list_hw(image, interpolate_pos_encoding))
-            return n.dual_packed(image, text, interpolate=interpolate_pos_encoding)
-        n = self.native(max(image.shape[0], text.shape[0]), require=True, hw=self._call_hw(image, interpolate_pos_encoding))
-        return n.dual(image, text, interpolate=interpolate_pos_encoding)
+        im = self._images(image, interpolate_pos_encoding)
+        n = self.native(max(len(im.x), text.shape[0]), require=True, hw=im.hw if interpolate_pos_encoding else None)
+        return n.dual(im, text)
 
     def set_comm(self, mode: str):
         """'peer' (default, fused NVLink peer-store kernel) | 'nccl' (torch.distributed all_gather baseline) | 'off'."""
@@ -74,10 +70,10 @@ class DualTower(_NativeOwner, nn.Module):
     def _call_distributed(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         import torch.distributed as dist
 
-        B = image.shape[0]
-        n = self.native(B, require=True, hw=self._call_hw(image, interpolate_pos_encoding))
-        x, ids = n._prep_images(image, interpolate_pos_encoding), n._prep_ids(text)
-        host_in = not x.is_cuda and not ids.is_cuda
+        im = self._images(image, interpolate_pos_encoding)
+        x, B = im.x, len(im.x)
+        n = self.native(B, require=True, hw=im.hw if interpolate_pos_encoding else None)
+        ids = n._prep_ids(text)
         with torch.cuda.device(n.device):
             cur = torch.cuda.current_stream(n.device)
             # host inputs: the ids go first (H2D copies share one engine), the images follow on a side stream and land while
@@ -92,7 +88,7 @@ class DualTower(_NativeOwner, nn.Module):
                     x_d = x.to(n.device, non_blocking=True)
             if x.is_cuda:
                 ie, te = n.dual_encode(x_d, ids_d)  # both towers concurrently (text forked onto the library's side stream)
-            elif x.dtype == torch.uint8:
+            elif im.u8:
                 # raw frames are a quarter of the bytes: take the short copy up front and run the two towers concurrently
                 cur.wait_stream(side)
                 x_d.record_stream(cur)
@@ -102,13 +98,7 @@ class DualTower(_NativeOwner, nn.Module):
                 cur.wait_stream(side)
                 x_d.record_stream(cur)
                 ie = n.vision(x_d, encode=True, interpolate=interpolate_pos_encoding)
-            out = self._distributed_logits(n, ie, te, B)
-            if not host_in:
-                return out
-            out_h = torch.empty(out.shape, dtype=torch.float32, pin_memory=True)
-            out_h.copy_(out, non_blocking=True)
-            cur.synchronize()
-            return out_h
+            return n._back(self._distributed_logits(n, ie, te, B), im.host and not ids.is_cuda).result()
 
     def _distributed_logits(self, n, ie, te, B) -> torch.Tensor:
         import torch.distributed as dist
@@ -125,12 +115,8 @@ class DualTower(_NativeOwner, nn.Module):
         dist.all_gather_into_tensor(gathered, t_n.contiguous())
         scale = self.logit_scale.to(n.device).reshape(1)
         bias = self.logit_bias.to(n.device).reshape(1) if "logit_bias" in self._params else None
-        import ctypes as C
-
         out = torch.empty((B, world * B), dtype=torch.float32, device=n.device)
-        _lib.check(n.lib.jimm_k_logits(C.c_void_p(i_n.data_ptr()), C.c_void_p(gathered.data_ptr()), C.c_void_p(scale.data_ptr()),
-                                       C.c_void_p(bias.data_ptr()) if bias is not None else None, C.c_void_p(out.data_ptr()), B,
-                                       world * B, t_n.shape[1], world * B, C.c_void_p(torch.cuda.current_stream(n.device).cuda_stream)))
+        _call(n.lib, n.device, "jimm_k_logits", i_n, gathered, scale, bias, out, B, world * B, t_n.shape[1], world * B)
         return out
 
 

@@ -11,7 +11,6 @@ from .. import _lib, nn
 from ..common.transformer import g_wrap
 from ..common import hf_loader as L
 from ..common.utils import load_params_and_config
-from .._runtime import PendingResult
 from ..common.vit import VisionTransformerBase, _NativeOwner, tower_config_fields
 
 
@@ -51,18 +50,13 @@ class VisionTransformer(_NativeOwner, nn.Module):
         keyword): images of any size of at least one patch, the position embeddings resampled bicubically to the patch grid.  A
         list / tuple of images [H_i, W_i, C] (or [1, H_i, W_i, C]) of different sizes runs in one packed call; row i is the result of
         x[i] alone."""
-        if isinstance(x, (list, tuple)):
-            return self._vision_list(x, interpolate_pos_encoding)
-        return self.native(x.shape[0], hw=self._call_hw(x, interpolate_pos_encoding)).vision(x, interpolate=interpolate_pos_encoding)
+        return self._vision(x, interpolate_pos_encoding)
 
     def forward_async(self, x, interpolate_pos_encoding: bool = False):
         """Asynchronous dispatch for host inputs (JAX dispatches asynchronously; examples/vit_inference.py:54-58 only blocks when
         it reads the logits): returns a `PendingResult`; back-to-back calls overlap their H2D copies with the previous forward.  A
         list of images runs as in __call__, synchronously for host images."""
-        if isinstance(x, (list, tuple)):
-            return PendingResult(self._vision_list(x, interpolate_pos_encoding), None)
-        n = self.native(x.shape[0], hw=self._call_hw(x, interpolate_pos_encoding))
-        return n.vision_async(x, interpolate=interpolate_pos_encoding)
+        return self._vision(x, interpolate_pos_encoding, wait=False)
 
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "VisionTransformer":
