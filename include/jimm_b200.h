@@ -149,6 +149,14 @@ JIMM_API int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype
  * eagerly and return without synchronising; back-to-back calls on one stream are safe. */
 JIMM_API int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
 JIMM_API int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
+/* B token sequences of different lengths in one jimm_encode_text call.  ids: device int32, the B sequences one after another; len: host
+ * int array [B], read during the call, every length in 1 .. ctx_len; out: device fp32 [B, E].  Row i equals jimm_encode_text on sequence
+ * i alone (T = len[i]): positions restart at 0 in every sequence, CLIP's causal mask and EOT argmax are taken within it, SigLIP pools its
+ * last token.  (For CLIP that is also the row of a padded call whenever sequence i is that row cut just after its first maximum id.)
+ * The tokens of consecutive sequences are packed into one stream (variable-length attention); a chunk takes the sequences in order while
+ * their tokens fit max_batch x ctx_len rows, up to 65535 sequences.  A bad length, a null argument or a model without a text tower is
+ * JIMM_EINVAL before anything is enqueued.  Runs eagerly and returns without synchronising; back-to-back calls on one stream are safe. */
+JIMM_API int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, float* out, void* stream);
 
 /* -- forward of a bare sub-module (kinds JIMM_ENCODER / JIMM_MAPHEAD; config fields used: v_width, v_heads, v_mlp, v_layers, v_act,
  *    v_eps_block, v_eps_outer, t_causal (attn_mask = tril), ctx_len = max tokens per sample, compute_dtype; parameters keyed
@@ -254,6 +262,10 @@ JIMM_API int jimm_k_attention_packed(const void* qkv, int io_type, void* out, in
                                      int head_dim, int reverse, void* stream);
 JIMM_API int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B,
                                          int max_S, int H, int head_dim, void* stream);
+/* jimm_k_attention_packed with a causal mask when causal != 0 (key <= query, counted from each sample's first row); jimm_k_attention_packed
+ * is this call with causal = 0.  Each sample's rows are the bits of jimm_k_attention_hd(..., causal, ...) on that sample alone. */
+JIMM_API int jimm_k_attention_packed_ex(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H,
+                                        int head_dim, int causal, int reverse, void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
 /* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left
  * untouched) and ldk (row stride in elements, 0 = P*P*C; more = pad columns, written as zeros). */
@@ -266,6 +278,10 @@ JIMM_API int jimm_k_activation(const float* x, float* y, long long n, int act, v
  * jimm_vit_forward_hw (pos fp32 [(1 +) g*g, D]); D a multiple of 4.  (gh, gw) == (g, g) gives the table itself, bit for bit. */
 JIMM_API int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream);
 JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream);
+/* jimm_k_embed on B sequences packed as for jimm_k_attention_packed (seq_off device int32 [B + 1], T_total = seq_off[B] rows of ids and
+ * x): x[r] = table[clamp(ids[r], 0, vocab - 1)] + pos[r - seq_off[b]] for the rows r of sequence b, whose positions restart at 0. */
+JIMM_API int jimm_k_embed_packed(const int32_t* ids, const float* table, const float* pos, float* x, const int32_t* seq_off, int B, int T_total,
+                                 int D, int vocab, void* stream);
 JIMM_API int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream);
 JIMM_API int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
                   int E, int ldl, void* stream);

@@ -74,6 +74,7 @@ SIGNATURES = {
     "jimm_dual_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _i, _i, _fp, _vp]),
     "jimm_vit_forward_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
     "jimm_encode_image_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
+    "jimm_encode_text_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -102,11 +103,13 @@ SIGNATURES = {
     "jimm_k_map_attention_hd": (_i, [_fp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_attention_packed": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention_packed": (_i, [_fp, _vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _vp]),
+    "jimm_k_attention_packed_ex": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),
     "jimm_k_tokens_init_interp": (_i, [_fp, _fp, _i, _i, _fp, _i, _i, _i, _vp]),
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
+    "jimm_k_embed_packed": (_i, [_ip, _fp, _fp, _fp, _ip, _i, _i, _i, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),
     "jimm_k_logits": (_i, [_fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_upload_rows": (_i, [_vp, _i, C.c_longlong, C.c_longlong, _vp, _i, C.c_longlong, _vp]),

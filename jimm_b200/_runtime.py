@@ -99,6 +99,41 @@ def prep_images(images, cfg: _lib.Config, preproc, interpolate: bool) -> Images:
     return Images(xs, not xs or not xs[0].is_cuda, bool(xs) and xs[0].dtype == torch.uint8, hw, hw == (cfg.img_size, cfg.img_size))
 
 
+class Texts(NamedTuple):
+    """The token sequences of one text call on a list, checked and concatenated once (prep_texts)."""
+
+    ids: torch.Tensor  # int32 [sum of the lengths]: the sequences one after another, on the device they came from
+    lens: List[int]
+    host: bool  # host memory: the result goes back to the host
+
+
+def prep_texts(texts, context_length: int) -> Texts:
+    """The input step of a text call on a list / tuple of token sequences of different lengths: each a 1-D (or [1, L]) integer torch
+    tensor (CUDA or host), numpy array or Python list of ints, 1 <= L <= context_length, all on one device.  They are concatenated
+    into one int32 tensor on that device, so host input crosses to the GPU in one copy."""
+    # A zero-shot classifier passes tens of thousands of short prompts: the per-sequence work stays in Python attribute reads, and the
+    # concatenation and the cast to int32 are one operation each for the whole list.
+    xs, lens = [], []
+    for i, t in enumerate(texts):
+        t = _as_tensor(t)
+        if t.ndim == 2 and t.shape[0] == 1:
+            t = t[0]
+        if t.ndim != 1:
+            raise ValueError(f"sequence {i} of the list: expected token ids of shape [length] or [1, length], got {tuple(t.shape)}")
+        n = t.shape[0]
+        if not 1 <= n <= context_length:
+            raise ValueError(f"sequence {i} of the list: length {n} outside 1 .. context_length={context_length}")
+        xs.append(t)
+        lens.append(int(n))
+    for i, t in enumerate(xs):
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise ValueError(f"sequence {i} of the list: token ids must be integers, got {t.dtype}")
+    if len({x.device for x in xs}) > 1:
+        raise ValueError(f"the sequences of a list must be on one device, got {sorted({str(x.device) for x in xs})}")
+    ids = torch.cat(xs).to(torch.int32) if xs else torch.empty(0, dtype=torch.int32)
+    return Texts(ids.contiguous(), lens, not ids.is_cuda)
+
+
 class PendingResult:
     """Result of an asynchronously dispatched forward: `.result()` waits for that call's work only."""
 
@@ -258,8 +293,28 @@ class NativeModel:
             self._run("jimm_encode_image_hw" if encode else "jimm_vit_forward_hw", xd, xd.dtype, B, xd.shape[1], xd.shape[2], out)
         return out
 
+    def _texts(self, text) -> Union[torch.Tensor, Texts]:
+        """The text input of a call: Texts for a list / tuple of sequences (or Texts already), else the [B, T] ids tensor."""
+        if isinstance(text, Texts):
+            return text
+        if isinstance(text, (list, tuple)):
+            return prep_texts(text, self.cfg.ctx_len)
+        return self._prep_ids(text)
+
+    def _text_packed_dev(self, tx: Texts) -> torch.Tensor:
+        """encode_text of the sequences of a list in one packed call (jimm_encode_text_packed): fp32 [B, E] on this GPU."""
+        B = len(tx.lens)
+        out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
+        if B:
+            self._run("jimm_encode_text_packed", tx.ids.to(self.device, non_blocking=True), B, (C.c_int * B)(*tx.lens), out)
+        return out
+
     def text(self, ids) -> torch.Tensor:
-        ids = self._prep_ids(ids)
+        """encode_text of a [B, T] ids tensor, or of a list of sequences of different lengths (one packed call).  CUDA input -> CUDA
+        output; host input -> host output."""
+        ids = self._texts(ids)
+        if isinstance(ids, Texts):
+            return self._back(self._text_packed_dev(ids), ids.host).result()
         B, T = ids.shape
         out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
         self._run("jimm_encode_text", ids.to(self.device, non_blocking=True), B, T, out)
@@ -284,10 +339,14 @@ class NativeModel:
         return out
 
     def dual(self, images, text, interpolate: bool = False) -> torch.Tensor:
-        """CLIP.__call__ / SigLIP.__call__ on one GPU, on Images or on a tensor / list prepared here.  The result is on the host
-        when the images and the ids were."""
+        """CLIP.__call__ / SigLIP.__call__ on one GPU, on Images or on a tensor / list prepared here, and on a [B, T] ids tensor or a
+        list of token sequences (Texts).  The result is on the host when the images and the ids were.  A list of sequences runs the
+        vision call, the packed text call and the logits one after another on the current stream."""
         im = images if isinstance(images, Images) else prep_images(images, self.cfg, self.preproc, interpolate)
-        ids = self._prep_ids(text)
+        ids = self._texts(text)
+        if isinstance(ids, Texts):
+            out = self.logits(self._vision_dev(im, True), self._text_packed_dev(ids))
+            return self._back(out, im.host and ids.host).result()
         host = im.host and not ids.is_cuda
         Bi, (Bt, T) = len(im.x), ids.shape
         if isinstance(im.x, list):

@@ -338,9 +338,11 @@ static int attn_launch_causal(const void* qkv, void* out, int B, int S, int H, i
   }
 }
 
-// the packed form is non-causal only
+// Packed and causal: the query tile, the key count n_kv and the mask are all relative to the sample's first row (row0), so each sample is
+// masked as it is alone.
 template <typename T, typename OutT>
 static int attn_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, int reverse, const int* seq_off) {
+  if (seq_off && causal) return attn_launch_causal<T, OutT, true, true>(qkv, out, B, S, H, d, stream, reverse, seq_off);
   if (seq_off) return attn_launch_causal<T, OutT, false, true>(qkv, out, B, S, H, d, stream, reverse, seq_off);
   if (causal) return attn_launch_causal<T, OutT, true, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
   return attn_launch_causal<T, OutT, false, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
@@ -367,9 +369,9 @@ int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, 
 }
 
 int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H, int head_dim,
-                         cudaStream_t stream, int reverse) {
+                         int causal, cudaStream_t stream, int reverse) {
   if (!seq_off) { set_last_error("attention_packed: null seq_off"); return -1; }
-  return attn_dispatch(qkv, io_type, out, out_type, B, max_S, H, head_dim, 0, stream, reverse, seq_off);
+  return attn_dispatch(qkv, io_type, out, out_type, B, max_S, H, head_dim, causal, stream, reverse, seq_off);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -410,21 +410,26 @@ int cls_row_run(float* x, const float* cls, const float* pos, int B, int S, int 
 }
 
 // ------------------------------------------------------------------------------------------
+// x[r, :] = table[clamp(ids[r]), :] + pos[t, :] by one warp
+__device__ __forceinline__ void embed_row(const int32_t* __restrict__ ids, const float* __restrict__ table, const float* __restrict__ pos,
+                                          float* __restrict__ x, int r, int t, int D4, int vocab, int lane) {
+  int id = ids[r];
+  id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);  // jnp take clamps out-of-range indices
+  const float4* e = reinterpret_cast<const float4*>(table) + static_cast<size_t>(id) * D4;
+  const float4* p = reinterpret_cast<const float4*>(pos) + static_cast<size_t>(t) * D4;
+  float4* o = reinterpret_cast<float4*>(x) + static_cast<size_t>(r) * D4;
+  for (int i = lane; i < D4; i += 32) {
+    const float4 a = __ldg(e + i), b = __ldg(p + i);
+    o[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
 __global__ void __launch_bounds__(256)
 embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ table, const float* __restrict__ pos, float* __restrict__ x,
              int rows, int T, int D4, int vocab) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= rows) return;
-  int id = ids[warp];
-  id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);  // jnp take clamps out-of-range indices
-  const int t = warp % T;
-  const float4* e = reinterpret_cast<const float4*>(table) + static_cast<size_t>(id) * D4;
-  const float4* p = reinterpret_cast<const float4*>(pos) + static_cast<size_t>(t) * D4;
-  float4* o = reinterpret_cast<float4*>(x) + static_cast<size_t>(warp) * D4;
-  for (int i = lane; i < D4; i += 32) {
-    const float4 a = __ldg(e + i), b = __ldg(p + i);
-    o[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-  }
+  embed_row(ids, table, pos, x, warp, warp % T, D4, vocab, lane);
 }
 int embed_run(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, cudaStream_t stream) {
   if (D % 4 != 0) { set_last_error("embed: D must be a multiple of 4"); return -1; }
@@ -435,24 +440,68 @@ int embed_run(const int32_t* ids, const float* table, const float* pos, float* x
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------
-__global__ void argmax_ids_kernel(const int32_t* __restrict__ ids, int* __restrict__ idx, int B, int T) {
+// one warp per row; the row's sequence is the last b with seq_off[b] <= row (binary search over the B + 1 offsets)
+__global__ void __launch_bounds__(256)
+embed_packed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ table, const float* __restrict__ pos, float* __restrict__ x,
+                    const int* __restrict__ seq_off, int B, int rows, int D4, int vocab) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp >= B) return;
+  if (warp >= rows) return;
+  int lo = 0, hi = B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (seq_off[mid] <= warp) lo = mid;
+    else hi = mid - 1;
+  }
+  embed_row(ids, table, pos, x, warp, warp - seq_off[lo], D4, vocab, lane);
+}
+int embed_packed_run(const int32_t* ids, const float* table, const float* pos, float* x, const int* seq_off, int B, int rows, int D, int vocab,
+                     cudaStream_t stream) {
+  if (D % 4 != 0) { set_last_error("embed_packed: D must be a multiple of 4"); return -1; }
+  if (B <= 0 || rows <= 0) return 0;
+  if (!seq_off) { set_last_error("embed_packed: null seq_off"); return -1; }
+  embed_packed_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(ids, table, pos, x, seq_off, B, rows, D / 4, vocab);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// first argmax of ids[0 .. T-1] by one warp: the largest id, the lowest position among equal ones
+__device__ __forceinline__ int warp_argmax_ids(const int32_t* __restrict__ ids, int T, int lane) {
   int best = INT_MIN, bi = 0x7fffffff;
   for (int t = lane; t < T; t += 32) {
-    const int v = ids[static_cast<size_t>(warp) * T + t];
+    const int v = ids[t];
     if (v > best) { best = v; bi = t; }
   }
   for (int o = 16; o > 0; o >>= 1) {
     const int ob = __shfl_xor_sync(0xffffffffu, best, o), oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
   }
+  return bi;
+}
+
+__global__ void argmax_ids_kernel(const int32_t* __restrict__ ids, int* __restrict__ idx, int B, int T) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B) return;
+  const int bi = warp_argmax_ids(ids + static_cast<size_t>(warp) * T, T, lane);
   if (lane == 0) idx[warp] = bi;
 }
 int argmax_ids_run(const int32_t* ids, int* idx, int B, int T, cudaStream_t stream) {
   if (B <= 0) return 0;
   argmax_ids_kernel<<<(B + 7) / 8, 256, 0, stream>>>(ids, idx, B, T);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+__global__ void argmax_ids_packed_kernel(const int32_t* __restrict__ ids, const int* __restrict__ seq_off, int* __restrict__ row, int B) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B) return;
+  const int r0 = seq_off[warp];
+  const int bi = warp_argmax_ids(ids + r0, seq_off[warp + 1] - r0, lane);
+  if (lane == 0) row[warp] = r0 + bi;
+}
+int argmax_ids_packed_run(const int32_t* ids, const int* seq_off, int* row, int B, cudaStream_t stream) {
+  if (B <= 0) return 0;
+  argmax_ids_packed_kernel<<<(B + 7) / 8, 256, 0, stream>>>(ids, seq_off, row, B);
   JIMM_LAUNCH_CHECK();
   return 0;
 }

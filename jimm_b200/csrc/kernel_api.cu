@@ -105,9 +105,13 @@ int jimm_k_attention(const void* qkv, int io_type, void* out, int out_type, int 
 int jimm_k_map_attention_hd(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, void* stream) {
   return map_attention_run(q, kv, io_type, out, out_type, B, S, H, head_dim, static_cast<cudaStream_t>(stream));
 }
+int jimm_k_attention_packed_ex(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H,
+                               int head_dim, int causal, int reverse, void* stream) {
+  return attention_packed_run(qkv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, causal, static_cast<cudaStream_t>(stream), reverse);
+}
 int jimm_k_attention_packed(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H, int head_dim,
                             int reverse, void* stream) {
-  return attention_packed_run(qkv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream), reverse);
+  return jimm_k_attention_packed_ex(qkv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, 0, reverse, stream);
 }
 int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S,
                                 int H, int head_dim, void* stream) {
@@ -132,6 +136,10 @@ int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, 
 }
 int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream) {
   return embed_run(ids, table, pos, x, B, T, D, vocab, static_cast<cudaStream_t>(stream));
+}
+int jimm_k_embed_packed(const int32_t* ids, const float* table, const float* pos, float* x, const int32_t* seq_off, int B, int T_total, int D,
+                        int vocab, void* stream) {
+  return embed_packed_run(ids, table, pos, x, seq_off, B, T_total, D, vocab, static_cast<cudaStream_t>(stream));
 }
 int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream) {
   return l2_normalize_run(x, out, ldo, B, E, static_cast<cudaStream_t>(stream));

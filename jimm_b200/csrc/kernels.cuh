@@ -50,8 +50,15 @@ int cls_row_run(float* x, const float* cls, const float* pos, int B, int S, int 
 // x[b,t,:] = table[ids[b,t], :] + pos[t, :]   (models/clip.py:159-160, models/siglip.py:146-147)
 int embed_run(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, cudaStream_t stream);
 
+// Packed form of embed_run for B sequences of different lengths: sequence b is rows seq_off[b] .. seq_off[b + 1] - 1 of ids / x
+// (seq_off: device int32 [B + 1], rows = seq_off[B]), its positions restart at 0: x[r, :] = table[ids[r], :] + pos[r - seq_off[b], :].
+int embed_packed_run(const int32_t* ids, const float* table, const float* pos, float* x, const int* seq_off, int B, int rows, int D, int vocab,
+                     cudaStream_t stream);
+
 // idx[b] = first argmax_t ids[b, t]    (models/clip.py:164)
 int argmax_ids_run(const int32_t* ids, int* idx, int B, int T, cudaStream_t stream);
+// Packed form over the sequences of embed_packed_run: row[b] = seq_off[b] + first argmax_t ids[seq_off[b] + t] (an absolute row)
+int argmax_ids_packed_run(const int32_t* ids, const int* seq_off, int* row, int B, cudaStream_t stream);
 
 // rows /= ||row||_2  (no epsilon; models/clip.py:183-184), fp32 [B,E] -> out (row stride ldo)
 int l2_normalize_run(const float* x, float* out, int ldo, int B, int E, cudaStream_t stream);
@@ -100,10 +107,10 @@ int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, 
                   int reverse = 0);
 
 // attention_run over B samples of different lengths packed into one [rows, 3D] qkv / [rows, D] out: sample b is rows seq_off[b] ..
-// seq_off[b + 1] - 1 (seq_off: device int32 [B + 1]), max_S >= every length.  Non-causal; each sample's rows are the bits
-// attention_run gives on that sample alone.
+// seq_off[b + 1] - 1 (seq_off: device int32 [B + 1]), max_S >= every length.  causal: key <= query within each sample.  Each sample's
+// rows are the bits attention_run gives on that sample alone.
 int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H, int head_dim,
-                         cudaStream_t stream, int reverse = 0);
+                         int causal, cudaStream_t stream, int reverse = 0);
 
 // MAP-head attention with a single (input-independent) probe query (common/vit.py:96-97).
 //   q: fp32 [H*d] (already projected + biased), kv: [B*S, 2D] (k | v) io_type, out [B, D] out_type; d as attention_run

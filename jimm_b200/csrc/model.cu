@@ -175,6 +175,7 @@ struct TextTower {
   LNW ln_final;
   LinearW head;  // text_projection
   GemmPlan p_head;
+  GemmPlan p_head_packed;  // packed calls (jimm_encode_text_packed): the pooled rows of up to TextWs::pk_seqs sequences, read from enc.h
 };
 
 struct EncBufs {  // the activation buffers one encoder stack works in, for `rows` rows of width D (alloc_stack)
@@ -193,6 +194,11 @@ struct TextWs {
   EncBufs enc;            // [Bmax*T, Dt]
   void* pooled = nullptr; // [Bmax, Dt]
   int* idx = nullptr;     // [Bmax] EOT positions
+  // packed calls: int32 token offsets [pk_seqs + 1] and pooled rows [pk_seqs] of the sequences of a chunk.  A chunk holds as many
+  // sequences as fit the Bmax*T token rows, up to the attention grid's 65535 samples.  Apart from ws.pk_meta, so that a packed text call
+  // on the text side stream may overlap a packed image call.
+  int* pk_meta = nullptr;
+  int pk_seqs = 0;
 };
 
 struct Workspace {
@@ -628,7 +634,7 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   for (BlockW& b : enc->blocks) {
     if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
     JIMM_TRY(run_gemm(m, b.p_qkv, ln_h, c.D, b.qkv, T, s, flip()));
-    if (pk) JIMM_TRY(attention_packed_run(ws.big, m->adt, ws.h, m->cdt, pk->seq_off, B, pk->max_S, c.H, c.D / c.H, s, flip()));
+    if (pk) JIMM_TRY(attention_packed_run(ws.big, m->adt, ws.h, m->cdt, pk->seq_off, B, pk->max_S, c.H, c.D / c.H, c.causal, s, flip()));
     else JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_out, ws.h, c.D, b.out, T, s, flip()));  // + residual (+ norm2 -> ws.h when fused)
     if (m->simt || !gemm_fuses_ln(&b.p_out, T))
@@ -750,6 +756,31 @@ static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out,
   p.epi.out = out;
   JIMM_TRY(run_gemm(m, p, ws.pooled, t.D, t.head, B, s));
   return 0;
+}
+
+// run_text on B token sequences of different lengths packed into one stream: sequence b is rows tok[b] .. tok[b + 1] - 1 of ids (host
+// offsets, tok[0] = 0), max_S the longest.  Positions restart at 0 in every sequence and the causal mask (CLIP) is taken within it; every
+// other kernel works row by row, so row b of out is the bits run_text gives on sequence b alone.
+static int run_text_packed(jimm_model* m, const int32_t* ids, int B, const int* tok, int max_S, float* out, cudaStream_t s) {
+  TextTower& t = m->txt;
+  TextWs& ws = m->wt;
+  // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
+  // on this stream has read its own offsets before this copy lands.  The pooled rows follow them: each sequence's last row (SigLIP's
+  // last-token pooling); CLIP's EOT rows overwrite them on the device.
+  std::vector<int> meta(2 * static_cast<size_t>(B) + 1);
+  for (int b = 0; b <= B; ++b) meta[b] = tok[b];
+  for (int b = 0; b < B; ++b) meta[B + 1 + b] = tok[b + 1] - 1;
+  JIMM_CUDA_CHECK(cudaMemcpyAsync(ws.pk_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  const PackedRows pk{ws.pk_meta, tok[B], max_S};
+  int* rows = ws.pk_meta + B + 1;
+  JIMM_TRY(embed_packed_run(ids, t.table, t.pos, ws.enc.x, pk.seq_off, B, pk.T, t.D, t.V, s));
+  JIMM_TRY(run_encoder(m, &t.enc, B, 0, s, ws.enc, &pk));
+  if (t.pool == JIMM_TPOOL_EOT_ARGMAX) JIMM_TRY(argmax_ids_packed_run(ids, pk.seq_off, rows, B, s));
+  // ln_final of the pooled rows only (group 0: the rows by index), into ws.enc.h -- free once the encoder has run -- for the head GEMM
+  JIMM_TRY(layernorm_run(ws.enc.x, t.D, 0, 0, rows, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.enc.h, m->cdt, t.D, B, t.D, s));
+  GemmPlan p = t.p_head_packed;
+  p.epi.out = out;
+  return run_gemm(m, p, ws.enc.h, t.D, t.head, B, s);
 }
 
 static int check_ready(const jimm_model* m, int B) {
@@ -1166,6 +1197,8 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
     JIMM_TRY(m->pool.alloc(&m->wt.pooled, Bm * t.D * cs));
     JIMM_TRY(m->pool.alloc(&m->wt.idx, Bm * sizeof(int)));
     JIMM_TRY(m->pool.alloc(&ws.in_ids, Bm * t.T * sizeof(int32_t)));
+    m->wt.pk_seqs = static_cast<int>(std::min<size_t>(Tt, 65535));  // one token each at most; the attention grid's z limit
+    JIMM_TRY(m->pool.alloc(&m->wt.pk_meta, (2 * static_cast<size_t>(m->wt.pk_seqs) + 1) * sizeof(int)));
   }
   JIMM_TRY(m->pool.alloc(&ws.emb_i, Bm * E * sizeof(float)));
   JIMM_TRY(m->pool.alloc(&ws.emb_t, Bm * E * sizeof(float)));
@@ -1195,6 +1228,8 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   if (dual) {
     JIMM_TRY(plan_encoder(m, &t.enc, static_cast<int>(Bm) * t.T, m->wt.enc));
     JIMM_TRY(gemm_plan_init(&t.p_head, m->cdt, m->wt.pooled, t.D, t.head.w, t.D, static_cast<int>(Bm), t.D, t.D,
+                            epi_plain(t.head, ACT_NONE, ws.out_dev, DT_F32, t.D, 0)));
+    JIMM_TRY(gemm_plan_init(&t.p_head_packed, m->cdt, m->wt.enc.h, t.D, t.head.w, t.D, m->wt.pk_seqs, t.D, t.D,
                             epi_plain(t.head, ACT_NONE, ws.out_dev, DT_F32, t.D, 0)));
   }
   JIMM_CUDA_CHECK(cudaDeviceSynchronize());
@@ -1362,6 +1397,28 @@ static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* o
   });
 }
 
+// B token sequences of lengths len[b] (ids: their concatenation): chunks of consecutive sequences, each as many as the text workspace's
+// max_batch x context_length token rows hold (at most pk_seqs), run packed.  The chunks are cut by tokens, not by sequences: short
+// prompts fill a chunk with several times max_batch sequences, and its GEMMs with as many rows as a padded call of max_batch.
+static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s) {
+  const int budget = m->max_batch * m->txt.T;
+  std::vector<int> tok;
+  size_t r0 = 0;  // the chunk's first row of ids
+  for (int b0 = 0; b0 < B;) {
+    tok.assign(1, 0);
+    int b1 = b0, max_S = 0;
+    while (b1 < B && b1 - b0 < m->wt.pk_seqs && tok.back() + len[b1] <= budget) {
+      tok.push_back(tok.back() + len[b1]);
+      max_S = std::max(max_S, len[b1]);
+      ++b1;
+    }
+    JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, out + static_cast<size_t>(b0) * m->txt.D, s));
+    r0 += tok.back();
+    b0 = b1;
+  }
+  return 0;
+}
+
 // The jimm_vit_forward* (vit_fn: its name) and jimm_encode_image* calls on device images
 static int encode_images(jimm_model* m, const char* vit_fn, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
   JIMM_TRY(check_ready(m, B));
@@ -1414,6 +1471,20 @@ int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* o
   JIMM_TRY(check_text_len(m, T));
   JIMM_TRY(set_device(m));
   return text_chunks(m, ids, B, T, out, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_text(m));
+  if (B > 0 && (!ids || !len || !out)) { set_last_error("jimm_encode_text_packed: null argument"); return JIMM_EINVAL; }
+  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
+    if (len[b] <= 0 || len[b] > m->txt.T) {
+      set_last_error("sequence %d: length %d outside (0, context_length=%d]", b, len[b], m->txt.T);
+      return JIMM_EINVAL;
+    }
+  }
+  JIMM_TRY(set_device(m));
+  return text_packed(m, ids, B, len, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const float* txt_e, int Bt, float* logits, void* stream) {

@@ -5,7 +5,7 @@ from __future__ import annotations
 import torch
 
 from .. import _lib, nn
-from .._runtime import _call
+from .._runtime import Texts, _call, prep_texts
 from ..common.transformer import Transformer, g_wrap
 from ..common.vit import _NativeOwner, tower_config_fields
 
@@ -42,22 +42,37 @@ class DualTower(_NativeOwner, nn.Module):
         embedding of image[i] alone."""
         return self._vision(image, interpolate_pos_encoding, encode=True)
 
+    def _texts(self, text):
+        """The text input step (prep_texts) for a list / tuple of token sequences, before any handle is built; a tensor as it is."""
+        return prep_texts(text, self.context_length) if isinstance(text, (list, tuple)) else text
+
     def encode_text(self, text) -> torch.Tensor:
-        return self.native(text.shape[0]).text(text)
+        """[B, T] token ids -> [B, E].  A list / tuple of token sequences of different lengths (each 1-D or [1, L], a tensor, numpy
+        array or list of ints, 1 <= L <= context_length) runs in one packed call that skips the padding: row i is
+        encode_text(text[i][None]), the call at T = len(text[i]).  For CLIP that is also the row of the padded call when text[i] is the
+        padded row cut just after its EOT (its first maximum id): nothing after the EOT reaches the pooled token.  SigLIP pools the last
+        token, so a list gives each sequence at its own length, not the padded embedding its checkpoint was trained on."""
+        text = self._texts(text)
+        return self.native().text(text) if isinstance(text, Texts) else self.native(text.shape[0]).text(text)
 
     def __call__(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """Similarity logits.  Single process: [B_img, B_txt].  Under torch.distributed (one process per GPU, batch sharded
         over ranks like the reference's P("batch") inputs, examples/clip_inference.py:41-42): this rank's row block
         [B_local, world*B_local], embeddings exchanged over NVLink peer memory inside the fused logits kernel.
-        interpolate_pos_encoding: as in encode_image.  `image` may be a list of images of different sizes (single process only)."""
+        interpolate_pos_encoding: as in encode_image.  `image` may be a list of images of different sizes and `text` a list of token
+        sequences of different lengths, as in encode_text (single process only)."""
         import torch.distributed as dist
 
         if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and self._comm_mode != "off":
             if isinstance(image, (list, tuple)):
                 raise ValueError("a list of images is not supported by the multi-GPU contrastive call; pass one [B, H, W, C] tensor per rank")
+            if isinstance(text, (list, tuple)):
+                raise ValueError("a list of token sequences is not supported by the multi-GPU contrastive call; pass one [B, T] tensor per rank")
             return self._call_distributed(image, text, interpolate_pos_encoding)
         im = self._images(image, interpolate_pos_encoding)
-        n = self.native(max(len(im.x), text.shape[0]), require=True, hw=im.hw if interpolate_pos_encoding else None)
+        text = self._texts(text)
+        Bt = len(text.lens) if isinstance(text, Texts) else text.shape[0]
+        n = self.native(max(len(im.x), Bt), require=True, hw=im.hw if interpolate_pos_encoding else None)
         return n.dual(im, text)
 
     def set_comm(self, mode: str):
