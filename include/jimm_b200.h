@@ -313,12 +313,20 @@ typedef struct jimm_preproc_config {
   float mean[3], std[3];    /* image_mean, image_std */
 } jimm_preproc_config_t;
 JIMM_API int jimm_preproc_create(const jimm_preproc_config_t* cfg, int device, jimm_preproc_t** out);
+/* Output size of H x W frames.  Refuses (JIMM_EINVAL) exactly the sizes jimm_preproc_run refuses: frames of H x W x 3 >= 2^31 bytes,
+ * a resized image (before the crop) of more than 2^24 pixels per edge, a crop larger than the resized image. */
 JIMM_API int jimm_preproc_output_size(const jimm_preproc_t* p, int H, int W, int* out_h, int* out_w);
-/* img: device uint8 [B,H,W,3] (same-sized RGB images); out: device [B,out_h,out_w,3] of out_dtype (JIMM_F32 | JIMM_F16 | JIMM_BF16). */
+/* img: device uint8 [B,H,W,3] (same-sized RGB images); out: device [B,out_h,out_w,3] of out_dtype (JIMM_F32 | JIMM_F16 | JIMM_BF16),
+ * aligned to four samples (16 bytes for JIMM_F32, 8 for the 16-bit types; JIMM_EINVAL otherwise).
+ * Sizes whose one-kernel plan does not fit in shared memory (4K, 12 MP, 8K frames into the bicubic front-ends) run in two passes
+ * through an 8-bit intermediate allocated in stream order per call, at most 64 MB per chunk of images; same bytes. */
 JIMM_API int jimm_preproc_run(jimm_preproc_t* p, const uint8_t* img, int B, int H, int W, void* out, int out_dtype, void* stream);
 JIMM_API int jimm_preproc_destroy(jimm_preproc_t* p);
 /* Host-only test entry: Pillow's resampling windows and 22-bit fixed-point weights for one axis. */
 JIMM_API int jimm_k_resample_coeffs(int in_size, int out_size, int resample, int* ksize, int* first, int* count, int* kk, int kk_capacity);
+/* Host-only test entry: the plan jimm_preproc_run uses for H x W frames.  path 0: one fused kernel with TY output rows per CTA, smem
+ * bytes of shared memory, chosen under shared-memory budget tier 0 / 1 / 2 (72 / 110 / 200 KB); path 1: two passes (tier -1, smem 0). */
+JIMM_API int jimm_k_preproc_plan(const jimm_preproc_config_t* cfg, int H, int W, int* path, int* tier, int* TY, long long* smem);
 /* ---- zero-shot / classification epilogue (SURVEY.md 8f.3): what the examples compute in JAX after the forward ----
  * logits: device fp32 [rows, cols] (leading dimension ld).  mode 0: probs = exp(x) / sum(exp(x)) per row, un-shifted like
  * examples/clip_inference.py:47; mode 1: probs = sigmoid(x) (SigLIP pair probabilities).  order (nullable, int32 [rows, cols]):

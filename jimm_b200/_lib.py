@@ -121,6 +121,7 @@ SIGNATURES = {
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),
     "jimm_preproc_destroy": (_i, [_vp]),
     "jimm_k_resample_coeffs": (_i, [_i, _i, _i, C.POINTER(_i), _ip, _ip, _ip, _i]),
+    "jimm_k_preproc_plan": (_i, [C.POINTER(PreprocConfig), _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_longlong)]),
 }
 
 _lib = None

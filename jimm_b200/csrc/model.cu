@@ -1677,6 +1677,15 @@ static int vit_forward_host_impl(jimm_model_t* m, const void* img_host, int in_d
   return for_chunks(B, m->max_batch, [&](int b0, int nb) {
     int sizes[jimm_model::kHostSlices];
     host_slices(m, nb, sizes, src_bytes);
+    if (pre && img_elems % 4) {
+      // the front-end writes each slice at off * img_elems floats and needs that 16 bytes aligned (8 for 16-bit outputs): with an odd
+      // image size, start every slice at a multiple of four images
+      for (int i = 0; i + 1 < jimm_model::kHostSlices && sizes[i + 1] > 0; ++i) {
+        const int r = sizes[i] % 4;
+        sizes[i] -= r;
+        sizes[i + 1] += r;
+      }
+    }
     bool same_layout = m->host_chain && m->host_chain_stream == s && m->host_chain_kind == kind;
     for (int i = 0; i < jimm_model::kHostSlices; ++i) same_layout = same_layout && sizes[i] == m->host_chain_sizes[i];
     if (!same_layout) {

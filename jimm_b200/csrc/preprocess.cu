@@ -8,11 +8,15 @@
 //      memory -- Pillow's temporary image, never written to HBM;
 //   2. the vertical pass reads that tile four bytes per thread, and each resulting 8-bit sample goes through a 768-entry
 //      table (channel, value) -> normalised float, then to the output dtype.
+// Sizes whose plan does not fit in shared memory (4K and larger frames into the bicubic front-ends) run the same two passes as two
+// kernels through an 8-bit intermediate in global memory (hpass_kernel, vpass_kernel); the planner (plan_size) is host-only.
 // All arithmetic is Pillow's: int32 fixed point with 22 fractional bits, taps and weights from the same double-precision
 // recipe, so the result is bit-exact (oracle/preprocess_oracle.py restates it and is pinned against Pillow itself).
 // HBM-bound byte work: algorithmic bytes = H*W*3 read + oh*ow*3*sizeof(out) written per image.
+#include <algorithm>
 #include <cmath>
 #include <map>
+#include <mutex>
 #include <utility>
 #include <vector>
 
@@ -61,7 +65,10 @@ struct ResampleTable {
   int smem_stride() const { return (kpad / 4) % 2 ? kpad : kpad + 4; }
 };
 
-ResampleTable make_table(int in_size, int out_size, int resample) {
+// Windows of output coordinates [begin, end) (default: all of them), stored from index 0: the front-end builds only the cropped
+// range, so its tables cost what the output needs whatever the size of the resize before the crop.
+ResampleTable make_table(int in_size, int out_size, int resample, int begin = 0, int end = -1) {
+  if (end < 0) end = out_size;
   double (*f)(double) = resample == 3 ? filter_bicubic : filter_bilinear;
   const double fsupport = resample == 3 ? 2.0 : 1.0;
   const double scale = static_cast<double>(in_size) / out_size;
@@ -70,12 +77,12 @@ ResampleTable make_table(int in_size, int out_size, int resample) {
   ResampleTable t;
   t.ksize = static_cast<int>(std::ceil(support)) * 2 + 1;
   t.kpad = (t.ksize + 3) / 4 * 4;
-  t.first.assign(out_size, 0);
-  t.count.assign(out_size, 0);
-  t.kk.assign(static_cast<size_t>(out_size) * t.ksize, 0);
+  t.first.assign(end - begin, 0);
+  t.count.assign(end - begin, 0);
+  t.kk.assign(static_cast<size_t>(end - begin) * t.ksize, 0);
   std::vector<double> w(t.ksize);
   const double ss = 1.0 / filterscale;
-  for (int xx = 0; xx < out_size; ++xx) {
+  for (int xx = begin; xx < end; ++xx) {
     const double center = 0.0 + (xx + 0.5) * scale;
     int xmin = static_cast<int>(center - support + 0.5);
     if (xmin < 0) xmin = 0;
@@ -89,11 +96,11 @@ ResampleTable make_table(int in_size, int out_size, int resample) {
     }
     for (int x = 0; x < xmax; ++x) {
       const double k = ww != 0.0 ? w[x] / ww : w[x];
-      t.kk[static_cast<size_t>(xx) * t.ksize + x] =
+      t.kk[static_cast<size_t>(xx - begin) * t.ksize + x] =
           k < 0 ? static_cast<int>(-0.5 + k * (1 << kPrecisionBits)) : static_cast<int>(0.5 + k * (1 << kPrecisionBits));
     }
-    t.first[xx] = xmin;
-    t.count[xx] = xmax;
+    t.first[xx - begin] = xmin;
+    t.count[xx - begin] = xmax;
   }
   return t;
 }
@@ -102,8 +109,8 @@ struct KernelArgs {
   const uint8_t* img;
   void* out;
   const float* lut;                    // [3][256] normalised value of an 8-bit sample
-  const int *hfirst, *hcount, *hk;     // horizontal tables, already offset to the first cropped column
-  const int *vfirst, *vcount, *vk;     // vertical tables, already offset to the first cropped row
+  const int *hfirst, *hcount, *hk;     // horizontal tables of the cropped columns
+  const int *vfirst, *vcount, *vk;     // vertical tables of the cropped rows
   int H, W, oh, ow, hks, hstride, vks;  // hks / vks: taps rounded up to a multiple of 4; hstride: row stride of hk
   int TY;                              // output rows per CTA
   int rowb;                            // bytes per tile row (ow*3 rounded up to 4)
@@ -121,6 +128,59 @@ __device__ __forceinline__ OUT to_out(float v);
 template <> __device__ __forceinline__ float to_out<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half to_out<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 to_out<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+// Vertical pass + normalise + store of output rows [yo0, yo1) of image b, from the 8-bit horizontal-pass rows in tile32 (input
+// rows from in_y0 on, rowb bytes apart): four consecutive samples per thread, four taps per step.
+template <typename OUT>
+__device__ __forceinline__ void vertical_pass(const KernelArgs& a, const uint32_t* tile32, int in_y0, int yo0, int yo1, int b) {
+  const int tid = threadIdx.x;
+  const int words = a.rowb / 4;
+  const int n_el = a.ow * 3;
+  OUT* out = static_cast<OUT*>(a.out);
+  for (int it = tid; it < (yo1 - yo0) * words; it += kThreads) {
+    const int r = it / words, wd = it - r * words;
+    const int yo = yo0 + r;
+    const uint32_t* tp = tile32 + (a.vfirst[yo] - in_y0) * words + wd;
+    const int vgroups = (a.vcount[yo] + 3) >> 2;
+    const int4* kp = reinterpret_cast<const int4*>(a.vk + static_cast<size_t>(yo) * a.vks);
+    int acc[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[j] = 1 << (kPrecisionBits - 1);
+    for (int g = 0; g < vgroups; ++g) {
+      const int4 k = __ldg(kp + g);
+      const uint32_t t0 = tp[(4 * g) * words], t1 = tp[(4 * g + 1) * words], t2 = tp[(4 * g + 2) * words], t3 = tp[(4 * g + 3) * words];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        acc[j] += static_cast<int>((t0 >> (8 * j)) & 255u) * k.x;
+        acc[j] += static_cast<int>((t1 >> (8 * j)) & 255u) * k.y;
+        acc[j] += static_cast<int>((t2 >> (8 * j)) & 255u) * k.z;
+        acc[j] += static_cast<int>((t3 >> (8 * j)) & 255u) * k.w;
+      }
+    }
+    const int e0 = wd * 4;
+    const size_t base = (static_cast<size_t>(b) * a.oh + yo) * n_el + e0;
+    OUT v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = (e0 + j) % 3;
+      v[j] = to_out<OUT>(__ldg(a.lut + c * 256 + clip8(acc[j])));
+    }
+    if (e0 + 3 < n_el && (base * sizeof(OUT)) % (4 * sizeof(OUT)) == 0) {
+      if constexpr (sizeof(OUT) == 4) {
+        *reinterpret_cast<float4*>(out + base) = make_float4(v[0], v[1], v[2], v[3]);
+      } else {
+        uint2 pk;
+        pk.x = static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[0])) | (static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[1])) << 16);
+        pk.y = static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[2])) | (static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[3])) << 16);
+        *reinterpret_cast<uint2*>(out + base) = pk;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (e0 + j < n_el) out[base + j] = v[j];
+    }
+  }
+}
 
 template <typename OUT>
 __global__ void __launch_bounds__(kThreads) preprocess_kernel(const KernelArgs a) {
@@ -205,55 +265,55 @@ __global__ void __launch_bounds__(kThreads) preprocess_kernel(const KernelArgs a
     __syncwarp();
   }
   __syncthreads();
+  vertical_pass<OUT>(a, reinterpret_cast<const uint32_t*>(tile), in_y0, yo0, yo1, b);
+}
 
-  // ---- vertical pass + normalise + store: four consecutive samples per thread, four taps per step ----
-  const int words = a.rowb / 4;
-  const int n_el = a.ow * 3;
-  const uint32_t* tile32 = reinterpret_cast<const uint32_t*>(tile);
-  OUT* out = static_cast<OUT*>(a.out);
-  for (int it = tid; it < (yo1 - yo0) * words; it += kThreads) {
-    const int r = it / words, wd = it - r * words;
-    const int yo = yo0 + r;
-    const uint32_t* tp = tile32 + (a.vfirst[yo] - in_y0) * words + wd;
-    const int vgroups = (a.vcount[yo] + 3) >> 2;
-    const int4* kp = reinterpret_cast<const int4*>(a.vk + static_cast<size_t>(yo) * a.vks);
-    int acc[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[j] = 1 << (kPrecisionBits - 1);
-    for (int g = 0; g < vgroups; ++g) {
-      const int4 k = __ldg(kp + g);
-      const uint32_t t0 = tp[(4 * g) * words], t1 = tp[(4 * g + 1) * words], t2 = tp[(4 * g + 2) * words], t3 = tp[(4 * g + 3) * words];
+// Two-pass path for sizes whose fused plan does not fit in shared memory (Resample.c's own order): the horizontal pass writes the
+// 8-bit intermediate -- the same clipped bytes the fused kernel keeps in its tile -- to global memory, one CTA per input row of one
+// image, for the cropped columns and the rows the cropped output reads only; vertical_pass then reads it from there.
+struct PassArgs {
+  KernelArgs k;
+  uint8_t* mid;  // [images][rows][rowb] bytes, plus zero-weight tap slack after the last image
+  int y0, rows;  // input rows [y0, y0 + rows) of each image
+  int b0;        // first image of this chunk: k.img and k.out stay the call's base pointers, so the vector stores' alignment
+                 // test in vertical_pass sees the absolute output index
+};
+
+__global__ void __launch_bounds__(kThreads) hpass_kernel(const PassArgs p) {
+  const KernelArgs& a = p.k;
+  const int row = blockIdx.x, b = blockIdx.y;
+  const uint8_t* src = a.img + (static_cast<size_t>(p.b0 + b) * a.H + p.y0 + row) * a.W * 3;
+  uint8_t* dst = p.mid + (static_cast<size_t>(b) * p.rows + row) * a.rowb;
+  const long long last = (a.W - 1) * 3LL;  // zero-weight taps past the window may run past the row: read its last pixel instead
+  for (int xo = threadIdx.x; xo < a.ow; xo += kThreads) {
+    const long long x0 = a.hfirst[xo] * 3LL;  // 64-bit: the padded taps may pass 2^31 in a row of nearly 2^31 bytes
+    const int hgroups = (a.hcount[xo] + 3) >> 2;
+    const int4* kp = reinterpret_cast<const int4*>(a.hk + static_cast<size_t>(xo) * a.hstride);
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    for (int g = 0; g < hgroups; ++g) {
+      const int4 k4 = __ldg(kp + g);
+      const int kw[4] = {k4.x, k4.y, k4.z, k4.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        acc[j] += static_cast<int>((t0 >> (8 * j)) & 255u) * k.x;
-        acc[j] += static_cast<int>((t1 >> (8 * j)) & 255u) * k.y;
-        acc[j] += static_cast<int>((t2 >> (8 * j)) & 255u) * k.z;
-        acc[j] += static_cast<int>((t3 >> (8 * j)) & 255u) * k.w;
+        const uint8_t* px = src + min(x0 + (4 * g + j) * 3, last);
+        a0 += static_cast<int>(__ldg(px)) * kw[j];
+        a1 += static_cast<int>(__ldg(px + 1)) * kw[j];
+        a2 += static_cast<int>(__ldg(px + 2)) * kw[j];
       }
     }
-    const int e0 = wd * 4;
-    const size_t base = (static_cast<size_t>(b) * a.oh + yo) * n_el + e0;
-    OUT v[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int c = (e0 + j) % 3;
-      v[j] = to_out<OUT>(__ldg(a.lut + c * 256 + clip8(acc[j])));
-    }
-    if (e0 + 3 < n_el && (base * sizeof(OUT)) % (4 * sizeof(OUT)) == 0) {
-      if constexpr (sizeof(OUT) == 4) {
-        *reinterpret_cast<float4*>(out + base) = make_float4(v[0], v[1], v[2], v[3]);
-      } else {
-        uint2 pk;
-        pk.x = static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[0])) | (static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[1])) << 16);
-        pk.y = static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[2])) | (static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&v[3])) << 16);
-        *reinterpret_cast<uint2*>(out + base) = pk;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (e0 + j < n_el) out[base + j] = v[j];
-    }
+    dst[xo * 3] = static_cast<uint8_t>(clip8(a0));
+    dst[xo * 3 + 1] = static_cast<uint8_t>(clip8(a1));
+    dst[xo * 3 + 2] = static_cast<uint8_t>(clip8(a2));
   }
+}
+
+template <typename OUT>
+__global__ void __launch_bounds__(kThreads) vpass_kernel(const PassArgs p) {
+  const int b = blockIdx.y;
+  const int yo0 = blockIdx.x * p.k.TY;
+  const int yo1 = min(yo0 + p.k.TY, p.k.oh);
+  const uint32_t* tile32 = reinterpret_cast<const uint32_t*>(p.mid + static_cast<size_t>(b) * p.rows * p.k.rowb);
+  vertical_pass<OUT>(p.k, tile32, p.y0, yo0, yo1, p.b0 + b);
 }
 
 struct DevTable {
@@ -261,11 +321,21 @@ struct DevTable {
   int *first = nullptr, *count = nullptr, *kk = nullptr;
 };
 
+enum { kFused = 0, kTwoPass = 1 };
+constexpr long long kMaxFrameBytes = (1LL << 31) - 1;  // H * W * 3 of one frame
+constexpr int kMaxResizedEdge = 1 << 24;               // each edge of the resized image before the crop: keeps pre-crop coordinates far inside int
+constexpr size_t kMidChunkBytes = size_t(64) << 20;    // two-pass intermediate of one chunk of images
+constexpr int kFusedImages = 65532;                   // images per fused launch
+constexpr int kTwoPassTY = 8;                          // output rows per CTA of the two-pass vertical kernel
+
 struct SizePlan {
   int rh = 0, rw = 0, top = 0, left = 0, oh = 0, ow = 0;
   DevTable h, v;
+  int path = kFused;
+  int tier = -1;  // fused: index of the shared-memory budget the plan was chosen under
   int TY = 0, tile_rows = 0, rowb = 0, stage_bytes = 0;
   size_t smem = 0;
+  int mid_y0 = 0, mid_rows = 0;  // two-pass: the input rows [mid_y0, mid_y0 + mid_rows) the cropped output reads
 };
 
 }  // namespace
@@ -277,6 +347,7 @@ struct jimm_preproc {
   jimm_preproc_config_t cfg;
   int device = 0;
   float* lut = nullptr;
+  mutable std::mutex mu;  // guards plans and allocs: one handle may be driven from several threads
   std::map<std::pair<int, int>, SizePlan> plans;
   std::vector<void*> allocs;
 };
@@ -292,12 +363,22 @@ int upload(jimm_preproc* p, const std::vector<int>& v, int** out) {
   return 0;
 }
 
-void resized_size(const jimm_preproc_config_t& c, int H, int W, int* rh, int* rw) {
-  if (!c.shortest_edge) { *rh = c.height; *rw = c.width; return; }
-  // transformers get_resize_output_image_size(size=shortest_edge, default_to_square=False)
-  const int s = W <= H ? W : H, l = W <= H ? H : W;
-  const int new_long = static_cast<int>(static_cast<double>(c.shortest_edge) * l / s);
-  if (W <= H) { *rw = c.shortest_edge; *rh = new_long; } else { *rh = c.shortest_edge; *rw = new_long; }
+int resized_size(const jimm_preproc_config_t& c, int H, int W, int* rh, int* rw) {
+  double h = c.height, w = c.width;
+  if (c.shortest_edge) {
+    // transformers get_resize_output_image_size(size=shortest_edge, default_to_square=False)
+    const int s = W <= H ? W : H, l = W <= H ? H : W;
+    const double new_long = static_cast<double>(c.shortest_edge) * l / s;
+    if (W <= H) { w = c.shortest_edge; h = new_long; } else { h = c.shortest_edge; w = new_long; }
+  }
+  if (h >= kMaxResizedEdge + 1.0 || w >= kMaxResizedEdge + 1.0) {
+    set_last_error("resize %dx%d -> %.0fx%.0f: the front-end resizes to at most %d pixels per edge before the crop", H, W, std::floor(h),
+                   std::floor(w), kMaxResizedEdge);
+    return JIMM_EINVAL;
+  }
+  *rh = static_cast<int>(h);
+  *rw = static_cast<int>(w);
+  return 0;
 }
 
 int check_cfg(const jimm_preproc_config_t* c) {
@@ -310,56 +391,97 @@ int check_cfg(const jimm_preproc_config_t* c) {
   return 0;
 }
 
-int get_plan(jimm_preproc* p, int H, int W, SizePlan** out) {
-  auto it = p->plans.find({H, W});
-  if (it != p->plans.end()) { *out = &it->second; return 0; }
+// The plan of one frame size, on the host only (jimm_preproc_output_size and the plan test hook run it without a GPU): output
+// geometry, Pillow's tables and the path.  Fused when the kernel's shared memory fits one of its budgets; otherwise two passes
+// through a global 8-bit intermediate.  A size is refused only past the limits checked here (INTEGRATION.md).
+int plan_size(const jimm_preproc_config_t& c, int H, int W, SizePlan* out, ResampleTable* th_out, ResampleTable* tv_out) {
   if (H <= 0 || W <= 0) { set_last_error("bad image size %dx%d", H, W); return JIMM_EINVAL; }
+  if (static_cast<long long>(H) * W * 3 > kMaxFrameBytes) {
+    set_last_error("frame %dx%d is %lld bytes: the front-end takes frames of at most 2^31 - 1 bytes (H x W x 3)", H, W,
+                   static_cast<long long>(H) * W * 3);
+    return JIMM_EINVAL;
+  }
   SizePlan s;
-  resized_size(p->cfg, H, W, &s.rh, &s.rw);
-  s.oh = p->cfg.crop_h ? p->cfg.crop_h : s.rh;
-  s.ow = p->cfg.crop_w ? p->cfg.crop_w : s.rw;
+  JIMM_TRY(resized_size(c, H, W, &s.rh, &s.rw));
+  s.oh = c.crop_h ? c.crop_h : s.rh;
+  s.ow = c.crop_w ? c.crop_w : s.rw;
   if (s.oh > s.rh || s.ow > s.rw) {
     set_last_error("centre crop %dx%d larger than the resized image %dx%d", s.oh, s.ow, s.rh, s.rw);
     return JIMM_EINVAL;
   }
   s.top = (s.rh - s.oh) / 2;
   s.left = (s.rw - s.ow) / 2;
-  ResampleTable th = make_table(W, s.rw, p->cfg.resample), tv = make_table(H, s.rh, p->cfg.resample);
+  ResampleTable& th = *th_out;
+  ResampleTable& tv = *tv_out;
+  th = make_table(W, s.rw, c.resample, s.left, s.left + s.ow);
+  tv = make_table(H, s.rh, c.resample, s.top, s.top + s.oh);
   s.h.ksize = th.kpad;
   s.h.stride = th.smem_stride();
   s.v.ksize = s.v.stride = tv.kpad;
+  s.rowb = (s.ow * 3 + 3) / 4 * 4;
+  // fused: one warp's row buffer holds a whole input row, and a window descriptor packs its four-tap group count in 7 bits
+  const size_t row_bytes = static_cast<size_t>(W) * 3;
+  int hgroups = 0;
+  for (int xo = 0; xo < s.ow; ++xo) hgroups = std::max(hgroups, (th.count[xo] + 3) >> 2);
+  if (row_bytes + 3 * th.kpad + 48 <= 64 * 1024 && hgroups < 128) {
+    // shared-memory budget: horizontal tables for the cropped columns + staging group + 8-bit tile
+    const size_t tables = (static_cast<size_t>(s.ow) * s.h.stride + s.ow) * sizeof(int) + 16;
+    s.stage_bytes = static_cast<int>((row_bytes + 15 + 3 * th.kpad + 8 + 15) / 16 * 16);  // alignment shift + zero-weight taps past the row + word read-ahead
+    // Largest tile of output rows (<= 32) that fits three CTAs per SM; when that leaves fewer than 16 rows (wide inputs, large
+    // outputs) the halo rows recomputed per tile dominate, so trade occupancy for a taller tile: two CTAs, then one.
+    const size_t budgets[3] = {72 * 1024, 110 * 1024, 200 * 1024};
+    for (int bi = 0; bi < 3; ++bi) {
+      s.tier = bi;
+      for (s.TY = 32; s.TY >= 1; s.TY /= 2) {
+        int rows = 0;  // worst-case number of input rows one tile of TY output rows touches
+        for (int y0 = 0; y0 < s.oh; y0 += s.TY) {
+          const int y1 = (y0 + s.TY < s.oh ? y0 + s.TY : s.oh) - 1;
+          const int r = tv.first[y1] + tv.count[y1] - tv.first[y0];
+          rows = r > rows ? r : rows;
+        }
+        s.tile_rows = rows;
+        s.smem = tables + static_cast<size_t>(kThreads / 32) * s.stage_bytes + static_cast<size_t>(rows + tv.kpad) * s.rowb + 16;  // zero-weight taps may run past the last row
+        if (s.smem <= budgets[bi] || s.TY == 1) break;
+      }
+      if (s.smem <= budgets[bi] && (s.TY >= 16 || s.TY >= s.oh)) break;
+    }
+    if (s.smem <= 200 * 1024) {
+      *out = s;
+      return 0;
+    }
+  }
+  s.path = kTwoPass;
+  s.tier = -1;
+  s.TY = kTwoPassTY;
+  s.tile_rows = s.stage_bytes = 0;
+  s.smem = 0;
+  s.mid_y0 = tv.first[0];
+  s.mid_rows = tv.first[s.oh - 1] + tv.count[s.oh - 1] - s.mid_y0;
+  const size_t mid_bytes = static_cast<size_t>(s.mid_rows + tv.kpad) * s.rowb;  // the vertical pass indexes one image's rows in int
+  if (mid_bytes > static_cast<size_t>(kMaxFrameBytes)) {
+    set_last_error("resize %dx%d -> %dx%d needs an 8-bit intermediate of %zu bytes per image: the front-end's limit is 2^31 - 1", H, W,
+                   s.rh, s.rw, mid_bytes);
+    return JIMM_EINVAL;
+  }
+  *out = s;
+  return 0;
+}
+
+int get_plan(jimm_preproc* p, int H, int W, SizePlan** out) {
+  std::lock_guard<std::mutex> lock(p->mu);
+  auto it = p->plans.find({H, W});
+  if (it != p->plans.end()) { *out = &it->second; return 0; }
+  SizePlan s;
+  ResampleTable th, tv;
+  JIMM_TRY(plan_size(p->cfg, H, W, &s, &th, &tv));
   JIMM_TRY(upload(p, th.first, &s.h.first));
   JIMM_TRY(upload(p, th.count, &s.h.count));
   JIMM_TRY(upload(p, th.padded(s.h.stride), &s.h.kk));
   JIMM_TRY(upload(p, tv.first, &s.v.first));
   JIMM_TRY(upload(p, tv.count, &s.v.count));
   JIMM_TRY(upload(p, tv.padded(s.v.stride), &s.v.kk));
-  // shared-memory budget: horizontal tables for the cropped columns + staging group + 8-bit tile
-  const size_t row_bytes = static_cast<size_t>(W) * 3;
-  if (row_bytes + 3 * th.kpad + 48 > 64 * 1024) { set_last_error("image width %d too large for the staging buffer", W); return JIMM_EINVAL; }
-  s.rowb = (s.ow * 3 + 3) / 4 * 4;
-  const size_t tables = (static_cast<size_t>(s.ow) * s.h.stride + s.ow) * sizeof(int) + 16;
-  s.stage_bytes = static_cast<int>((row_bytes + 15 + 3 * th.kpad + 8 + 15) / 16 * 16);  // alignment shift + zero-weight taps past the row + word read-ahead
-  // Largest tile of output rows (<= 32) that fits three CTAs per SM; when that leaves fewer than 16 rows (wide inputs, large
-  // outputs) the halo rows recomputed per tile dominate, so trade occupancy for a taller tile: two CTAs, then one.
-  const size_t budgets[3] = {72 * 1024, 110 * 1024, 200 * 1024};
-  for (int bi = 0; bi < 3; ++bi) {
-    for (s.TY = 32; s.TY >= 1; s.TY /= 2) {
-      int rows = 0;  // worst-case number of input rows one tile of TY output rows touches
-      for (int y0 = 0; y0 < s.oh; y0 += s.TY) {
-        const int y1 = (y0 + s.TY < s.oh ? y0 + s.TY : s.oh) - 1;
-        const int r = tv.first[s.top + y1] + tv.count[s.top + y1] - tv.first[s.top + y0];
-        rows = r > rows ? r : rows;
-      }
-      s.tile_rows = rows;
-      s.smem = tables + static_cast<size_t>(kThreads / 32) * s.stage_bytes + static_cast<size_t>(rows + tv.kpad) * s.rowb + 16;  // zero-weight taps may run past the last row
-      if (s.smem <= budgets[bi] || s.TY == 1) break;
-    }
-    if (s.smem <= budgets[bi] && (s.TY >= 16 || s.TY >= s.oh)) break;
-  }
-  if (s.smem > 200 * 1024) { set_last_error("resize %dx%d -> %dx%d needs %zu bytes of shared memory", H, W, s.rh, s.rw, s.smem); return JIMM_EINVAL; }
   auto ins = p->plans.emplace(std::make_pair(H, W), s);
-  *out = &ins.first->second;
+  *out = &ins.first->second;  // map nodes never move: the pointer stays valid while other sizes are added
   return 0;
 }
 
@@ -375,6 +497,54 @@ int launch(const KernelArgs& a, const SizePlan& s, int B, cudaStream_t stream) {
   JIMM_CUDA_CHECK(launch_k(preprocess_kernel<OUT>, grid, dim3(kThreads), s.smem, stream, 1, false, a));
   note_launch();
   return 0;
+}
+
+template <typename OUT>
+int launch_two_pass(const PassArgs& pa, const SizePlan& s, int B, cudaStream_t stream) {
+  JIMM_CUDA_CHECK(launch_k(hpass_kernel, dim3(s.mid_rows, B), dim3(kThreads), 0, stream, 1, false, pa));
+  note_launch();
+  JIMM_CUDA_CHECK(launch_k(vpass_kernel<OUT>, dim3((s.oh + s.TY - 1) / s.TY, B), dim3(kThreads), 0, stream, 1, false, pa));
+  note_launch();
+  return 0;
+}
+
+// All B images of one size: the fused kernel, up to 65532 images per launch; or the two passes, whose intermediate is allocated in
+// stream order for this call alone, so that calls in flight on other streams of the same handle never share it, and sized for a
+// chunk of images rather than the batch.  (The device's default pool returns it to the driver at each synchronisation unless
+// the application raises the pool's release threshold; the cost of that has not been measured.)
+template <typename OUT>
+int run_sized(const SizePlan& s, KernelArgs a, int B, cudaStream_t st) {
+  const uint8_t* img = a.img;
+  OUT* out = static_cast<OUT*>(a.out);
+  const size_t in_image = static_cast<size_t>(a.H) * a.W * 3, out_image = static_cast<size_t>(s.oh) * s.ow * 3;
+  if (s.path == kFused) {
+    // 65532 images per launch (the grid's y limit is 65535): a multiple of four, so every launch's output pointer keeps the
+    // alignment of `out` that the kernel's vector stores test relative to it
+    for (int b0 = 0; b0 < B; b0 += kFusedImages) {
+      a.img = img + static_cast<size_t>(b0) * in_image;
+      a.out = out + static_cast<size_t>(b0) * out_image;
+      JIMM_TRY(launch<OUT>(a, s, std::min(B - b0, kFusedImages), st));
+    }
+    return 0;
+  }
+  const size_t mid_image = static_cast<size_t>(s.mid_rows) * s.rowb;
+  const int chunk = static_cast<int>(std::min<size_t>(std::max<size_t>(kMidChunkBytes / mid_image, 1), std::min(B, 65535)));
+  PassArgs pa;
+  pa.k = a;
+  pa.y0 = s.mid_y0;
+  pa.rows = s.mid_rows;
+  pa.mid = nullptr;
+  pa.b0 = 0;
+  // + zero-weight taps of the last image's last rows, which may run past its intermediate
+  JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&pa.mid), chunk * mid_image + static_cast<size_t>(s.v.ksize) * s.rowb, st));
+  int rc = 0;
+  for (int b0 = 0; b0 < B && rc == 0; b0 += chunk) {
+    pa.b0 = b0;
+    rc = launch_two_pass<OUT>(pa, s, std::min(B - b0, chunk), st);
+  }
+  const cudaError_t fe = cudaFreeAsync(pa.mid, st);
+  if (rc == 0 && fe != cudaSuccess) { set_last_error("cudaFreeAsync -> %s", cudaGetErrorString(fe)); return JIMM_ECUDA; }
+  return rc;
 }
 
 }  // namespace
@@ -408,13 +578,20 @@ int jimm_preproc_create(const jimm_preproc_config_t* cfg, int device, jimm_prepr
 }
 
 int jimm_preproc_output_size(const jimm_preproc_t* p, int H, int W, int* out_h, int* out_w) {
-  if (!p || H <= 0 || W <= 0) { set_last_error("bad arguments"); return JIMM_EINVAL; }
-  int rh, rw;
-  resized_size(p->cfg, H, W, &rh, &rw);
-  const int oh = p->cfg.crop_h ? p->cfg.crop_h : rh, ow = p->cfg.crop_w ? p->cfg.crop_w : rw;
-  if (oh > rh || ow > rw) { set_last_error("centre crop %dx%d larger than the resized image %dx%d", oh, ow, rh, rw); return JIMM_EINVAL; }
-  if (out_h) *out_h = oh;
-  if (out_w) *out_w = ow;
+  if (!p) { set_last_error("bad arguments"); return JIMM_EINVAL; }
+  SizePlan s;
+  bool known = false;
+  {
+    std::lock_guard<std::mutex> lock(p->mu);
+    auto it = p->plans.find({H, W});
+    if (it != p->plans.end()) { s = it->second; known = true; }
+  }
+  if (!known) {  // the planner jimm_preproc_run uses: a size it would refuse is refused here, before a caller stages anything
+    ResampleTable th, tv;
+    JIMM_TRY(plan_size(p->cfg, H, W, &s, &th, &tv));
+  }
+  if (out_h) *out_h = s.oh;
+  if (out_w) *out_w = s.ow;
   return 0;
 }
 
@@ -422,6 +599,12 @@ int jimm_preproc_run(jimm_preproc_t* p, const uint8_t* img, int B, int H, int W,
   if (!p || !img || !out) { set_last_error("null argument"); return JIMM_EINVAL; }
   if (B <= 0) return 0;
   if (out_dtype < JIMM_F32 || out_dtype > JIMM_BF16) { set_last_error("bad output dtype %d", out_dtype); return JIMM_EINVAL; }
+  // the kernels store four samples at once wherever the index allows: out must be aligned for that
+  const size_t vec_bytes = out_dtype == JIMM_F32 ? 16 : 8;
+  if (reinterpret_cast<uintptr_t>(out) % vec_bytes) {
+    set_last_error("output pointer must be %zu-byte aligned for this dtype", vec_bytes);
+    return JIMM_EINVAL;
+  }
   JIMM_CUDA_CHECK(cudaSetDevice(p->device));
   SizePlan* s = nullptr;
   JIMM_TRY(get_plan(p, H, W, &s));
@@ -429,27 +612,19 @@ int jimm_preproc_run(jimm_preproc_t* p, const uint8_t* img, int B, int H, int W,
   a.img = img;
   a.out = out;
   a.lut = p->lut;
-  a.hfirst = s->h.first + s->left;
-  a.hcount = s->h.count + s->left;
-  a.hk = s->h.kk + static_cast<size_t>(s->left) * s->h.stride;
-  a.vfirst = s->v.first + s->top;
-  a.vcount = s->v.count + s->top;
-  a.vk = s->v.kk + static_cast<size_t>(s->top) * s->v.ksize;
+  a.hfirst = s->h.first;  // tables of the cropped columns and rows only
+  a.hcount = s->h.count;
+  a.hk = s->h.kk;
+  a.vfirst = s->v.first;
+  a.vcount = s->v.count;
+  a.vk = s->v.kk;
   a.H = H; a.W = W; a.oh = s->oh; a.ow = s->ow; a.hks = s->h.ksize; a.hstride = s->h.stride; a.vks = s->v.ksize;
   a.TY = s->TY; a.rowb = s->rowb; a.stage_bytes = s->stage_bytes;
   a.vec_ok = (reinterpret_cast<uintptr_t>(img) & 15) == 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the grid's y dimension is limited to 65535 images per launch
-  for (int b0 = 0; b0 < B; b0 += 65535) {
-    const int nb = B - b0 < 65535 ? B - b0 : 65535;
-    KernelArgs c = a;
-    c.img = img + static_cast<size_t>(b0) * H * W * 3;
-    const size_t out_off = static_cast<size_t>(b0) * s->oh * s->ow * 3;
-    if (out_dtype == JIMM_F32) { c.out = static_cast<float*>(out) + out_off; JIMM_TRY(launch<float>(c, *s, nb, st)); }
-    else if (out_dtype == JIMM_F16) { c.out = static_cast<__half*>(out) + out_off; JIMM_TRY(launch<__half>(c, *s, nb, st)); }
-    else { c.out = static_cast<__nv_bfloat16*>(out) + out_off; JIMM_TRY(launch<__nv_bfloat16>(c, *s, nb, st)); }
-  }
-  return 0;
+  if (out_dtype == JIMM_F32) return run_sized<float>(*s, a, B, st);
+  if (out_dtype == JIMM_F16) return run_sized<__half>(*s, a, B, st);
+  return run_sized<__nv_bfloat16>(*s, a, B, st);
 }
 
 int jimm_preproc_destroy(jimm_preproc_t* p) {
@@ -471,6 +646,19 @@ int jimm_k_resample_coeffs(int in_size, int out_size, int resample, int* ksize, 
     if (kk_capacity < out_size * t.ksize) { set_last_error("kk buffer too small: %d < %d", kk_capacity, out_size * t.ksize); return JIMM_EINVAL; }
     for (int i = 0; i < out_size * t.ksize; ++i) kk[i] = t.kk[i];
   }
+  return 0;
+}
+
+// Host-only: the plan jimm_preproc_run would use for H x W frames, for the CPU tests that pin the planner.
+int jimm_k_preproc_plan(const jimm_preproc_config_t* cfg, int H, int W, int* path, int* tier, int* TY, long long* smem) {
+  JIMM_TRY(check_cfg(cfg));
+  SizePlan s;
+  ResampleTable th, tv;
+  JIMM_TRY(plan_size(*cfg, H, W, &s, &th, &tv));
+  if (path) *path = s.path;
+  if (tier) *tier = s.tier;
+  if (TY) *TY = s.TY;
+  if (smem) *smem = static_cast<long long>(s.smem);
   return 0;
 }
 

@@ -46,6 +46,35 @@ def _size_fields(size, default_to_square: bool = True) -> dict:
     raise ValueError(f"Size must contain 'height' and 'width' keys, or a 'shortest_edge' key. Got {size}.")
 
 
+def _config(size=None, crop_size=None, resample: int = BILINEAR, do_center_crop: Optional[bool] = None,
+            rescale_factor: float = 1 / 255, image_mean: Sequence[float] = (0.5, 0.5, 0.5), image_std: Sequence[float] = (0.5, 0.5, 0.5),
+            do_resize: bool = True, do_rescale: bool = True, do_normalize: bool = True, default_to_square: bool = True) -> _lib.PreprocConfig:
+    """jimm_preproc_config_t of ImagePreprocessor's keywords (checked here; no GPU needed)."""
+    if not (do_resize and do_rescale and do_normalize):
+        raise ValueError("the GPU front-end implements the full resize -> rescale -> normalize pipeline of the reference's examples")
+    if int(resample) not in (BILINEAR, BICUBIC):
+        raise ValueError(f"resample must be PIL BILINEAR (2) or BICUBIC (3), got {resample}")
+    if len(image_mean) != 3 or len(image_std) != 3:
+        raise ValueError("mean must have 3 elements if it is an iterable")
+    if not all(image_std):
+        raise ValueError("std evaluated to zero, leading to division by zero.")
+    f = _size_fields(size if size is not None else {"height": 224, "width": 224}, default_to_square)
+    cfg = _lib.PreprocConfig()
+    cfg.height, cfg.width, cfg.shortest_edge = f.get("height", 0), f.get("width", 0), f.get("shortest_edge", 0)
+    if do_center_crop is None:
+        do_center_crop = crop_size is not None
+    if do_center_crop:
+        c = _size_fields(crop_size if not isinstance(crop_size, int) else (crop_size, crop_size))
+        if "height" not in c:
+            raise ValueError(f"The size dictionary must have keys 'height' and 'width'. Got {crop_size}")
+        cfg.crop_h, cfg.crop_w = c["height"], c["width"]
+    cfg.resample = int(resample)
+    cfg.rescale_factor = float(rescale_factor)
+    cfg.mean = (C.c_float * 3)(*[float(v) for v in image_mean])
+    cfg.std = (C.c_float * 3)(*[float(v) for v in image_std])
+    return cfg
+
+
 class ImagePreprocessor:
     """Mirror of `ViTImageProcessor` / `CLIPImageProcessor` / `SiglipImageProcessor` for uint8 RGB batches on the GPU."""
 
@@ -53,28 +82,8 @@ class ImagePreprocessor:
                  rescale_factor: float = 1 / 255, image_mean: Sequence[float] = (0.5, 0.5, 0.5),
                  image_std: Sequence[float] = (0.5, 0.5, 0.5), do_resize: bool = True, do_rescale: bool = True,
                  do_normalize: bool = True, device: Optional[int] = None, default_to_square: bool = True, **unused):
-        if not (do_resize and do_rescale and do_normalize):
-            raise ValueError("the GPU front-end implements the full resize -> rescale -> normalize pipeline of the reference's examples")
-        if int(resample) not in (BILINEAR, BICUBIC):
-            raise ValueError(f"resample must be PIL BILINEAR (2) or BICUBIC (3), got {resample}")
-        if len(image_mean) != 3 or len(image_std) != 3:
-            raise ValueError("mean must have 3 elements if it is an iterable")
-        if not all(image_std):
-            raise ValueError("std evaluated to zero, leading to division by zero.")
-        f = _size_fields(size if size is not None else {"height": 224, "width": 224}, default_to_square)
-        cfg = _lib.PreprocConfig()
-        cfg.height, cfg.width, cfg.shortest_edge = f.get("height", 0), f.get("width", 0), f.get("shortest_edge", 0)
-        if do_center_crop is None:
-            do_center_crop = crop_size is not None
-        if do_center_crop:
-            c = _size_fields(crop_size if not isinstance(crop_size, int) else (crop_size, crop_size))
-            if "height" not in c:
-                raise ValueError(f"The size dictionary must have keys 'height' and 'width'. Got {crop_size}")
-            cfg.crop_h, cfg.crop_w = c["height"], c["width"]
-        cfg.resample = int(resample)
-        cfg.rescale_factor = float(rescale_factor)
-        cfg.mean = (C.c_float * 3)(*[float(v) for v in image_mean])
-        cfg.std = (C.c_float * 3)(*[float(v) for v in image_std])
+        cfg = _config(size, crop_size, resample, do_center_crop, rescale_factor, image_mean, image_std, do_resize, do_rescale,
+                      do_normalize, default_to_square)
         if not torch.cuda.is_available():
             raise _lib.JimmError("jimm_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
@@ -165,3 +174,17 @@ def resample_coeffs(in_size: int, out_size: int, resample: int):
     _lib.check(lib.jimm_k_resample_coeffs(in_size, out_size, resample, C.byref(ks), first.ctypes.data_as(C.c_void_p),
                                           count.ctypes.data_as(C.c_void_p), kk.ctypes.data_as(C.c_void_p), kk.size))
     return first, count, kk
+
+
+FUSED, TWO_PASS = 0, 1
+
+
+def plan(height: int, width: int, **config):
+    """Host-only: how the library runs height x width frames under ImagePreprocessor(**config) -- (path, tier, TY, smem): FUSED with
+    TY output rows per CTA and smem bytes of shared memory chosen under budget tier 0 / 1 / 2 (72 / 110 / 200 KB), or TWO_PASS
+    (-1, 8, 0).  Raises ValueError for a size the front-end refuses (test hook)."""
+    lib = _lib.load()
+    cfg = _config(**config)
+    path, tier, ty, smem = C.c_int(), C.c_int(), C.c_int(), C.c_longlong()
+    _lib.check(lib.jimm_k_preproc_plan(C.byref(cfg), int(height), int(width), C.byref(path), C.byref(tier), C.byref(ty), C.byref(smem)))
+    return path.value, tier.value, ty.value, smem.value
