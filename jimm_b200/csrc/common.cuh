@@ -540,7 +540,11 @@ __device__ __forceinline__ float to_float(__nv_fp8_e4m3 v) { return static_cast<
 // a = 0; k is clamped at -126 so that s stays a normal fp32 (rows with a < 2^-117 only).  k comes from the exponent bits (frexpf is
 // exact): a = f 2^E with f in [0.5, 1), and a <= 448 2^k = 0.875 2^(9 + k) holds from k = E - 9 on when f <= 0.875, else from E - 8.
 // x / s is then an exact multiplication by 2^-k, and the dequantised value q s is exact.
+// A row holding an infinity (amax = inf; NaN never reaches amax, fmaxf drops it) gets k = 255: s = 2^255 = inf and 2^-k = 0, so its
+// finite elements store 0, its infinities and NaNs store NaN, and every dequantised value 0 inf / NaN inf is NaN.  The row stays
+// non-finite, as it does in the 16-bit modes, instead of saturating to +-448 at a finite scale.
 __device__ __forceinline__ int e4m3_scale_exp(float amax) {
+  if (amax == INFINITY) return 255;
   if (!(amax > 0.f)) return 0;
   int e;
   const float f = frexpf(amax, &e);

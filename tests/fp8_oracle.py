@@ -29,6 +29,7 @@ def e4m3_scale(amax: torch.Tensor) -> torch.Tensor:
     m, e = torch.frexp(a)  # a = m 2^e, m in [0.5, 1); a <= 448 2^k = 0.875 2^(9 + k)
     k = e.to(torch.int64) - 9 + (m > 0.875).to(torch.int64)
     k = torch.where(a > 0, torch.clamp(k, min=-126), torch.zeros_like(k))
+    k = torch.where(torch.isinf(a), torch.full_like(k, 255), k)  # an infinite row: s = inf, the row dequantises to NaN
     return torch.ldexp(torch.ones_like(a), k.to(torch.float64)).to(torch.float32)
 
 
@@ -46,7 +47,7 @@ def round_e4m3(y: torch.Tensor) -> torch.Tensor:
 def quantize_rows(x: torch.Tensor):
     """fp32 rows -> (float8_e4m3fn values, fp32 scales [rows]), as the LayerNorm kernel and the weight quantiser store them."""
     x = x.to(torch.float32)
-    s = e4m3_scale(x.abs().amax(-1))
+    s = e4m3_scale(torch.where(torch.isnan(x), 0.0, x.abs()).amax(-1))  # NaN does not count towards the maximum (fmaxf on the device)
     q = round_e4m3(x / s.unsqueeze(-1))  # division by a power of two: exact (also into fp32 subnormals, as on the device)
     return q.to(torch.float8_e4m3fn), s
 
