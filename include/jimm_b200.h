@@ -39,7 +39,8 @@ enum jimm_dtype { JIMM_F32 = 0, JIMM_F16 = 1, JIMM_BF16 = 2, JIMM_I32 = 3, JIMM_
 enum jimm_kind {
   JIMM_VIT = 0, JIMM_CLIP = 1, JIMM_SIGLIP = 2, JIMM_TOWER = 3 /* bare VisionTransformerBase */,
   JIMM_ENCODER = 4 /* bare Transformer / TransformerEncoder stack (common/transformer.py:22-196) */,
-  JIMM_MAPHEAD = 5 /* bare MultiHeadAttentionPoolingHead (common/vit.py:12-101) */
+  JIMM_MAPHEAD = 5 /* bare MultiHeadAttentionPoolingHead (common/vit.py:12-101) */,
+  JIMM_SIGLIP_NAFLEX = 6 /* SigLIP 2 NaFlex: SigLIP whose vision tower takes each image at its own patch grid, see jimm_encode_image_patches */
 };
 enum jimm_pool { JIMM_POOL_CLS = 0, JIMM_POOL_MAP = 1 };
 enum jimm_act { JIMM_GELU_TANH = 0, JIMM_QUICK_GELU = 1 };
@@ -149,6 +150,17 @@ JIMM_API int jimm_dual_forward_hw(jimm_model_t* m, const void* img, int in_dtype
  * eagerly and return without synchronising; back-to-back calls on one stream are safe. */
 JIMM_API int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
 JIMM_API int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream);
+/* SigLIP 2 NaFlex (kind JIMM_SIGLIP_NAFLEX; config as JIMM_SIGLIP with img_size = g * patch, g * g the position table's rows, MAP pooling,
+ * no pre-norm, patch bias).  Every vision call on this kind resamples the g x g position table to the image's patch grid with
+ * F.interpolate(mode="bilinear", align_corners=False, antialias=True) instead of bicubically -- at img_size x img_size the table itself,
+ * so jimm_encode_image is the plain SigLIP tower -- and the *_hw and *_packed calls above run on it unchanged.
+ * jimm_encode_image_patches takes the HuggingFace Siglip2ImageProcessor's output as it is: patches device [B, N, patch*patch*in_ch] of
+ * in_dtype (pixel_values; each row a patch flattened in (py, px, c) order), grid host int [B][2] = (gh, gw) (spatial_shapes), read during
+ * the call.  Sample b's rows 0 .. gh*gw - 1 are its patches, row-major over its grid; the rows after them (the processor's padding, what
+ * pixel_attention_mask marks 0) are never read.  out: device fp32 [B, v_width]; row b equals jimm_encode_image_packed on the gh*patch x
+ * gw*patch image with those patches.  Chunks, the token budget and the MAP head's limit are those of jimm_encode_image_packed.  A grid
+ * edge < 1, gh*gw > N, a null argument or a model of another kind is JIMM_EINVAL before anything is enqueued. */
+JIMM_API int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream);
 /* B token sequences of different lengths in one jimm_encode_text call.  ids: device int32, the B sequences one after another; len: host
  * int array [B], read during the call, every length in 1 .. ctx_len; out: device fp32 [B, E].  Row i equals jimm_encode_text on sequence
  * i alone (T = len[i]): positions restart at 0 in every sequence, CLIP's causal mask and EOT argmax are taken within it, SigLIP pools its
@@ -277,6 +289,20 @@ JIMM_API int jimm_k_activation(const float* x, float* y, long long n, int act, v
  * row 0 = cls + pos[0] when cls (fp32 [D]) is not NULL, the patch rows the bicubic resampling of pos's g x g patch rows described at
  * jimm_vit_forward_hw (pos fp32 [(1 +) g*g, D]); D a multiple of 4.  (gh, gw) == (g, g) gives the table itself, bit for bit. */
 JIMM_API int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream);
+/* jimm_k_tokens_init_interp with the resampling chosen by mode: 0 bicubic (jimm_k_tokens_init_interp itself), 1 antialiased bilinear
+ * (F.interpolate(mode="bilinear", align_corners=False, antialias=True), the NaFlex rule; up to g table rows per axis). */
+JIMM_API int jimm_k_tokens_init_interp_ex(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, int mode,
+                                          void* stream);
+/* The position add of a packed vision call: image b is rows seq_off[b] .. seq_off[b+1]-1 of x fp32 [rows, D] (seq_off device int32 [B + 1]),
+ * its grid (n_b / gw[b]) x gw[b] (gw device int32 [B]; n_b its rows less the CLS row when cls is not NULL).  The CLS row is set to cls +
+ * pos[0]; each patch row gets += the table resampled as jimm_k_tokens_init_interp_ex (mode) gives it.  max_S: the most rows of one image. */
+JIMM_API int jimm_k_tokens_add_interp_packed(const float* cls, const float* pos, int g, int D, float* x, const int32_t* seq_off, const int32_t* gw,
+                                             int B, int max_S, int mode, void* stream);
+/* The patch-GEMM operand of jimm_encode_image_patches: patches [B, N, K] of in_type (0 fp32 | 1 fp16 | 2 bf16), sample b's rows 0 .. n_b - 1
+ * (n_b = seq_off[b+1] - seq_off[b] <= max_rows <= N) -> rows seq_off[b] + r of out [*, ldk] of out_type (0 fp32 | 1 fp16 | 2 bf16 | 3 tf32),
+ * columns K .. ldk - 1 written as zeros; other rows of out untouched, other rows of patches never read. */
+JIMM_API int jimm_k_patch_rows_packed(const void* patches, int in_type, int N, int K, const int32_t* seq_off, int B, int max_rows, void* out,
+                                      int out_type, int ldk, void* stream);
 JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream);
 /* jimm_k_embed on B sequences packed as for jimm_k_attention_packed (seq_off device int32 [B + 1], T_total = seq_off[B] rows of ids and
  * x): x[r] = table[clamp(ids[r], 0, vocab - 1)] + pos[r - seq_off[b]] for the rows r of sequence b, whose positions restart at 0. */

@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libjimm_b200.so")
 
 F32, F16, BF16, I32, F8E4M3 = 0, 1, 2, 3, 4
 PARAM_TRANSPOSED = 1
-KIND_VIT, KIND_CLIP, KIND_SIGLIP, KIND_TOWER, KIND_ENCODER, KIND_MAPHEAD = 0, 1, 2, 3, 4, 5
+KIND_VIT, KIND_CLIP, KIND_SIGLIP, KIND_TOWER, KIND_ENCODER, KIND_MAPHEAD, KIND_SIGLIP_NAFLEX = 0, 1, 2, 3, 4, 5, 6
 POOL_CLS, POOL_MAP = 0, 1
 ACT_GELU_TANH, ACT_QUICK_GELU = 0, 1
 TPOOL_EOT_ARGMAX, TPOOL_LAST = 0, 1
@@ -75,6 +75,7 @@ SIGNATURES = {
     "jimm_vit_forward_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
     "jimm_encode_image_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
     "jimm_encode_text_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), _fp, _vp]),
+    "jimm_encode_image_patches": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_i), _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -108,6 +109,9 @@ SIGNATURES = {
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),
     "jimm_k_tokens_init_interp": (_i, [_fp, _fp, _i, _i, _fp, _i, _i, _i, _vp]),
+    "jimm_k_tokens_init_interp_ex": (_i, [_fp, _fp, _i, _i, _fp, _i, _i, _i, _i, _vp]),
+    "jimm_k_tokens_add_interp_packed": (_i, [_fp, _fp, _i, _i, _fp, _ip, _ip, _i, _i, _i, _vp]),
+    "jimm_k_patch_rows_packed": (_i, [_vp, _i, _i, _i, _ip, _i, _i, _vp, _i, _i, _vp]),
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_embed_packed": (_i, [_ip, _fp, _fp, _fp, _ip, _i, _i, _i, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),

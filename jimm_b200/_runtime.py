@@ -37,11 +37,12 @@ def _call(lib, device: torch.device, name: str, *args):
 class Images(NamedTuple):
     """The images of one vision call, checked and prepared once (prep_images)."""
 
-    x: Union[torch.Tensor, List[torch.Tensor]]  # [B, H, W, C], or a list of [H, W, C]
+    x: Union[torch.Tensor, List[torch.Tensor]]  # [B, H, W, C], or a list of [H, W, C], or NaFlex patch rows [B, N, P*P*C] (grid)
     host: bool  # host memory: the result goes back to the host
     u8: bool  # raw RGB frames for the image front-end
     hw: Optional[Tuple[int, int]]  # the (height, width) the tower sees; for a list the one with the most tokens (None: empty list)
     trained: bool  # hw is the trained size
+    grid: Optional[List[Tuple[int, int]]] = None  # NaFlex patch rows: each sample's patch grid (rows, columns)
 
 
 def _prep_batch(x, cfg: _lib.Config, preproc, interpolate: bool):
@@ -97,6 +98,35 @@ def prep_images(images, cfg: _lib.Config, preproc, interpolate: bool) -> Images:
     hw = max((hw for _, hw in prepped), key=lambda s: grid_tokens(cfg, *s), default=None)
     xs = [x[0] for x, _ in prepped]
     return Images(xs, not xs or not xs[0].is_cuda, bool(xs) and xs[0].dtype == torch.uint8, hw, hw == (cfg.img_size, cfg.img_size))
+
+
+def prep_patches(pixel_values, spatial_shapes, pixel_attention_mask, cfg: _lib.Config) -> Images:
+    """The input step of a SigLIP 2 NaFlex call on the HF processor's output: pixel_values [B, N, P*P*C] (each row a patch flattened in
+    (py, px, c) order), spatial_shapes [B, 2] integer (patch rows, patch columns) with 1 <= rows * columns <= N, and optionally
+    pixel_attention_mask [B, N], which must be the prefix mask the shapes imply (sample b's first rows * columns entries set).  The
+    masked rows are never read, so the mask itself is not needed."""
+    x = _as_tensor(pixel_values)
+    K = cfg.patch * cfg.patch * cfg.in_ch
+    if x.ndim != 3 or x.shape[2] != K:
+        raise ValueError(f"expected pixel_values of shape [batch, max_num_patches, {K}] (patch {cfg.patch}, {cfg.in_ch} channels), "
+                         f"got {tuple(x.shape)}")
+    B, N = x.shape[0], x.shape[1]
+    ss = _as_tensor(spatial_shapes)
+    if tuple(ss.shape) != (B, 2) or ss.dtype.is_floating_point or ss.dtype.is_complex or ss.dtype == torch.bool:
+        raise ValueError(f"expected integer spatial_shapes of shape [{B}, 2] (patch rows, patch columns), got {tuple(ss.shape)} {ss.dtype}")
+    grid = [(int(h), int(w)) for h, w in ss.tolist()]
+    for i, (h, w) in enumerate(grid):
+        if h < 1 or w < 1 or h * w > N:
+            raise ValueError(f"sample {i}: spatial shape {h}x{w} needs 1 .. {N} (max_num_patches) patch rows")
+    if pixel_attention_mask is not None:
+        mk = _as_tensor(pixel_attention_mask)
+        n = torch.tensor([h * w for h, w in grid], dtype=torch.long)
+        if tuple(mk.shape) != (B, N) or not torch.equal(mk.cpu() != 0, torch.arange(N)[None, :] < n[:, None]):
+            raise ValueError("pixel_attention_mask is not the mask spatial_shapes implies (each sample's first rows * columns patches)")
+    if x.dtype not in _TORCH_TO_CODE:
+        x = x.to(torch.float32)
+    hw = max(((h * cfg.patch, w * cfg.patch) for h, w in grid), key=lambda s: grid_tokens(cfg, *s), default=None)
+    return Images(x.contiguous(), not x.is_cuda, False, hw, False, grid)
 
 
 class Texts(NamedTuple):
@@ -280,7 +310,10 @@ class NativeModel:
         xd = self._device_images(im.x)
         B = len(xd)
         out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-        if isinstance(xd, list):
+        if im.grid is not None:
+            if B:
+                self._run("jimm_encode_image_patches", xd, xd.dtype, B, xd.shape[1], (C.c_int * (2 * B))(*[v for hw in im.grid for v in hw]), out)
+        elif isinstance(xd, list):
             if B:
                 self._run("jimm_encode_image_packed" if encode else "jimm_vit_forward_packed", (C.c_void_p * B)(*[t.data_ptr() for t in xd]),
                           xd[0].dtype, B, (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]), out)
@@ -349,7 +382,7 @@ class NativeModel:
             return self._back(out, im.host and ids.host).result()
         host = im.host and not ids.is_cuda
         Bi, (Bt, T) = len(im.x), ids.shape
-        if isinstance(im.x, list):
+        if isinstance(im.x, list) or im.grid is not None:
             out = self.logits(self._vision_dev(im, True), self.text(ids.to(self.device, non_blocking=True)))
         elif host and im.trained and not im.u8:
             # float pixels and ids: the library's pipeline copies both in and the logits out

@@ -21,6 +21,7 @@ QKV_W = "qkv_w"        # q/k/v projection weight (H*d, D)      -> (D, H, d)
 QKV_B = "qkv_b"        # q/k/v projection bias (H*d)           -> (H, d)
 OUT_W = "out_w"        # attention output weight (D, H*d)      -> (H, d, D)
 CONV = "conv"          # patch conv weight (D, C, P, P)        -> HWIO (P, P, C, D)
+PATCH_LINEAR = "patch_linear"  # SigLIP 2 NaFlex patch Linear weight (D, P*P*C), columns in (py, px, c) order -> HWIO (P, P, C, D)
 
 KNOWN_UNUSED = {"text_model.embeddings.position_ids", "vision_model.embeddings.position_ids"}  # models/vit.py:262-265
 
@@ -42,6 +43,10 @@ def convert(t: torch.Tensor, kind: str, flax_shape: Tuple[int, ...], rows: Optio
             return None
         v = t.permute(2, 3, 1, 0)
         return v if tuple(v.shape) == tuple(flax_shape) else None
+    if kind == PATCH_LINEAR:  # the (P*P*C, D) view of the HWIO kernel, transposed: the K-major operand as stored
+        if t.ndim != 2 or tuple(t.shape) != (flax_shape[-1], numel // flax_shape[-1]):
+            return None
+        return LazyParam(t if t.is_contiguous() else t.contiguous(), flax_shape, transposed=True)
     if kind in (LINEAR, QKV_W, OUT_W):
         if t.ndim != 2 or t.numel() != numel:
             return None

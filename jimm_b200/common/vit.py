@@ -125,10 +125,11 @@ class _NativeOwner:
         n = self._native
         return prep_images(images, n.cfg if n is not None else self._native_config(), self._preproc, interpolate_pos_encoding)
 
-    def _vision(self, images, interpolate_pos_encoding: bool, encode: bool = False, wait: bool = True):
+    def _vision(self, images, interpolate_pos_encoding: bool, encode: bool = False, wait: bool = True, **inputs):
         """A vision call (NativeModel.vision) on a [B, H, W, C] batch or a list / tuple of images of different sizes (one packed
-        call).  The handle is rebuilt only when the largest image of an interpolate_pos_encoding call does not fit it."""
-        im = self._images(images, interpolate_pos_encoding)
+        call).  The handle is rebuilt only when the largest image of an interpolate_pos_encoding call does not fit it.  `inputs`: the
+        further image inputs a model's _images takes (SigLIP 2 NaFlex's spatial_shapes / pixel_attention_mask)."""
+        im = self._images(images, interpolate_pos_encoding, **inputs)
         return self.native(hw=im.hw if interpolate_pos_encoding else None).vision(im, encode=encode, wait=wait)
 
     def set_max_image_size(self, height: int, width: int):

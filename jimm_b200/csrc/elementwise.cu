@@ -300,8 +300,38 @@ __device__ __forceinline__ void bicubic_taps(int in, int out, int dst, int (&idx
   for (int k = 0; k < 4; ++k) idx[k] = max(min(i0 - 1 + k, in - 1), 0);
 }
 
+// Antialiased bilinear resampling (torch.nn.functional.interpolate(mode="bilinear", align_corners=False, antialias=True), the operation
+// SigLIP 2 NaFlex applies to its position table; PyTorch's _upsample_bilinear2d_aa weight rule) along an axis of `in` -> `out` samples:
+// output index `dst` reads taps i0 .. i1 - 1, each weighted by the triangle filter stretched by max(scale, 1) and normalised by the sum.
+// Downscaling reads up to `in` taps (all of them for out = 1).  At out == in the taps are (dst, dst + 1) with weights exactly (1, 0).
+struct AaAxis {
+  int i0, i1;
+  float center, invscale, total;
+  __device__ __forceinline__ float raw(int j) const {
+    const float x = fabsf(__fmul_rn(__fadd_rn(__fsub_rn(static_cast<float>(j), center), 0.5f), invscale));
+    return x < 1.f ? __fsub_rn(1.f, x) : 0.f;
+  }
+  __device__ __forceinline__ float weight(int j) const { return __fdiv_rn(raw(j), total); }
+};
+__device__ __forceinline__ AaAxis aa_axis(int in, int out, int dst) {
+  AaAxis a;
+  const float scale = __fdiv_rn(static_cast<float>(in), static_cast<float>(out));
+  const float support = scale >= 1.f ? scale : 1.f;
+  a.invscale = scale >= 1.f ? __fdiv_rn(1.f, scale) : 1.f;
+  a.center = __fmul_rn(scale, __fadd_rn(static_cast<float>(dst), 0.5f));
+  a.i0 = max(static_cast<int>(__fadd_rn(__fsub_rn(a.center, support), 0.5f)), 0);
+  a.i1 = min(static_cast<int>(__fadd_rn(__fadd_rn(a.center, support), 0.5f)), in);
+  a.total = 0.f;
+  for (int j = a.i0; j < a.i1; ++j) a.total = __fadd_rn(a.total, a.raw(j));
+  return a;
+}
+
+__device__ __forceinline__ float4 mul4(float4 p, float w) { return make_float4(__fmul_rn(p.x, w), __fmul_rn(p.y, w), __fmul_rn(p.z, w), __fmul_rn(p.w, w)); }
+__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w)); }
+
 // Row r of the initial residual stream of a gh x gw grid, columns 4 c .. 4 c + 3: cls + pos[0] for the CLS row (cls != null), else
-// the bicubic resampling of pos's g x g patch rows.
+// the resampling (Mode: bicubic or antialiased bilinear) of pos's g x g patch rows.
+template <int Mode>
 __device__ __forceinline__ float4 interp_token(const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int gh, int gw, int r,
                                                int c) {
   const int off = cls != nullptr ? 1 : 0;
@@ -309,6 +339,29 @@ __device__ __forceinline__ float4 interp_token(const float4* __restrict__ cls, c
   if (r < off) {
     const float4 a = __ldg(pos + c), b = __ldg(cls + c);
     v = make_float4(b.x + a.x, b.y + a.y, b.z + a.z, b.w + a.w);
+  } else if (Mode == POS_BILINEAR_AA) {
+    const int q = r - off, gy = q / gw, gx = q - gy * gw;
+    const AaAxis ay = aa_axis(g, gh, gy), ax = aa_axis(g, gw, gx);
+    const float4* src = pos + static_cast<size_t>(off) * D4 + c;
+    // sum over rows of (sum over columns of tap * wx) * wy, each sum in tap order: PyTorch's separable accumulation.  Zero-weight taps
+    // are skipped (each sum starts at its first weighted tap), so the (g, g) resample returns the table itself.
+    bool first_row = true;
+    for (int a = ay.i0; a < ay.i1; ++a) {
+      const float wy = ay.weight(a);
+      if (wy == 0.f) continue;
+      const float4* row = src + static_cast<size_t>(a) * g * D4;
+      float4 h = make_float4(0.f, 0.f, 0.f, 0.f);
+      bool first_col = true;
+      for (int b = ax.i0; b < ax.i1; ++b) {
+        const float wx = ax.weight(b);
+        if (wx == 0.f) continue;
+        const float4 t = mul4(__ldg(row + static_cast<size_t>(b) * D4), wx);
+        h = first_col ? t : add4(h, t);
+        first_col = false;
+      }
+      v = first_row ? mul4(h, wy) : add4(v, mul4(h, wy));
+      first_row = false;
+    }
   } else {
     const int q = r - off, gy = q / gw, gx = q - gy * gw;
     int iy[4], ix[4];
@@ -340,18 +393,20 @@ __device__ __forceinline__ float4 interp_token(const float4* __restrict__ cls, c
 }
 
 // One thread per (token r, 4 columns): the value is the same for every sample, so it is computed once and stored B times.
+template <int Mode>
 __global__ void __launch_bounds__(256)
 tokens_init_interp_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4, int B,
                           int gh, int gw, int S) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= S * D4) return;
   const int r = i / D4, c = i - r * D4;
-  const float4 v = interp_token(cls, pos, g, D4, gh, gw, r, c);
+  const float4 v = interp_token<Mode>(cls, pos, g, D4, gh, gw, r, c);
   const size_t SD4 = static_cast<size_t>(S) * D4;
   for (int b = 0; b < B; ++b) x[b * SD4 + i] = v;
 }
 
 // blockIdx.y = image; one thread per (token r of the image, 4 columns)
+template <int Mode>
 __global__ void __launch_bounds__(256)
 tokens_add_interp_packed_kernel(float4* __restrict__ x, const float4* __restrict__ cls, const float4* __restrict__ pos, int g, int D4,
                                 const int* __restrict__ seq_off, const int* __restrict__ gw_of) {
@@ -360,7 +415,7 @@ tokens_add_interp_packed_kernel(float4* __restrict__ x, const float4* __restrict
   if (i >= S * D4) return;
   const int r = i / D4, c = i - r * D4;
   const int gw = gw_of[b], gh = (S - (cls != nullptr ? 1 : 0)) / gw;
-  const float4 v = interp_token(cls, pos, g, D4, gh, gw, r, c);
+  const float4 v = interp_token<Mode>(cls, pos, g, D4, gh, gw, r, c);
   float4* dst = x + static_cast<size_t>(row0) * D4 + i;
   if (cls != nullptr && r == 0) {
     *dst = v;
@@ -370,26 +425,79 @@ tokens_add_interp_packed_kernel(float4* __restrict__ x, const float4* __restrict
   }
 }
 
+static int check_interp_mode(const char* fn, int mode) {
+  if (mode != POS_BICUBIC && mode != POS_BILINEAR_AA) { set_last_error("%s: bad resampling mode %d", fn, mode); return -1; }
+  return 0;
+}
+
 int tokens_add_interp_packed_run(float* x, const float* cls, const float* pos, int g, int D, const int* seq_off, const int* gw, int B, int max_S,
-                                 cudaStream_t stream) {
+                                 int mode, cudaStream_t stream) {
   if (B <= 0) return 0;
+  if (check_interp_mode("tokens_add_interp_packed", mode)) return -1;
   if (D % 4 != 0) { set_last_error("tokens_add_interp_packed: D must be a multiple of 4"); return -1; }
   if (B > 65535) { set_last_error("tokens_add_interp_packed: %d images exceed the grid", B); return -1; }
   const int D4 = D / 4, n = max_S * D4;
-  tokens_add_interp_packed_kernel<<<dim3((n + 255) / 256, B), 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls),
-                                                                                reinterpret_cast<const float4*>(pos), g, D4, seq_off, gw);
+  const dim3 grid((n + 255) / 256, B);
+  auto kernel = mode == POS_BILINEAR_AA ? tokens_add_interp_packed_kernel<POS_BILINEAR_AA> : tokens_add_interp_packed_kernel<POS_BICUBIC>;
+  kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls), reinterpret_cast<const float4*>(pos), g, D4,
+                                   seq_off, gw);
   JIMM_LAUNCH_CHECK();
   return 0;
 }
 
-int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream) {
+int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, int mode, cudaStream_t stream) {
   if (B <= 0) return 0;
+  if (check_interp_mode("tokens_init_interp", mode)) return -1;
   if (D % 4 != 0) { set_last_error("tokens_init_interp: D must be a multiple of 4"); return -1; }
   if (g <= 0 || gh <= 0 || gw <= 0) { set_last_error("tokens_init_interp: empty grid (g=%d, output %dx%d)", g, gh, gw); return -1; }
   const int S = gh * gw + (cls != nullptr ? 1 : 0), D4 = D / 4;
   const int n = S * D4;
-  tokens_init_interp_kernel<<<(n + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls),
-                                                                  reinterpret_cast<const float4*>(pos), g, D4, B, gh, gw, S);
+  auto kernel = mode == POS_BILINEAR_AA ? tokens_init_interp_kernel<POS_BILINEAR_AA> : tokens_init_interp_kernel<POS_BICUBIC>;
+  kernel<<<(n + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls), reinterpret_cast<const float4*>(pos),
+                                              g, D4, B, gh, gw, S);
+  JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Patch rows of the HuggingFace NaFlex processor ([B, N, K] pixel_values, sample b's first n_b rows valid) into the packed patch-GEMM
+// operand: blockIdx.y = sample, one thread per (row, column) of its n_b = seq_off[b + 1] - seq_off[b] rows; columns K .. ldk - 1 are zeros.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(256)
+patch_rows_packed_kernel(const InT* __restrict__ pv, OutT* __restrict__ out, const int* __restrict__ seq_off, int N, int K, int ldk) {
+  const int b = blockIdx.y;
+  const int row0 = seq_off[b];
+  const size_t total = static_cast<size_t>(seq_off[b + 1] - row0) * ldk;
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int r = static_cast<int>(i / ldk), k = static_cast<int>(i % ldk);
+  const float v = k < K ? to_float(pv[(static_cast<size_t>(b) * N + r) * K + k]) : 0.f;
+  out[static_cast<size_t>(row0 + r) * ldk + k] = from_float<OutT>(v);
+}
+
+template <typename InT>
+static void patch_rows_packed_launch(const void* pv, void* out, int out_type, const int* seq_off, int B, int max_rows, int N, int K, int ldk,
+                                     cudaStream_t stream) {
+  const dim3 grid(static_cast<unsigned>((static_cast<size_t>(max_rows) * ldk + 255) / 256), B);
+  const InT* in = static_cast<const InT*>(pv);
+  if (out_type == DT_F32) patch_rows_packed_kernel<InT, float><<<grid, 256, 0, stream>>>(in, static_cast<float*>(out), seq_off, N, K, ldk);
+  else if (out_type == DT_TF32) patch_rows_packed_kernel<InT, tf32_t><<<grid, 256, 0, stream>>>(in, static_cast<tf32_t*>(out), seq_off, N, K, ldk);
+  else if (out_type == DT_F16) patch_rows_packed_kernel<InT, __half><<<grid, 256, 0, stream>>>(in, static_cast<__half*>(out), seq_off, N, K, ldk);
+  else patch_rows_packed_kernel<InT, __nv_bfloat16><<<grid, 256, 0, stream>>>(in, static_cast<__nv_bfloat16*>(out), seq_off, N, K, ldk);
+}
+
+int patch_rows_packed_run(const void* pv, int in_type, int N, int K, const int* seq_off, int B, int max_rows, void* out, int out_type, int ldk,
+                          cudaStream_t stream) {
+  if (B <= 0 || max_rows <= 0) return 0;
+  if (in_type < DT_F32 || in_type > DT_BF16 || out_type < DT_F32 || out_type > DT_TF32) {
+    set_last_error("patch_rows_packed: bad type codes (in %d, out %d)", in_type, out_type);
+    return -1;
+  }
+  if (K <= 0 || ldk < K || max_rows > N) { set_last_error("patch_rows_packed: bad shape (N %d, K %d, ldk %d, max_rows %d)", N, K, ldk, max_rows); return -1; }
+  if (B > 65535) { set_last_error("patch_rows_packed: %d samples exceed the grid", B); return -1; }
+  if (in_type == DT_F32) patch_rows_packed_launch<float>(pv, out, out_type, seq_off, B, max_rows, N, K, ldk, stream);
+  else if (in_type == DT_F16) patch_rows_packed_launch<__half>(pv, out, out_type, seq_off, B, max_rows, N, K, ldk, stream);
+  else patch_rows_packed_launch<__nv_bfloat16>(pv, out, out_type, seq_off, B, max_rows, N, K, ldk, stream);
   JIMM_LAUNCH_CHECK();
   return 0;
 }

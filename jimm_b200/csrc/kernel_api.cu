@@ -131,8 +131,21 @@ int jimm_k_activation(const float* x, float* y, long long n, int act, void* stre
   if (n < 0 || (n > 0 && (!x || !y))) { set_last_error("jimm_k_activation: bad arguments"); return JIMM_EINVAL; }
   return activation_run(x, y, static_cast<size_t>(n), act, static_cast<cudaStream_t>(stream));
 }
+int jimm_k_tokens_init_interp_ex(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, int mode, void* stream) {
+  return tokens_init_interp_run(x, cls, pos, g, D, B, gh, gw, mode, static_cast<cudaStream_t>(stream));
+}
 int jimm_k_tokens_init_interp(const float* cls, const float* pos, int g, int D, float* x, int B, int gh, int gw, void* stream) {
-  return tokens_init_interp_run(x, cls, pos, g, D, B, gh, gw, static_cast<cudaStream_t>(stream));
+  return jimm_k_tokens_init_interp_ex(cls, pos, g, D, x, B, gh, gw, POS_BICUBIC, stream);
+}
+int jimm_k_tokens_add_interp_packed(const float* cls, const float* pos, int g, int D, float* x, const int32_t* seq_off, const int32_t* gw, int B,
+                                    int max_S, int mode, void* stream) {
+  if (B > 0 && (!pos || !x || !seq_off || !gw || g <= 0)) { set_last_error("jimm_k_tokens_add_interp_packed: null argument or empty table"); return JIMM_EINVAL; }
+  return tokens_add_interp_packed_run(x, cls, pos, g, D, seq_off, gw, B, max_S, mode, static_cast<cudaStream_t>(stream));
+}
+int jimm_k_patch_rows_packed(const void* patches, int in_type, int N, int K, const int32_t* seq_off, int B, int max_rows, void* out, int out_type,
+                             int ldk, void* stream) {
+  if (B > 0 && (!patches || !seq_off || !out)) { set_last_error("jimm_k_patch_rows_packed: null argument"); return JIMM_EINVAL; }
+  return patch_rows_packed_run(patches, in_type, N, K, seq_off, B, max_rows, out, out_type, ldk, static_cast<cudaStream_t>(stream));
 }
 int jimm_k_embed(const int32_t* ids, const float* table, const float* pos, float* x, int B, int T, int D, int vocab, void* stream) {
   return embed_run(ids, table, pos, x, B, T, D, vocab, static_cast<cudaStream_t>(stream));

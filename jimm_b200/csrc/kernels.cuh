@@ -32,17 +32,28 @@ int patchify_run(const void* img, int in_type, int B, int H, int W, int C, int P
 // patch embeddings into rows tok_off.. (common/vit.py:231-236)
 int tokens_init_run(float* x, const float* cls, const float* pos, int B, int S, int D, cudaStream_t stream);
 
+// How the position table is resampled to another patch grid: bicubic (HF's interpolate_pos_encoding) or antialiased bilinear (SigLIP 2
+// NaFlex); both F.interpolate with align_corners=False.
+enum PosInterp : int { POS_BICUBIC = 0, POS_BILINEAR_AA = 1 };
+
 // tokens_init_run on a gh x gw patch grid for a table trained on a g x g grid: x[b, 0, :] = cls + pos[0] (cls != null), and the patch
-// rows (row-major over (gh, gw)) are the bicubic resampling of pos's g x g patch rows (F.interpolate, align_corners=False), computed
-// on the fly from 16 table rows each.  x: fp32 [B, gh*gw (+1), D]; at (gh, gw) == (g, g) the same bits as tokens_init_run.
-int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, cudaStream_t stream);
+// rows (row-major over (gh, gw)) are the resampling (mode: PosInterp) of pos's g x g patch rows, computed on the fly from 16 table rows
+// each (bicubic) or the rows under the antialias window (up to g per axis).  x: fp32 [B, gh*gw (+1), D]; at (gh, gw) == (g, g) the same
+// bits as tokens_init_run in either mode.
+int tokens_init_interp_run(float* x, const float* cls, const float* pos, int g, int D, int B, int gh, int gw, int mode, cudaStream_t stream);
 
 // Packed form of tokens_init_interp_run for B images of different grids, after the patch GEMM: image b is rows seq_off[b] ..
 // seq_off[b + 1] - 1 of x (device int32 [B + 1]), its grid is (n_b / gw[b]) x gw[b] (gw: device int32 [B]).  Its CLS row (cls != null) is
 // set to cls + pos[0]; every patch row, which holds that patch's embedding, gets the resampled table row added -- the bits the
 // per-image path gives by reduce-adding the embedding onto the table.  max_S: the longest image's rows.
 int tokens_add_interp_packed_run(float* x, const float* cls, const float* pos, int g, int D, const int* seq_off, const int* gw, int B, int max_S,
-                                 cudaStream_t stream);
+                                 int mode, cudaStream_t stream);
+
+// The patch-GEMM operand of a packed call from HuggingFace NaFlex patch rows: pv [B, N, K] of in_type (K = P*P*C in (py, px, c) order, the
+// order patchify writes), sample b's rows 0 .. n_b - 1 (n_b = seq_off[b + 1] - seq_off[b] <= max_rows <= N; seq_off device int32 [B + 1])
+// -> rows seq_off[b] + r of out [*, ldk] in out_type, columns K .. ldk - 1 zeros.  The other rows of pv are never read.
+int patch_rows_packed_run(const void* pv, int in_type, int N, int K, const int* seq_off, int B, int max_rows, void* out, int out_type, int ldk,
+                          cudaStream_t stream);
 
 // x[b, 0, :] = cls + pos[0]   (common/vit.py:231-236), fp32 residual stream [B, S, D]
 int cls_row_run(float* x, const float* cls, const float* pos, int B, int S, int D, cudaStream_t stream);

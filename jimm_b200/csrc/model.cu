@@ -147,6 +147,7 @@ struct VisionTower {
   int img = 0, P = 0, C = 0, D = 0, n = 0, n_pad = 0, S = 0, pooling = 0, pre_norm = 0, patch_bias = 0;
   int Kp = 0;  // patch GEMM K = P*P*C rounded up to a multiple of 8 (16-byte rows for TMA; the pad columns are zeros on both operands)
   bool patch_scatter = false;  // patch GEMM reduce-adds into the pos-initialised residual stream through a 3-D TMA map
+  int interp = POS_BICUBIC;    // how the position table is resampled to another patch grid (antialiased bilinear for SigLIP 2 NaFlex)
   float eps_outer = 1e-5f;
   Encoder enc;
   LinearW patch;
@@ -301,6 +302,9 @@ struct jimm_model {
 namespace jimm {
 
 static size_t cdt_size(const jimm_model* m) { return dtype_size(m->cdt); }
+
+// CLIP, SigLIP and SigLIP 2 NaFlex: a vision and a text tower and the contrastive head
+static bool dual_kind(int kind) { return kind == JIMM_CLIP || kind == JIMM_SIGLIP || kind == JIMM_SIGLIP_NAFLEX; }
 
 // The buffers of an encoder stack over `rows` rows of width D, with `big` bytes of b->big.
 static int alloc_stack(jimm_model* m, size_t rows, size_t D, size_t big, EncBufs* b) {
@@ -694,7 +698,7 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H
   // patch embed + pos (+cls)
   if (grid) {
     // resampled pos (+cls) first; the patch GEMM adds onto it (token scatter, or a residual-reading epilogue with row remap)
-    JIMM_TRY(tokens_init_interp_run(x, cls, v.pos, v.img / v.P, D, B, grid->gh, grid->gw, s));
+    JIMM_TRY(tokens_init_interp_run(x, cls, v.pos, v.img / v.P, D, B, grid->gh, grid->gw, v.interp, s));
     const int rows = v.patch_scatter ? grid->n_pad : grid->n;
     JIMM_TRY(patchify_run(img, in_dtype, B, H, W, v.C, v.P, big, m->cdt, s, v.patch_scatter ? grid->n_pad : 0, v.Kp));
     JIMM_TRY(run_gemm(m, grid->patch, big, v.patch.K, v.patch, B * rows, s));
@@ -712,10 +716,25 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H
   return run_pool(m, B, S, out, s);
 }
 
-// run_vision on B images of different sizes packed into one token stream: image b (imgs[b], NHWC H[b] x W[b]) is token rows tok[b] ..
-// tok[b + 1] - 1 (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets,
-// image by image, so row b of out is the bits run_vision gives on image b alone.
-static int run_vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, const int* tok, int max_S,
+// The pixels of a packed call: B NHWC images imgs[b] of H[b] x W[b], or (patches not null) the HuggingFace NaFlex patch rows of B
+// samples, patches [B, N, P*P*C], of which sample b's first (H[b] / P) * (W[b] / P) rows are its patches (jimm_encode_image_patches).
+struct PackedSrc {
+  const void* const* imgs = nullptr;
+  const void* patches = nullptr;
+  int N = 0;
+  size_t sample_bytes = 0;  // bytes of one sample's N patch rows
+  PackedSrc from(int b0) const {  // the samples from b0 on
+    PackedSrc p = *this;
+    if (imgs) p.imgs += b0;
+    else p.patches = static_cast<const uint8_t*>(patches) + b0 * sample_bytes;
+    return p;
+  }
+};
+
+// run_vision on B images of different sizes packed into one token stream: image b (H[b] x W[b]) is token rows tok[b] .. tok[b + 1] - 1
+// (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets, image by image,
+// so row b of out is the bits run_vision gives on image b alone.
+static int run_vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, const int* tok, int max_S,
                              float* out, cudaStream_t s) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
@@ -730,11 +749,15 @@ static int run_vision_packed(jimm_model* m, const void* const* imgs, int in_dtyp
   JIMM_CUDA_CHECK(cudaMemcpyAsync(ws.pk_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
   const PackedRows pk{ws.pk_meta, T, max_S};
   const size_t row_bytes = static_cast<size_t>(v.Kp) * cdt_size(m);
-  for (int b = 0; b < B; ++b)
-    JIMM_TRY(patchify_run(imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.enc.big) + (tok[b] + off) * row_bytes, m->cdt, s, 0,
-                          v.Kp));
+  if (src.patches) {  // NaFlex patch rows: no CLS token, so patch rows are token rows
+    JIMM_TRY(patch_rows_packed_run(src.patches, in_dtype, src.N, v.P * v.P * v.C, pk.seq_off, B, max_S, ws.enc.big, m->cdt, v.Kp, s));
+  } else {
+    for (int b = 0; b < B; ++b)
+      JIMM_TRY(patchify_run(src.imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.enc.big) + (tok[b] + off) * row_bytes, m->cdt,
+                            s, 0, v.Kp));
+  }
   JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.enc.big, v.Kp, v.patch, T, s));
-  JIMM_TRY(tokens_add_interp_packed_run(x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, s));
+  JIMM_TRY(tokens_add_interp_packed_run(x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, v.interp, s));
   if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, T, D, s));
   JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, ws.enc, &pk));
   return run_pool(m, B, 0, out, s, &pk);
@@ -989,7 +1012,7 @@ static int finalize_sub(jimm_model* m, int max_batch) {
 // pk.done() whatever the result.
 static int pack_model(jimm_model* m, Packer& pk) {
   const jimm_config_t& c = m->cfg;
-  const bool dual = c.kind == JIMM_CLIP || c.kind == JIMM_SIGLIP;
+  const bool dual = dual_kind(c.kind);
   const std::string vp = c.kind == JIMM_VIT ? "encoder." : (dual ? "vision_model." : "");
   VisionTower& v = m->vis;
   const int D = v.D, PPC0 = c.patch * c.patch * c.in_ch;
@@ -1013,7 +1036,7 @@ static int pack_model(jimm_model* m, Packer& pk) {
   JIMM_TRY(pk.encoder("text_model.", &t.enc));
   JIMM_TRY(pk.linear("text_projection", t.D, t.D, c.t_head_bias != 0, &t.head));
   JIMM_TRY(pk.upload_f32("logit_scale", {}, &m->logit_scale));
-  if (c.kind == JIMM_SIGLIP) JIMM_TRY(pk.upload_f32("logit_bias", {}, &m->logit_bias));
+  if (c.kind != JIMM_CLIP) JIMM_TRY(pk.upload_f32("logit_bias", {}, &m->logit_bias));
   return 0;
 }
 
@@ -1042,13 +1065,13 @@ static int check_heads(const char* tower, int width, int heads) {
 
 int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) {
   if (!cfg || !out) { set_last_error("jimm_model_create: null argument"); return JIMM_EINVAL; }
-  if (cfg->kind < JIMM_VIT || cfg->kind > JIMM_MAPHEAD) { set_last_error("bad kind %d", cfg->kind); return JIMM_EINVAL; }
+  if (cfg->kind < JIMM_VIT || cfg->kind > JIMM_SIGLIP_NAFLEX) { set_last_error("bad kind %d", cfg->kind); return JIMM_EINVAL; }
   const bool sub = cfg->kind == JIMM_ENCODER || cfg->kind == JIMM_MAPHEAD;  // a bare Transformer / MultiHeadAttentionPoolingHead
   if (cfg->pooling != JIMM_POOL_CLS && cfg->pooling != JIMM_POOL_MAP) {
     set_last_error("pooling_type must be either MAP or CLS.");  // common/vit.py:178
     return JIMM_EINVAL;
   }
-  const bool dual = cfg->kind == JIMM_CLIP || cfg->kind == JIMM_SIGLIP;
+  const bool dual = dual_kind(cfg->kind);
   if (check_heads(sub ? "" : "vision ", cfg->v_width, cfg->v_heads) || (dual && check_heads("text ", cfg->t_width, cfg->t_heads))) return JIMM_EINVAL;
   const int cd = cfg->compute_dtype;
   if (cd != JIMM_F32 && cd != JIMM_F16 && cd != JIMM_BF16 && cd != JIMM_F8E4M3) { set_last_error("bad compute_dtype %d", cd); return JIMM_EINVAL; }
@@ -1062,6 +1085,12 @@ int jimm_model_create(const jimm_config_t* cfg, int device, jimm_model_t** out) 
   if (sub && cfg->ctx_len <= 0) { set_last_error("sub-module handle: ctx_len (max tokens per sample) must be positive"); return JIMM_EINVAL; }
   if (!sub && (cfg->patch <= 0 || cfg->img_size < cfg->patch || cfg->in_ch <= 0)) {
     set_last_error("unsupported patch/img/channels (%d/%d/%d)", cfg->patch, cfg->img_size, cfg->in_ch);
+    return JIMM_EINVAL;
+  }
+  // SigLIP 2 NaFlex is SigLIP's tower (MAP head, no pre-norm, patch bias) on a g x g position table, img_size = g * patch
+  if (cfg->kind == JIMM_SIGLIP_NAFLEX && (cfg->pooling != JIMM_POOL_MAP || cfg->pre_norm != 0 || cfg->patch_bias != 1 || cfg->img_size % cfg->patch != 0)) {
+    set_last_error("SigLIP 2 NaFlex: needs MAP pooling, pre_norm 0, patch_bias 1 and img_size a multiple of patch (got pooling %d, pre_norm %d, "
+                   "patch_bias %d, img_size %d, patch %d)", cfg->pooling, cfg->pre_norm, cfg->patch_bias, cfg->img_size, cfg->patch);
     return JIMM_EINVAL;
   }
   // limits of the kernels, reported at construction (not on the first forward): widths are TMA rows (16-byte multiples), LayerNorm keeps
@@ -1152,7 +1181,7 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
     const size_t g = static_cast<size_t>(c.img_size / c.patch);
     JIMM_TRY(map_seq_fits(m, g * g, "the trained image size"));
   }
-  const bool dual = c.kind == JIMM_CLIP || c.kind == JIMM_SIGLIP;
+  const bool dual = dual_kind(c.kind);
 
   // ---- towers ----
   VisionTower& v = m->vis;
@@ -1163,6 +1192,7 @@ int jimm_model_finalize(jimm_model_t* m, int max_batch) {
   v.S = v.n + (v.pooling == JIMM_POOL_CLS ? 1 : 0);
   v.n_pad = ((v.n + 31) / 32) * 32;
   v.patch_scatter = !m->simt && m->epi_mode_res == 2;
+  v.interp = c.kind == JIMM_SIGLIP_NAFLEX ? POS_BILINEAR_AA : POS_BICUBIC;
   v.Kp = (c.patch * c.patch * c.in_ch + 7) / 8 * 8;  // K of the patch GEMM, zero-padded (patch 14: 588 -> 592)
   v.enc.c.D = c.v_width; v.enc.c.H = c.v_heads; v.enc.c.M = c.v_mlp; v.enc.c.L = c.v_layers;
   v.enc.c.act = c.v_act; v.enc.c.causal = 0; v.enc.c.eps = c.v_eps_block;
@@ -1364,11 +1394,11 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
 static bool packed_fit(const jimm_model* m, size_t T) { return T <= m->ws_rows && big_bytes(m, T, T) <= m->ws_big; }
 
 // B images of different sizes: chunks of consecutive images, each as many as fit (packed_fit, at most max_batch), run packed.
-static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s) {
+static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s) {
   const VisionTower& v = m->vis;
   const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
   for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
-    if (!imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
+    if (src.imgs && !src.imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
     if (H[b] < v.P || W[b] < v.P) { set_last_error("image %d: %dx%d is smaller than one %dx%d patch", b, H[b], W[b], v.P, v.P); return JIMM_EINVAL; }
     JIMM_TRY(image_map_fits(m, H[b], W[b]));
     if (!packed_fit(m, static_cast<size_t>(H[b] / v.P) * (W[b] / v.P) + off)) return image_too_large(m, H[b], W[b]);
@@ -1385,7 +1415,7 @@ static int vision_packed(jimm_model* m, const void* const* imgs, int in_dtype, i
       max_S = std::max(max_S, S);
       ++b1;
     }
-    JIMM_TRY(run_vision_packed(m, imgs + b0, in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, out + static_cast<size_t>(b0) * od, s));
+    JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, out + static_cast<size_t>(b0) * od, s));
     b0 = b1;
   }
   return 0;
@@ -1454,7 +1484,9 @@ static int encode_packed(jimm_model* m, const char* vit_fn, const void* const* i
   JIMM_TRY(check_vision(m, vit_fn));
   if (B > 0 && (!imgs || !H || !W || !out)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
-  return vision_packed(m, imgs, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
+  PackedSrc src;
+  src.imgs = imgs;
+  return vision_packed(m, src, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
@@ -1463,6 +1495,39 @@ int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dty
 
 int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
   return encode_packed(m, nullptr, imgs, in_dtype, B, H, W, out, stream);
+}
+
+// HuggingFace NaFlex patch rows: sample b is the (gh*P) x (gw*P) image of its first gh*gw rows, run through the packed chunker
+int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  if (m->cfg.kind != JIMM_SIGLIP_NAFLEX) {
+    set_last_error("jimm_encode_image_patches: the model is not a SigLIP 2 NaFlex handle (kind %d); use jimm_encode_image_packed", m->cfg.kind);
+    return JIMM_EINVAL;
+  }
+  if (B > 0 && (!patches || !grid || !out)) { set_last_error("jimm_encode_image_patches: null argument"); return JIMM_EINVAL; }
+  const VisionTower& v = m->vis;
+  std::vector<int> H(B), W(B);
+  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
+    const int gh = grid[2 * b], gw = grid[2 * b + 1];
+    if (gh < 1 || gw < 1 || gh > INT32_MAX / v.P || gw > INT32_MAX / v.P) {
+      set_last_error("jimm_encode_image_patches: sample %d has a %dx%d patch grid (each edge from 1 up)", b, gh, gw);
+      return JIMM_EINVAL;
+    }
+    if (static_cast<int64_t>(gh) * gw > N) {
+      set_last_error("jimm_encode_image_patches: sample %d has a %dx%d patch grid, %lld patches, more than its N = %d rows", b, gh, gw,
+                     static_cast<long long>(gh) * gw, N);
+      return JIMM_EINVAL;
+    }
+    H[b] = gh * v.P;
+    W[b] = gw * v.P;
+  }
+  JIMM_TRY(set_device(m));
+  PackedSrc src;
+  src.patches = patches;
+  src.N = N;
+  src.sample_bytes = static_cast<size_t>(N) * v.P * v.P * v.C * dtype_size(in_dtype);
+  return vision_packed(m, src, in_dtype, B, H.data(), W.data(), out, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {

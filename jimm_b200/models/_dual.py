@@ -61,6 +61,11 @@ class DualTower(_NativeOwner, nn.Module):
         [B_local, world*B_local], embeddings exchanged over NVLink peer memory inside the fused logits kernel.
         interpolate_pos_encoding: as in encode_image.  `image` may be a list of images of different sizes and `text` a list of token
         sequences of different lengths, as in encode_text (single process only)."""
+        return self._dual_call(image, text, interpolate_pos_encoding)
+
+    def _dual_call(self, image, text, interpolate_pos_encoding: bool, **inputs):
+        """__call__, with the further image inputs a model's _images takes (SigLIP 2 NaFlex's spatial_shapes / pixel_attention_mask;
+        single process only)."""
         import torch.distributed as dist
 
         if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and self._comm_mode != "off":
@@ -68,8 +73,11 @@ class DualTower(_NativeOwner, nn.Module):
                 raise ValueError("a list of images is not supported by the multi-GPU contrastive call; pass one [B, H, W, C] tensor per rank")
             if isinstance(text, (list, tuple)):
                 raise ValueError("a list of token sequences is not supported by the multi-GPU contrastive call; pass one [B, T] tensor per rank")
+            if any(v is not None for v in inputs.values()):
+                raise ValueError("NaFlex pixel_values (spatial_shapes / pixel_attention_mask) are not supported by the multi-GPU contrastive "
+                                 "call; pass one [B, H, W, C] tensor per rank")
             return self._call_distributed(image, text, interpolate_pos_encoding)
-        im = self._images(image, interpolate_pos_encoding)
+        im = self._images(image, interpolate_pos_encoding, **inputs)
         text = self._texts(text)
         Bt = len(text.lens) if isinstance(text, Texts) else text.shape[0]
         n = self.native(max(len(im.x), Bt), require=True, hw=im.hw if interpolate_pos_encoding else None)

@@ -1,6 +1,8 @@
-"""Mirror of jimm.models.siglip (reference: src/jimm/models/siglip.py)."""
+"""Mirror of jimm.models.siglip (reference: src/jimm/models/siglip.py), and SigLIP 2 NaFlex checkpoints on the same parameter tree."""
 
 from __future__ import annotations
+
+import math
 
 import torch
 
@@ -8,18 +10,29 @@ from .. import _lib, nn
 from ..common.transformer import g_wrap
 from ..common import hf_loader as L
 from ..common.utils import load_params_and_config
+from .._runtime import prep_patches
 from ..common.vit import VisionTransformerBase, tower_config_fields
 from ._dual import DualTower, build_text_tower
 
 
 class SigLIP(DualTower):
-    """models/siglip.py:15-174."""
+    """models/siglip.py:15-174.
+
+    naflex=True: the vision tower of a SigLIP 2 NaFlex checkpoint (HF `Siglip2Model`).  The parameter tree is SigLIP's, with a
+    (image_resolution / vision_patch_size)^2-row position table; every image keeps its own aspect ratio and patch grid, and the table is
+    resampled to that grid with F.interpolate(mode="bilinear", align_corners=False, antialias=True).  encode_image / __call__ then take the
+    HF processor's `pixel_values` [B, max_num_patches, P*P*3] with `spatial_shapes` [B, 2] (and optionally its `pixel_attention_mask`),
+    or NHWC images of any size of at least one patch (a list for different sizes), trailing pixels dropped."""
 
     def __init__(self, image_resolution: int, vision_layers: int, vision_width: int, vision_patch_size: int, context_length: int,
                  vocab_size: int, transformer_width: int, transformer_heads: int, transformer_layers: int, rngs=None,
-                 dtype=torch.float32, param_dtype=torch.float32, mesh=None):
+                 dtype=torch.float32, param_dtype=torch.float32, mesh=None, naflex: bool = False):
+        if naflex and image_resolution % vision_patch_size:
+            raise ValueError(f"naflex: image_resolution {image_resolution} must be a multiple of vision_patch_size {vision_patch_size} "
+                             "(the position table is a square grid of patches)")
         self._init_common(image_resolution, vision_layers, vision_width, vision_patch_size, context_length, vocab_size,
                           transformer_width, transformer_heads, transformer_layers, dtype)
+        object.__setattr__(self, "naflex", bool(naflex))
         g = nn._gen(rngs)
         object.__setattr__(self, "vision_heads", vision_width // 64)  # models/siglip.py:59
         # models/siglip.py:60-78: MAP pooling, patch bias, tanh-GELU, eps 1e-6
@@ -33,30 +46,68 @@ class SigLIP(DualTower):
 
     def _native_config(self) -> _lib.Config:
         cfg = _lib.Config()
-        cfg.kind = _lib.KIND_SIGLIP
+        cfg.kind = _lib.KIND_SIGLIP_NAFLEX if self.naflex else _lib.KIND_SIGLIP
         tower_config_fields(cfg, **self.vision_model._hp)
         cfg.num_classes = 0
         # text: no mask, tanh-GELU, ln_final eps 1e-6 (:104), last-token pooling (:151), Linear head with bias (:111-119,152)
         return self._text_config(cfg, act=_lib.ACT_GELU_TANH, causal=0, pool=_lib.TPOOL_LAST, head_bias=1, eps_outer=1e-6)
 
+    # ---- SigLIP 2 NaFlex inputs ----
+    def _images(self, images, interpolate_pos_encoding: bool, spatial_shapes=None, pixel_attention_mask=None):
+        """The image input of a call: on a NaFlex model the HF processor's pixel_values with spatial_shapes (prep_patches), or images of
+        any size; otherwise as for SigLIP."""
+        if spatial_shapes is None and pixel_attention_mask is None:
+            return super()._images(images, interpolate_pos_encoding or self.naflex)
+        if not self.naflex:
+            raise ValueError("spatial_shapes / pixel_attention_mask are inputs of SigLIP 2 NaFlex models (SigLIP(..., naflex=True))")
+        if spatial_shapes is None:
+            raise ValueError("pixel_attention_mask needs the spatial_shapes it was made for")
+        n = self._native
+        return prep_patches(images, spatial_shapes, pixel_attention_mask, n.cfg if n is not None else self._native_config())
+
+    def encode_image(self, image, interpolate_pos_encoding: bool = False, spatial_shapes=None, pixel_attention_mask=None) -> torch.Tensor:
+        """As DualTower.encode_image.  On a NaFlex model: `image` is the HF processor's pixel_values [B, N, P*P*3] when spatial_shapes
+        [B, 2] = (patch rows, patch columns) is given -- sample b's first rows_b * cols_b rows are its patches, the rest padding that is
+        never read; a pixel_attention_mask, if given, must be the prefix mask those shapes imply (ValueError otherwise) -- else NHWC images
+        of any size (interpolate_pos_encoding is implied)."""
+        return self._vision(image, interpolate_pos_encoding or self.naflex, encode=True, spatial_shapes=spatial_shapes,
+                            pixel_attention_mask=pixel_attention_mask)
+
+    def __call__(self, image, text, spatial_shapes=None, pixel_attention_mask=None, interpolate_pos_encoding: bool = False) -> torch.Tensor:
+        """As DualTower.__call__, with the NaFlex image inputs of encode_image (single process only)."""
+        return self._dual_call(image, text, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,
+                               pixel_attention_mask=pixel_attention_mask)
+
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "SigLIP":
         """Load a HF `SiglipModel` checkpoint (models/siglip.py:176-385): shapes always inferred from the tensors, except
-        `image_size`, which must come from config["vision_config"] (:210)."""
+        `image_size`, which must come from config["vision_config"] (:210).  A SigLIP 2 NaFlex checkpoint (`Siglip2Model`: a 2-D
+        `patch_embedding.weight`, the Linear over flattened (py, px, c) patches) loads as SigLIP(..., naflex=True): patch_size from
+        config["vision_config"], image_resolution = sqrt(num_patches) * patch_size."""
         hf, config = load_params_and_config(model_name_or_path, use_pytorch)
 
         def depth(tower, suffix):
             return max((int(k.split(".")[3]) + 1 for k in hf if k.startswith(f"{tower}.encoder.layers.") and k.endswith(suffix)), default=0)
 
         pw = hf["vision_model.embeddings.patch_embedding.weight"]
-        vision_width, vision_patch = pw.shape[0], pw.shape[3]
+        naflex = pw.ndim == 2
+        if naflex:
+            vision_width, vision_patch = pw.shape[0], int(config["vision_config"]["patch_size"])
+            num_patches = hf["vision_model.embeddings.position_embedding.weight"].shape[0]
+            g = math.isqrt(num_patches)
+            if g * g != num_patches:
+                raise ValueError(f"SigLIP 2 NaFlex checkpoint: num_patches = {num_patches} position rows is not a square grid")
+            image_resolution = g * vision_patch
+        else:
+            vision_width, vision_patch = pw.shape[0], pw.shape[3]
+            image_resolution = config["vision_config"]["image_size"]
         vocab_size, text_width = hf["text_model.embeddings.token_embedding.weight"].shape
         v_layers, t_layers = depth("vision_model", ".mlp.fc2.bias"), depth("text_model", ".self_attn.q_proj.weight")
         with nn.deferred_init():  # every parameter is replaced below
-            model = cls(image_resolution=config["vision_config"]["image_size"], vision_layers=v_layers, vision_width=vision_width,
+            model = cls(image_resolution=image_resolution, vision_layers=v_layers, vision_width=vision_width,
                         vision_patch_size=vision_patch, context_length=hf["text_model.embeddings.position_embedding.weight"].shape[0],
                         vocab_size=vocab_size, transformer_width=text_width, transformer_heads=text_width // 64, transformer_layers=t_layers,
-                        mesh=mesh, dtype=dtype, param_dtype=dtype)
+                        mesh=mesh, dtype=dtype, param_dtype=dtype, naflex=naflex)
         v, mh = "vision_model.", "vision_model.MAPHead."
         rules = [
             ("logit_scale", "logit_scale", L.ASIS),                                      # (1,) -> ()          models/siglip.py:322-323
@@ -67,7 +118,7 @@ class SigLIP(DualTower):
             ("ln_final.bias", "text_model.final_layer_norm.bias", L.ASIS),
             ("text_projection.kernel", "text_model.head.weight", L.LINEAR),
             ("text_projection.bias", "text_model.head.bias", L.ASIS),
-            (v + "patch_embeddings.kernel", v + "embeddings.patch_embedding.weight", L.CONV),
+            (v + "patch_embeddings.kernel", v + "embeddings.patch_embedding.weight", L.PATCH_LINEAR if naflex else L.CONV),
             (v + "patch_embeddings.bias", v + "embeddings.patch_embedding.bias", L.ASIS),
             (v + "position_embeddings", v + "embeddings.position_embedding.weight", L.ASIS),  # (S,D) -> (1,S,D)    :320-321
             (v + "ln_post.scale", v + "post_layernorm.weight", L.ASIS),
