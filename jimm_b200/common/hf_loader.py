@@ -98,6 +98,21 @@ def apply_mapping(model, hf: Dict[str, torch.Tensor], rules: Iterable[Tuple], *,
     assert len(unexpected) == 0, f"Some unexpected HuggingFace checkpoint parameters were not used: {sorted(unexpected)}"
 
 
+def tower_arch(tower_config: dict, field: str, width: int, hf: Dict[str, torch.Tensor], prefix: str, default_act: str):
+    """(heads, MLP width, use_quick_gelu) of one `width`-wide tower of a HF CLIP / SigLIP checkpoint from its `field` ("vision_config" /
+    "text_config") dict.  A key the dict lacks takes its default: heads width // 64, the MLP width of the `prefix` tower's first fc1
+    weight, hidden_act `default_act`.  hidden_act "quick_gelu" is QuickGELU; "gelu", "gelu_new" and "gelu_pytorch_tanh" run the tanh
+    GELU, as VisionTransformer.from_pretrained maps "gelu"; any other value raises ValueError."""
+    fc1 = hf.get(f"{prefix}.encoder.layers.0.mlp.fc1.weight")
+    heads = int(tower_config.get("num_attention_heads", width // 64))
+    mlp = int(tower_config.get("intermediate_size", fc1.shape[0] if fc1 is not None else 4 * width))
+    act = tower_config.get("hidden_act", default_act)
+    if act not in ("quick_gelu", "gelu", "gelu_new", "gelu_pytorch_tanh"):
+        raise ValueError(f"{field}.hidden_act = {act!r} is not supported: the towers run 'quick_gelu' or the tanh GELU "
+                         "('gelu', 'gelu_new', 'gelu_pytorch_tanh')")
+    return heads, mlp, act == "quick_gelu"
+
+
 def block_rules(flax_base: str, hf_base: str, names: Dict[str, str]):
     """The 16 entries of one encoder block.  `names` maps the role to the HF sub-path (they differ between ViT and CLIP / SigLIP)."""
     r = []

@@ -22,11 +22,11 @@ class MultiHeadAttentionPoolingHead(_SubModuleRunner, nn.Module):
                  dtype=None, param_dtype=None, mesh=None):
         nn.Module.__init__(self)
         self._sub_init(dtype)
-        if intermediate_size != 4 * hidden_size:
-            raise ValueError("the MAP head kernels take intermediate_size == 4 * hidden_size (the only value the reference uses, common/vit.py:175)")
+        if intermediate_size <= 0 or intermediate_size % 8:
+            raise ValueError(f"MAP head intermediate_size {intermediate_size}: the GEMM kernels take a positive multiple of 8")
         g = nn._gen(rngs)
         object.__setattr__(self, "layernorm_epsilon", layernorm_epsilon)
-        object.__setattr__(self, "_dims", (hidden_size, num_heads))
+        object.__setattr__(self, "_dims", (hidden_size, num_heads, intermediate_size))
         self.add_param("probe", nn.zeros((1, 1, hidden_size)))
         self.add_child("attn", nn.MultiHeadAttention(num_heads, hidden_size, rngs=g_wrap(g)))
         self.add_child("layernorm", nn.LayerNorm(hidden_size, layernorm_epsilon))
@@ -35,10 +35,10 @@ class MultiHeadAttentionPoolingHead(_SubModuleRunner, nn.Module):
                                             nn.Linear(intermediate_size, hidden_size, rngs=g_wrap(g))))
 
     def _sub_config(self, max_seq):
-        D, H = self._dims
+        D, H, M = self._dims
         cfg = _lib.Config()
         cfg.kind = _lib.KIND_MAPHEAD
-        cfg.v_width, cfg.v_heads, cfg.v_mlp, cfg.v_layers = D, H, 4 * D, 0
+        cfg.v_width, cfg.v_heads, cfg.v_mlp, cfg.v_layers = D, H, M, 0
         cfg.v_eps_outer = cfg.v_eps_block = float(self.layernorm_epsilon)
         cfg.ctx_len = int(max_seq)
         cfg.compute_dtype = self._sub_dtype
@@ -169,12 +169,13 @@ def tower_config_fields(cfg: _lib.Config, *, img_size, patch_size, in_channels, 
 
 
 class VisionTransformerBase(_NativeOwner, nn.Module):
-    """common/vit.py:104-248."""
+    """common/vit.py:104-248.  map_mlp_dim: the MAP head's MLP width; None is the reference's 4 * hidden_size (common/vit.py:175),
+    HF SigLIP checkpoints use the tower's intermediate_size."""
 
     def __init__(self, img_size: int, patch_size: int, in_channels: int, hidden_size: int, num_layers: int, num_heads: int,
                  mlp_dim: int, pooling_type: str = "CLS", dropout_rate: float = 0.0, use_quick_gelu: bool = False,
                  use_pre_norm: bool = False, use_patch_bias: bool = True, layernorm_epsilon: float = 1e-5, rngs=None, dtype=None,
-                 param_dtype=None, mesh=None):
+                 param_dtype=None, mesh=None, map_mlp_dim: Optional[int] = None):
         nn.Module.__init__(self)
         self._native_init(dtype)
         g = nn._gen(rngs)
@@ -192,8 +193,8 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
             pos = nn.truncated_normal(g, (1, n_patches + 1, hidden_size), 0.02)
         elif pooling_type == "MAP":
             pos = nn.truncated_normal(g, (1, n_patches, hidden_size), 0.02)
-            self.add_child("MAPHead", MultiHeadAttentionPoolingHead(hidden_size, 4 * hidden_size, num_heads, layernorm_epsilon,
-                                                                      rngs=g_wrap(g)))
+            self.add_child("MAPHead", MultiHeadAttentionPoolingHead(hidden_size, map_mlp_dim or 4 * hidden_size, num_heads,
+                                                                      layernorm_epsilon, rngs=g_wrap(g)))
         else:
             raise ValueError("pooling_type must be either MAP or CLS.")  # common/vit.py:178
         self.add_param("position_embeddings", pos)

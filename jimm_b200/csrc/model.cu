@@ -206,7 +206,7 @@ struct Workspace {
   EncBufs enc;            // [Tmax, D] (ws_rows x D), ws.big ws_big bytes
   void* pooled = nullptr; // [Bmax, D] compute dtype
   float* feat = nullptr;  // [Bmax, D] fp32 (MAP attention out-proj / residual)
-  void* mid2 = nullptr;   // [Bmax, 4*D] compute dtype (MAP MLP hidden)
+  void* mid2 = nullptr;   // [Bmax, M] compute dtype (MAP MLP hidden, M = vis.map_fc1.N)
   float* emb_i = nullptr; // [Bmax, E] fp32 encoder outputs
   float* emb_t = nullptr;
   float* nrm_i = nullptr; // normalised
@@ -454,8 +454,16 @@ struct Packer {
     JIMM_TRY(fused_proj(mp + "attn", {"key", "value"}, D, H, &v->map_kv));
     JIMM_TRY(out_proj(mp + "attn", D, H, &v->map_out));
     JIMM_TRY(upload_ln(mp + "layernorm", D, &v->map_ln));
-    JIMM_TRY(linear(mp + "mlp.layers.0", D, 4 * D, true, &v->map_fc1));  // intermediate_size = 4*hidden (common/vit.py:175)
-    JIMM_TRY(linear(mp + "mlp.layers.2", 4 * D, D, true, &v->map_fc2));
+    // the MLP width is that of the staged (D, M) fc1 kernel: 4 * D in the reference's towers (common/vit.py:175), the checkpoint's
+    // intermediate_size in HF SigLIP (4304 in so400m)
+    auto fc1 = m->host.find(mp + "mlp.layers.0.kernel");
+    const int M = fc1 != m->host.end() && fc1->second.shape.size() == 2 ? static_cast<int>(fc1->second.shape[1]) : 4 * D;
+    if (M <= 0 || M % 8 != 0) {
+      set_last_error("MAP head mlp width %d (%smlp.layers.0.kernel): must be a positive multiple of 8", M, mp.c_str());
+      return JIMM_EINVAL;
+    }
+    JIMM_TRY(linear(mp + "mlp.layers.0", D, M, true, &v->map_fc1));
+    JIMM_TRY(linear(mp + "mlp.layers.2", M, D, true, &v->map_fc2));
     // probe query is input independent: q = probe . Wq + bq  (common/vit.py:96-97), done once on the host in fp64
     HostParam* probe = find(mp + "probe", {1, 1, D});
     HostParam* wq = find(mp + "attn.query.kernel", {D, H, d});
@@ -587,13 +595,13 @@ static int plan_encoder(jimm_model* m, Encoder* enc, int Tmax, const EncBufs& ws
 static int plan_map_head(jimm_model* m, int Bm, int Tv) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
-  const int D = v.D;
+  const int D = v.D, M = v.map_fc1.N;
   JIMM_TRY(gemm_plan_init(&v.p_map_kv, m->cdt, ws.enc.h, D, v.map_kv.w, D, Tv, 2 * D, D, epi_plain(v.map_kv, ACT_NONE, ws.enc.big, m->adt, 2 * D, m->epi_mode_16)));
   JIMM_TRY(gemm_plan_init(&v.p_map_out, m->cdt, ws.pooled, D, v.map_out.w, D, Bm, D, D, epi_plain(v.map_out, ACT_NONE, ws.feat, DT_F32, D, 0)));
-  JIMM_TRY(gemm_plan_init(&v.p_map_fc1, m->cdt, ws.pooled, D, v.map_fc1.w, D, Bm, 4 * D, D, epi_plain(v.map_fc1, ACT_GELU_TANH, ws.mid2, m->cdt, 4 * D, 0)));
+  JIMM_TRY(gemm_plan_init(&v.p_map_fc1, m->cdt, ws.pooled, D, v.map_fc1.w, D, Bm, M, D, epi_plain(v.map_fc1, ACT_GELU_TANH, ws.mid2, m->cdt, M, 0)));
   GemmEpilogue e = epi_plain(v.map_fc2, ACT_NONE, ws.out_dev, DT_F32, D, 0);
   e.residual = ws.feat; e.ldr = D;
-  JIMM_TRY(gemm_plan_init(&v.p_map_fc2, m->cdt, ws.mid2, 4 * D, v.map_fc2.w, 4 * D, Bm, D, 4 * D, e));
+  JIMM_TRY(gemm_plan_init(&v.p_map_fc2, m->cdt, ws.mid2, M, v.map_fc2.w, M, Bm, D, M, e));
   return 0;
 }
 
@@ -661,10 +669,10 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s,
   else JIMM_TRY(map_attention_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s)); // [B, D]
   JIMM_TRY(run_gemm(m, v.p_map_out, ws.pooled, D, v.map_out, B, s));                                 // -> feat fp32 [B, D]
   JIMM_TRY(layernorm_run(ws.feat, D, 1, 0, nullptr, v.map_ln.scale, v.map_ln.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
-  JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, 4D]
+  JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, M]
   GemmPlan p = v.p_map_fc2;  // + bias + residual(feat) -> out fp32 [B, D]
   p.epi.out = out;
-  return run_gemm(m, p, ws.mid2, 4 * D, v.map_fc2, B, s);
+  return run_gemm(m, p, ws.mid2, v.map_fc1.N, v.map_fc2, B, s);
 }
 
 // ln_post + the pooling head of B samples of S tokens (pk: the packed rows instead) in ws.x.  CLS: ln_post is per-row and only row 0 of
@@ -972,7 +980,7 @@ static int alloc_workspace(jimm_model* m, size_t Bm, size_t Tv, size_t big, size
   JIMM_TRY(alloc_stack(m, Tv, D, big, &ws.enc));
   JIMM_TRY(m->pool.alloc(&ws.pooled, Bm * D * cs));
   JIMM_TRY(m->pool.alloc(&ws.feat, Bm * D * sizeof(float)));
-  JIMM_TRY(m->pool.alloc(&ws.mid2, Bm * 4 * D * cs));
+  JIMM_TRY(m->pool.alloc(&ws.mid2, Bm * m->vis.map_fc1.N * cs));
   ws.out_dev_elems = out_elems;
   JIMM_TRY(m->pool.alloc(&ws.out_dev, out_elems * sizeof(float)));
   m->ws_rows = Tv;

@@ -16,20 +16,26 @@ class DualTower(_NativeOwner, nn.Module):
     _kind = None
 
     def _init_common(self, image_resolution, vision_layers, vision_width, vision_patch_size, context_length, vocab_size,
-                     transformer_width, transformer_heads, transformer_layers, dtype):
+                     transformer_width, transformer_heads, transformer_layers, dtype, *, vision_heads, vision_mlp_dim, text_mlp_dim,
+                     vision_quick_gelu, text_quick_gelu):
+        """The shared attributes.  vision_heads / vision_mlp_dim / text_mlp_dim None: the reference's rule, vision_width // 64 heads
+        (models/clip.py:60, models/siglip.py:59) and MLPs 4x the width."""
         nn.Module.__init__(self)
         self._native_init(dtype)
         for k, v in dict(image_resolution=image_resolution, vision_layers=vision_layers, vision_width=vision_width,
                          vision_patch_size=vision_patch_size, context_length=context_length, vocab_size=vocab_size,
                          transformer_width=transformer_width, transformer_heads=transformer_heads,
-                         transformer_layers=transformer_layers, dtype=dtype).items():
+                         transformer_layers=transformer_layers, dtype=dtype, vision_heads=vision_heads or vision_width // 64,
+                         vision_mlp_dim=vision_mlp_dim or 4 * vision_width, text_mlp_dim=text_mlp_dim or 4 * transformer_width,
+                         vision_quick_gelu=bool(vision_quick_gelu), text_quick_gelu=bool(text_quick_gelu)).items():
             object.__setattr__(self, k, v)
         object.__setattr__(self, "_comm_mode", None)
 
-    def _text_config(self, cfg: _lib.Config, *, act, causal, pool, head_bias, eps_outer):
+    def _text_config(self, cfg: _lib.Config, *, causal, pool, head_bias, eps_outer):
         cfg.ctx_len, cfg.vocab, cfg.t_width = self.context_length, self.vocab_size, self.transformer_width
-        cfg.t_heads, cfg.t_layers, cfg.t_mlp = self.transformer_heads, self.transformer_layers, self.transformer_width * 4
-        cfg.t_act, cfg.t_causal, cfg.t_pool, cfg.t_head_bias = act, causal, pool, head_bias
+        cfg.t_heads, cfg.t_layers, cfg.t_mlp = self.transformer_heads, self.transformer_layers, self.text_mlp_dim
+        cfg.t_act = _lib.ACT_QUICK_GELU if self.text_quick_gelu else _lib.ACT_GELU_TANH
+        cfg.t_causal, cfg.t_pool, cfg.t_head_bias = causal, pool, head_bias
         cfg.t_eps_outer = eps_outer
         cfg.t_eps_block = 1e-6  # Transformer default (common/transformer.py:142); CLIP does not forward 1e-5 (models/clip.py:92-104)
         cfg.compute_dtype = self._compute_dtype
@@ -143,10 +149,11 @@ class DualTower(_NativeOwner, nn.Module):
         return out
 
 
-def build_text_tower(model: DualTower, g, *, head_bias: bool, layernorm_epsilon, use_quick_gelu: bool, attn_mask):
+def build_text_tower(model: DualTower, g, *, head_bias: bool, layernorm_epsilon, attn_mask):
     Dt, T, V = model.transformer_width, model.context_length, model.vocab_size
-    model.add_child("text_model", Transformer(width=Dt, mlp_dim=Dt * 4, layers=model.transformer_layers, num_heads=model.transformer_heads,
-                                              dropout_rate=0.0, attn_mask=attn_mask, use_quick_gelu=use_quick_gelu,
+    model.add_child("text_model", Transformer(width=Dt, mlp_dim=model.text_mlp_dim, layers=model.transformer_layers,
+                                              num_heads=model.transformer_heads, dropout_rate=0.0, attn_mask=attn_mask,
+                                              use_quick_gelu=model.text_quick_gelu,
                                               layernorm_epsilon=layernorm_epsilon, rngs=g_wrap(g)))
     model.add_child("token_embedding", nn.Embed(V, Dt, rngs=g_wrap(g)))
     model.add_param("positional_embedding", nn.truncated_normal(g, (T, Dt), 0.02))

@@ -2,6 +2,8 @@
 
 from __future__ import annotations
 
+from typing import Optional
+
 import torch
 
 from .. import _lib, nn
@@ -13,23 +15,30 @@ from ._dual import DualTower, build_text_tower
 
 
 class CLIP(DualTower):
-    """models/clip.py:15-188."""
+    """models/clip.py:15-188.
+
+    vision_heads, vision_mlp_dim, text_mlp_dim, vision_quick_gelu, text_quick_gelu: the architecture of checkpoints that depart from the
+    reference's rule (vision_width // 64 heads, MLPs 4x the width, QuickGELU on both towers), such as OpenCLIP's ViT-H/14 (16 heads of
+    80, tanh GELU where HF declares hidden_act "gelu").  None / the defaults are the reference's values."""
 
     def __init__(self, image_resolution: int, vision_layers: int, vision_width: int, vision_patch_size: int, context_length: int,
                  vocab_size: int, transformer_width: int, transformer_heads: int, transformer_layers: int, rngs=None,
-                 dtype=torch.float32, param_dtype=torch.float32, mesh=None):
+                 dtype=torch.float32, param_dtype=torch.float32, mesh=None, vision_heads: Optional[int] = None,
+                 vision_mlp_dim: Optional[int] = None, text_mlp_dim: Optional[int] = None, vision_quick_gelu: bool = True,
+                 text_quick_gelu: bool = True):
         self._init_common(image_resolution, vision_layers, vision_width, vision_patch_size, context_length, vocab_size,
-                          transformer_width, transformer_heads, transformer_layers, dtype)
+                          transformer_width, transformer_heads, transformer_layers, dtype, vision_heads=vision_heads,
+                          vision_mlp_dim=vision_mlp_dim, text_mlp_dim=text_mlp_dim, vision_quick_gelu=vision_quick_gelu,
+                          text_quick_gelu=text_quick_gelu)
         g = nn._gen(rngs)
-        vision_heads = vision_width // 64  # models/clip.py:60
         object.__setattr__(self, "attn_mask", torch.tril(torch.ones(context_length, context_length)))  # :62
         # models/clip.py:64-81: pre-norm, no patch bias, QuickGELU, CLS, eps 1e-5
         self.add_child("vision_model", VisionTransformerBase(
             img_size=image_resolution, patch_size=vision_patch_size, in_channels=3, hidden_size=vision_width,
-            num_layers=vision_layers, num_heads=vision_heads, mlp_dim=vision_width * 4, use_pre_norm=True, use_patch_bias=False,
-            use_quick_gelu=True, pooling_type="CLS", layernorm_epsilon=1e-5, dtype=dtype, rngs=g_wrap(g)))
+            num_layers=vision_layers, num_heads=self.vision_heads, mlp_dim=self.vision_mlp_dim, use_pre_norm=True, use_patch_bias=False,
+            use_quick_gelu=self.vision_quick_gelu, pooling_type="CLS", layernorm_epsilon=1e-5, dtype=dtype, rngs=g_wrap(g)))
         self.add_child("visual_projection", nn.Linear(vision_width, transformer_width, use_bias=False, rngs=g_wrap(g)))
-        build_text_tower(self, g, head_bias=False, layernorm_epsilon=1e-6, use_quick_gelu=True, attn_mask=self.attn_mask)
+        build_text_tower(self, g, head_bias=False, layernorm_epsilon=1e-6, attn_mask=self.attn_mask)
         self.add_param("logit_scale", nn.ones(()))
 
     def _native_config(self) -> _lib.Config:
@@ -38,11 +47,13 @@ class CLIP(DualTower):
         tower_config_fields(cfg, **self.vision_model._hp)
         cfg.num_classes = 0
         # text: causal tril mask (:62,:98), QuickGELU (:99), ln_final eps 1e-5 (:117), EOT = argmax(ids) pooling (:164), bias-free projection (:166)
-        return self._text_config(cfg, act=_lib.ACT_QUICK_GELU, causal=1, pool=_lib.TPOOL_EOT_ARGMAX, head_bias=0, eps_outer=1e-5)
+        return self._text_config(cfg, causal=1, pool=_lib.TPOOL_EOT_ARGMAX, head_bias=0, eps_outer=1e-5)
 
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "CLIP":
-        """Load a HF `CLIPModel` checkpoint (models/clip.py:190-416)."""
+        """Load a HF `CLIPModel` checkpoint (models/clip.py:190-416).  Heads, MLP widths and hidden_act of each tower come from
+        config.json's vision_config / text_config (hf_loader.tower_arch); without a config.json, heads are width // 64, the MLP widths
+        those of the fc1 weights and both towers QuickGELU."""
         hf, config = load_params_and_config(model_name_or_path, use_pytorch)
         if config == {}:
             if use_pytorch:
@@ -64,11 +75,14 @@ class CLIP(DualTower):
                                   "image_size": grid * vp, "patch_size": vp},
             }
         tc, vc = config["text_config"], config["vision_config"]
+        v_heads, v_mlp, v_quick = L.tower_arch(vc, "vision_config", vc["hidden_size"], hf, "vision_model", "quick_gelu")
+        t_heads, t_mlp, t_quick = L.tower_arch(tc, "text_config", tc["hidden_size"], hf, "text_model", "quick_gelu")
         with nn.deferred_init():  # every parameter is replaced below (and asserted to be)
             model = cls(image_resolution=vc["image_size"], vision_layers=vc["num_hidden_layers"], vision_width=vc["hidden_size"],
                         vision_patch_size=vc["patch_size"], context_length=tc["max_position_embeddings"], vocab_size=tc["vocab_size"],
-                        transformer_width=tc["hidden_size"], transformer_heads=tc["num_attention_heads"],
-                        transformer_layers=tc["num_hidden_layers"], mesh=mesh, dtype=dtype, param_dtype=dtype)
+                        transformer_width=tc["hidden_size"], transformer_heads=t_heads, transformer_layers=tc["num_hidden_layers"],
+                        mesh=mesh, dtype=dtype, param_dtype=dtype, vision_heads=v_heads, vision_mlp_dim=v_mlp, text_mlp_dim=t_mlp,
+                        vision_quick_gelu=v_quick, text_quick_gelu=t_quick)
         v = "vision_model."
         rules = [
             ("logit_scale", "logit_scale", L.ASIS),

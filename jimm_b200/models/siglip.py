@@ -3,6 +3,7 @@
 from __future__ import annotations
 
 import math
+from typing import Optional
 
 import torch
 
@@ -22,25 +23,36 @@ class SigLIP(DualTower):
     (image_resolution / vision_patch_size)^2-row position table; every image keeps its own aspect ratio and patch grid, and the table is
     resampled to that grid with F.interpolate(mode="bilinear", align_corners=False, antialias=True).  encode_image / __call__ then take the
     HF processor's `pixel_values` [B, max_num_patches, P*P*3] with `spatial_shapes` [B, 2] (and optionally its `pixel_attention_mask`),
-    or NHWC images of any size of at least one patch (a list for different sizes), trailing pixels dropped."""
+    or NHWC images of any size of at least one patch (a list for different sizes), trailing pixels dropped.
+
+    vision_heads, vision_mlp_dim, text_mlp_dim, vision_quick_gelu, text_quick_gelu: the architecture of checkpoints that depart from the
+    reference's rule (vision_width // 64 heads, MLPs 4x the width, tanh GELU), such as so400m (16 heads of 72 and MLPs 4304 wide on
+    both towers).  The MAP head's MLP is vision_mlp_dim wide, as in HF's SigLIP; its GELU is always tanh.  None / the defaults are the
+    reference's values."""
 
     def __init__(self, image_resolution: int, vision_layers: int, vision_width: int, vision_patch_size: int, context_length: int,
                  vocab_size: int, transformer_width: int, transformer_heads: int, transformer_layers: int, rngs=None,
-                 dtype=torch.float32, param_dtype=torch.float32, mesh=None, naflex: bool = False):
+                 dtype=torch.float32, param_dtype=torch.float32, mesh=None, naflex: bool = False, vision_heads: Optional[int] = None,
+                 vision_mlp_dim: Optional[int] = None, text_mlp_dim: Optional[int] = None, vision_quick_gelu: bool = False,
+                 text_quick_gelu: bool = False):
         if naflex and image_resolution % vision_patch_size:
             raise ValueError(f"naflex: image_resolution {image_resolution} must be a multiple of vision_patch_size {vision_patch_size} "
                              "(the position table is a square grid of patches)")
+        if vision_quick_gelu:
+            raise ValueError("vision_quick_gelu: the MAP head runs the tanh GELU, so the vision tower of SigLIP cannot be QuickGELU")
         self._init_common(image_resolution, vision_layers, vision_width, vision_patch_size, context_length, vocab_size,
-                          transformer_width, transformer_heads, transformer_layers, dtype)
+                          transformer_width, transformer_heads, transformer_layers, dtype, vision_heads=vision_heads,
+                          vision_mlp_dim=vision_mlp_dim, text_mlp_dim=text_mlp_dim, vision_quick_gelu=vision_quick_gelu,
+                          text_quick_gelu=text_quick_gelu)
         object.__setattr__(self, "naflex", bool(naflex))
         g = nn._gen(rngs)
-        object.__setattr__(self, "vision_heads", vision_width // 64)  # models/siglip.py:59
-        # models/siglip.py:60-78: MAP pooling, patch bias, tanh-GELU, eps 1e-6
+        # models/siglip.py:59-78: MAP pooling, patch bias, tanh-GELU, eps 1e-6
         self.add_child("vision_model", VisionTransformerBase(
             img_size=image_resolution, patch_size=vision_patch_size, in_channels=3, hidden_size=vision_width,
-            num_layers=vision_layers, num_heads=self.vision_heads, mlp_dim=vision_width * 4, use_pre_norm=False,
-            use_patch_bias=True, use_quick_gelu=False, pooling_type="MAP", layernorm_epsilon=1e-6, dtype=dtype, rngs=g_wrap(g)))
-        build_text_tower(self, g, head_bias=True, layernorm_epsilon=1e-6, use_quick_gelu=False, attn_mask=None)
+            num_layers=vision_layers, num_heads=self.vision_heads, mlp_dim=self.vision_mlp_dim, use_pre_norm=False,
+            use_patch_bias=True, use_quick_gelu=False, pooling_type="MAP", layernorm_epsilon=1e-6, dtype=dtype, rngs=g_wrap(g),
+            map_mlp_dim=self.vision_mlp_dim))
+        build_text_tower(self, g, head_bias=True, layernorm_epsilon=1e-6, attn_mask=None)
         self.add_param("logit_scale", nn.ones(()))
         self.add_param("logit_bias", nn.ones(()))
 
@@ -50,7 +62,7 @@ class SigLIP(DualTower):
         tower_config_fields(cfg, **self.vision_model._hp)
         cfg.num_classes = 0
         # text: no mask, tanh-GELU, ln_final eps 1e-6 (:104), last-token pooling (:151), Linear head with bias (:111-119,152)
-        return self._text_config(cfg, act=_lib.ACT_GELU_TANH, causal=0, pool=_lib.TPOOL_LAST, head_bias=1, eps_outer=1e-6)
+        return self._text_config(cfg, causal=0, pool=_lib.TPOOL_LAST, head_bias=1, eps_outer=1e-6)
 
     # ---- SigLIP 2 NaFlex inputs ----
     def _images(self, images, interpolate_pos_encoding: bool, spatial_shapes=None, pixel_attention_mask=None):
@@ -81,7 +93,8 @@ class SigLIP(DualTower):
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "SigLIP":
         """Load a HF `SiglipModel` checkpoint (models/siglip.py:176-385): shapes always inferred from the tensors, except
-        `image_size`, which must come from config["vision_config"] (:210).  A SigLIP 2 NaFlex checkpoint (`Siglip2Model`: a 2-D
+        `image_size`, which must come from config["vision_config"] (:210), and each tower's heads, MLP width and hidden_act, which come
+        from config["vision_config"] / config["text_config"] (hf_loader.tower_arch).  A SigLIP 2 NaFlex checkpoint (`Siglip2Model`: a 2-D
         `patch_embedding.weight`, the Linear over flattened (py, px, c) patches) loads as SigLIP(..., naflex=True): patch_size from
         config["vision_config"], image_resolution = sqrt(num_patches) * patch_size."""
         hf, config = load_params_and_config(model_name_or_path, use_pytorch)
@@ -103,11 +116,14 @@ class SigLIP(DualTower):
             image_resolution = config["vision_config"]["image_size"]
         vocab_size, text_width = hf["text_model.embeddings.token_embedding.weight"].shape
         v_layers, t_layers = depth("vision_model", ".mlp.fc2.bias"), depth("text_model", ".self_attn.q_proj.weight")
+        v_heads, v_mlp, v_quick = L.tower_arch(config["vision_config"], "vision_config", vision_width, hf, "vision_model", "gelu_pytorch_tanh")
+        t_heads, t_mlp, t_quick = L.tower_arch(config.get("text_config", {}), "text_config", text_width, hf, "text_model", "gelu_pytorch_tanh")
         with nn.deferred_init():  # every parameter is replaced below
             model = cls(image_resolution=image_resolution, vision_layers=v_layers, vision_width=vision_width,
                         vision_patch_size=vision_patch, context_length=hf["text_model.embeddings.position_embedding.weight"].shape[0],
-                        vocab_size=vocab_size, transformer_width=text_width, transformer_heads=text_width // 64, transformer_layers=t_layers,
-                        mesh=mesh, dtype=dtype, param_dtype=dtype, naflex=naflex)
+                        vocab_size=vocab_size, transformer_width=text_width, transformer_heads=t_heads, transformer_layers=t_layers,
+                        mesh=mesh, dtype=dtype, param_dtype=dtype, naflex=naflex, vision_heads=v_heads, vision_mlp_dim=v_mlp,
+                        text_mlp_dim=t_mlp, vision_quick_gelu=v_quick, text_quick_gelu=t_quick)
         v, mh = "vision_model.", "vision_model.MAPHead."
         rules = [
             ("logit_scale", "logit_scale", L.ASIS),                                      # (1,) -> ()          models/siglip.py:322-323

@@ -76,6 +76,43 @@ def tiny_siglip_config():
     )
 
 
+# HF checkpoint families at their real tower widths: model class, vision (width, heads, MLP width, hidden_act, patch) and text (width,
+# heads, MLP width, hidden_act).  family_config builds one at a small depth and image size.
+FAMILIES = {
+    "openai-clip-b32": ("clip", (768, 12, 3072, "quick_gelu", 32), (512, 8, 2048, "quick_gelu")),
+    "openclip-vit-h14": ("clip", (1280, 16, 5120, "gelu", 14), (1024, 16, 4096, "gelu")),
+    "openclip-vit-g14": ("clip", (1408, 16, 6144, "gelu", 14), (1024, 16, 4096, "gelu")),
+    "siglip-base": ("siglip", (768, 12, 3072, "gelu_pytorch_tanh", 16), (768, 12, 3072, "gelu_pytorch_tanh")),
+    "siglip-so400m": ("siglip", (1152, 16, 4304, "gelu_pytorch_tanh", 14), (1152, 16, 4304, "gelu_pytorch_tanh")),
+    "siglip2-giant-opt": ("siglip", (1536, 16, 6144, "gelu_pytorch_tanh", 16), (1152, 16, 4304, "gelu_pytorch_tanh")),
+    "siglip2-so400m-naflex": ("siglip2", (1152, 16, 4304, "gelu_pytorch_tanh", 16), (1152, 16, 4304, "gelu_pytorch_tanh")),
+}
+
+
+def family_config(name, vision_layers=2, text_layers=2, grid=4, context_length=16, vocab_size=100):
+    """The HF config of FAMILIES[name] with `grid` x `grid` patches per image (NaFlex: a 16 x 16 position table)."""
+    from transformers import CLIPConfig, Siglip2Config, SiglipConfig
+
+    kind, (vw, vh, vm, va, P), (tw, th, tm, ta) = FAMILIES[name]
+    v = dict(hidden_size=vw, num_attention_heads=vh, intermediate_size=vm, hidden_act=va, num_hidden_layers=vision_layers, patch_size=P)
+    t = dict(hidden_size=tw, num_attention_heads=th, intermediate_size=tm, hidden_act=ta, num_hidden_layers=text_layers,
+             max_position_embeddings=context_length, vocab_size=vocab_size)
+    if kind == "clip":
+        return CLIPConfig(text_config=dict(t, eos_token_id=vocab_size - 1, bos_token_id=vocab_size - 2, pad_token_id=1),
+                          vision_config=dict(v, image_size=grid * P), projection_dim=tw)
+    t["projection_size"] = vw  # SigLIP's text head projects to the vision width (1152 -> 1536 in giant-opt)
+    if kind == "siglip":
+        return SiglipConfig(text_config=t, vision_config=dict(v, image_size=grid * P))
+    return Siglip2Config(text_config=t, vision_config=dict(v, num_patches=256))  # the 16 x 16 table of the NaFlex checkpoints
+
+
+def hf_semantics(cfg) -> O.Semantics:
+    """The oracle in HF semantics: erf GELU on the towers whose hidden_act is "gelu", HF's LayerNorm eps in the blocks."""
+    acts = {cfg.vision_config.hidden_act, cfg.text_config.hidden_act} - {"quick_gelu"}
+    assert len(acts) <= 1, f"one GELU form for both towers, got {acts}"
+    return O.Semantics(gelu="erf" if acts == {"gelu"} else "tanh", block_eps=cfg.vision_config.layer_norm_eps)
+
+
 def rel(a, b):
     return float((a - b).abs().max() / b.abs().max())
 
@@ -106,7 +143,15 @@ def _dual_cfg(cfg) -> O.DualCfg:
     return O.DualCfg(image_resolution=v.image_size, vision_layers=v.num_hidden_layers, vision_width=v.hidden_size,
                      vision_patch_size=v.patch_size, context_length=t.max_position_embeddings, vocab_size=t.vocab_size,
                      transformer_width=t.hidden_size, transformer_heads=t.num_attention_heads,
-                     transformer_layers=t.num_hidden_layers)
+                     transformer_layers=t.num_hidden_layers, **arch_fields(cfg))
+
+
+def arch_fields(cfg) -> dict:
+    """The DualCfg fields a HF config declares beyond the reference's rule: heads, MLP widths (the MAP head's is the vision tower's,
+    as in HF's SigLIP) and each tower's activation."""
+    t, v = cfg.text_config, cfg.vision_config
+    return dict(vision_heads=v.num_attention_heads, vision_mlp=v.intermediate_size, text_mlp=t.intermediate_size,
+                map_mlp=v.intermediate_size, vision_quick_gelu=v.hidden_act == "quick_gelu", text_quick_gelu=t.hidden_act == "quick_gelu")
 
 
 def check_clip(cfg=None, B=3, dtype=torch.float64, seed=0):
@@ -117,15 +162,17 @@ def check_clip(cfg=None, B=3, dtype=torch.float64, seed=0):
     m = perturb_(CLIPModel(cfg)).eval().to(dtype)
     sd = {k: v.detach() for k, v in m.state_dict().items()}
     oc = _dual_cfg(cfg)
-    assert cfg.vision_config.num_attention_heads == oc.vision_width // 64, "jimm hard-codes vision heads = width // 64"
     p = O.hf_to_flax_clip(sd, oc)
     img = O.synthetic_images(B, oc.image_resolution, dtype=dtype)
     txt = O.synthetic_tokens(B + 1, oc.context_length, oc.vocab_size, "clip")
+    sem = hf_semantics(cfg)
     with torch.no_grad():
         ref = m(pixel_values=img.permute(0, 3, 1, 2), input_ids=txt).logits_per_image
-        out_hf = O.clip_forward(p, oc, img, txt, O.Semantics(block_eps=cfg.vision_config.layer_norm_eps))
+        ref_i, ref_t = m.get_image_features(pixel_values=img.permute(0, 3, 1, 2)).pooler_output, m.get_text_features(input_ids=txt).pooler_output
+        out_hf = O.clip_forward(p, oc, img, txt, sem)
+        ie, te = O.clip_encode_image(p, oc, img, sem), O.clip_encode_text(p, oc, txt, sem)
         out_jimm = O.clip_forward(p, oc, img, txt)
-    return dict(hf_abs=float((out_hf - ref).abs().max()), hf_rel=rel(out_hf, ref),
+    return dict(hf_abs=float((out_hf - ref).abs().max()), hf_rel=rel(out_hf, ref), img_rel=rel(ie, ref_i), txt_rel=rel(te, ref_t),
                 jimm_abs=float((out_jimm - ref).abs().max()), jimm_rel=rel(out_jimm, ref))
 
 
@@ -140,14 +187,13 @@ def check_siglip(cfg=None, B=3, dtype=torch.float64, seed=0):
         m.logit_bias.fill_(-1.7)
     sd = {k: v.detach() for k, v in m.state_dict().items()}
     oc = _dual_cfg(cfg)
-    assert cfg.vision_config.num_attention_heads == oc.vision_width // 64
-    assert cfg.text_config.num_attention_heads == oc.transformer_width // 64
     p = O.hf_to_flax_siglip(sd, oc)
     img = O.synthetic_images(B, oc.image_resolution, dtype=dtype)
     txt = O.synthetic_tokens(B + 1, oc.context_length, oc.vocab_size, "siglip")
     with torch.no_grad():
         out = m(pixel_values=img.permute(0, 3, 1, 2), input_ids=txt)
-        ie, te, lg = O.siglip_encode_image(p, oc, img), O.siglip_encode_text(p, oc, txt), O.siglip_forward(p, oc, img, txt)
+        sem = hf_semantics(cfg)
+        ie, te, lg = O.siglip_encode_image(p, oc, img, sem), O.siglip_encode_text(p, oc, txt, sem), O.siglip_forward(p, oc, img, txt, sem)
         # HF returns the un-normalised pooled outputs from the sub-models; image_embeds/text_embeds are normalised
         ref_i = m.vision_model(pixel_values=img.permute(0, 3, 1, 2)).pooler_output
         ref_t = m.text_model(input_ids=txt).pooler_output

@@ -227,6 +227,7 @@ class TowerCfg:
     use_pre_norm: bool = False
     use_patch_bias: bool = True
     layernorm_epsilon: float = 1e-5
+    map_mlp: Optional[int] = None  # MAP head MLP width; None: 4 * hidden_size (common/vit.py:175)
 
 
 def patch_embed(p: Params, prefix: str, img, cfg: TowerCfg, sem: Semantics = JIMM):
@@ -312,16 +313,37 @@ class DualCfg:
     transformer_width: int
     transformer_heads: int
     transformer_layers: int
+    # HF checkpoints that depart from the reference's rule; None is the rule: vision heads vision_width // 64 (models/clip.py:60,
+    # models/siglip.py:59), MLPs 4x the width (the MAP head's too, common/vit.py:175), QuickGELU on CLIP's towers and tanh GELU on SigLIP's
+    vision_heads: Optional[int] = None
+    vision_mlp: Optional[int] = None
+    text_mlp: Optional[int] = None
+    map_mlp: Optional[int] = None
+    vision_quick_gelu: Optional[bool] = None
+    text_quick_gelu: Optional[bool] = None
+
+    @property
+    def v_heads(self) -> int:
+        return self.vision_heads or self.vision_width // 64
+
+    @property
+    def t_mlp(self) -> int:
+        return self.text_mlp or 4 * self.transformer_width
+
+    def text_quick(self, kind: str) -> bool:
+        return (kind == "clip") if self.text_quick_gelu is None else self.text_quick_gelu
 
     def clip_tower(self) -> TowerCfg:
         # models/clip.py:60-81
+        quick = True if self.vision_quick_gelu is None else self.vision_quick_gelu
         return TowerCfg(self.image_resolution, self.vision_patch_size, 3, self.vision_width, self.vision_layers,
-                        self.vision_width // 64, self.vision_width * 4, "CLS", True, True, False, 1e-5)
+                        self.v_heads, self.vision_mlp or self.vision_width * 4, "CLS", quick, True, False, 1e-5)
 
     def siglip_tower(self) -> TowerCfg:
         # models/siglip.py:59-78
+        quick = False if self.vision_quick_gelu is None else self.vision_quick_gelu
         return TowerCfg(self.image_resolution, self.vision_patch_size, 3, self.vision_width, self.vision_layers,
-                        self.vision_width // 64, self.vision_width * 4, "MAP", False, False, True, 1e-6)
+                        self.v_heads, self.vision_mlp or self.vision_width * 4, "MAP", quick, False, True, 1e-6, self.map_mlp)
 
 
 def clip_encode_image(p: Params, cfg: DualCfg, img, sem: Semantics = JIMM):
@@ -336,7 +358,7 @@ def clip_encode_text(p: Params, cfg: DualCfg, text, sem: Semantics = JIMM):
     x = _prm(p["token_embedding.embedding"][text], sem)  # :159
     x = _out(x + _prm(p["positional_embedding"][:seq], sem), sem)  # :160
     mask = torch.tril(torch.ones(cfg.context_length, cfg.context_length, dtype=x.dtype))  # :62
-    x = transformer(p, "text_model.", x, cfg.transformer_layers, cfg.transformer_heads, True, mask, 1e-6, sem)  # :161 (eps not forwarded :92-104)
+    x = transformer(p, "text_model.", x, cfg.transformer_layers, cfg.transformer_heads, cfg.text_quick("clip"), mask, 1e-6, sem)  # :161 (eps not forwarded :92-104)
     x = layer_norm(x, p["ln_final.scale"], p["ln_final.bias"], 1e-5, sem)  # :162 (:117)
     eot = text.argmax(dim=-1)  # :164
     x = x[torch.arange(x.shape[0]), eot]
@@ -368,7 +390,7 @@ def siglip_encode_text(p: Params, cfg: DualCfg, text, sem: Semantics = JIMM):
     seq = text.shape[1]
     x = _prm(p["token_embedding.embedding"][text], sem)
     x = _out(x + _prm(p["positional_embedding"][:seq], sem), sem)
-    x = transformer(p, "text_model.", x, cfg.transformer_layers, cfg.transformer_heads, False, None, 1e-6, sem)  # :81-92 eps 1e-6
+    x = transformer(p, "text_model.", x, cfg.transformer_layers, cfg.transformer_heads, cfg.text_quick("siglip"), None, 1e-6, sem)  # :81-92 eps 1e-6
     x = layer_norm(x, p["ln_final.scale"], p["ln_final.bias"], 1e-6, sem)  # :104
     return linear(x[:, -1, :], p["text_projection.kernel"], p["text_projection.bias"], sem)  # :151-152
 
@@ -460,7 +482,7 @@ def hf_to_flax_clip(sd, cfg: DualCfg) -> Params:
     o["vision_model.ln_post.bias"] = sd["vision_model.post_layernorm.bias"]
     o["visual_projection.kernel"] = sd["visual_projection.weight"].T
     _dual_blocks(o, sd, "text_model.", "text_model.", cfg.transformer_layers, cfg.transformer_heads)
-    _dual_blocks(o, sd, "vision_model.transformer.", "vision_model.", cfg.vision_layers, cfg.vision_width // 64)
+    _dual_blocks(o, sd, "vision_model.transformer.", "vision_model.", cfg.vision_layers, cfg.v_heads)
     return {k: v.contiguous() for k, v in o.items()}
 
 
@@ -482,7 +504,7 @@ def hf_to_flax_siglip(sd, cfg: DualCfg) -> Params:
     o[v + "position_embeddings"] = pe.reshape(1, *pe.shape)
     o[v + "ln_post.scale"] = sd[v + "post_layernorm.weight"]
     o[v + "ln_post.bias"] = sd[v + "post_layernorm.bias"]
-    H = cfg.vision_width // 64
+    H = cfg.v_heads
     m = v + "MAPHead."
     o[m + "probe"] = sd[v + "head.probe"]
     o[m + "layernorm.scale"] = sd[v + "head.layernorm.weight"]
@@ -559,9 +581,10 @@ def _rand_tower(o: Params, g, prefix, t: TowerCfg):
         o[m + "attn.out.bias"] = _small(g, D)
         o[m + "layernorm.scale"] = 1.0 + _small(g, D, s=0.1)
         o[m + "layernorm.bias"] = _small(g, D, s=0.1)
-        o[m + "mlp.layers.0.kernel"] = _xavier(g, D, 4 * D, fan_in=D, fan_out=4 * D)
-        o[m + "mlp.layers.0.bias"] = _small(g, 4 * D)
-        o[m + "mlp.layers.2.kernel"] = _xavier(g, 4 * D, D, fan_in=4 * D, fan_out=D)
+        M = t.map_mlp or 4 * D
+        o[m + "mlp.layers.0.kernel"] = _xavier(g, D, M, fan_in=D, fan_out=M)
+        o[m + "mlp.layers.0.bias"] = _small(g, M)
+        o[m + "mlp.layers.2.kernel"] = _xavier(g, M, D, fan_in=M, fan_out=D)
         o[m + "mlp.layers.2.bias"] = _small(g, D)
     if t.use_pre_norm:
         o[prefix + "ln_pre.scale"] = 1.0 + _small(g, D, s=0.1)
@@ -609,7 +632,7 @@ def random_dual_params(cfg: DualCfg, kind: str, seed=0, dtype=torch.float32) -> 
     o["positional_embedding"] = _small(g, T, Dt, s=0.1)
     o["ln_final.scale"] = 1.0 + _small(g, Dt, s=0.1)
     o["ln_final.bias"] = _small(g, Dt, s=0.1)
-    _rand_blocks(o, g, "text_model.", cfg.transformer_layers, Dt, cfg.transformer_heads, 4 * Dt)
+    _rand_blocks(o, g, "text_model.", cfg.transformer_layers, Dt, cfg.transformer_heads, cfg.t_mlp)
     return cast_params(o, dtype)
 
 

@@ -17,6 +17,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+import check_vs_hf as H
 import jimm_oracle as O
 
 
@@ -102,7 +103,8 @@ def dual_cfg(cfg) -> O.DualCfg:
     g = math.isqrt(v.num_patches)
     return O.DualCfg(image_resolution=g * v.patch_size, vision_layers=v.num_hidden_layers, vision_width=v.hidden_size,
                      vision_patch_size=v.patch_size, context_length=t.max_position_embeddings, vocab_size=t.vocab_size,
-                     transformer_width=t.hidden_size, transformer_heads=t.num_attention_heads, transformer_layers=t.num_hidden_layers)
+                     transformer_width=t.hidden_size, transformer_heads=t.num_attention_heads, transformer_layers=t.num_hidden_layers,
+                     **H.arch_fields(cfg))
 
 
 def tiny_siglip2_config():
