@@ -170,6 +170,39 @@ JIMM_API int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int
  * JIMM_EINVAL before anything is enqueued.  Runs eagerly and returns without synchronising; back-to-back calls on one stream are safe. */
 JIMM_API int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, float* out, void* stream);
 
+/* -- per-token hidden states (HF output_hidden_states) of the vision and text towers ---------------------------------------------
+ * With x_k the fp32 residual stream after k of a tower's L blocks: layer k in 0 .. L returns x_k (x_0: the embeddings -- vision: patch
+ * embedding + position table, resampled on another grid, CLS row first on CLS towers, after ln_pre when the tower has it; text: token
+ * embedding + positions); JIMM_LAYER_FINAL returns the final-normed tokens, ln_post(x_L) (vision) / ln_final(x_L) (text).  Rows: per
+ * image its S = gh*gw (+1 CLS) tokens in the order the tower holds them (CLS, then patches row-major); per sequence its T tokens, those
+ * after an EOT or padding as computed.  Each request j writes out[j]: a device buffer [rows, D] row-major, contiguous, 16-byte aligned,
+ * of out_dtype (JIMM_F32: the residual stream's bits; JIMM_F16 / JIMM_BF16: those rounded to nearest even); rows = B * S (dense), the
+ * sum of the samples' token counts (packed, in sample order).  pooled (device fp32 [B, out_dim], or NULL for none) receives exactly
+ * what the matching pooled call writes: jimm_vit_forward* on a ViT / tower handle, jimm_encode_image* / jimm_encode_text* on a dual one.
+ * Without JIMM_LAYER_FINAL and pooled, only max(k) blocks run.  These calls never replay a CUDA graph and leave the graph cache as it
+ * is; they allocate nothing.  A bad request (n outside 1 .. L + 2, a layer outside 0 .. L and not JIMM_LAYER_FINAL, a bad out_dtype,
+ * a null or misaligned pointer) and every refusal of the matching pooled call is JIMM_EINVAL before anything is enqueued. */
+#define JIMM_LAYER_FINAL (-1)
+typedef struct jimm_tokens_req {
+  int n;                                   /* requests, 1 .. L + 2 */
+  const int* layers;                       /* host [n]: each 0 .. L, or JIMM_LAYER_FINAL */
+  void* const* out;                        /* host [n] of device buffers: [rows, D] row-major, contiguous */
+  int out_dtype;                           /* JIMM_F32 / JIMM_F16 / JIMM_BF16 */
+} jimm_tokens_req_t;
+/* The vision tower on images as jimm_vit_forward_hw / jimm_encode_image_hw take them (H == W == img_size: the trained size). */
+JIMM_API int jimm_image_tokens(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_tokens_req_t* req, float* pooled,
+                               void* stream);
+/* ... on images of different sizes as jimm_vit_forward_packed / jimm_encode_image_packed take them */
+JIMM_API int jimm_image_tokens_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W,
+                                      const jimm_tokens_req_t* req, float* pooled, void* stream);
+/* ... on HF NaFlex patch rows as jimm_encode_image_patches takes them (kind JIMM_SIGLIP_NAFLEX); sample b has gh*gw rows */
+JIMM_API int jimm_image_tokens_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid,
+                                       const jimm_tokens_req_t* req, float* pooled, void* stream);
+/* The text tower on ids as jimm_encode_text / jimm_encode_text_packed take them */
+JIMM_API int jimm_text_tokens(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_tokens_req_t* req, float* pooled, void* stream);
+JIMM_API int jimm_text_tokens_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_tokens_req_t* req, float* pooled,
+                                     void* stream);
+
 /* -- forward of a bare sub-module (kinds JIMM_ENCODER / JIMM_MAPHEAD; config fields used: v_width, v_heads, v_mlp, v_layers, v_act,
  *    v_eps_block, v_eps_outer, t_causal (attn_mask = tril), ctx_len = max tokens per sample, compute_dtype; parameters keyed
  *    "blocks.layers.{i}.<...>" resp. "probe", "attn.<...>", "layernorm.<...>", "mlp.layers.{0,2}.<...>") ---------------------------- */
@@ -308,6 +341,10 @@ JIMM_API int jimm_k_embed(const int32_t* ids, const float* table, const float* p
  * x): x[r] = table[clamp(ids[r], 0, vocab - 1)] + pos[r - seq_off[b]] for the rows r of sequence b, whose positions restart at 0. */
 JIMM_API int jimm_k_embed_packed(const int32_t* ids, const float* table, const float* pos, float* x, const int32_t* seq_off, int B, int T_total,
                                  int D, int vocab, void* stream);
+/* The copy of the per-token calls: out[r, :] = x[r, :] for r < rows, x fp32 [rows, D] and out [rows, D] of out_type (0 fp32: the same
+ * bits | 1 fp16 | 2 bf16: round to nearest even), both contiguous and 16-byte aligned, D a multiple of 8; nothing after rows * D
+ * elements of out is written. */
+JIMM_API int jimm_k_tokens_out(const float* x, long long rows, int D, void* out, int out_type, void* stream);
 JIMM_API int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream);
 JIMM_API int jimm_k_logits(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
                   int E, int ldl, void* stream);

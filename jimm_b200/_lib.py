@@ -38,6 +38,15 @@ class Config(C.Structure):
 
 _vp, _i, _f, _fp, _ip = C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p
 
+LAYER_FINAL = -1  # JIMM_LAYER_FINAL: the final-normed tokens
+
+
+class TokensReq(C.Structure):
+    """jimm_tokens_req_t"""
+
+    _fields_ = [("n", C.c_int), ("layers", C.POINTER(C.c_int)), ("out", C.POINTER(C.c_void_p)), ("out_dtype", C.c_int)]
+
+
 # name -> (restype, argtypes): every symbol include/jimm_b200.h declares
 class PreprocConfig(C.Structure):
     """jimm_preproc_config_t"""
@@ -76,6 +85,11 @@ SIGNATURES = {
     "jimm_encode_image_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), _fp, _vp]),
     "jimm_encode_text_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), _fp, _vp]),
     "jimm_encode_image_patches": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_i), _fp, _vp]),
+    "jimm_image_tokens": (_i, [_vp, _vp, _i, _i, _i, _i, C.POINTER(TokensReq), _fp, _vp]),
+    "jimm_image_tokens_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(TokensReq), _fp, _vp]),
+    "jimm_image_tokens_patches": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_i), C.POINTER(TokensReq), _fp, _vp]),
+    "jimm_text_tokens": (_i, [_vp, _ip, _i, _i, C.POINTER(TokensReq), _fp, _vp]),
+    "jimm_text_tokens_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), C.POINTER(TokensReq), _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -114,6 +128,7 @@ SIGNATURES = {
     "jimm_k_patch_rows_packed": (_i, [_vp, _i, _i, _i, _ip, _i, _i, _vp, _i, _i, _vp]),
     "jimm_k_embed": (_i, [_ip, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_embed_packed": (_i, [_ip, _fp, _fp, _fp, _ip, _i, _i, _i, _i, _vp]),
+    "jimm_k_tokens_out": (_i, [_fp, C.c_longlong, _i, _vp, _i, _vp]),
     "jimm_k_l2_normalize": (_i, [_fp, _fp, _i, _i, _i, _vp]),
     "jimm_k_logits": (_i, [_fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
     "jimm_k_upload_rows": (_i, [_vp, _i, C.c_longlong, C.c_longlong, _vp, _i, C.c_longlong, _vp]),

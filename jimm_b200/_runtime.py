@@ -164,6 +164,60 @@ def prep_texts(texts, context_length: int) -> Texts:
     return Texts(ids.contiguous(), lens, not ids.is_cuda)
 
 
+_TOKEN_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+class TokenLayers(NamedTuple):
+    """The layer requests of a per-token call, checked once (prep_layers)."""
+
+    codes: List[int]  # the distinct requests as the library takes them: 0 .. L, or LAYER_FINAL
+    index: List[int]  # request i is codes[index[i]]
+    single: bool  # one request (an int or None), not a list / tuple
+    dtype: torch.dtype
+
+
+def prep_layers(layers, num_layers: int, dtype) -> TokenLayers:
+    """The layer step of a per-token call on a tower of num_layers blocks: `layers` is one request or a list / tuple of them, each an int
+    k in [-(L+1), L] (x_k, the residual stream after k blocks, negative k counting from the end as Python indexing does: -1 is x_L) or
+    None (the final-normed tokens); dtype the output type, float32, float16 or bfloat16."""
+    L = int(num_layers)
+    if dtype not in _TOKEN_DTYPES:
+        raise ValueError(f"hidden states come as torch.float32, torch.float16 or torch.bfloat16, got dtype={dtype}")
+    single = layers is None or not isinstance(layers, (list, tuple))
+    reqs = [layers] if single else list(layers)
+    if not reqs:
+        raise ValueError("layers: an empty list requests nothing; pass an int, None or a non-empty list of them")
+    codes, index = [], []
+    for k in reqs:
+        if k is None:
+            c = _lib.LAYER_FINAL
+        elif isinstance(k, (int, np.integer)) and not isinstance(k, bool):
+            k = int(k)
+            if not -(L + 1) <= k <= L:
+                raise ValueError(f"layer {k} outside [-{L + 1}, {L}] for a tower of {L} blocks (0 is the embeddings, {L} the last block)")
+            c = k % (L + 1)
+        else:
+            raise ValueError(f"a layer request is an int or None, got {k!r}")
+        if c not in codes:
+            codes.append(c)
+        index.append(codes.index(c))
+    return TokenLayers(codes, index, single, dtype)
+
+
+def prep_ids(t) -> torch.Tensor:
+    """A [B, T] token-id tensor as the library takes it: int32, contiguous."""
+    t = _as_tensor(t)
+    if t.ndim != 2:
+        raise ValueError(f"expected token ids of shape [batch, context_length], got {tuple(t.shape)}")
+    return t.to(torch.int32).contiguous()
+
+
+def tokens_result(toks, req: TokenLayers, pooled, return_pooled: bool):
+    """What a per-token call returns: one result per request (a tuple for a list of requests), and the pooled output when asked."""
+    res = toks[req.index[0]] if req.single else tuple(toks[i] for i in req.index)
+    return (res, pooled) if return_pooled else res
+
+
 class PendingResult:
     """Result of an asynchronously dispatched forward: `.result()` waits for that call's work only."""
 
@@ -352,6 +406,71 @@ class NativeModel:
         out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
         self._run("jimm_encode_text", ids.to(self.device, non_blocking=True), B, T, out)
         return self._back(out, not ids.is_cuda).result()
+
+    # ---- per-token hidden states ----
+    def _tokens_call(self, name: str, inputs, rows: int, D: int, req: TokenLayers, B: int, pooled_dim: int, pooled: bool):
+        """Entry point `name` (jimm_image_tokens* / jimm_text_tokens*) on `inputs`: one [rows, D] output of req.dtype on this GPU per
+        distinct request, and the fp32 [B, pooled_dim] pooled output when asked (else None)."""
+        outs = [torch.empty((rows, D), dtype=req.dtype, device=self.device) for _ in req.codes]
+        pool = torch.empty((B, pooled_dim), dtype=torch.float32, device=self.device) if pooled else None
+        if B:
+            n = len(req.codes)
+            r = _lib.TokensReq(n, (C.c_int * n)(*req.codes), (C.c_void_p * n)(*[o.data_ptr() for o in outs]), _TORCH_TO_CODE[req.dtype])
+            self._run(name, *inputs, C.byref(r), pool if pooled else None)
+        return outs, pool
+
+    def image_tokens(self, im: Images, req: TokenLayers, pooled: bool = False):
+        """Hidden states of the vision tower on prepared images: per distinct request [B, S, D] for a batch, a list of [S_i, D] views of
+        one packed [sum S_i, D] buffer for a list or NaFlex patch rows; and the pooled output (the vision call's result) when asked.
+        Host images are copied over and run eagerly; their results come back to the host."""
+        xd = self._device_images(im.x)
+        B, D, cfg = len(xd), self.cfg.v_width, self.cfg
+        if im.grid is not None:
+            counts = [h * w for h, w in im.grid]
+            inputs = (xd, xd.dtype, B, xd.shape[1], (C.c_int * (2 * B))(*[v for hw in im.grid for v in hw]))
+            name = "jimm_image_tokens_patches"
+        elif isinstance(xd, list):
+            counts = [grid_tokens(cfg, t.shape[0], t.shape[1]) for t in xd]
+            inputs = ((C.c_void_p * B)(*[t.data_ptr() for t in xd]), xd[0].dtype if B else torch.float32, B,
+                      (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]))
+            name = "jimm_image_tokens_packed"
+        else:
+            counts = None
+            S = grid_tokens(cfg, xd.shape[1], xd.shape[2])
+            inputs = (xd, xd.dtype, B, xd.shape[1], xd.shape[2])
+            name = "jimm_image_tokens"
+        rows = sum(counts) if counts is not None else B * S
+        outs, pool = self._tokens_call(name, inputs, rows, D, req, B, self.vision_out, pooled)
+        if isinstance(xd, list) and not im.host:
+            for t in xd:  # freshly made device copies are freed only after the call's work
+                t.record_stream(torch.cuda.current_stream(self.device))
+        return self._tokens_back(outs, pool, im.host, counts, None if counts is not None else (B, S))
+
+    def text_tokens(self, ids, req: TokenLayers, pooled: bool = False):
+        """Hidden states of the text tower on a [B, T] ids tensor (per distinct request [B, T, D]) or on Texts (a list of [L_i, D] views
+        of one packed [sum L_i, D] buffer); and the pooled output (encode_text's result) when asked.  Host ids give host results."""
+        ids = self._texts(ids)
+        D = self.cfg.t_width
+        if isinstance(ids, Texts):
+            B = len(ids.lens)
+            inputs = (ids.ids.to(self.device, non_blocking=True), B, (C.c_int * max(B, 1))(*ids.lens))
+            outs, pool = self._tokens_call("jimm_text_tokens_packed", inputs, sum(ids.lens), D, req, B, self.text_out, pooled)
+            return self._tokens_back(outs, pool, ids.host, ids.lens, None)
+        B, T = ids.shape
+        outs, pool = self._tokens_call("jimm_text_tokens", (ids.to(self.device, non_blocking=True), B, T), B * T, D, req, B, self.text_out, pooled)
+        return self._tokens_back(outs, pool, not ids.is_cuda, None, (B, T))
+
+    def _tokens_back(self, outs, pool, host: bool, counts, shape):
+        """The outputs of a per-token call as its caller gets them: on the host for host inputs, [B, S, D] (shape = (B, S)) or split into
+        per-sample views of `counts` rows."""
+        if host:
+            outs = [self._back(o, True).result() for o in outs]
+            pool = self._back(pool, True).result() if pool is not None else None
+        if counts is not None:
+            outs = [list(torch.split(o, counts)) if counts else [] for o in outs]
+        else:
+            outs = [o.view(shape[0], shape[1], o.shape[1]) for o in outs]
+        return outs, pool
 
     def dual_encode(self, x: torch.Tensor, ids: torch.Tensor):
         """encode_image + encode_text of device-resident inputs with the two towers running concurrently (jimm_dual_encode)."""

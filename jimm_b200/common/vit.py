@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _lib, nn
-from .._runtime import Images, NativeModel, default_max_batch, grid_tokens, prep_images
+from .._runtime import Images, NativeModel, default_max_batch, grid_tokens, prep_images, prep_layers, tokens_result
 from .transformer import Transformer, _SubModuleRunner, g_wrap
 
 
@@ -132,6 +132,14 @@ class _NativeOwner:
         im = self._images(images, interpolate_pos_encoding, **inputs)
         return self.native(hw=im.hw if interpolate_pos_encoding else None).vision(im, encode=encode, wait=wait)
 
+    def _vision_tokens(self, images, layers, dtype, return_pooled: bool, interpolate_pos_encoding: bool, **inputs):
+        """A per-token vision call (NativeModel.image_tokens) on the inputs _vision takes.  The layers, the dtype and the images are
+        checked before any handle is built, and the handle is chosen (or rebuilt) as for the pooled call."""
+        req = prep_layers(layers, self._native_config().v_layers, dtype)
+        im = self._images(images, interpolate_pos_encoding, **inputs)
+        toks, pooled = self.native(hw=im.hw if interpolate_pos_encoding else None).image_tokens(im, req, return_pooled)
+        return tokens_result(toks, req, pooled, return_pooled)
+
     def set_max_image_size(self, height: int, width: int):
         """Size the vision workspace for interpolate_pos_encoding calls on images up to height x width: `max_batch` such images run
         in one chunk, and no call on them rebuilds the handle.  The default holds `max_batch` images of the native size (larger
@@ -224,3 +232,12 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
         only blocks when it reads the logits): returns a `PendingResult`; back-to-back calls overlap their copies with compute.  A
         list of images runs as in __call__, synchronously for host images."""
         return self._vision(img, interpolate_pos_encoding, wait=False)
+
+    def forward_tokens(self, img, layers=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False):
+        """Per-token hidden states (HF's output_hidden_states) of the inputs __call__ takes.  layers: an int k in [-(L+1), L] -- x_k, the
+        fp32 residual stream after k blocks (0: the embeddings, after ln_pre when the tower has it; negative k counts from the end, -1 is
+        x_L) -- or None, the final-normed tokens ln_post(x_L); or a list / tuple of these, giving a tuple in request order.  Each result
+        is [batch, S, hidden_size] of `dtype` (float32, float16 or bfloat16), S = patches (+1 CLS, first), patches row-major; a list of
+        images gives a list of [S_i, hidden_size].  Without None or return_pooled only the blocks up to the deepest request run.
+        return_pooled: also return __call__'s result on the same input, bit for bit: (tokens, pooled)."""
+        return self._vision_tokens(img, layers, dtype, return_pooled, interpolate_pos_encoding)

@@ -3,6 +3,7 @@
 #include <limits.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "common.cuh"
@@ -737,6 +738,54 @@ int cast_run(const float* src, void* dst, int out_type, size_t n, cudaStream_t s
   else if (out_type == DT_F16) cast_kernel<__half><<<grid, 256, 0, stream>>>(src, static_cast<__half*>(dst), n);
   else cast_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(src, static_cast<__nv_bfloat16*>(dst), n);
   JIMM_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Per-token hidden states: fp32 residual-stream rows -> the caller's buffer.  Each thread moves 8 elements per step (two 16-byte
+// loads; one 16-byte store for 16-bit outputs, two for fp32).  Launched with PDL between two encoder blocks, so it waits for the
+// previous block's FC2 reduce-add before it reads x -- every thread, before any exit, so the kernel never completes ahead of its
+// producer.
+// ------------------------------------------------------------------------------------------
+template <typename OutT>
+__global__ void __launch_bounds__(256)
+tokens_out_kernel(const float4* __restrict__ x, OutT* __restrict__ out, size_t n8) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const float4 a = x[2 * i], b = x[2 * i + 1];
+    if constexpr (sizeof(OutT) == 4) {
+      reinterpret_cast<float4*>(out)[2 * i] = a;
+      reinterpret_cast<float4*>(out)[2 * i + 1] = b;
+    } else {
+      constexpr int ot = std::is_same<OutT, __half>::value ? 1 : 2;
+      uint4 p;
+      p.x = pack2(a.x, a.y, ot);
+      p.y = pack2(a.z, a.w, ot);
+      p.z = pack2(b.x, b.y, ot);
+      p.w = pack2(b.z, b.w, ot);
+      reinterpret_cast<uint4*>(out)[i] = p;
+    }
+  }
+}
+
+int tokens_out_run(const float* x, size_t rows, int D, void* out, int out_type, cudaStream_t stream) {
+  if (D <= 0 || D % 8 != 0 || (out_type != DT_F32 && out_type != DT_F16 && out_type != DT_BF16)) {
+    set_last_error("tokens_out: D=%d must be a positive multiple of 8 and the output type fp32 / fp16 / bf16 (got %d)", D, out_type);
+    return -1;
+  }
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) % 16 != 0) {
+    set_last_error("tokens_out: x and out must be 16-byte aligned");
+    return -1;
+  }
+  if (rows == 0) return 0;
+  const size_t n8 = rows * static_cast<size_t>(D) / 8;
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>((n8 + 255) / 256, static_cast<size_t>(device_sm_count()) * 8));
+  const float4* x4 = reinterpret_cast<const float4*>(x);
+  if (out_type == DT_F32) JIMM_CUDA_CHECK(launch_k(tokens_out_kernel<float>, dim3(grid), dim3(256), 0, stream, 1, true, x4, static_cast<float*>(out), n8));
+  else if (out_type == DT_F16) JIMM_CUDA_CHECK(launch_k(tokens_out_kernel<__half>, dim3(grid), dim3(256), 0, stream, 1, true, x4, static_cast<__half*>(out), n8));
+  else JIMM_CUDA_CHECK(launch_k(tokens_out_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, stream, 1, true, x4, static_cast<__nv_bfloat16*>(out), n8));
+  note_launch();
   return 0;
 }
 

@@ -154,6 +154,10 @@ int jimm_k_embed_packed(const int32_t* ids, const float* table, const float* pos
                         int vocab, void* stream) {
   return embed_packed_run(ids, table, pos, x, seq_off, B, T_total, D, vocab, static_cast<cudaStream_t>(stream));
 }
+int jimm_k_tokens_out(const float* x, long long rows, int D, void* out, int out_type, void* stream) {
+  if (rows < 0 || (rows > 0 && (!x || !out))) { set_last_error("jimm_k_tokens_out: bad arguments"); return JIMM_EINVAL; }
+  return tokens_out_run(x, static_cast<size_t>(rows), D, out, out_type, static_cast<cudaStream_t>(stream));
+}
 int jimm_k_l2_normalize(const float* x, float* out, int ldo, int B, int E, void* stream) {
   return l2_normalize_run(x, out, ldo, B, E, static_cast<cudaStream_t>(stream));
 }

@@ -82,6 +82,11 @@ int logits_run(const float* img, const float* txt, const float* logit_scale, con
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);
 int cast_run(const float* src, void* dst, int out_type, size_t n, cudaStream_t stream);
 
+// Per-token hidden states: out[r, :] = x[r, :] for rows r < rows of a contiguous fp32 [rows, D] residual stream, out contiguous of
+// out_type DT_F32 (a bit copy) | DT_F16 | DT_BF16 (round to nearest even).  D a multiple of 8, x and out 16-byte aligned; nothing past
+// rows * D elements of out is written.  Launched with PDL: it waits for its stream predecessor before it reads x.
+int tokens_out_run(const float* x, size_t rows, int D, void* out, int out_type, cudaStream_t stream);
+
 // ---- checkpoint ingestion (pack.cu) ----
 // rows of K elements of src_type (DT_F32 | DT_F16 | DT_BF16), row-major -> dst[r * ldd + k] of out_type
 int pack_rows_run(const void* src, int src_type, size_t rows, size_t K, void* dst, int out_type, size_t ldd, cudaStream_t stream);

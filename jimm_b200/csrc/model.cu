@@ -632,10 +632,40 @@ struct PackedRows {
   int T, max_S;
 };
 
+// Where a per-token call (jimm_image_tokens* / jimm_text_tokens*) puts the hidden states of one chunk: request j copies x_layers[j]
+// (JIMM_LAYER_FINAL: the final-normed tokens) into out[j] from output row row0 on.  run_encoder runs `blocks` blocks; the pooling tail
+// runs only when the call asked for the pooled output too.
+struct TokenSink {
+  int n = 0;
+  const int* layers = nullptr;
+  void* const* out = nullptr;
+  int out_type = DT_F32;
+  size_t row0 = 0;             // the chunk's first output row
+  int blocks = 0;              // max(requested layer), or every block for JIMM_LAYER_FINAL / a pooled output
+  const LNW* ln = nullptr;     // the final norm: ln_post (vision) / ln_final (text)
+  float eps = 0.f;
+  TokenSink at(size_t r) const { TokenSink t = *this; t.row0 = r; return t; }
+};
+
+// The requests of `sink` for layer k (JIMM_LAYER_FINAL: the final norm) on the T rows of x
+static int sink_rows(const TokenSink& sink, int k, const float* x, int T, int D, cudaStream_t s) {
+  for (int j = 0; j < sink.n; ++j) {
+    if (sink.layers[j] != k) continue;
+    void* dst = static_cast<uint8_t*>(sink.out[j]) + sink.row0 * D * dtype_size(sink.out_type);
+    if (k == JIMM_LAYER_FINAL) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, sink.ln->scale, sink.ln->bias, sink.eps, dst, sink.out_type, D, T, D, s));
+    else JIMM_TRY(tokens_out_run(x, static_cast<size_t>(T), D, dst, sink.out_type, s));
+  }
+  return 0;
+}
+
 // x: fp32 [B*S, D] residual stream in ws.x (pk: the packed rows instead).  TransformerEncoder.__call__ x L (common/transformer.py:116-132,190-196).
-static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, const EncBufs& ws, const PackedRows* pk = nullptr) {
+// sink: also copy the requested layers out, and run only sink->blocks blocks.
+static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s, const EncBufs& ws, const PackedRows* pk = nullptr,
+                       const TokenSink* sink = nullptr) {
   const EncoderCfg& c = enc->c;
   const int T = pk ? pk->T : B * S;
+  const int nblocks = sink ? sink->blocks : static_cast<int>(enc->blocks.size());
+  if (sink) JIMM_TRY(sink_rows(*sink, 0, ws.x, T, c.D, s));
   // Boustrophedon schedule: every kernel walks its rows / tiles / items in the direction opposite to its producer, so it
   // starts on the data written last -- the part of the 77-310 MB activation still resident in the 50 MB L2.
   int dir = m->l2_alternate ? 1 : 0;  // the patch GEMM / embedding kernels ran forward -> the first LayerNorm runs backward
@@ -643,7 +673,8 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
   bool h_ready = false;  // ws.h already holds norm1(x) of the coming block (written by the previous block's FC2 epilogue)
   const int ln_t = m->f8 ? DT_E4M3 : m->cdt;  // the block LayerNorms feed QKV / FC1 (see plan_encoder)
   void* ln_h = m->f8 ? ws.h8 : ws.h;
-  for (BlockW& b : enc->blocks) {
+  for (int bi = 0; bi < nblocks; ++bi) {
+    BlockW& b = enc->blocks[bi];
     if (!h_ready) JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm1.scale, b.norm1.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
     JIMM_TRY(run_gemm(m, b.p_qkv, ln_h, c.D, b.qkv, T, s, flip()));
     if (pk) JIMM_TRY(attention_packed_run(ws.big, m->adt, ws.h, m->cdt, pk->seq_off, B, pk->max_S, c.H, c.D / c.H, c.causal, s, flip()));
@@ -654,7 +685,9 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
     JIMM_TRY(run_gemm(m, b.p_fc1, ln_h, c.D, b.fc1, T, s, flip()));
     JIMM_TRY(run_gemm(m, b.p_fc2, ws.big, c.M, b.fc2, T, s, flip()));  // + residual (+ the next block's norm1 -> ws.h when fused)
     h_ready = !m->simt && gemm_fuses_ln(&b.p_fc2, T);
+    if (sink) JIMM_TRY(sink_rows(*sink, bi + 1, ws.x, T, c.D, s));
   }
+  if (sink) JIMM_TRY(sink_rows(*sink, JIMM_LAYER_FINAL, ws.x, T, c.D, s));
   return 0;
 }
 
@@ -697,7 +730,8 @@ static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, con
 
 // VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  img: [B, H, W, C]; grid: null for the trained patch
 // grid, else the grid of H x W (position table resampled).  out: fp32 [B, out_dim]
-static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, const PatchGrid* grid, float* out, cudaStream_t s) {
+static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, const PatchGrid* grid, float* out, cudaStream_t s,
+                      const TokenSink* sink = nullptr) {
   VisionTower& v = m->vis;
   float* x = m->ws.enc.x;
   void* big = m->ws.enc.big;
@@ -720,7 +754,8 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H
     if (cls) JIMM_TRY(cls_row_run(x, v.cls, v.pos, B, S, D, s));
   }
   if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, B * S, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc));
+  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc, nullptr, sink));
+  if (sink && !out) return 0;
   return run_pool(m, B, S, out, s);
 }
 
@@ -743,7 +778,7 @@ struct PackedSrc {
 // (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets, image by image,
 // so row b of out is the bits run_vision gives on image b alone.
 static int run_vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, const int* tok, int max_S,
-                             float* out, cudaStream_t s) {
+                             float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
   float* x = ws.enc.x;
@@ -767,16 +802,18 @@ static int run_vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, 
   JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.enc.big, v.Kp, v.patch, T, s));
   JIMM_TRY(tokens_add_interp_packed_run(x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, v.interp, s));
   if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, T, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, ws.enc, &pk));
+  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, ws.enc, &pk, sink));
+  if (sink && !out) return 0;
   return run_pool(m, B, 0, out, s, &pk);
 }
 
 // CLIP.encode_text (models/clip.py:148-167) / SigLIP.encode_text (models/siglip.py:135-153).  out fp32 [B, Dt]
-static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
+static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
   TextTower& t = m->txt;
   TextWs& ws = m->wt;
   JIMM_TRY(embed_run(ids, t.table, t.pos, ws.enc.x, B, T, t.D, t.V, s));
-  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, ws.enc));
+  JIMM_TRY(run_encoder(m, &t.enc, B, T, s, ws.enc, nullptr, sink));
+  if (sink && !out) return 0;
   if (t.pool == JIMM_TPOOL_EOT_ARGMAX) {
     JIMM_TRY(argmax_ids_run(ids, ws.idx, B, T, s));
     JIMM_TRY(layernorm_run(ws.enc.x, t.D, T, 0, ws.idx, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.pooled, m->cdt, t.D, B, t.D, s));
@@ -792,7 +829,8 @@ static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out,
 // run_text on B token sequences of different lengths packed into one stream: sequence b is rows tok[b] .. tok[b + 1] - 1 of ids (host
 // offsets, tok[0] = 0), max_S the longest.  Positions restart at 0 in every sequence and the causal mask (CLIP) is taken within it; every
 // other kernel works row by row, so row b of out is the bits run_text gives on sequence b alone.
-static int run_text_packed(jimm_model* m, const int32_t* ids, int B, const int* tok, int max_S, float* out, cudaStream_t s) {
+static int run_text_packed(jimm_model* m, const int32_t* ids, int B, const int* tok, int max_S, float* out, cudaStream_t s,
+                           const TokenSink* sink = nullptr) {
   TextTower& t = m->txt;
   TextWs& ws = m->wt;
   // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
@@ -805,7 +843,8 @@ static int run_text_packed(jimm_model* m, const int32_t* ids, int B, const int* 
   const PackedRows pk{ws.pk_meta, tok[B], max_S};
   int* rows = ws.pk_meta + B + 1;
   JIMM_TRY(embed_packed_run(ids, t.table, t.pos, ws.enc.x, pk.seq_off, B, pk.T, t.D, t.V, s));
-  JIMM_TRY(run_encoder(m, &t.enc, B, 0, s, ws.enc, &pk));
+  JIMM_TRY(run_encoder(m, &t.enc, B, 0, s, ws.enc, &pk, sink));
+  if (sink && !out) return 0;
   if (t.pool == JIMM_TPOOL_EOT_ARGMAX) JIMM_TRY(argmax_ids_packed_run(ids, pk.seq_off, rows, B, s));
   // ln_final of the pooled rows only (group 0: the rows by index), into ws.enc.h -- free once the encoder has run -- for the head GEMM
   JIMM_TRY(layernorm_run(ws.enc.x, t.D, 0, 0, rows, t.ln_final.scale, t.ln_final.bias, t.eps_outer, ws.enc.h, m->cdt, t.D, B, t.D, s));
@@ -849,6 +888,17 @@ static int check_text_len(const jimm_model* m, int T) {
 }
 static int check_patch(const jimm_model* m, int H, int W) {
   if (H < m->vis.P || W < m->vis.P) { set_last_error("image %dx%d is smaller than one %dx%d patch", H, W, m->vis.P, m->vis.P); return JIMM_EINVAL; }
+  return 0;
+}
+
+// every length of a packed text call in 1 .. context_length
+static int check_lens(const jimm_model* m, int B, const int* len) {
+  for (int b = 0; b < B; ++b) {
+    if (len[b] <= 0 || len[b] > m->txt.T) {
+      set_last_error("sequence %d: length %d outside (0, context_length=%d]", b, len[b], m->txt.T);
+      return JIMM_EINVAL;
+    }
+  }
   return 0;
 }
 
@@ -1368,8 +1418,10 @@ static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
   return 0;
 }
 
-// Vision forward of B images of H x W.  The native size goes through exec_vision (graphs, staging); other sizes run eagerly.
-static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s) {
+// Vision forward of B images of H x W.  The native size goes through exec_vision (graphs, staging); other sizes run eagerly.  A token
+// call (sink) always runs eagerly, its chunk of images from b0 on writing from output row b0 * S on; out may then be null.
+static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s,
+                         const TokenSink* sink = nullptr) {
   const VisionTower& v = m->vis;
   JIMM_TRY(check_patch(m, H, W));
   const bool native = H == v.img && W == v.img;
@@ -1379,7 +1431,11 @@ static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, in
   const int od = vision_out_dim(m);
   return for_chunks(B, grid ? grid->chunk : m->max_batch, [&](int b0, int nb) {
     const void* src = static_cast<const uint8_t*>(img) + b0 * img_bytes;
-    float* dst = out + static_cast<size_t>(b0) * od;
+    float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
+    if (sink) {
+      const TokenSink at = sink->at(static_cast<size_t>(b0) * (grid ? grid->S : v.S));
+      return run_vision(m, src, in_dtype, nb, H, W, grid, dst, s, &at);
+    }
     return native ? exec_vision(m, src, in_dtype, nb, dst, s) : run_vision(m, src, in_dtype, nb, H, W, grid, dst, s);
   });
 }
@@ -1402,7 +1458,9 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
 static bool packed_fit(const jimm_model* m, size_t T) { return T <= m->ws_rows && big_bytes(m, T, T) <= m->ws_big; }
 
 // B images of different sizes: chunks of consecutive images, each as many as fit (packed_fit, at most max_batch), run packed.
-static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s) {
+// A token call (sink): each chunk writes from its first token row on; out may then be null.
+static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s,
+                         const TokenSink* sink = nullptr) {
   const VisionTower& v = m->vis;
   const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
   for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
@@ -1413,6 +1471,7 @@ static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int 
   }
   const int od = vision_out_dim(m);
   std::vector<int> tok;
+  size_t t0 = 0;  // the chunk's first token row
   for (int b0 = 0; b0 < B;) {
     tok.assign(1, 0);
     int b1 = b0, max_S = 0;
@@ -1423,22 +1482,37 @@ static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int 
       max_S = std::max(max_S, S);
       ++b1;
     }
-    JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, out + static_cast<size_t>(b0) * od, s));
+    float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
+    if (sink) {
+      const TokenSink at = sink->at(t0);
+      JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, dst, s, &at));
+    } else {
+      JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, dst, s));
+    }
+    t0 += tok.back();
     b0 = b1;
   }
   return 0;
 }
 
-static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s) {
+// A token call (sink) runs eagerly, the chunk from sequence b0 on writing from output row b0 * T on; out may then be null.
+static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
   return for_chunks(B, m->max_batch, [&](int b0, int nb) {
-    return exec_text(m, ids + static_cast<size_t>(b0) * T, nb, T, out + static_cast<size_t>(b0) * m->txt.D, s);
+    const int32_t* src = ids + static_cast<size_t>(b0) * T;
+    float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
+    if (sink) {
+      const TokenSink at = sink->at(static_cast<size_t>(b0) * T);
+      return run_text(m, src, nb, T, dst, s, &at);
+    }
+    return exec_text(m, src, nb, T, dst, s);
   });
 }
 
 // B token sequences of lengths len[b] (ids: their concatenation): chunks of consecutive sequences, each as many as the text workspace's
 // max_batch x context_length token rows hold (at most pk_seqs), run packed.  The chunks are cut by tokens, not by sequences: short
 // prompts fill a chunk with several times max_batch sequences, and its GEMMs with as many rows as a padded call of max_batch.
-static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s) {
+// A token call (sink): each chunk writes from its first row of ids on; out may then be null.
+static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
   const int budget = m->max_batch * m->txt.T;
   std::vector<int> tok;
   size_t r0 = 0;  // the chunk's first row of ids
@@ -1450,7 +1524,13 @@ static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len,
       max_S = std::max(max_S, len[b1]);
       ++b1;
     }
-    JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, out + static_cast<size_t>(b0) * m->txt.D, s));
+    float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
+    if (sink) {
+      const TokenSink at = sink->at(r0);
+      JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s, &at));
+    } else {
+      JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s));
+    }
     r0 += tok.back();
     b0 = b1;
   }
@@ -1505,36 +1585,47 @@ int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dt
   return encode_packed(m, nullptr, imgs, in_dtype, B, H, W, out, stream);
 }
 
-// HuggingFace NaFlex patch rows: sample b is the (gh*P) x (gw*P) image of its first gh*gw rows, run through the packed chunker
-int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
+// The checks and the packed source of a call on HuggingFace NaFlex patch rows (fn names it): a NaFlex handle, and every sample's grid
+// within its N rows; H, W [B] receive the image sizes the grids cut.
+static int naflex_src(const jimm_model* m, const char* fn, const void* patches, int in_dtype, int B, int N, const int* grid, int* H, int* W,
+                      PackedSrc* src) {
   if (m->cfg.kind != JIMM_SIGLIP_NAFLEX) {
-    set_last_error("jimm_encode_image_patches: the model is not a SigLIP 2 NaFlex handle (kind %d); use jimm_encode_image_packed", m->cfg.kind);
+    set_last_error("%s: the model is not a SigLIP 2 NaFlex handle (kind %d); use jimm_encode_image_packed", fn, m->cfg.kind);
     return JIMM_EINVAL;
   }
-  if (B > 0 && (!patches || !grid || !out)) { set_last_error("jimm_encode_image_patches: null argument"); return JIMM_EINVAL; }
   const VisionTower& v = m->vis;
-  std::vector<int> H(B), W(B);
   for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
     const int gh = grid[2 * b], gw = grid[2 * b + 1];
     if (gh < 1 || gw < 1 || gh > INT32_MAX / v.P || gw > INT32_MAX / v.P) {
-      set_last_error("jimm_encode_image_patches: sample %d has a %dx%d patch grid (each edge from 1 up)", b, gh, gw);
+      set_last_error("%s: sample %d has a %dx%d patch grid (each edge from 1 up)", fn, b, gh, gw);
       return JIMM_EINVAL;
     }
     if (static_cast<int64_t>(gh) * gw > N) {
-      set_last_error("jimm_encode_image_patches: sample %d has a %dx%d patch grid, %lld patches, more than its N = %d rows", b, gh, gw,
+      set_last_error("%s: sample %d has a %dx%d patch grid, %lld patches, more than its N = %d rows", fn, b, gh, gw,
                      static_cast<long long>(gh) * gw, N);
       return JIMM_EINVAL;
     }
     H[b] = gh * v.P;
     W[b] = gw * v.P;
   }
-  JIMM_TRY(set_device(m));
+  src->patches = patches;
+  src->N = N;
+  src->sample_bytes = static_cast<size_t>(N) * v.P * v.P * v.C * dtype_size(in_dtype);
+  return 0;
+}
+
+// HuggingFace NaFlex patch rows: sample b is the (gh*P) x (gw*P) image of its first gh*gw rows, run through the packed chunker
+int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  if (m->cfg.kind == JIMM_SIGLIP_NAFLEX && B > 0 && (!patches || !grid || !out)) {
+    set_last_error("jimm_encode_image_patches: null argument");
+    return JIMM_EINVAL;
+  }
+  std::vector<int> H(B), W(B);
   PackedSrc src;
-  src.patches = patches;
-  src.N = N;
-  src.sample_bytes = static_cast<size_t>(N) * v.P * v.P * v.C * dtype_size(in_dtype);
+  JIMM_TRY(naflex_src(m, "jimm_encode_image_patches", patches, in_dtype, B, N, grid, H.data(), W.data(), &src));
+  JIMM_TRY(set_device(m));
   return vision_packed(m, src, in_dtype, B, H.data(), W.data(), out, static_cast<cudaStream_t>(stream));
 }
 
@@ -1550,14 +1641,108 @@ int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const in
   JIMM_TRY(check_ready(m, B));
   JIMM_TRY(check_text(m));
   if (B > 0 && (!ids || !len || !out)) { set_last_error("jimm_encode_text_packed: null argument"); return JIMM_EINVAL; }
-  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
-    if (len[b] <= 0 || len[b] > m->txt.T) {
-      set_last_error("sequence %d: length %d outside (0, context_length=%d]", b, len[b], m->txt.T);
-      return JIMM_EINVAL;
-    }
-  }
+  JIMM_TRY(check_lens(m, B, len));
   JIMM_TRY(set_device(m));
   return text_packed(m, ids, B, len, out, static_cast<cudaStream_t>(stream));
+}
+
+// ---- per-token hidden states ----
+// The request of a per-token call (fn names it) on the tower with encoder `enc` and final norm (ln, eps), as the sink of its chunks.
+// pooled: the call writes the pooled output too, so every block runs.
+static int tokens_sink(const char* fn, const jimm_tokens_req_t* req, const Encoder& enc, const LNW& ln, float eps, bool pooled, TokenSink* sink) {
+  const int L = enc.c.L;
+  if (!req || !req->layers || !req->out) { set_last_error("%s: null request", fn); return JIMM_EINVAL; }
+  if (req->n < 1 || req->n > L + 2) { set_last_error("%s: %d layer requests, outside 1 .. L + 2 = %d", fn, req->n, L + 2); return JIMM_EINVAL; }
+  if (req->out_dtype != JIMM_F32 && req->out_dtype != JIMM_F16 && req->out_dtype != JIMM_BF16) {
+    set_last_error("%s: output dtype %d; hidden states are JIMM_F32, JIMM_F16 or JIMM_BF16", fn, req->out_dtype);
+    return JIMM_EINVAL;
+  }
+  int blocks = pooled ? L : 0;
+  for (int j = 0; j < req->n; ++j) {
+    const int k = req->layers[j];
+    if (k != JIMM_LAYER_FINAL && (k < 0 || k > L)) {
+      set_last_error("%s: request %d asks for layer %d, outside 0 .. %d (or JIMM_LAYER_FINAL)", fn, j, k, L);
+      return JIMM_EINVAL;
+    }
+    if (!req->out[j] || reinterpret_cast<uintptr_t>(req->out[j]) % 16 != 0) {
+      set_last_error("%s: output buffer %d is null or not 16-byte aligned", fn, j);
+      return JIMM_EINVAL;
+    }
+    blocks = std::max(blocks, k == JIMM_LAYER_FINAL ? L : k);
+  }
+  *sink = TokenSink{};
+  sink->n = req->n;
+  sink->layers = req->layers;
+  sink->out = req->out;
+  sink->out_type = req->out_dtype;
+  sink->blocks = blocks;
+  sink->ln = &ln;
+  sink->eps = eps;
+  return 0;
+}
+
+int jimm_image_tokens(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_tokens_req_t* req, float* pooled, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_vision(m, nullptr));
+  TokenSink sink;
+  JIMM_TRY(tokens_sink("jimm_image_tokens", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
+  if (B > 0 && !img) { set_last_error("jimm_image_tokens: null images"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  return vision_chunks(m, img, in_dtype, B, H, W, pooled, static_cast<cudaStream_t>(stream), &sink);
+}
+
+int jimm_image_tokens_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, const jimm_tokens_req_t* req,
+                             float* pooled, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  JIMM_TRY(check_vision(m, nullptr));
+  TokenSink sink;
+  JIMM_TRY(tokens_sink("jimm_image_tokens_packed", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
+  if (B > 0 && (!imgs || !H || !W)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  PackedSrc src;
+  src.imgs = imgs;
+  return vision_packed(m, src, in_dtype, B, H, W, pooled, static_cast<cudaStream_t>(stream), &sink);
+}
+
+int jimm_image_tokens_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, const jimm_tokens_req_t* req,
+                              float* pooled, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_image_dtype(in_dtype));
+  if (m->cfg.kind == JIMM_SIGLIP_NAFLEX && B > 0 && (!patches || !grid)) {
+    set_last_error("jimm_image_tokens_patches: null argument");
+    return JIMM_EINVAL;
+  }
+  std::vector<int> H(B), W(B);
+  PackedSrc src;
+  JIMM_TRY(naflex_src(m, "jimm_image_tokens_patches", patches, in_dtype, B, N, grid, H.data(), W.data(), &src));
+  TokenSink sink;
+  JIMM_TRY(tokens_sink("jimm_image_tokens_patches", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
+  JIMM_TRY(set_device(m));
+  return vision_packed(m, src, in_dtype, B, H.data(), W.data(), pooled, static_cast<cudaStream_t>(stream), &sink);
+}
+
+int jimm_text_tokens(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_tokens_req_t* req, float* pooled, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_text(m));
+  JIMM_TRY(check_text_len(m, T));
+  TokenSink sink;
+  JIMM_TRY(tokens_sink("jimm_text_tokens", req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, pooled != nullptr, &sink));
+  if (B > 0 && !ids) { set_last_error("jimm_text_tokens: null ids"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  return text_chunks(m, ids, B, T, pooled, static_cast<cudaStream_t>(stream), &sink);
+}
+
+int jimm_text_tokens_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_tokens_req_t* req, float* pooled, void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_text(m));
+  TokenSink sink;
+  JIMM_TRY(tokens_sink("jimm_text_tokens_packed", req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, pooled != nullptr, &sink));
+  if (B > 0 && (!ids || !len)) { set_last_error("jimm_text_tokens_packed: null argument"); return JIMM_EINVAL; }
+  JIMM_TRY(check_lens(m, B, len));
+  JIMM_TRY(set_device(m));
+  return text_packed(m, ids, B, len, pooled, static_cast<cudaStream_t>(stream), &sink);
 }
 
 int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const float* txt_e, int Bt, float* logits, void* stream) {

@@ -5,7 +5,7 @@ from __future__ import annotations
 import torch
 
 from .. import _lib, nn
-from .._runtime import Texts, _call, prep_texts
+from .._runtime import Texts, _call, prep_ids, prep_layers, prep_texts, tokens_result
 from ..common.transformer import Transformer, g_wrap
 from ..common.vit import _NativeOwner, tower_config_fields
 
@@ -60,6 +60,28 @@ class DualTower(_NativeOwner, nn.Module):
         token, so a list gives each sequence at its own length, not the padded embedding its checkpoint was trained on."""
         text = self._texts(text)
         return self.native().text(text) if isinstance(text, Texts) else self.native(text.shape[0]).text(text)
+
+    def encode_image_tokens(self, image, layers=None, *, dtype=torch.float32, return_pooled: bool = False,
+                            interpolate_pos_encoding: bool = False):
+        """Per-token hidden states of the vision tower (HF's output_hidden_states) on the inputs encode_image takes: as
+        VisionTransformerBase.forward_tokens, None being ln_post(x_L).  return_pooled: also return encode_image's result, bit for bit."""
+        return self._vision_tokens(image, layers, dtype, return_pooled, interpolate_pos_encoding)
+
+    def encode_text_tokens(self, text, layers=None, *, dtype=torch.float32, return_pooled: bool = False):
+        """Per-token hidden states of the text tower on the inputs encode_text takes.  layers: an int k in [-(L+1), L] -- x_k, the fp32
+        residual stream after k blocks (0: token embedding + positions; -1 is x_L) -- or None, the final-normed tokens ln_final(x_L); or a
+        list / tuple of these, giving a tuple in request order.  Each result is [batch, T, width] of `dtype` (float32, float16 or
+        bfloat16), every row as computed, those after an EOT or padding included; a list of sequences gives a list of [L_i, width].
+        Without None or return_pooled only the blocks up to the deepest request run.  return_pooled: also return encode_text's result,
+        bit for bit: (tokens, pooled)."""
+        req = prep_layers(layers, self.transformer_layers, dtype)
+        text = self._texts(text)
+        if not isinstance(text, Texts):
+            text = prep_ids(text)
+            if not 1 <= text.shape[1] <= self.context_length:
+                raise ValueError(f"sequence length {text.shape[1]} outside 1 .. context_length={self.context_length}")
+        toks, pooled = self.native().text_tokens(text, req, return_pooled)
+        return tokens_result(toks, req, pooled, return_pooled)
 
     def __call__(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """Similarity logits.  Single process: [B_img, B_txt].  Under torch.distributed (one process per GPU, batch sharded

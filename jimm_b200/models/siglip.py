@@ -85,6 +85,13 @@ class SigLIP(DualTower):
         return self._vision(image, interpolate_pos_encoding or self.naflex, encode=True, spatial_shapes=spatial_shapes,
                             pixel_attention_mask=pixel_attention_mask)
 
+    def encode_image_tokens(self, image, layers=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False,
+                            spatial_shapes=None, pixel_attention_mask=None):
+        """As DualTower.encode_image_tokens, with the NaFlex image inputs of encode_image: on pixel_values with spatial_shapes each
+        sample's result is [rows_b * cols_b, D] (no CLS token), its patches row-major."""
+        return self._vision_tokens(image, layers, dtype, return_pooled, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,
+                                   pixel_attention_mask=pixel_attention_mask)
+
     def __call__(self, image, text, spatial_shapes=None, pixel_attention_mask=None, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """As DualTower.__call__, with the NaFlex image inputs of encode_image (single process only)."""
         return self._dual_call(image, text, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,

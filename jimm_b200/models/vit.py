@@ -58,6 +58,11 @@ class VisionTransformer(_NativeOwner, nn.Module):
         list of images runs as in __call__, synchronously for host images."""
         return self._vision(x, interpolate_pos_encoding, wait=False)
 
+    def forward_tokens(self, x, layers=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False):
+        """Per-token hidden states of the encoder (HF's output_hidden_states; VisionTransformerBase.forward_tokens), on the inputs
+        __call__ takes.  return_pooled: also return the logits __call__ gives on the same input, bit for bit: (tokens, logits)."""
+        return self._vision_tokens(x, layers, dtype, return_pooled, interpolate_pos_encoding)
+
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "VisionTransformer":
         """Load a HF `ViTForImageClassification` checkpoint (models/vit.py:105-273): same config parsing, shape
