@@ -110,6 +110,16 @@ JIMM_API int jimm_model_output_dim(const jimm_model_t* m, int* vision_out, int* 
 JIMM_API int jimm_model_max_batch(const jimm_model_t* m);
 
 /* -- forward: device-resident inputs/outputs ---------------------------------------------------------------------- */
+/* The forward calls on device inputs (jimm_vit_forward*, jimm_encode_image*, jimm_encode_text*, jimm_image_tokens*, jimm_text_tokens*)
+ * check their arguments in one order and report the first fault, before anything is enqueued:
+ *   1. the handle: not null, finalized (else JIMM_ESTATE), B >= 0;
+ *   2. the image dtype (image calls);
+ *   3. the tower: a vision / text tower, a ViT / tower handle for jimm_vit_forward*, a JIMM_SIGLIP_NAFLEX handle for the *_patches calls;
+ *   4. the request of a per-token call;
+ *   5. when B > 0, null arguments ("<call>: null argument"): the inputs, and out on the pooled calls (pooled stays optional);
+ *   6. the shapes: image sizes, NaFlex patch grids, the workspace and the MAP head's sequence limit; sequence lengths;
+ *   7. the handle's device is made current.
+ * Every refusal is JIMM_EINVAL unless stated. */
 /* VisionTransformer.__call__ (models/vit.py:91-103) / VisionTransformerBase.__call__ (common/vit.py:216-248).
  * img: device NHWC [B,img,img,in_ch] of in_dtype; out: device fp32 [B, num_classes | v_width]. */
 JIMM_API int jimm_vit_forward(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream);

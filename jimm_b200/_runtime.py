@@ -312,12 +312,6 @@ class NativeModel:
     def _operand_dtype(self) -> torch.dtype:
         return {_lib.F32: torch.float32, _lib.F16: torch.float16, _lib.BF16: torch.bfloat16, _lib.F8E4M3: torch.float16}[self.cfg.compute_dtype]
 
-    def _prep_ids(self, t) -> torch.Tensor:
-        t = _as_tensor(t)
-        if t.ndim != 2:
-            raise ValueError(f"expected token ids of shape [batch, context_length], got {tuple(t.shape)}")
-        return t.to(torch.int32).contiguous()
-
     def _run(self, name: str, *args):
         """Entry point `name` on this handle (see _call)."""
         _call(self.lib, self.device, name, self.handle, *args)
@@ -359,25 +353,36 @@ class NativeModel:
         res = self._back(self._vision_dev(im, encode), im.host, keep=im.x).result()
         return res if wait else PendingResult(res, None)
 
+    def _image_inputs(self, im: Images, xd):
+        """The arguments of a vision call on im's images xd (on this GPU) up to `out` / `req`: the input form ("patches": NaFlex rows,
+        "packed": a list, "trained" / "dense": a batch of the trained size or not), the ctypes argument tuple (a batch's with H and W)
+        and each sample's token count (None for a batch).  Freshly made device copies of list images are freed only after the call's
+        work."""
+        B = len(xd)
+        if im.grid is not None:
+            return "patches", (xd, xd.dtype, B, xd.shape[1], (C.c_int * (2 * B))(*[v for hw in im.grid for v in hw])), [h * w for h, w in im.grid]
+        if isinstance(xd, list):
+            if not im.host:
+                for t in xd:
+                    t.record_stream(torch.cuda.current_stream(self.device))
+            args = ((C.c_void_p * B)(*[t.data_ptr() for t in xd]), xd[0].dtype if B else torch.float32, B,
+                    (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]))
+            return "packed", args, [grid_tokens(self.cfg, t.shape[0], t.shape[1]) for t in xd]
+        return "trained" if im.trained else "dense", (xd, xd.dtype, B, xd.shape[1], xd.shape[2]), None
+
     def _vision_dev(self, im: Images, encode: bool) -> torch.Tensor:
         """The vision call on the images on this GPU (host images copied over): fp32 [B, out_dim] on this GPU."""
         xd = self._device_images(im.x)
         B = len(xd)
         out = torch.empty((B, self.vision_out), dtype=torch.float32, device=self.device)
-        if im.grid is not None:
-            if B:
-                self._run("jimm_encode_image_patches", xd, xd.dtype, B, xd.shape[1], (C.c_int * (2 * B))(*[v for hw in im.grid for v in hw]), out)
-        elif isinstance(xd, list):
-            if B:
-                self._run("jimm_encode_image_packed" if encode else "jimm_vit_forward_packed", (C.c_void_p * B)(*[t.data_ptr() for t in xd]),
-                          xd[0].dtype, B, (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]), out)
-                if not im.host:
-                    for t in xd:  # freshly made device copies are freed only after the call's work
-                        t.record_stream(torch.cuda.current_stream(self.device))
-        elif im.trained:
-            self._run("jimm_encode_image" if encode else "jimm_vit_forward", xd, xd.dtype, B, out)
-        else:
-            self._run("jimm_encode_image_hw" if encode else "jimm_vit_forward_hw", xd, xd.dtype, B, xd.shape[1], xd.shape[2], out)
+        form, args, _ = self._image_inputs(im, xd)
+        name = "jimm_encode_image" if encode else "jimm_vit_forward"
+        if form == "trained":
+            self._run(name, *args[:3], out)
+        elif form == "dense":
+            self._run(name + "_hw", *args, out)
+        elif B:
+            self._run("jimm_encode_image_patches" if form == "patches" else name + "_packed", *args, out)
         return out
 
     def _texts(self, text) -> Union[torch.Tensor, Texts]:
@@ -386,26 +391,32 @@ class NativeModel:
             return text
         if isinstance(text, (list, tuple)):
             return prep_texts(text, self.cfg.ctx_len)
-        return self._prep_ids(text)
+        return prep_ids(text)
 
-    def _text_packed_dev(self, tx: Texts) -> torch.Tensor:
-        """encode_text of the sequences of a list in one packed call (jimm_encode_text_packed): fp32 [B, E] on this GPU."""
-        B = len(tx.lens)
-        out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
-        if B:
-            self._run("jimm_encode_text_packed", tx.ids.to(self.device, non_blocking=True), B, (C.c_int * B)(*tx.lens), out)
+    def _text_inputs(self, ids: Union[torch.Tensor, Texts]):
+        """The arguments of a text call on a [B, T] ids tensor or on Texts up to `out` / `req`, the ids copied to this GPU: the ctypes
+        argument tuple, each sequence's length (None for a tensor) and whether the result goes back to the host."""
+        if isinstance(ids, Texts):
+            B = len(ids.lens)
+            return (ids.ids.to(self.device, non_blocking=True), B, (C.c_int * max(B, 1))(*ids.lens)), ids.lens, ids.host
+        B, T = ids.shape
+        return (ids.to(self.device, non_blocking=True), B, T), None, not ids.is_cuda
+
+    def _text_dev(self, ids: Union[torch.Tensor, Texts]) -> torch.Tensor:
+        """encode_text of a [B, T] ids tensor, or of Texts in one packed call (jimm_encode_text_packed): fp32 [B, E] on this GPU."""
+        args, lens, _ = self._text_inputs(ids)
+        out = torch.empty((args[1], self.text_out), dtype=torch.float32, device=self.device)
+        if lens is None:
+            self._run("jimm_encode_text", *args, out)
+        elif lens:
+            self._run("jimm_encode_text_packed", *args, out)
         return out
 
     def text(self, ids) -> torch.Tensor:
         """encode_text of a [B, T] ids tensor, or of a list of sequences of different lengths (one packed call).  CUDA input -> CUDA
         output; host input -> host output."""
         ids = self._texts(ids)
-        if isinstance(ids, Texts):
-            return self._back(self._text_packed_dev(ids), ids.host).result()
-        B, T = ids.shape
-        out = torch.empty((B, self.text_out), dtype=torch.float32, device=self.device)
-        self._run("jimm_encode_text", ids.to(self.device, non_blocking=True), B, T, out)
-        return self._back(out, not ids.is_cuda).result()
+        return self._back(self._text_dev(ids), ids.host if isinstance(ids, Texts) else not ids.is_cuda).result()
 
     # ---- per-token hidden states ----
     def _tokens_call(self, name: str, inputs, rows: int, D: int, req: TokenLayers, B: int, pooled_dim: int, pooled: bool):
@@ -424,41 +435,22 @@ class NativeModel:
         one packed [sum S_i, D] buffer for a list or NaFlex patch rows; and the pooled output (the vision call's result) when asked.
         Host images are copied over and run eagerly; their results come back to the host."""
         xd = self._device_images(im.x)
-        B, D, cfg = len(xd), self.cfg.v_width, self.cfg
-        if im.grid is not None:
-            counts = [h * w for h, w in im.grid]
-            inputs = (xd, xd.dtype, B, xd.shape[1], (C.c_int * (2 * B))(*[v for hw in im.grid for v in hw]))
-            name = "jimm_image_tokens_patches"
-        elif isinstance(xd, list):
-            counts = [grid_tokens(cfg, t.shape[0], t.shape[1]) for t in xd]
-            inputs = ((C.c_void_p * B)(*[t.data_ptr() for t in xd]), xd[0].dtype if B else torch.float32, B,
-                      (C.c_int * B)(*[t.shape[0] for t in xd]), (C.c_int * B)(*[t.shape[1] for t in xd]))
-            name = "jimm_image_tokens_packed"
-        else:
-            counts = None
-            S = grid_tokens(cfg, xd.shape[1], xd.shape[2])
-            inputs = (xd, xd.dtype, B, xd.shape[1], xd.shape[2])
-            name = "jimm_image_tokens"
+        B = len(xd)
+        form, args, counts = self._image_inputs(im, xd)
+        name = {"patches": "jimm_image_tokens_patches", "packed": "jimm_image_tokens_packed"}.get(form, "jimm_image_tokens")
+        S = grid_tokens(self.cfg, xd.shape[1], xd.shape[2]) if counts is None else None
         rows = sum(counts) if counts is not None else B * S
-        outs, pool = self._tokens_call(name, inputs, rows, D, req, B, self.vision_out, pooled)
-        if isinstance(xd, list) and not im.host:
-            for t in xd:  # freshly made device copies are freed only after the call's work
-                t.record_stream(torch.cuda.current_stream(self.device))
+        outs, pool = self._tokens_call(name, args, rows, self.cfg.v_width, req, B, self.vision_out, pooled)
         return self._tokens_back(outs, pool, im.host, counts, None if counts is not None else (B, S))
 
     def text_tokens(self, ids, req: TokenLayers, pooled: bool = False):
         """Hidden states of the text tower on a [B, T] ids tensor (per distinct request [B, T, D]) or on Texts (a list of [L_i, D] views
         of one packed [sum L_i, D] buffer); and the pooled output (encode_text's result) when asked.  Host ids give host results."""
-        ids = self._texts(ids)
-        D = self.cfg.t_width
-        if isinstance(ids, Texts):
-            B = len(ids.lens)
-            inputs = (ids.ids.to(self.device, non_blocking=True), B, (C.c_int * max(B, 1))(*ids.lens))
-            outs, pool = self._tokens_call("jimm_text_tokens_packed", inputs, sum(ids.lens), D, req, B, self.text_out, pooled)
-            return self._tokens_back(outs, pool, ids.host, ids.lens, None)
-        B, T = ids.shape
-        outs, pool = self._tokens_call("jimm_text_tokens", (ids.to(self.device, non_blocking=True), B, T), B * T, D, req, B, self.text_out, pooled)
-        return self._tokens_back(outs, pool, not ids.is_cuda, None, (B, T))
+        args, lens, host = self._text_inputs(self._texts(ids))
+        B = args[1]
+        name, rows = ("jimm_text_tokens", B * args[2]) if lens is None else ("jimm_text_tokens_packed", sum(lens))
+        outs, pool = self._tokens_call(name, args, rows, self.cfg.t_width, req, B, self.text_out, pooled)
+        return self._tokens_back(outs, pool, host, lens, (B, args[2]) if lens is None else None)
 
     def _tokens_back(self, outs, pool, host: bool, counts, shape):
         """The outputs of a per-token call as its caller gets them: on the host for host inputs, [B, S, D] (shape = (B, S)) or split into
@@ -497,12 +489,12 @@ class NativeModel:
         im = images if isinstance(images, Images) else prep_images(images, self.cfg, self.preproc, interpolate)
         ids = self._texts(text)
         if isinstance(ids, Texts):
-            out = self.logits(self._vision_dev(im, True), self._text_packed_dev(ids))
+            out = self.logits(self._vision_dev(im, True), self._text_dev(ids))
             return self._back(out, im.host and ids.host).result()
         host = im.host and not ids.is_cuda
         Bi, (Bt, T) = len(im.x), ids.shape
         if isinstance(im.x, list) or im.grid is not None:
-            out = self.logits(self._vision_dev(im, True), self.text(ids.to(self.device, non_blocking=True)))
+            out = self.logits(self._vision_dev(im, True), self._text_dev(ids))
         elif host and im.trained and not im.u8:
             # float pixels and ids: the library's pipeline copies both in and the logits out
             out = torch.empty((Bi, Bt), dtype=torch.float32, pin_memory=True)

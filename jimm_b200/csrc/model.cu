@@ -728,6 +728,18 @@ static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, con
   return run_gemm(m, p, ws.pooled, D, v.head, B, s);
 }
 
+// The vision tower after the patch embedding, on B samples of S tokens (pk: the packed rows instead) in ws.x: ln_pre, the encoder and,
+// unless a token call (sink) asked for no pooled output, the pooling head into out.
+static int vision_tail(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk, const TokenSink* sink) {
+  VisionTower& v = m->vis;
+  float* x = m->ws.enc.x;
+  if (v.pre_norm)
+    JIMM_TRY(layernorm_run(x, v.D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, v.D, pk ? pk->T : B * S, v.D, s));
+  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc, pk, sink));
+  if (sink && !out) return 0;
+  return run_pool(m, B, S, out, s, pk);
+}
+
 // VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  img: [B, H, W, C]; grid: null for the trained patch
 // grid, else the grid of H x W (position table resampled).  out: fp32 [B, out_dim]
 static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, const PatchGrid* grid, float* out, cudaStream_t s,
@@ -753,58 +765,74 @@ static int run_vision(jimm_model* m, const void* img, int in_dtype, int B, int H
     JIMM_TRY(run_gemm(m, v.p_patch, big, v.patch.K, v.patch, B * n, s));
     if (cls) JIMM_TRY(cls_row_run(x, v.cls, v.pos, B, S, D, s));
   }
-  if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, B * S, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc, nullptr, sink));
-  if (sink && !out) return 0;
-  return run_pool(m, B, S, out, s);
+  return vision_tail(m, B, S, out, s, nullptr, sink);
 }
 
-// The pixels of a packed call: B NHWC images imgs[b] of H[b] x W[b], or (patches not null) the HuggingFace NaFlex patch rows of B
-// samples, patches [B, N, P*P*C], of which sample b's first (H[b] / P) * (W[b] / P) rows are its patches (jimm_encode_image_patches).
-struct PackedSrc {
+// The pixels of a vision call, in one of three forms:
+//   IMG_DENSE: img [B, H, W, C], every image H x W (native: the trained size, which image_call fills in);
+//   IMG_LIST:  B NHWC images imgs[b] of Hs[b] x Ws[b];
+//   IMG_ROWS:  the HuggingFace NaFlex patch rows of B samples, img = patches [B, N, P*P*C], of which sample b's first gh * gw rows are
+//              its patches, (gh, gw) = (grid[2b], grid[2b + 1]); image_call points Hs, Ws at the sizes the grids cut.
+enum ImageForm { IMG_DENSE, IMG_LIST, IMG_ROWS };
+struct ImageSrc {
+  ImageForm form = IMG_DENSE;
+  const void* img = nullptr;
   const void* const* imgs = nullptr;
-  const void* patches = nullptr;
+  int H = 0, W = 0;
+  bool native = false;
+  const int* Hs = nullptr;
+  const int* Ws = nullptr;
+  const int* grid = nullptr;
   int N = 0;
-  size_t sample_bytes = 0;  // bytes of one sample's N patch rows
-  PackedSrc from(int b0) const {  // the samples from b0 on
-    PackedSrc p = *this;
+  size_t sample_bytes = 0;  // IMG_DENSE / IMG_ROWS: bytes of one sample (image_call fills it in)
+  static ImageSrc dense(const void* img, int H, int W) { ImageSrc s; s.img = img; s.H = H; s.W = W; return s; }
+  static ImageSrc trained(const void* img) { ImageSrc s; s.img = img; s.native = true; return s; }
+  static ImageSrc list(const void* const* imgs, const int* H, const int* W) { ImageSrc s; s.form = IMG_LIST; s.imgs = imgs; s.Hs = H; s.Ws = W; return s; }
+  static ImageSrc rows(const void* patches, int N, const int* grid) { ImageSrc s; s.form = IMG_ROWS; s.img = patches; s.N = N; s.grid = grid; return s; }
+  ImageSrc from(int b0) const {  // the samples from b0 on
+    ImageSrc p = *this;
     if (imgs) p.imgs += b0;
-    else p.patches = static_cast<const uint8_t*>(patches) + b0 * sample_bytes;
+    else p.img = static_cast<const uint8_t*>(img) + b0 * sample_bytes;
+    if (Hs) { p.Hs += b0; p.Ws += b0; }
+    if (grid) p.grid += 2 * b0;
     return p;
   }
 };
 
-// run_vision on B images of different sizes packed into one token stream: image b (H[b] x W[b]) is token rows tok[b] .. tok[b + 1] - 1
-// (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets, image by image,
-// so row b of out is the bits run_vision gives on image b alone.
-static int run_vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, const int* tok, int max_S,
-                             float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
+// Uploads the offsets tok[0 .. B] of a packed chunk and one int per sequence, col(b), to meta [2B + 1].  The copy is stream-ordered from
+// pageable memory, which is staged before the call returns: an earlier call or chunk on this stream has read its own offsets before this
+// copy lands.
+template <typename F>
+static int upload_offsets(int* meta, const int* tok, int B, F&& col, cudaStream_t s) {
+  std::vector<int> h(2 * static_cast<size_t>(B) + 1);
+  for (int b = 0; b <= B; ++b) h[b] = tok[b];
+  for (int b = 0; b < B; ++b) h[B + 1 + b] = col(b);
+  JIMM_CUDA_CHECK(cudaMemcpyAsync(meta, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// run_vision on B images of different sizes (src: IMG_LIST or IMG_ROWS) packed into one token stream: image b is token rows tok[b] ..
+// tok[b + 1] - 1 (host offsets, tok[0] = 0), max_S the most tokens of one image.  Every kernel works row by row or, given the offsets,
+// image by image, so row b of out is the bits run_vision gives on image b alone.
+static int run_vision_packed(jimm_model* m, const ImageSrc& src, int in_dtype, int B, const int* tok, int max_S, float* out, cudaStream_t s,
+                             const TokenSink* sink) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
-  float* x = ws.enc.x;
-  const int D = v.D, T = tok[B], off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
-  const float* cls = off ? v.cls : nullptr;
-  // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
-  // on this stream has read its own offsets before this copy lands.
-  std::vector<int> meta(2 * static_cast<size_t>(B) + 1);
-  for (int b = 0; b <= B; ++b) meta[b] = tok[b];
-  for (int b = 0; b < B; ++b) meta[B + 1 + b] = W[b] / v.P;
-  JIMM_CUDA_CHECK(cudaMemcpyAsync(ws.pk_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  const int T = tok[B], off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  JIMM_TRY(upload_offsets(ws.pk_meta, tok, B, [&](int b) { return src.Ws[b] / v.P; }, s));
   const PackedRows pk{ws.pk_meta, T, max_S};
   const size_t row_bytes = static_cast<size_t>(v.Kp) * cdt_size(m);
-  if (src.patches) {  // NaFlex patch rows: no CLS token, so patch rows are token rows
-    JIMM_TRY(patch_rows_packed_run(src.patches, in_dtype, src.N, v.P * v.P * v.C, pk.seq_off, B, max_S, ws.enc.big, m->cdt, v.Kp, s));
+  if (src.form == IMG_ROWS) {  // NaFlex patch rows: no CLS token, so patch rows are token rows
+    JIMM_TRY(patch_rows_packed_run(src.img, in_dtype, src.N, v.P * v.P * v.C, pk.seq_off, B, max_S, ws.enc.big, m->cdt, v.Kp, s));
   } else {
     for (int b = 0; b < B; ++b)
-      JIMM_TRY(patchify_run(src.imgs[b], in_dtype, 1, H[b], W[b], v.C, v.P, static_cast<uint8_t*>(ws.enc.big) + (tok[b] + off) * row_bytes, m->cdt,
-                            s, 0, v.Kp));
+      JIMM_TRY(patchify_run(src.imgs[b], in_dtype, 1, src.Hs[b], src.Ws[b], v.C, v.P, static_cast<uint8_t*>(ws.enc.big) + (tok[b] + off) * row_bytes,
+                            m->cdt, s, 0, v.Kp));
   }
   JIMM_TRY(run_gemm(m, v.p_patch_packed, ws.enc.big, v.Kp, v.patch, T, s));
-  JIMM_TRY(tokens_add_interp_packed_run(x, cls, v.pos, v.img / v.P, D, pk.seq_off, ws.pk_meta + B + 1, B, max_S, v.interp, s));
-  if (v.pre_norm) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, D, T, D, s));
-  JIMM_TRY(run_encoder(m, &v.enc, B, 0, s, ws.enc, &pk, sink));
-  if (sink && !out) return 0;
-  return run_pool(m, B, 0, out, s, &pk);
+  JIMM_TRY(tokens_add_interp_packed_run(ws.enc.x, off ? v.cls : nullptr, v.pos, v.img / v.P, v.D, pk.seq_off, ws.pk_meta + B + 1, B, max_S,
+                                        v.interp, s));
+  return vision_tail(m, B, 0, out, s, &pk, sink);
 }
 
 // CLIP.encode_text (models/clip.py:148-167) / SigLIP.encode_text (models/siglip.py:135-153).  out fp32 [B, Dt]
@@ -830,16 +858,11 @@ static int run_text(jimm_model* m, const int32_t* ids, int B, int T, float* out,
 // offsets, tok[0] = 0), max_S the longest.  Positions restart at 0 in every sequence and the causal mask (CLIP) is taken within it; every
 // other kernel works row by row, so row b of out is the bits run_text gives on sequence b alone.
 static int run_text_packed(jimm_model* m, const int32_t* ids, int B, const int* tok, int max_S, float* out, cudaStream_t s,
-                           const TokenSink* sink = nullptr) {
+                           const TokenSink* sink) {
   TextTower& t = m->txt;
   TextWs& ws = m->wt;
-  // The offsets travel by a stream-ordered copy from pageable memory, which is staged before the call returns: an earlier call or chunk
-  // on this stream has read its own offsets before this copy lands.  The pooled rows follow them: each sequence's last row (SigLIP's
-  // last-token pooling); CLIP's EOT rows overwrite them on the device.
-  std::vector<int> meta(2 * static_cast<size_t>(B) + 1);
-  for (int b = 0; b <= B; ++b) meta[b] = tok[b];
-  for (int b = 0; b < B; ++b) meta[B + 1 + b] = tok[b + 1] - 1;
-  JIMM_CUDA_CHECK(cudaMemcpyAsync(ws.pk_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  // The pooled rows follow the offsets: each sequence's last row (SigLIP's last-token pooling); CLIP's EOT rows overwrite them on the device.
+  JIMM_TRY(upload_offsets(ws.pk_meta, tok, B, [&](int b) { return tok[b + 1] - 1; }, s));
   const PackedRows pk{ws.pk_meta, tok[B], max_S};
   int* rows = ws.pk_meta + B + 1;
   JIMM_TRY(embed_packed_run(ids, t.table, t.pos, ws.enc.x, pk.seq_off, B, pk.T, t.D, t.V, s));
@@ -1418,25 +1441,20 @@ static int get_grid(jimm_model* m, int H, int W, PatchGrid** out) {
   return 0;
 }
 
-// Vision forward of B images of H x W.  The native size goes through exec_vision (graphs, staging); other sizes run eagerly.  A token
-// call (sink) always runs eagerly, its chunk of images from b0 on writing from output row b0 * S on; out may then be null.
-static int vision_chunks(jimm_model* m, const void* img, int in_dtype, int B, int H, int W, float* out, cudaStream_t s,
+// Vision forward of B images of src.H x src.W (IMG_DENSE) on the patch grid `grid` (null: the trained grid).  The native size goes through
+// exec_vision (graphs, staging); other sizes run eagerly.  A token call (sink) always runs eagerly, its chunk of images from b0 on writing
+// from output row b0 * S on; out may then be null.
+static int vision_chunks(jimm_model* m, const ImageSrc& src, int in_dtype, int B, const PatchGrid* grid, float* out, cudaStream_t s,
                          const TokenSink* sink = nullptr) {
   const VisionTower& v = m->vis;
-  JIMM_TRY(check_patch(m, H, W));
-  const bool native = H == v.img && W == v.img;
-  PatchGrid* grid = nullptr;  // null: the trained grid
-  if (!trained_grid(v, H, W)) JIMM_TRY(get_grid(m, H, W, &grid));
-  const size_t img_bytes = static_cast<size_t>(H) * W * v.C * dtype_size(in_dtype);
+  const bool native = src.H == v.img && src.W == v.img;
   const int od = vision_out_dim(m);
   return for_chunks(B, grid ? grid->chunk : m->max_batch, [&](int b0, int nb) {
-    const void* src = static_cast<const uint8_t*>(img) + b0 * img_bytes;
+    const void* img = src.from(b0).img;
     float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
-    if (sink) {
-      const TokenSink at = sink->at(static_cast<size_t>(b0) * (grid ? grid->S : v.S));
-      return run_vision(m, src, in_dtype, nb, H, W, grid, dst, s, &at);
-    }
-    return native ? exec_vision(m, src, in_dtype, nb, dst, s) : run_vision(m, src, in_dtype, nb, H, W, grid, dst, s);
+    if (native && !sink) return exec_vision(m, img, in_dtype, nb, dst, s);
+    const TokenSink at = sink ? sink->at(static_cast<size_t>(b0) * (grid ? grid->S : v.S)) : TokenSink{};
+    return run_vision(m, img, in_dtype, nb, src.H, src.W, grid, dst, s, sink ? &at : nullptr);
   });
 }
 
@@ -1457,18 +1475,11 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
 // token-layout patch rows (S rather than the padded n_pad) outgrow every other term of a handle without a set_max_tokens budget.
 static bool packed_fit(const jimm_model* m, size_t T) { return T <= m->ws_rows && big_bytes(m, T, T) <= m->ws_big; }
 
-// B images of different sizes: chunks of consecutive images, each as many as fit (packed_fit, at most max_batch), run packed.
-// A token call (sink): each chunk writes from its first token row on; out may then be null.
-static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int B, const int* H, const int* W, float* out, cudaStream_t s,
-                         const TokenSink* sink = nullptr) {
+// B images of different sizes (IMG_LIST / IMG_ROWS): chunks of consecutive images, each as many as fit (packed_fit, at most max_batch),
+// run packed.  A token call (sink): each chunk writes from its first token row on; out may then be null.
+static int vision_packed(jimm_model* m, const ImageSrc& src, int in_dtype, int B, float* out, cudaStream_t s, const TokenSink* sink) {
   const VisionTower& v = m->vis;
   const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
-  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
-    if (src.imgs && !src.imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
-    if (H[b] < v.P || W[b] < v.P) { set_last_error("image %d: %dx%d is smaller than one %dx%d patch", b, H[b], W[b], v.P, v.P); return JIMM_EINVAL; }
-    JIMM_TRY(image_map_fits(m, H[b], W[b]));
-    if (!packed_fit(m, static_cast<size_t>(H[b] / v.P) * (W[b] / v.P) + off)) return image_too_large(m, H[b], W[b]);
-  }
   const int od = vision_out_dim(m);
   std::vector<int> tok;
   size_t t0 = 0;  // the chunk's first token row
@@ -1476,19 +1487,15 @@ static int vision_packed(jimm_model* m, const PackedSrc& src, int in_dtype, int 
     tok.assign(1, 0);
     int b1 = b0, max_S = 0;
     while (b1 < B && b1 - b0 < m->max_batch) {
-      const int S = (H[b1] / v.P) * (W[b1] / v.P) + off;
+      const int S = (src.Hs[b1] / v.P) * (src.Ws[b1] / v.P) + off;
       if (!packed_fit(m, static_cast<size_t>(tok.back()) + S)) break;
       tok.push_back(tok.back() + S);
       max_S = std::max(max_S, S);
       ++b1;
     }
     float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
-    if (sink) {
-      const TokenSink at = sink->at(t0);
-      JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, dst, s, &at));
-    } else {
-      JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, H + b0, W + b0, tok.data(), max_S, dst, s));
-    }
+    const TokenSink at = sink ? sink->at(t0) : TokenSink{};
+    JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, tok.data(), max_S, dst, s, sink ? &at : nullptr));
     t0 += tok.back();
     b0 = b1;
   }
@@ -1500,11 +1507,9 @@ static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* o
   return for_chunks(B, m->max_batch, [&](int b0, int nb) {
     const int32_t* src = ids + static_cast<size_t>(b0) * T;
     float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
-    if (sink) {
-      const TokenSink at = sink->at(static_cast<size_t>(b0) * T);
-      return run_text(m, src, nb, T, dst, s, &at);
-    }
-    return exec_text(m, src, nb, T, dst, s);
+    if (!sink) return exec_text(m, src, nb, T, dst, s);
+    const TokenSink at = sink->at(static_cast<size_t>(b0) * T);
+    return run_text(m, src, nb, T, dst, s, &at);
   });
 }
 
@@ -1512,7 +1517,7 @@ static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* o
 // max_batch x context_length token rows hold (at most pk_seqs), run packed.  The chunks are cut by tokens, not by sequences: short
 // prompts fill a chunk with several times max_batch sequences, and its GEMMs with as many rows as a padded call of max_batch.
 // A token call (sink): each chunk writes from its first row of ids on; out may then be null.
-static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s, const TokenSink* sink = nullptr) {
+static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s, const TokenSink* sink) {
   const int budget = m->max_batch * m->txt.T;
   std::vector<int> tok;
   size_t r0 = 0;  // the chunk's first row of ids
@@ -1525,128 +1530,15 @@ static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len,
       ++b1;
     }
     float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
-    if (sink) {
-      const TokenSink at = sink->at(r0);
-      JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s, &at));
-    } else {
-      JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s));
-    }
+    const TokenSink at = sink ? sink->at(r0) : TokenSink{};
+    JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s, sink ? &at : nullptr));
     r0 += tok.back();
     b0 = b1;
   }
   return 0;
 }
 
-// The jimm_vit_forward* (vit_fn: its name) and jimm_encode_image* calls on device images
-static int encode_images(jimm_model* m, const char* vit_fn, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
-  JIMM_TRY(check_vision(m, vit_fn));
-  JIMM_TRY(set_device(m));
-  return vision_chunks(m, img, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
-}
-
-int jimm_vit_forward(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  return encode_images(m, "jimm_vit_forward", img, in_dtype, B, m->vis.img, m->vis.img, out, stream);
-}
-
-int jimm_encode_image(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  return encode_images(m, nullptr, img, in_dtype, B, m->vis.img, m->vis.img, out, stream);
-}
-
-int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
-  return encode_images(m, "jimm_vit_forward_hw", img, in_dtype, B, H, W, out, stream);
-}
-
-int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
-  return encode_images(m, nullptr, img, in_dtype, B, H, W, out, stream);
-}
-
-// The jimm_vit_forward_packed (vit_fn: its name) and jimm_encode_image_packed calls
-static int encode_packed(jimm_model* m, const char* vit_fn, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out,
-                         void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
-  JIMM_TRY(check_vision(m, vit_fn));
-  if (B > 0 && (!imgs || !H || !W || !out)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  PackedSrc src;
-  src.imgs = imgs;
-  return vision_packed(m, src, in_dtype, B, H, W, out, static_cast<cudaStream_t>(stream));
-}
-
-int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
-  return encode_packed(m, "jimm_vit_forward_packed", imgs, in_dtype, B, H, W, out, stream);
-}
-
-int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
-  return encode_packed(m, nullptr, imgs, in_dtype, B, H, W, out, stream);
-}
-
-// The checks and the packed source of a call on HuggingFace NaFlex patch rows (fn names it): a NaFlex handle, and every sample's grid
-// within its N rows; H, W [B] receive the image sizes the grids cut.
-static int naflex_src(const jimm_model* m, const char* fn, const void* patches, int in_dtype, int B, int N, const int* grid, int* H, int* W,
-                      PackedSrc* src) {
-  if (m->cfg.kind != JIMM_SIGLIP_NAFLEX) {
-    set_last_error("%s: the model is not a SigLIP 2 NaFlex handle (kind %d); use jimm_encode_image_packed", fn, m->cfg.kind);
-    return JIMM_EINVAL;
-  }
-  const VisionTower& v = m->vis;
-  for (int b = 0; b < B; ++b) {  // refuse the call before anything is enqueued
-    const int gh = grid[2 * b], gw = grid[2 * b + 1];
-    if (gh < 1 || gw < 1 || gh > INT32_MAX / v.P || gw > INT32_MAX / v.P) {
-      set_last_error("%s: sample %d has a %dx%d patch grid (each edge from 1 up)", fn, b, gh, gw);
-      return JIMM_EINVAL;
-    }
-    if (static_cast<int64_t>(gh) * gw > N) {
-      set_last_error("%s: sample %d has a %dx%d patch grid, %lld patches, more than its N = %d rows", fn, b, gh, gw,
-                     static_cast<long long>(gh) * gw, N);
-      return JIMM_EINVAL;
-    }
-    H[b] = gh * v.P;
-    W[b] = gw * v.P;
-  }
-  src->patches = patches;
-  src->N = N;
-  src->sample_bytes = static_cast<size_t>(N) * v.P * v.P * v.C * dtype_size(in_dtype);
-  return 0;
-}
-
-// HuggingFace NaFlex patch rows: sample b is the (gh*P) x (gw*P) image of its first gh*gw rows, run through the packed chunker
-int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
-  if (m->cfg.kind == JIMM_SIGLIP_NAFLEX && B > 0 && (!patches || !grid || !out)) {
-    set_last_error("jimm_encode_image_patches: null argument");
-    return JIMM_EINVAL;
-  }
-  std::vector<int> H(B), W(B);
-  PackedSrc src;
-  JIMM_TRY(naflex_src(m, "jimm_encode_image_patches", patches, in_dtype, B, N, grid, H.data(), W.data(), &src));
-  JIMM_TRY(set_device(m));
-  return vision_packed(m, src, in_dtype, B, H.data(), W.data(), out, static_cast<cudaStream_t>(stream));
-}
-
-int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_text(m));
-  JIMM_TRY(check_text_len(m, T));
-  JIMM_TRY(set_device(m));
-  return text_chunks(m, ids, B, T, out, static_cast<cudaStream_t>(stream));
-}
-
-int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, float* out, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_text(m));
-  if (B > 0 && (!ids || !len || !out)) { set_last_error("jimm_encode_text_packed: null argument"); return JIMM_EINVAL; }
-  JIMM_TRY(check_lens(m, B, len));
-  JIMM_TRY(set_device(m));
-  return text_packed(m, ids, B, len, out, static_cast<cudaStream_t>(stream));
-}
-
-// ---- per-token hidden states ----
+// ---- the forward calls on device inputs ----
 // The request of a per-token call (fn names it) on the tower with encoder `enc` and final norm (ln, eps), as the sink of its chunks.
 // pooled: the call writes the pooled output too, so every block runs.
 static int tokens_sink(const char* fn, const jimm_tokens_req_t* req, const Encoder& enc, const LNW& ln, float eps, bool pooled, TokenSink* sink) {
@@ -1681,68 +1573,166 @@ static int tokens_sink(const char* fn, const jimm_tokens_req_t* req, const Encod
   return 0;
 }
 
-int jimm_image_tokens(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_tokens_req_t* req, float* pooled, void* stream) {
+// The kinds of forward call: the pooled output (jimm_encode_*), the same on a ViT / tower handle only (jimm_vit_forward*), and the
+// hidden states of a request with the pooled output optional (jimm_image_tokens* / jimm_text_tokens*)
+enum CallKind { CALL_ENCODE, CALL_VIT, CALL_TOKENS };
+
+static int null_argument(const char* fn) {
+  set_last_error("%s: null argument", fn);
+  return JIMM_EINVAL;
+}
+
+// The shape step of a vision call (fn names it), which fills in src's sizes.  IMG_DENSE: images of at least one patch, and off the
+// trained grid its plan (*grid; null on the trained grid).  IMG_ROWS: every sample's grid within its N rows, the image sizes it cuts
+// written to cut.  IMG_LIST and IMG_ROWS: every image present, of at least one patch, within the MAP head's limit and alone fitting
+// a packed chunk.
+static int image_shapes(jimm_model* m, const char* fn, ImageSrc* src, int in_dtype, int B, std::vector<int>* cut, PatchGrid** grid) {
+  const VisionTower& v = m->vis;
+  *grid = nullptr;
+  if (src->form == IMG_DENSE) {
+    if (src->native) src->H = src->W = v.img;
+    JIMM_TRY(check_patch(m, src->H, src->W));
+    if (!trained_grid(v, src->H, src->W)) JIMM_TRY(get_grid(m, src->H, src->W, grid));
+    src->sample_bytes = static_cast<size_t>(src->H) * src->W * v.C * dtype_size(in_dtype);
+    return 0;
+  }
+  if (src->form == IMG_ROWS) {
+    cut->resize(2 * static_cast<size_t>(B));
+    for (int b = 0; b < B; ++b) {
+      const int gh = src->grid[2 * b], gw = src->grid[2 * b + 1];
+      if (gh < 1 || gw < 1 || gh > INT32_MAX / v.P || gw > INT32_MAX / v.P) {
+        set_last_error("%s: sample %d has a %dx%d patch grid (each edge from 1 up)", fn, b, gh, gw);
+        return JIMM_EINVAL;
+      }
+      if (static_cast<int64_t>(gh) * gw > src->N) {
+        set_last_error("%s: sample %d has a %dx%d patch grid, %lld patches, more than its N = %d rows", fn, b, gh, gw,
+                       static_cast<long long>(gh) * gw, src->N);
+        return JIMM_EINVAL;
+      }
+      (*cut)[b] = gh * v.P;
+      (*cut)[B + b] = gw * v.P;
+    }
+    src->Hs = cut->data();
+    src->Ws = cut->data() + B;
+    src->sample_bytes = static_cast<size_t>(src->N) * v.P * v.P * v.C * dtype_size(in_dtype);
+  }
+  const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
+  for (int b = 0; b < B; ++b) {
+    const int H = src->Hs[b], W = src->Ws[b];
+    if (src->imgs && !src->imgs[b]) { set_last_error("packed call: image %d is a null pointer", b); return JIMM_EINVAL; }
+    if (H < v.P || W < v.P) { set_last_error("image %d: %dx%d is smaller than one %dx%d patch", b, H, W, v.P, v.P); return JIMM_EINVAL; }
+    JIMM_TRY(image_map_fits(m, H, W));
+    if (!packed_fit(m, static_cast<size_t>(H / v.P) * (W / v.P) + off)) return image_too_large(m, H, W);
+  }
+  return 0;
+}
+
+// Every vision call on device images (fn names it): the checks in the order include/jimm_b200.h states, then the chunker of the form.
+static int image_call(jimm_model* m, const char* fn, CallKind kind, ImageSrc src, int in_dtype, int B, float* out, const jimm_tokens_req_t* req,
+                      void* stream) {
   JIMM_TRY(check_ready(m, B));
   JIMM_TRY(check_image_dtype(in_dtype));
-  JIMM_TRY(check_vision(m, nullptr));
+  if (src.form != IMG_ROWS) {
+    JIMM_TRY(check_vision(m, kind == CALL_VIT ? fn : nullptr));
+  } else if (m->cfg.kind != JIMM_SIGLIP_NAFLEX) {
+    set_last_error("%s: the model is not a SigLIP 2 NaFlex handle (kind %d); use jimm_encode_image_packed", fn, m->cfg.kind);
+    return JIMM_EINVAL;
+  }
   TokenSink sink;
-  JIMM_TRY(tokens_sink("jimm_image_tokens", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
-  if (B > 0 && !img) { set_last_error("jimm_image_tokens: null images"); return JIMM_EINVAL; }
+  if (kind == CALL_TOKENS) JIMM_TRY(tokens_sink(fn, req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, out != nullptr, &sink));
+  const bool inputs = src.form == IMG_LIST ? src.imgs && src.Hs && src.Ws : src.img && (src.form == IMG_DENSE || src.grid);
+  if (B > 0 && (!inputs || (kind != CALL_TOKENS && !out))) return null_argument(fn);
+  std::vector<int> cut;
+  PatchGrid* grid = nullptr;
+  JIMM_TRY(image_shapes(m, fn, &src, in_dtype, B, &cut, &grid));
   JIMM_TRY(set_device(m));
-  return vision_chunks(m, img, in_dtype, B, H, W, pooled, static_cast<cudaStream_t>(stream), &sink);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const TokenSink* sk = kind == CALL_TOKENS ? &sink : nullptr;
+  if (src.form == IMG_DENSE) return vision_chunks(m, src, in_dtype, B, grid, out, s, sk);
+  return vision_packed(m, src, in_dtype, B, out, s, sk);
+}
+
+// The token ids of a text call: B sequences of T ids each (ids [B, T]), or, packed, of len[b] ids one after another
+struct TextSrc {
+  const int32_t* ids;
+  int T;
+  const int* len;
+  bool packed;
+};
+
+// Every text call on device ids (fn names it), on the pattern of image_call
+static int text_call(jimm_model* m, const char* fn, CallKind kind, const TextSrc& src, int B, float* out, const jimm_tokens_req_t* req,
+                     void* stream) {
+  JIMM_TRY(check_ready(m, B));
+  JIMM_TRY(check_text(m));
+  TokenSink sink;
+  if (kind == CALL_TOKENS) JIMM_TRY(tokens_sink(fn, req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, out != nullptr, &sink));
+  if (B > 0 && (!src.ids || (src.packed && !src.len) || (kind != CALL_TOKENS && !out))) return null_argument(fn);
+  JIMM_TRY(src.packed ? check_lens(m, B, src.len) : check_text_len(m, src.T));
+  JIMM_TRY(set_device(m));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const TokenSink* sk = kind == CALL_TOKENS ? &sink : nullptr;
+  if (src.packed) return text_packed(m, src.ids, B, src.len, out, s, sk);
+  return text_chunks(m, src.ids, B, src.T, out, s, sk);
+}
+
+int jimm_vit_forward(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
+  return image_call(m, "jimm_vit_forward", CALL_VIT, ImageSrc::trained(img), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_encode_image(jimm_model_t* m, const void* img, int in_dtype, int B, float* out, void* stream) {
+  return image_call(m, "jimm_encode_image", CALL_ENCODE, ImageSrc::trained(img), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_vit_forward_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
+  return image_call(m, "jimm_vit_forward_hw", CALL_VIT, ImageSrc::dense(img, H, W), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_encode_image_hw(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, float* out, void* stream) {
+  return image_call(m, "jimm_encode_image_hw", CALL_ENCODE, ImageSrc::dense(img, H, W), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_vit_forward_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
+  return image_call(m, "jimm_vit_forward_packed", CALL_VIT, ImageSrc::list(imgs, H, W), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_encode_image_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, float* out, void* stream) {
+  return image_call(m, "jimm_encode_image_packed", CALL_ENCODE, ImageSrc::list(imgs, H, W), in_dtype, B, out, nullptr, stream);
+}
+
+// HuggingFace NaFlex patch rows: sample b is the (gh*P) x (gw*P) image of its first gh*gw rows, run through the packed chunker
+int jimm_encode_image_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, float* out, void* stream) {
+  return image_call(m, "jimm_encode_image_patches", CALL_ENCODE, ImageSrc::rows(patches, N, grid), in_dtype, B, out, nullptr, stream);
+}
+
+int jimm_encode_text(jimm_model_t* m, const int32_t* ids, int B, int T, float* out, void* stream) {
+  return text_call(m, "jimm_encode_text", CALL_ENCODE, TextSrc{ids, T, nullptr, false}, B, out, nullptr, stream);
+}
+
+int jimm_encode_text_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, float* out, void* stream) {
+  return text_call(m, "jimm_encode_text_packed", CALL_ENCODE, TextSrc{ids, 0, len, true}, B, out, nullptr, stream);
+}
+
+int jimm_image_tokens(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_tokens_req_t* req, float* pooled, void* stream) {
+  return image_call(m, "jimm_image_tokens", CALL_TOKENS, ImageSrc::dense(img, H, W), in_dtype, B, pooled, req, stream);
 }
 
 int jimm_image_tokens_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, const jimm_tokens_req_t* req,
                              float* pooled, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
-  JIMM_TRY(check_vision(m, nullptr));
-  TokenSink sink;
-  JIMM_TRY(tokens_sink("jimm_image_tokens_packed", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
-  if (B > 0 && (!imgs || !H || !W)) { set_last_error("packed call: null argument"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  PackedSrc src;
-  src.imgs = imgs;
-  return vision_packed(m, src, in_dtype, B, H, W, pooled, static_cast<cudaStream_t>(stream), &sink);
+  return image_call(m, "jimm_image_tokens_packed", CALL_TOKENS, ImageSrc::list(imgs, H, W), in_dtype, B, pooled, req, stream);
 }
 
 int jimm_image_tokens_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, const jimm_tokens_req_t* req,
                               float* pooled, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_image_dtype(in_dtype));
-  if (m->cfg.kind == JIMM_SIGLIP_NAFLEX && B > 0 && (!patches || !grid)) {
-    set_last_error("jimm_image_tokens_patches: null argument");
-    return JIMM_EINVAL;
-  }
-  std::vector<int> H(B), W(B);
-  PackedSrc src;
-  JIMM_TRY(naflex_src(m, "jimm_image_tokens_patches", patches, in_dtype, B, N, grid, H.data(), W.data(), &src));
-  TokenSink sink;
-  JIMM_TRY(tokens_sink("jimm_image_tokens_patches", req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, pooled != nullptr, &sink));
-  JIMM_TRY(set_device(m));
-  return vision_packed(m, src, in_dtype, B, H.data(), W.data(), pooled, static_cast<cudaStream_t>(stream), &sink);
+  return image_call(m, "jimm_image_tokens_patches", CALL_TOKENS, ImageSrc::rows(patches, N, grid), in_dtype, B, pooled, req, stream);
 }
 
 int jimm_text_tokens(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_tokens_req_t* req, float* pooled, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_text(m));
-  JIMM_TRY(check_text_len(m, T));
-  TokenSink sink;
-  JIMM_TRY(tokens_sink("jimm_text_tokens", req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, pooled != nullptr, &sink));
-  if (B > 0 && !ids) { set_last_error("jimm_text_tokens: null ids"); return JIMM_EINVAL; }
-  JIMM_TRY(set_device(m));
-  return text_chunks(m, ids, B, T, pooled, static_cast<cudaStream_t>(stream), &sink);
+  return text_call(m, "jimm_text_tokens", CALL_TOKENS, TextSrc{ids, T, nullptr, false}, B, pooled, req, stream);
 }
 
 int jimm_text_tokens_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_tokens_req_t* req, float* pooled, void* stream) {
-  JIMM_TRY(check_ready(m, B));
-  JIMM_TRY(check_text(m));
-  TokenSink sink;
-  JIMM_TRY(tokens_sink("jimm_text_tokens_packed", req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, pooled != nullptr, &sink));
-  if (B > 0 && (!ids || !len)) { set_last_error("jimm_text_tokens_packed: null argument"); return JIMM_EINVAL; }
-  JIMM_TRY(check_lens(m, B, len));
-  JIMM_TRY(set_device(m));
-  return text_packed(m, ids, B, len, pooled, static_cast<cudaStream_t>(stream), &sink);
+  return text_call(m, "jimm_text_tokens_packed", CALL_TOKENS, TextSrc{ids, 0, len, true}, B, pooled, req, stream);
 }
 
 int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const float* txt_e, int Bt, float* logits, void* stream) {
@@ -1788,16 +1778,15 @@ int jimm_dual_encode_hw(jimm_model_t* m, const void* img, int in_dtype, int Bi, 
   JIMM_TRY(check_text(m));
   JIMM_TRY(check_image_dtype(in_dtype));
   JIMM_TRY(check_text_len(m, T));
-  JIMM_TRY(check_patch(m, H, W));
+  ImageSrc src = ImageSrc::dense(img, H, W);
+  std::vector<int> cut;
+  PatchGrid* grid = nullptr;
+  JIMM_TRY(image_shapes(m, "jimm_dual_encode_hw", &src, in_dtype, Bi, &cut, &grid));  // refuse the images before the text tower runs
   JIMM_TRY(set_device(m));
-  if (!trained_grid(m->vis, H, W)) {  // refuse an image that does not fit before the text tower runs
-    PatchGrid* grid = nullptr;
-    JIMM_TRY(get_grid(m, H, W, &grid));
-  }
   cudaStream_t s = static_cast<cudaStream_t>(stream), ts = s;
   JIMM_TRY(fork_text(m, s, &ts));
   JIMM_TRY(text_chunks(m, ids, Bt, T, txt_e, ts));
-  JIMM_TRY(vision_chunks(m, img, in_dtype, Bi, H, W, img_e, s));
+  JIMM_TRY(vision_chunks(m, src, in_dtype, Bi, grid, img_e, s));
   return join_text(m, s, ts);
 }
 

@@ -124,7 +124,7 @@ class DualTower(_NativeOwner, nn.Module):
         im = self._images(image, interpolate_pos_encoding)
         x, B = im.x, len(im.x)
         n = self.native(B, require=True, hw=im.hw if interpolate_pos_encoding else None)
-        ids = n._prep_ids(text)
+        ids = prep_ids(text)
         with torch.cuda.device(n.device):
             cur = torch.cuda.current_stream(n.device)
             # host inputs: the ids go first (H2D copies share one engine), the images follow on a side stream and land while
