@@ -404,7 +404,9 @@ JIMM_API int jimm_k_preproc_plan(const jimm_preproc_config_t* cfg, int H, int W,
  * logits: device fp32 [rows, cols] (leading dimension ld).  mode 0: probs = exp(x) / sum(exp(x)) per row, un-shifted like
  * examples/clip_inference.py:47; mode 1: probs = sigmoid(x) (SigLIP pair probabilities).  order (nullable, int32 [rows, cols]):
  * `argsort(x)[::-1]` per row -- descending, equal scores with the larger index first (examples/clip_inference.py:49);
- * argmax (nullable, int32 [rows]): first maximum per row (examples/vit_inference.py:58).  order / argmax need cols <= 4096. */
+ * argmax (nullable, int32 [rows]): first maximum per row (examples/vit_inference.py:58).  Any cols: the order of a row wider than
+ * 4096 columns is sorted in scratch allocated in stream order on `stream` (cudaMallocAsync / cudaFreeAsync), 16 bytes per column
+ * per row (8 when cols <= 8192), for at most 256 MB of rows at a time (or one row, if a row needs more). */
 JIMM_API int jimm_postprocess(const float* logits, int rows, int cols, int ld, int mode, float* probs, int ldp, int32_t* order, int32_t* argmax,
                               void* stream);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads

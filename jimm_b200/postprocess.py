@@ -14,6 +14,8 @@ import torch
 
 from . import _lib
 
+_INT32_MAX = 2**31 - 1  # rows and columns are C ints, and the order holds int32 column indices
+
 
 def _run(logits: torch.Tensor, mode: int, want_probs: bool, want_order: bool, want_argmax: bool):
     if not isinstance(logits, torch.Tensor) or not logits.is_cuda:
@@ -22,10 +24,13 @@ def _run(logits: torch.Tensor, mode: int, want_probs: bool, want_order: bool, wa
         logits = logits[None]
     if logits.ndim != 2:
         raise ValueError(f"expected logits of shape [rows, cols], got {tuple(logits.shape)}")
+    rows, cols = logits.shape
+    if rows > _INT32_MAX or cols > _INT32_MAX:  # before the cast / copy below allocates anything
+        raise ValueError(f"postprocess takes at most {_INT32_MAX} rows and columns, got {tuple(logits.shape)}")
     x = logits.to(torch.float32)
-    if x.stride(1) != 1:
+    # the library reads rows `ld` floats apart with unit column stride: expanded (stride-0) or overlapping rows are copied first
+    if x.stride(1) != 1 or (rows > 1 and not cols <= x.stride(0) <= _INT32_MAX):
         x = x.contiguous()
-    rows, cols = x.shape
     lib = _lib.load()
     with torch.cuda.device(x.device):
         probs = torch.empty((rows, cols), dtype=torch.float32, device=x.device) if want_probs else None
