@@ -110,12 +110,12 @@ JIMM_API int jimm_model_output_dim(const jimm_model_t* m, int* vision_out, int* 
 JIMM_API int jimm_model_max_batch(const jimm_model_t* m);
 
 /* -- forward: device-resident inputs/outputs ---------------------------------------------------------------------- */
-/* The forward calls on device inputs (jimm_vit_forward*, jimm_encode_image*, jimm_encode_text*, jimm_image_tokens*, jimm_text_tokens*)
- * check their arguments in one order and report the first fault, before anything is enqueued:
+/* The forward calls on device inputs (jimm_vit_forward*, jimm_encode_image*, jimm_encode_text*, jimm_image_tokens*, jimm_text_tokens*,
+ * jimm_image_attn*, jimm_text_attn*) check their arguments in one order and report the first fault, before anything is enqueued:
  *   1. the handle: not null, finalized (else JIMM_ESTATE), B >= 0;
  *   2. the image dtype (image calls);
  *   3. the tower: a vision / text tower, a ViT / tower handle for jimm_vit_forward*, a JIMM_SIGLIP_NAFLEX handle for the *_patches calls;
- *   4. the request of a per-token call;
+ *   4. the request of a per-token or attention call;
  *   5. when B > 0, null arguments ("<call>: null argument"): the inputs, and out on the pooled calls (pooled stays optional);
  *   6. the shapes: image sizes, NaFlex patch grids, the workspace and the MAP head's sequence limit; sequence lengths;
  *   7. the handle's device is made current.
@@ -212,6 +212,40 @@ JIMM_API int jimm_image_tokens_patches(jimm_model_t* m, const void* patches, int
 JIMM_API int jimm_text_tokens(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_tokens_req_t* req, float* pooled, void* stream);
 JIMM_API int jimm_text_tokens_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_tokens_req_t* req, float* pooled,
                                      void* stream);
+
+/* -- attention weights (HF output_attentions) of the vision and text towers, and the MAP head's probe weights ------------------------
+ * Block k (0 .. L-1) gives softmax(q k^T / sqrt(d)) of each of its H heads, computed in fp32 on the q / k its attention reads (the qkv
+ * buffer in the attention I/O type: fp16, or bf16 in bf16 mode).  Each request j writes out[j], a device buffer, contiguous, 16-byte
+ * aligned, of out_dtype (JIMM_F32; JIMM_F16 / JIMM_BF16: the fp32 weights rounded to nearest even): per sample b its [H, S_b, S_b]
+ * weights, row-major (query rows, key columns), sample b from element H * sum_{j<b} S_j^2 on -- [B, H, S, S] for a dense call.  The
+ * CLIP text tower is causal: the entries above the diagonal are 0.  JIMM_ATTN_MAP (MAP-pooled vision towers) gives the MAP head's
+ * probe weights, the ones its pooled output sums with: per sample [H, 1, S_b], sample b from element H * sum_{j<b} S_j on.  Rows and
+ * samples are those of jimm_image_tokens* / jimm_text_tokens*; sample b of a packed call equals the call on that sample alone.
+ * pooled (device fp32 [B, out_dim], or NULL) receives exactly what the matching pooled call writes.  Without JIMM_ATTN_MAP and pooled,
+ * only the blocks up to the deepest request run.  These calls never replay a CUDA graph, leave the graph cache as it is and allocate
+ * nothing.  A bad request (n outside 1 .. L + 1, a block outside 0 .. L-1 and not JIMM_ATTN_MAP, JIMM_ATTN_MAP on a CLS-pooled or a
+ * text tower, a bad out_dtype, a null or misaligned pointer) and every refusal of the matching pooled call is JIMM_EINVAL before
+ * anything is enqueued, in the order stated above the forward calls (the request is step 4). */
+#define JIMM_ATTN_MAP (-2)
+typedef struct jimm_attn_req {
+  int n;                                   /* requests, 1 .. L + 1 */
+  const int* blocks;                       /* host [n]: each 0 .. L-1, or JIMM_ATTN_MAP */
+  void* const* out;                        /* host [n] of device buffers, 16-byte aligned */
+  int out_dtype;                           /* JIMM_F32 / JIMM_F16 / JIMM_BF16 */
+} jimm_attn_req_t;
+/* The vision tower on images as jimm_image_tokens takes them */
+JIMM_API int jimm_image_attn(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_attn_req_t* req, float* pooled,
+                             void* stream);
+/* ... as jimm_image_tokens_packed takes them */
+JIMM_API int jimm_image_attn_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W,
+                                    const jimm_attn_req_t* req, float* pooled, void* stream);
+/* ... as jimm_image_tokens_patches takes them (kind JIMM_SIGLIP_NAFLEX) */
+JIMM_API int jimm_image_attn_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, const jimm_attn_req_t* req,
+                                     float* pooled, void* stream);
+/* The text tower on ids as jimm_text_tokens / jimm_text_tokens_packed take them */
+JIMM_API int jimm_text_attn(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_attn_req_t* req, float* pooled, void* stream);
+JIMM_API int jimm_text_attn_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_attn_req_t* req, float* pooled,
+                                   void* stream);
 
 /* -- forward of a bare sub-module (kinds JIMM_ENCODER / JIMM_MAPHEAD; config fields used: v_width, v_heads, v_mlp, v_layers, v_act,
  *    v_eps_block, v_eps_outer, t_causal (attn_mask = tril), ctx_len = max tokens per sample, compute_dtype; parameters keyed
@@ -321,6 +355,15 @@ JIMM_API int jimm_k_map_attention_packed(const float* q, const void* kv, int io_
  * is this call with causal = 0.  Each sample's rows are the bits of jimm_k_attention_hd(..., causal, ...) on that sample alone. */
 JIMM_API int jimm_k_attention_packed_ex(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int max_S, int H,
                                         int head_dim, int causal, int reverse, void* stream);
+/* The attention weights of jimm_k_attention_hd / jimm_k_attention_packed_ex (HF output_attentions): softmax((q/sqrt(d)) k^T masked) in
+ * fp32, written as out_type JIMM_F32 / JIMM_F16 / JIMM_BF16 (the fp32 value rounded to nearest even).  out: sample b's [H, S_b, S_b] block,
+ * row-major, from element H * sum_{j<b} S_j^2 on (dense, seq_off NULL: S_b = S); causal: the entries above the diagonal are 0. */
+JIMM_API int jimm_k_attn_probs(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int S, int H, int head_dim,
+                               int causal, void* stream);
+/* jimm_k_map_attention_hd (seq_off NULL) / jimm_k_map_attention_packed that also writes the weights its output sums with, probs
+ * [B, H, 1, S] of probs_type (packed: sample b's [H, 1, S_b] from element H * seq_off[b] on); probs NULL is the plain call. */
+JIMM_API int jimm_k_map_attention_probs(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B,
+                                        int S, int H, int head_dim, void* probs, int probs_type, void* stream);
 JIMM_API int jimm_k_patchify(const void* img, int in_type, int B, int H, int W, int C, int P, void* out, int out_type, void* stream);
 /* jimm_k_patchify into the patch GEMM's padded layout: rows_per_sample (0 = patches per image; more = pad rows per sample, left
  * untouched) and ldk (row stride in elements, 0 = P*P*C; more = pad columns, written as zeros). */

@@ -47,6 +47,15 @@ class TokensReq(C.Structure):
     _fields_ = [("n", C.c_int), ("layers", C.POINTER(C.c_int)), ("out", C.POINTER(C.c_void_p)), ("out_dtype", C.c_int)]
 
 
+ATTN_MAP = -2  # JIMM_ATTN_MAP: the MAP head's probe weights
+
+
+class AttnReq(C.Structure):
+    """jimm_attn_req_t"""
+
+    _fields_ = [("n", C.c_int), ("blocks", C.POINTER(C.c_int)), ("out", C.POINTER(C.c_void_p)), ("out_dtype", C.c_int)]
+
+
 # name -> (restype, argtypes): every symbol include/jimm_b200.h declares
 class PreprocConfig(C.Structure):
     """jimm_preproc_config_t"""
@@ -90,6 +99,11 @@ SIGNATURES = {
     "jimm_image_tokens_patches": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_i), C.POINTER(TokensReq), _fp, _vp]),
     "jimm_text_tokens": (_i, [_vp, _ip, _i, _i, C.POINTER(TokensReq), _fp, _vp]),
     "jimm_text_tokens_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), C.POINTER(TokensReq), _fp, _vp]),
+    "jimm_image_attn": (_i, [_vp, _vp, _i, _i, _i, _i, C.POINTER(AttnReq), _fp, _vp]),
+    "jimm_image_attn_packed": (_i, [_vp, C.POINTER(_vp), _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(AttnReq), _fp, _vp]),
+    "jimm_image_attn_patches": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_i), C.POINTER(AttnReq), _fp, _vp]),
+    "jimm_text_attn": (_i, [_vp, _ip, _i, _i, C.POINTER(AttnReq), _fp, _vp]),
+    "jimm_text_attn_packed": (_i, [_vp, _ip, _i, C.POINTER(_i), C.POINTER(AttnReq), _fp, _vp]),
     "jimm_encoder_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_map_head_forward": (_i, [_vp, _fp, _i, _i, _fp, _vp]),
     "jimm_vit_forward_host": (_i, [_vp, _vp, _i, _i, _fp, _vp]),
@@ -119,6 +133,8 @@ SIGNATURES = {
     "jimm_k_attention_packed": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _vp]),
     "jimm_k_map_attention_packed": (_i, [_fp, _vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _vp]),
     "jimm_k_attention_packed_ex": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_attn_probs": (_i, [_vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _i, _vp]),
+    "jimm_k_map_attention_probs": (_i, [_fp, _vp, _i, _vp, _i, _ip, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "jimm_k_patchify_ex": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "jimm_k_activation": (_i, [_fp, _fp, C.c_longlong, _i, _vp]),

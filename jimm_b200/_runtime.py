@@ -4,6 +4,7 @@ Python mirror classes.  PyTorch is used only for device memory, streams and torc
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
@@ -168,9 +169,9 @@ _TOKEN_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 
 
 class TokenLayers(NamedTuple):
-    """The layer requests of a per-token call, checked once (prep_layers)."""
+    """The requests of a per-token call (prep_layers) or of an attention call (prep_blocks), checked once."""
 
-    codes: List[int]  # the distinct requests as the library takes them: 0 .. L, or LAYER_FINAL
+    codes: List[int]  # the distinct requests as the library takes them: layers 0 .. L or LAYER_FINAL; blocks 0 .. L-1 or ATTN_MAP
     index: List[int]  # request i is codes[index[i]]
     single: bool  # one request (an int or None), not a list / tuple
     dtype: torch.dtype
@@ -198,6 +199,37 @@ def prep_layers(layers, num_layers: int, dtype) -> TokenLayers:
             c = k % (L + 1)
         else:
             raise ValueError(f"a layer request is an int or None, got {k!r}")
+        if c not in codes:
+            codes.append(c)
+        index.append(codes.index(c))
+    return TokenLayers(codes, index, single, dtype)
+
+
+def prep_blocks(blocks, num_layers: int, dtype, map_head: bool) -> TokenLayers:
+    """The block step of an attention call on a tower of num_layers blocks: `blocks` is an int k in [-L, L-1] (block k's self-attention
+    weights, negative k counting from the end), "map" (the MAP head's probe weights; map_head: the tower has one), None (every block in
+    order, HF's `attentions` tuple, "map" not included) or a list / tuple of these; dtype the output type, float32, float16 or bfloat16.
+    One int or "map" gives one result; None or a list gives a tuple."""
+    L = int(num_layers)
+    if dtype not in _TOKEN_DTYPES:
+        raise ValueError(f"attention weights come as torch.float32, torch.float16 or torch.bfloat16, got dtype={dtype}")
+    single = blocks is not None and not isinstance(blocks, (list, tuple))
+    reqs = [blocks] if single else list(range(L)) if blocks is None else list(blocks)
+    if not reqs:
+        raise ValueError("blocks: an empty list requests nothing; pass an int, \"map\", None or a non-empty list of them")
+    codes, index = [], []
+    for k in reqs:
+        if isinstance(k, str) and k == "map":
+            if not map_head:
+                raise ValueError('blocks="map": the tower has no MAP head (CLS-pooled vision towers and text towers)')
+            c = _lib.ATTN_MAP
+        elif isinstance(k, (int, np.integer)) and not isinstance(k, bool):
+            k = int(k)
+            if not -L <= k <= L - 1:
+                raise ValueError(f"block {k} outside [-{L}, {L - 1}] for a tower of {L} blocks")
+            c = k % L
+        else:
+            raise ValueError(f'a block request is an int or "map" (or None for every block, alone), got {k!r}')
         if c not in codes:
             codes.append(c)
         index.append(codes.index(c))
@@ -418,51 +450,75 @@ class NativeModel:
         ids = self._texts(ids)
         return self._back(self._text_dev(ids), ids.host if isinstance(ids, Texts) else not ids.is_cuda).result()
 
-    # ---- per-token hidden states ----
-    def _tokens_call(self, name: str, inputs, rows: int, D: int, req: TokenLayers, B: int, pooled_dim: int, pooled: bool):
-        """Entry point `name` (jimm_image_tokens* / jimm_text_tokens*) on `inputs`: one [rows, D] output of req.dtype on this GPU per
-        distinct request, and the fp32 [B, pooled_dim] pooled output when asked (else None)."""
-        outs = [torch.empty((rows, D), dtype=req.dtype, device=self.device) for _ in req.codes]
+    # ---- per-token hidden states and attention weights ----
+    def _sink_call(self, name: str, struct, inputs, shapes, req: TokenLayers, B: int, pooled_dim: int, pooled: bool, host: bool):
+        """Entry point `name` (jimm_image_tokens* / jimm_text_tokens* with struct TokensReq, jimm_image_attn* / jimm_text_attn* with
+        AttnReq) on `inputs`: per distinct request i one output of req.dtype shaped by shapes[i] -- a tuple for a dense batch, or a list
+        of per-sample shapes, views of one packed buffer in sample order -- and the fp32 [B, pooled_dim] pooled output when asked (else
+        None).  host: the results come back to the host."""
+        outs = [torch.empty(sum(math.prod(x) for x in ([sh] if isinstance(sh, tuple) else sh)), dtype=req.dtype, device=self.device)
+                for sh in shapes]
         pool = torch.empty((B, pooled_dim), dtype=torch.float32, device=self.device) if pooled else None
         if B:
             n = len(req.codes)
-            r = _lib.TokensReq(n, (C.c_int * n)(*req.codes), (C.c_void_p * n)(*[o.data_ptr() for o in outs]), _TORCH_TO_CODE[req.dtype])
+            r = struct(n, (C.c_int * n)(*req.codes), (C.c_void_p * n)(*[o.data_ptr() for o in outs]), _TORCH_TO_CODE[req.dtype])
             self._run(name, *inputs, C.byref(r), pool if pooled else None)
-        return outs, pool
+        if host:
+            outs = [self._back(o, True).result() for o in outs]
+            pool = self._back(pool, True).result() if pool is not None else None
+        res = []
+        for o, sh in zip(outs, shapes):
+            if isinstance(sh, tuple):
+                res.append(o.view(sh))
+            else:
+                res.append([p.view(x) for p, x in zip(torch.split(o, [math.prod(x) for x in sh]), sh)] if sh else [])
+        return res, pool
+
+    @staticmethod
+    def _sink_shapes(attn: bool, req: TokenLayers, B: int, S, counts, D: int, H: int):
+        """Each request's output shape (see _sink_call) for B samples of S tokens each (counts None) or of counts[b] tokens: hidden
+        states [S, D] per sample; attention weights [H, S, S], or [H, 1, S] for the MAP head's."""
+        def one(c, n):
+            return (n, D) if not attn else (H, 1, n) if c == _lib.ATTN_MAP else (H, n, n)
+        return [(B, *one(c, S)) if counts is None else [one(c, n) for n in counts] for c in req.codes]
+
+    def _image_sink(self, im: Images, req: TokenLayers, pooled: bool, attn: bool):
+        xd = self._device_images(im.x)
+        B = len(xd)
+        form, args, counts = self._image_inputs(im, xd)
+        name = ("jimm_image_attn" if attn else "jimm_image_tokens") + {"patches": "_patches", "packed": "_packed"}.get(form, "")
+        S = grid_tokens(self.cfg, xd.shape[1], xd.shape[2]) if counts is None else None
+        shapes = self._sink_shapes(attn, req, B, S, counts, self.cfg.v_width, self.cfg.v_heads)
+        return self._sink_call(name, _lib.AttnReq if attn else _lib.TokensReq, args, shapes, req, B, self.vision_out, pooled, im.host)
+
+    def _text_sink(self, ids, req: TokenLayers, pooled: bool, attn: bool):
+        args, lens, host = self._text_inputs(self._texts(ids))
+        B = args[1]
+        name = ("jimm_text_attn" if attn else "jimm_text_tokens") + ("" if lens is None else "_packed")
+        shapes = self._sink_shapes(attn, req, B, args[2] if lens is None else None, lens, self.cfg.t_width, self.cfg.t_heads)
+        return self._sink_call(name, _lib.AttnReq if attn else _lib.TokensReq, args, shapes, req, B, self.text_out, pooled, host)
 
     def image_tokens(self, im: Images, req: TokenLayers, pooled: bool = False):
         """Hidden states of the vision tower on prepared images: per distinct request [B, S, D] for a batch, a list of [S_i, D] views of
         one packed [sum S_i, D] buffer for a list or NaFlex patch rows; and the pooled output (the vision call's result) when asked.
         Host images are copied over and run eagerly; their results come back to the host."""
-        xd = self._device_images(im.x)
-        B = len(xd)
-        form, args, counts = self._image_inputs(im, xd)
-        name = {"patches": "jimm_image_tokens_patches", "packed": "jimm_image_tokens_packed"}.get(form, "jimm_image_tokens")
-        S = grid_tokens(self.cfg, xd.shape[1], xd.shape[2]) if counts is None else None
-        rows = sum(counts) if counts is not None else B * S
-        outs, pool = self._tokens_call(name, args, rows, self.cfg.v_width, req, B, self.vision_out, pooled)
-        return self._tokens_back(outs, pool, im.host, counts, None if counts is not None else (B, S))
+        return self._image_sink(im, req, pooled, False)
 
     def text_tokens(self, ids, req: TokenLayers, pooled: bool = False):
         """Hidden states of the text tower on a [B, T] ids tensor (per distinct request [B, T, D]) or on Texts (a list of [L_i, D] views
         of one packed [sum L_i, D] buffer); and the pooled output (encode_text's result) when asked.  Host ids give host results."""
-        args, lens, host = self._text_inputs(self._texts(ids))
-        B = args[1]
-        name, rows = ("jimm_text_tokens", B * args[2]) if lens is None else ("jimm_text_tokens_packed", sum(lens))
-        outs, pool = self._tokens_call(name, args, rows, self.cfg.t_width, req, B, self.text_out, pooled)
-        return self._tokens_back(outs, pool, host, lens, (B, args[2]) if lens is None else None)
+        return self._text_sink(ids, req, pooled, False)
 
-    def _tokens_back(self, outs, pool, host: bool, counts, shape):
-        """The outputs of a per-token call as its caller gets them: on the host for host inputs, [B, S, D] (shape = (B, S)) or split into
-        per-sample views of `counts` rows."""
-        if host:
-            outs = [self._back(o, True).result() for o in outs]
-            pool = self._back(pool, True).result() if pool is not None else None
-        if counts is not None:
-            outs = [list(torch.split(o, counts)) if counts else [] for o in outs]
-        else:
-            outs = [o.view(shape[0], shape[1], o.shape[1]) for o in outs]
-        return outs, pool
+    def image_attn(self, im: Images, req: TokenLayers, pooled: bool = False):
+        """Attention weights of the vision tower on prepared images (req from prep_blocks): per distinct request [B, H, S, S] for a batch
+        ([B, H, 1, S] for the MAP head's), a list of [H, S_i, S_i] ([H, 1, S_i]) views of one packed buffer for a list or NaFlex patch
+        rows; and the pooled output when asked.  Host images give host results."""
+        return self._image_sink(im, req, pooled, True)
+
+    def text_attn(self, ids, req: TokenLayers, pooled: bool = False):
+        """Attention weights of the text tower on a [B, T] ids tensor ([B, H, T, T] per distinct request) or on Texts (a list of
+        [H, L_i, L_i] views of one packed buffer); and the pooled output when asked.  Host ids give host results."""
+        return self._text_sink(ids, req, pooled, True)
 
     def dual_encode(self, x: torch.Tensor, ids: torch.Tensor):
         """encode_image + encode_text of device-resident inputs with the two towers running concurrently (jimm_dual_encode)."""

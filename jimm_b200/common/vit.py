@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _lib, nn
-from .._runtime import Images, NativeModel, default_max_batch, grid_tokens, prep_images, prep_layers, tokens_result
+from .._runtime import Images, NativeModel, default_max_batch, grid_tokens, prep_blocks, prep_images, prep_layers, tokens_result
 from .transformer import Transformer, _SubModuleRunner, g_wrap
 
 
@@ -132,12 +132,15 @@ class _NativeOwner:
         im = self._images(images, interpolate_pos_encoding, **inputs)
         return self.native(hw=im.hw if interpolate_pos_encoding else None).vision(im, encode=encode, wait=wait)
 
-    def _vision_tokens(self, images, layers, dtype, return_pooled: bool, interpolate_pos_encoding: bool, **inputs):
-        """A per-token vision call (NativeModel.image_tokens) on the inputs _vision takes.  The layers, the dtype and the images are
-        checked before any handle is built, and the handle is chosen (or rebuilt) as for the pooled call."""
-        req = prep_layers(layers, self._native_config().v_layers, dtype)
+    def _vision_tokens(self, images, layers, dtype, return_pooled: bool, interpolate_pos_encoding: bool, attn: bool = False, **inputs):
+        """A per-token vision call (NativeModel.image_tokens) or, attn, an attention call (NativeModel.image_attn, `layers` being the
+        blocks) on the inputs _vision takes.  The requests, the dtype and the images are checked before any handle is built, and the
+        handle is chosen (or rebuilt) as for the pooled call."""
+        cfg = self._native_config()
+        req = prep_blocks(layers, cfg.v_layers, dtype, cfg.pooling == _lib.POOL_MAP) if attn else prep_layers(layers, cfg.v_layers, dtype)
         im = self._images(images, interpolate_pos_encoding, **inputs)
-        toks, pooled = self.native(hw=im.hw if interpolate_pos_encoding else None).image_tokens(im, req, return_pooled)
+        n = self.native(hw=im.hw if interpolate_pos_encoding else None)
+        toks, pooled = (n.image_attn if attn else n.image_tokens)(im, req, return_pooled)
         return tokens_result(toks, req, pooled, return_pooled)
 
     def set_max_image_size(self, height: int, width: int):
@@ -241,3 +244,13 @@ class VisionTransformerBase(_NativeOwner, nn.Module):
         images gives a list of [S_i, hidden_size].  Without None or return_pooled only the blocks up to the deepest request run.
         return_pooled: also return __call__'s result on the same input, bit for bit: (tokens, pooled)."""
         return self._vision_tokens(img, layers, dtype, return_pooled, interpolate_pos_encoding)
+
+    def forward_attentions(self, img, blocks=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False):
+        """Self-attention weights (HF's output_attentions) of the inputs __call__ takes.  blocks: an int k in [-L, L-1] -- block k's
+        softmax(q k^T / sqrt(d)) per head, computed in fp32 on the q / k the forward's attention reads (negative k counts from the end)
+        -- or "map" on a MAP-pooled tower, its pooling head's probe weights (the weights the pooled output sums the tokens with); None
+        gives every block in order, a tuple like HF's `attentions`; a list / tuple of these gives a tuple in request order.  Each result
+        is [batch, heads, S, S] ("map": [batch, heads, 1, S]) of `dtype` (float32, float16 or bfloat16), S the tokens as forward_tokens
+        orders them; a list of images gives a list of [heads, S_i, S_i].  Without "map" or return_pooled only the blocks up to the
+        deepest request run.  return_pooled: also return __call__'s result on the same input, bit for bit: (weights, pooled)."""
+        return self._vision_tokens(img, blocks, dtype, return_pooled, interpolate_pos_encoding, attn=True)

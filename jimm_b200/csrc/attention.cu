@@ -375,13 +375,254 @@ int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, 
 }
 
 // ------------------------------------------------------------------------------------------
+// Attention weights (HF output_attentions): softmax(q k^T / sqrt(d)) of one block, written out.
+// ------------------------------------------------------------------------------------------
+// One CTA = one warpgroup = 64 query rows of one (sample, head), the tiles, descriptors and S = Q K^T of attention_kernel.  Two passes over
+// the sample's 64-key tiles: the first keeps the fp32 online row max m and sum l (exp2 with scale_log2, as attention_kernel does), the
+// second recomputes each score tile and writes p = exp2(s c - m) / l.  Each warp stages its 16 x 64 tile in shared memory and writes it
+// as row segments of consecutive keys: rows are S elements long, so no store can assume more than the element's alignment.  Causal:
+// key tiles entirely above the diagonal are written as zeros without being computed.  Rows q >= S and keys >= S are never stored.
+// out: sample b's [H, S_b, S_b] block starts at element H * sum_{j<b} S_j^2 (dense: b * H * S^2); every offset is 64-bit.
+template <int DP, int OUTB>
+struct ProbsSmem {
+  static constexpr int STAGE_LD = OUTB == 4 ? 72 : 36;  // 32-bit words per staged row (64 fp32 or 64 16-bit + padding: no bank conflicts)
+  static constexpr int STAGE = QT * STAGE_LD * 4;
+  static constexpr int BYTES = 3 * HeadTile<DP>::BYTES + STAGE;  // Q + double-buffered K + the staged output tile
+};
+
+template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED>
+__global__ void __launch_bounds__(128)
+attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, int H, int d, float scale_log2, const int* __restrict__ seq_off) {
+  using L = HeadTile<DP>;
+  using PS = ProbsSmem<DP, static_cast<int>(sizeof(OutT))>;
+  uint8_t* smem = AttnSmem<PS::BYTES>::get();
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int D = H * d;
+  const size_t ld = static_cast<size_t>(3) * D;
+  uint32_t* stage = reinterpret_cast<uint32_t*>(smem + 3 * L::BYTES);
+  pdl_launch_dependents();
+  pdl_wait();  // qkv is the QKV GEMM's output (and the offsets may come from the previous kernel)
+  int S = S_arg;
+  size_t row0 = static_cast<size_t>(b) * S_arg;
+  size_t obase = static_cast<size_t>(b) * H * S_arg * S_arg;
+  if constexpr (PACKED) {
+    row0 = static_cast<size_t>(seq_off[b]);
+    S = seq_off[b + 1] - seq_off[b];
+    if (qt * QT >= S) return;
+    // H * sum_{j<b} S_j^2, reduced over the CTA
+    unsigned long long acc = 0;
+    for (int j = tid; j < b; j += 128) {
+      const unsigned long long n = static_cast<unsigned long long>(seq_off[j + 1] - seq_off[j]);
+      acc += n * n;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    unsigned long long* red = reinterpret_cast<unsigned long long*>(stage);  // free until pass 2
+    if (lane == 0) red[warp] = acc;
+    __syncthreads();
+    obase = static_cast<size_t>(H) * (red[0] + red[1] + red[2] + red[3]);
+  }
+  obase += static_cast<size_t>(h) * S * S;
+  const T* gq = qkv + row0 * ld + h * d;
+  const T* gk = gq + D;
+  const uint32_t sQ = smem_u32(smem);
+  const uint32_t sK0 = sQ + L::BYTES;
+  const int q0 = qt * QT;
+  const int n_all = (S + KT - 1) / KT;
+  const int n_kv = CAUSAL ? min(n_all, qt + 1) : n_all;  // the tiles with a key at or below the diagonal
+
+  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  const uint64_t qdesc = make_wgmma_desc<L::SW>(sQ, 16);
+  const int g = lane >> 2, t4 = lane & 3;
+  const int row_lo = q0 + warp * 16 + g;  // this thread's two query rows: row_lo, row_lo + 8
+
+  // S = Q K^T of key tile j (this warp's 16 rows, m16n8 accumulator layout), masked to -inf past S and above the diagonal.  The K tile
+  // of step `it` of a pass is in buffer it & 1; the next one is prefetched while this one is used.
+  auto scores = [&](int j, int it, int n_it, float (&s)[8][4]) {
+    const int buf = it & 1;
+    if (it + 1 < n_it) {
+      load_tile<T, DP>(sK0 + (buf ^ 1) * L::BYTES, gk, ld, (j + 1) * KT, S, d, tid);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    float (&s_acc)[32] = reinterpret_cast<float (&)[32]>(s);
+    const uint64_t kdesc = make_wgmma_desc<L::SW>(sK0 + buf * L::BYTES, 16);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s_acc[i] = 0.f;
+    wgmma_fence_operands(s_acc);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < DP / 16; ++ks) wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + L::kstep(ks), kdesc + L::kstep(ks), ks != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s_acc);
+    __syncthreads();  // every warp is done reading buf before it is refilled by the next step's prefetch
+    const int k0 = j * KT;
+    if ((k0 + KT > S) || (CAUSAL && (k0 + KT - 1 > q0))) {
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = k0 + nt * 8 + t4 * 2 + (e & 1);
+          if (!(key < S && (!CAUSAL || key <= row_lo + (e >> 1) * 8))) s[nt][e] = -INFINITY;
+        }
+    }
+  };
+
+  // ---- pass 1: row max and sum ----
+  load_tile<T, DP>(sQ, gq, ld, q0, S, d, tid);
+  load_tile<T, DP>(sK0, gk, ld, 0, S, d, tid);
+  cp_async_commit();
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  for (int j = 0; j < n_kv; ++j) {
+    float s[8][4];
+    scores(j, j, n_kv, s);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[nt][0], s[nt][1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[nt][2], s[nt][3]));
+    }
+    float moff[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mnew = fmaxf(m_run[r], mx[r]);
+      const float muse = (mnew == -INFINITY) ? 0.f : mnew;
+      l_run[r] *= exp2f((m_run[r] - muse) * scale_log2);
+      m_run[r] = mnew;
+      moff[r] = muse * scale_log2;
+    }
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      l_run[0] += exp2f(s[nt][0] * scale_log2 - moff[0]) + exp2f(s[nt][1] * scale_log2 - moff[0]);
+      l_run[1] += exp2f(s[nt][2] * scale_log2 - moff[1]) + exp2f(s[nt][3] * scale_log2 - moff[1]);
+    }
+  }
+  float inv[2], moff[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv[r] = 1.0f / l;
+    moff[r] = (m_run[r] == -INFINITY ? 0.f : m_run[r]) * scale_log2;
+  }
+
+  // ---- pass 2: the probabilities, staged per warp and stored as row segments ----
+  uint32_t* wst = stage + warp * 16 * PS::STAGE_LD;
+  OutT* orow = out + obase + static_cast<size_t>(q0 + warp * 16) * S;  // this warp's first row
+  const int rows = min(16, S - (q0 + warp * 16));                       // this warp's rows inside the sample (may be <= 0)
+  load_tile<T, DP>(sK0, gk, ld, 0, S, d, tid);
+  cp_async_commit();
+  for (int j = 0; j < n_all; ++j) {
+    const int k0 = j * KT, cols = min(KT, S - k0);
+    if (j < n_kv) {
+      float s[8][4];
+      scores(j, j, n_kv, s);
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const float p0 = exp2f(s[nt][2 * r] * scale_log2 - moff[r]) * inv[r];
+          const float p1 = exp2f(s[nt][2 * r + 1] * scale_log2 - moff[r]) * inv[r];
+          const int srow = g + r * 8, c = nt * 8 + t4 * 2;
+          if constexpr (sizeof(OutT) == 4) *reinterpret_cast<float2*>(wst + srow * PS::STAGE_LD + c) = make_float2(p0, p1);
+          else wst[srow * PS::STAGE_LD + c / 2] = pack_pair<OutT>(p0, p1);
+        }
+      }
+      __syncwarp();
+      for (int r = 0; r < rows; ++r) {
+        OutT* dst = orow + static_cast<size_t>(r) * S + k0;
+        const OutT* src = reinterpret_cast<const OutT*>(wst + r * PS::STAGE_LD);
+        if (lane < cols) dst[lane] = src[lane];
+        if (lane + 32 < cols) dst[lane + 32] = src[lane + 32];
+      }
+      __syncwarp();  // the staged tile is read before the next one overwrites it
+    } else {  // causal: every key of the tile is above the diagonal
+      const OutT z = from_float<OutT>(0.f);
+      for (int r = 0; r < rows; ++r) {
+        OutT* dst = orow + static_cast<size_t>(r) * S + k0;
+        if (lane < cols) dst[lane] = z;
+        if (lane + 32 < cols) dst[lane + 32] = z;
+      }
+    }
+  }
+}
+
+template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED>
+static int probs_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
+  constexpr int SMEM = ProbsSmem<DP, static_cast<int>(sizeof(OutT))>::BYTES;
+  constexpr size_t dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
+  auto* kernel = attn_probs_kernel<T, OutT, CAUSAL, DP, PACKED>;
+  if constexpr (dyn > 0) {
+    static DeviceOnce attr_set;
+    if (int rc = attr_set.run([&]() -> int {
+          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+          return 0;
+        }))
+      return rc;
+  }
+  dim3 grid((S + QT - 1) / QT, H, B);
+  JIMM_CUDA_CHECK(launch_k(kernel, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d,
+                           attn_scale_log2(d), seq_off));
+  note_launch();
+  return 0;
+}
+
+template <typename T, typename OutT, bool CAUSAL, bool PACKED>
+static int probs_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
+  switch (padded_head_dim(d)) {
+    case 16: return probs_launch_dp<T, OutT, CAUSAL, 16, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+    case 32: return probs_launch_dp<T, OutT, CAUSAL, 32, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+    case 64: return probs_launch_dp<T, OutT, CAUSAL, 64, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+    case 80: return probs_launch_dp<T, OutT, CAUSAL, 80, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+    case 96: return probs_launch_dp<T, OutT, CAUSAL, 96, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+    default: return probs_launch_dp<T, OutT, CAUSAL, 128, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
+  }
+}
+
+template <typename T, typename OutT>
+static int probs_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, const int* seq_off) {
+  if (seq_off && causal) return probs_launch_causal<T, OutT, true, true>(qkv, out, B, S, H, d, stream, seq_off);
+  if (seq_off) return probs_launch_causal<T, OutT, false, true>(qkv, out, B, S, H, d, stream, seq_off);
+  if (causal) return probs_launch_causal<T, OutT, true, false>(qkv, out, B, S, H, d, stream, nullptr);
+  return probs_launch_causal<T, OutT, false, false>(qkv, out, B, S, H, d, stream, nullptr);
+}
+
+template <typename T>
+static int probs_out(const void* qkv, void* out, int out_type, int B, int S, int H, int d, int causal, cudaStream_t stream, const int* seq_off) {
+  if (out_type == DT_F32) return probs_launch<T, float>(qkv, out, B, S, H, d, causal, stream, seq_off);
+  if (out_type == DT_F16) return probs_launch<T, __half>(qkv, out, B, S, H, d, causal, stream, seq_off);
+  return probs_launch<T, __nv_bfloat16>(qkv, out, B, S, H, d, causal, stream, seq_off);
+}
+
+int attn_probs_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int S, int H, int head_dim, int causal,
+                   cudaStream_t stream) {
+  if (!head_dim_ok(head_dim)) { set_last_error("attn_probs: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
+  if (out_type != DT_F32 && out_type != DT_F16 && out_type != DT_BF16) { set_last_error("attn_probs: output dtype %d", out_type); return -1; }
+  if (B <= 0 || S <= 0) return 0;
+  if (B > 65535 || H > 65535) { set_last_error("attn_probs: grid too large (B=%d H=%d)", B, H); return -1; }
+  if (io_type == DT_F16) return probs_out<__half>(qkv, out, out_type, B, S, H, head_dim, causal, stream, seq_off);
+  if (io_type == DT_BF16) return probs_out<__nv_bfloat16>(qkv, out, out_type, B, S, H, head_dim, causal, stream, seq_off);
+  set_last_error("attn_probs: qkv dtype %d; the attention I/O is fp16 or bf16", io_type);
+  return -1;
+}
+
+// ------------------------------------------------------------------------------------------
 // MAP-head attention: one CTA (256 threads) per (sample, head); scores in smem; HBM-bound on K/V.
 // ------------------------------------------------------------------------------------------
 // PACKED: sample b is rows seq_off[b] .. seq_off[b + 1] - 1 of kv (S_arg: the longest sample, which the scores' smem is sized for)
 template <typename T, typename OutT, bool PACKED = false>
 __global__ void __launch_bounds__(256)
 map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT* __restrict__ out, int S_arg, int H, int d, float qscale,
-                     const int* __restrict__ seq_off) {
+                     const int* __restrict__ seq_off, void* __restrict__ probs, int probs_type) {
   extern __shared__ float sm[];
   float* sq = sm;              // [128]
   float* red = sm + 128;       // [8 * 128] cross-group reduction / [8] block reductions
@@ -434,6 +675,15 @@ map_attention_kernel(const float* __restrict__ q, const T* __restrict__ kv, OutT
 #pragma unroll
   for (int w = 0; w < 8; ++w) bsum += red[w];
   __syncthreads();
+  if (probs) {  // the weights the output sums with, [B, H, 1, S]: sample b from element H * (its first token row) on
+    const size_t pb = row0 * H + static_cast<size_t>(h) * S;
+    for (int s = tid; s < S; s += 256) {
+      const float p = sc[s] / bsum;
+      if (probs_type == DT_F32) static_cast<float*>(probs)[pb + s] = p;
+      else if (probs_type == DT_F16) static_cast<__half*>(probs)[pb + s] = __float2half_rn(p);
+      else static_cast<__nv_bfloat16*>(probs)[pb + s] = __float2bfloat16_rn(p);
+    }
+  }
   // output: warp = key group, lane = dim pairs lane and lane + 32 (columns 2 lane, 2 lane + 1 and 64 more)
   float a[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
   for (int s = warp; s < S; s += 8) {
@@ -477,7 +727,8 @@ int map_attention_max_seq(int device, int* max_S) {
 }
 
 template <typename T, typename OutT, bool PACKED>
-static int map_launch_k(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
+static int map_launch_k(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off, void* probs,
+                        int probs_type) {
   auto* kernel = map_attention_kernel<T, OutT, PACKED>;
   const size_t smem = (kMapSmemFloats + S) * sizeof(float);
   if (smem > 48 * 1024) {  // opt in once per device to all the shared memory map_attention_max_seq counts on
@@ -492,42 +743,48 @@ static int map_launch_k(const float* q, const void* kv, void* out, int B, int S,
       return rc;
   }
   const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(d)));  // 0.125f for d = 64
-  kernel<<<dim3(H, B), 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off);
+  kernel<<<dim3(H, B), 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off, probs, probs_type);
   JIMM_LAUNCH_CHECK();
   return 0;
 }
 
 template <typename T, typename OutT>
-static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
-  if (seq_off) return map_launch_k<T, OutT, true>(q, kv, out, B, S, H, d, stream, seq_off);
-  return map_launch_k<T, OutT, false>(q, kv, out, B, S, H, d, stream, nullptr);
+static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off, void* probs,
+                      int probs_type) {
+  if (seq_off) return map_launch_k<T, OutT, true>(q, kv, out, B, S, H, d, stream, seq_off, probs, probs_type);
+  return map_launch_k<T, OutT, false>(q, kv, out, B, S, H, d, stream, nullptr, probs, probs_type);
 }
 
 static int map_dispatch(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
-                        const int* seq_off) {
+                        const int* seq_off, void* probs, int probs_type) {
   if (!head_dim_ok(head_dim)) { set_last_error("map_attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0) return 0;
   int dev = 0, max_S = 0;
   JIMM_CUDA_CHECK(cudaGetDevice(&dev));
   if (int rc = map_attention_max_seq(dev, &max_S)) return rc;
   if (S > max_S) { set_last_error("map_attention: S=%d too large (the scores of a sample live in shared memory: at most %d tokens on device %d)", S, max_S, dev); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream, seq_off);
-  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream, seq_off);
-  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream, seq_off);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream, seq_off);
-  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream, seq_off);
+  if (probs && probs_type != DT_F32 && probs_type != DT_F16 && probs_type != DT_BF16) {
+    set_last_error("map_attention: probs dtype %d", probs_type);
+    return -1;
+  }
+  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
+  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
+  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
+  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
+  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
   set_last_error("map_attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
   return -1;
 }
 
-int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream) {
-  return map_dispatch(q, kv, io_type, out, out_type, B, S, H, head_dim, stream, nullptr);
+int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
+                      void* probs, int probs_type) {
+  return map_dispatch(q, kv, io_type, out, out_type, B, S, H, head_dim, stream, nullptr, probs, probs_type);
 }
 
 int map_attention_packed_run(const float* q, const void* kv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H,
-                             int head_dim, cudaStream_t stream) {
+                             int head_dim, cudaStream_t stream, void* probs, int probs_type) {
   if (!seq_off) { set_last_error("map_attention_packed: null seq_off"); return -1; }
-  return map_dispatch(q, kv, io_type, out, out_type, B, max_S, H, head_dim, stream, seq_off);
+  return map_dispatch(q, kv, io_type, out, out_type, B, max_S, H, head_dim, stream, seq_off, probs, probs_type);
 }
 
 }  // namespace jimm

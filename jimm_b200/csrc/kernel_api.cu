@@ -117,6 +117,16 @@ int jimm_k_map_attention_packed(const float* q, const void* kv, int io_type, voi
                                 int H, int head_dim, void* stream) {
   return map_attention_packed_run(q, kv, io_type, out, out_type, seq_off, B, max_S, H, head_dim, static_cast<cudaStream_t>(stream));
 }
+int jimm_k_attn_probs(const void* qkv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int S, int H, int head_dim, int causal,
+                      void* stream) {
+  if (B > 0 && S > 0 && (!qkv || !out)) { set_last_error("jimm_k_attn_probs: null argument"); return JIMM_EINVAL; }
+  return attn_probs_run(qkv, io_type, out, out_type, seq_off, B, S, H, head_dim, causal, static_cast<cudaStream_t>(stream));
+}
+int jimm_k_map_attention_probs(const float* q, const void* kv, int io_type, void* out, int out_type, const int32_t* seq_off, int B, int S, int H,
+                               int head_dim, void* probs, int probs_type, void* stream) {
+  if (seq_off) return map_attention_packed_run(q, kv, io_type, out, out_type, seq_off, B, S, H, head_dim, static_cast<cudaStream_t>(stream), probs, probs_type);
+  return map_attention_run(q, kv, io_type, out, out_type, B, S, H, head_dim, static_cast<cudaStream_t>(stream), probs, probs_type);
+}
 int jimm_k_map_attention(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, void* stream) {
   return jimm_k_map_attention_hd(q, kv, io_type, out, out_type, B, S, H, 64, stream);
 }

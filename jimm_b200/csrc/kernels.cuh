@@ -128,12 +128,22 @@ int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, 
 int attention_packed_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H, int head_dim,
                          int causal, cudaStream_t stream, int reverse = 0);
 
+// The attention weights attention_run computes (HF output_attentions): p[b, h, q, k] = softmax_k((q/sqrt(d)) k^T masked) in fp32, written as
+// out_type DT_F32 | DT_F16 | DT_BF16 (round to nearest even).  out: sample b's [H, S_b, S_b] block starts at element H * sum_{j<b} S_j^2,
+// row-major; causal: the entries above the diagonal are 0.  seq_off null: B samples of S rows; else packed as in attention_packed_run
+// (S = max_S).  io_type fp16/bf16.  Launched with PDL: it waits for its stream predecessor before it reads qkv.
+int attn_probs_run(const void* qkv, int io_type, void* out, int out_type, const int* seq_off, int B, int S, int H, int head_dim, int causal,
+                   cudaStream_t stream);
+
 // MAP-head attention with a single (input-independent) probe query (common/vit.py:96-97).
 //   q: fp32 [H*d] (already projected + biased), kv: [B*S, 2D] (k | v) io_type, out [B, D] out_type; d as attention_run
-int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream);
-// map_attention_run on samples packed as in attention_packed_run (kv: [rows, 2D]); out [B, D]
+//   probs (optional): the weights the output sums with, [B, H, 1, S] of probs_type DT_F32 | DT_F16 | DT_BF16
+int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
+                      void* probs = nullptr, int probs_type = DT_F32);
+// map_attention_run on samples packed as in attention_packed_run (kv: [rows, 2D]); out [B, D]; probs: sample b's [H, 1, S_b] from element
+// H * seq_off[b] on
 int map_attention_packed_run(const float* q, const void* kv, int io_type, void* out, int out_type, const int* seq_off, int B, int max_S, int H,
-                             int head_dim, cudaStream_t stream);
+                             int head_dim, cudaStream_t stream, void* probs = nullptr, int probs_type = DT_F32);
 // The longest sequence the MAP-head attention takes on `device` (its scores live in shared memory): into *max_S; 0 or an error code.
 int map_attention_max_seq(int device, int* max_S);
 

@@ -633,8 +633,10 @@ struct PackedRows {
 };
 
 // Where a per-token call (jimm_image_tokens* / jimm_text_tokens*) puts the hidden states of one chunk: request j copies x_layers[j]
-// (JIMM_LAYER_FINAL: the final-normed tokens) into out[j] from output row row0 on.  run_encoder runs `blocks` blocks; the pooling tail
-// runs only when the call asked for the pooled output too.
+// (JIMM_LAYER_FINAL: the final-normed tokens) into out[j] from output row row0 on.  An attention call (jimm_image_attn* /
+// jimm_text_attn*) instead writes block ablocks[j]'s weights into aout[j] from element H * sq0 on (JIMM_ATTN_MAP: the MAP head's probe
+// weights, from element H * row0 on).  run_encoder runs `blocks` blocks; the pooling tail runs only when the call asked for the pooled
+// output too, or for the MAP head's weights.
 struct TokenSink {
   int n = 0;
   const int* layers = nullptr;
@@ -644,7 +646,13 @@ struct TokenSink {
   int blocks = 0;              // max(requested layer), or every block for JIMM_LAYER_FINAL / a pooled output
   const LNW* ln = nullptr;     // the final norm: ln_post (vision) / ln_final (text)
   float eps = 0.f;
-  TokenSink at(size_t r) const { TokenSink t = *this; t.row0 = r; return t; }
+  int an = 0;                  // attention requests
+  const int* ablocks = nullptr;
+  void* const* aout = nullptr;
+  int aout_type = DT_F32;
+  bool map = false;            // one of them is JIMM_ATTN_MAP
+  size_t sq0 = 0;              // sum of S_b^2 over the samples before the chunk
+  TokenSink at(size_t r, size_t sq) const { TokenSink t = *this; t.row0 = r; t.sq0 = sq; return t; }
 };
 
 // The requests of `sink` for layer k (JIMM_LAYER_FINAL: the final norm) on the T rows of x
@@ -654,6 +662,16 @@ static int sink_rows(const TokenSink& sink, int k, const float* x, int T, int D,
     void* dst = static_cast<uint8_t*>(sink.out[j]) + sink.row0 * D * dtype_size(sink.out_type);
     if (k == JIMM_LAYER_FINAL) JIMM_TRY(layernorm_run(x, D, 1, 0, nullptr, sink.ln->scale, sink.ln->bias, sink.eps, dst, sink.out_type, D, T, D, s));
     else JIMM_TRY(tokens_out_run(x, static_cast<size_t>(T), D, dst, sink.out_type, s));
+  }
+  return 0;
+}
+
+// The attention requests of `sink` for block bi, on the qkv that block's attention read
+static int sink_attn(const TokenSink& sink, int bi, const void* qkv, int adt, const EncoderCfg& c, int B, int S, const PackedRows* pk, cudaStream_t s) {
+  for (int j = 0; j < sink.an; ++j) {
+    if (sink.ablocks[j] != bi) continue;
+    void* dst = static_cast<uint8_t*>(sink.aout[j]) + sink.sq0 * c.H * dtype_size(sink.aout_type);
+    JIMM_TRY(attn_probs_run(qkv, adt, dst, sink.aout_type, pk ? pk->seq_off : nullptr, B, pk ? pk->max_S : S, c.H, c.D / c.H, c.causal, s));
   }
   return 0;
 }
@@ -679,6 +697,7 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
     JIMM_TRY(run_gemm(m, b.p_qkv, ln_h, c.D, b.qkv, T, s, flip()));
     if (pk) JIMM_TRY(attention_packed_run(ws.big, m->adt, ws.h, m->cdt, pk->seq_off, B, pk->max_S, c.H, c.D / c.H, c.causal, s, flip()));
     else JIMM_TRY(attention_run(ws.big, m->adt, ws.h, m->cdt, B, S, c.H, c.D / c.H, c.causal, s, flip()));
+    if (sink) JIMM_TRY(sink_attn(*sink, bi, ws.big, m->adt, c, B, S, pk, s));  // before FC1 overwrites ws.big
     JIMM_TRY(run_gemm(m, b.p_out, ws.h, c.D, b.out, T, s, flip()));  // + residual (+ norm2 -> ws.h when fused)
     if (m->simt || !gemm_fuses_ln(&b.p_out, T))
       JIMM_TRY(layernorm_run(ws.x, c.D, 1, 0, nullptr, b.norm2.scale, b.norm2.bias, c.eps, ln_h, ln_t, c.D, T, c.D, s, flip(), ws.sa));
@@ -692,14 +711,24 @@ static int run_encoder(jimm_model* m, Encoder* enc, int B, int S, cudaStream_t s
 }
 
 // MultiHeadAttentionPoolingHead.__call__ (common/vit.py:87-101) on the tokens in ws.h (compute dtype, [B*S, D], or the packed rows pk);
-// out fp32 [B, D]
-static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr) {
+// out fp32 [B, D].  sink: each JIMM_ATTN_MAP request also receives the probe weights; without out the head stops after its attention.
+static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr, const TokenSink* sink = nullptr) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
   const int D = v.D, T = pk ? pk->T : B * S, H = v.enc.c.H, d = v.enc.c.D / v.enc.c.H;
   JIMM_TRY(run_gemm(m, v.p_map_kv, ws.enc.h, D, v.map_kv, T, s));                                    // k | v  [T, 2D]
-  if (pk) JIMM_TRY(map_attention_packed_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, pk->seq_off, B, pk->max_S, H, d, s));
-  else JIMM_TRY(map_attention_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s)); // [B, D]
+  auto attend = [&](void* probs, int probs_type) -> int {                                            // [B, D]
+    if (pk) return map_attention_packed_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, pk->seq_off, B, pk->max_S, H, d, s, probs, probs_type);
+    return map_attention_run(v.map_q, ws.enc.big, m->adt, ws.pooled, m->cdt, B, S, H, d, s, probs, probs_type);
+  };
+  bool probed = false;
+  for (int j = 0; sink && j < sink->an; ++j) {
+    if (sink->ablocks[j] != JIMM_ATTN_MAP) continue;
+    JIMM_TRY(attend(static_cast<uint8_t*>(sink->aout[j]) + sink->row0 * H * dtype_size(sink->aout_type), sink->aout_type));
+    probed = true;
+  }
+  if (!probed) JIMM_TRY(attend(nullptr, DT_F32));
+  if (!out) return 0;
   JIMM_TRY(run_gemm(m, v.p_map_out, ws.pooled, D, v.map_out, B, s));                                 // -> feat fp32 [B, D]
   JIMM_TRY(layernorm_run(ws.feat, D, 1, 0, nullptr, v.map_ln.scale, v.map_ln.bias, v.eps_outer, ws.pooled, m->cdt, D, B, D, s));
   JIMM_TRY(run_gemm(m, v.p_map_fc1, ws.pooled, D, v.map_fc1, B, s));                                 // gelu -> mid2 [B, M]
@@ -711,13 +740,13 @@ static int run_map_head(jimm_model* m, int B, int S, float* out, cudaStream_t s,
 // ln_post + the pooling head of B samples of S tokens (pk: the packed rows instead) in ws.x.  CLS: ln_post is per-row and only row 0 of
 // each sample is consumed (common/vit.py:244-246): every S-th row, or the packed offsets as row index (group 0).  MAP: ln_post of every
 // row, then the MAP head (common/vit.py:87-101).  out: fp32 [B, out_dim]
-static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr) {
+static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk = nullptr, const TokenSink* sink = nullptr) {
   VisionTower& v = m->vis;
   Workspace& ws = m->ws;
   const int D = v.D;
   if (v.pooling == JIMM_POOL_MAP) {
     JIMM_TRY(layernorm_run(ws.enc.x, D, 1, 0, nullptr, v.ln_post.scale, v.ln_post.bias, v.eps_outer, ws.enc.h, m->cdt, D, pk ? pk->T : B * S, D, s));
-    return run_map_head(m, B, S, out, s, pk);
+    return run_map_head(m, B, S, out, s, pk, sink);
   }
   const int group = pk ? 0 : S;
   const int* row_index = pk ? pk->seq_off : nullptr;
@@ -729,15 +758,15 @@ static int run_pool(jimm_model* m, int B, int S, float* out, cudaStream_t s, con
 }
 
 // The vision tower after the patch embedding, on B samples of S tokens (pk: the packed rows instead) in ws.x: ln_pre, the encoder and,
-// unless a token call (sink) asked for no pooled output, the pooling head into out.
+// unless a token or attention call (sink) asked for no pooled output and no MAP weights, the pooling head into out.
 static int vision_tail(jimm_model* m, int B, int S, float* out, cudaStream_t s, const PackedRows* pk, const TokenSink* sink) {
   VisionTower& v = m->vis;
   float* x = m->ws.enc.x;
   if (v.pre_norm)
     JIMM_TRY(layernorm_run(x, v.D, 1, 0, nullptr, v.ln_pre.scale, v.ln_pre.bias, v.eps_outer, x, DT_F32, v.D, pk ? pk->T : B * S, v.D, s));
   JIMM_TRY(run_encoder(m, &v.enc, B, S, s, m->ws.enc, pk, sink));
-  if (sink && !out) return 0;
-  return run_pool(m, B, S, out, s, pk);
+  if (sink && !out && !sink->map) return 0;
+  return run_pool(m, B, S, out, s, pk, sink);
 }
 
 // VisionTransformerBase.__call__ (common/vit.py:216-248) + the model's head.  img: [B, H, W, C]; grid: null for the trained patch
@@ -1453,7 +1482,8 @@ static int vision_chunks(jimm_model* m, const ImageSrc& src, int in_dtype, int B
     const void* img = src.from(b0).img;
     float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
     if (native && !sink) return exec_vision(m, img, in_dtype, nb, dst, s);
-    const TokenSink at = sink ? sink->at(static_cast<size_t>(b0) * (grid ? grid->S : v.S)) : TokenSink{};
+    const size_t S = grid ? grid->S : v.S;
+    const TokenSink at = sink ? sink->at(b0 * S, b0 * S * S) : TokenSink{};
     return run_vision(m, img, in_dtype, nb, src.H, src.W, grid, dst, s, sink ? &at : nullptr);
   });
 }
@@ -1475,6 +1505,13 @@ int jimm_model_images_per_call(const jimm_model_t* m, int H, int W, int* images)
 // token-layout patch rows (S rather than the padded n_pad) outgrow every other term of a handle without a set_max_tokens budget.
 static bool packed_fit(const jimm_model* m, size_t T) { return T <= m->ws_rows && big_bytes(m, T, T) <= m->ws_big; }
 
+// sum of (tok[b + 1] - tok[b])^2 over the samples of a packed chunk's offsets: what an attention call's outputs advance by, per head
+static size_t sum_squares(const std::vector<int>& tok) {
+  size_t n = 0;
+  for (size_t b = 0; b + 1 < tok.size(); ++b) n += static_cast<size_t>(tok[b + 1] - tok[b]) * (tok[b + 1] - tok[b]);
+  return n;
+}
+
 // B images of different sizes (IMG_LIST / IMG_ROWS): chunks of consecutive images, each as many as fit (packed_fit, at most max_batch),
 // run packed.  A token call (sink): each chunk writes from its first token row on; out may then be null.
 static int vision_packed(jimm_model* m, const ImageSrc& src, int in_dtype, int B, float* out, cudaStream_t s, const TokenSink* sink) {
@@ -1482,7 +1519,7 @@ static int vision_packed(jimm_model* m, const ImageSrc& src, int in_dtype, int B
   const int off = v.pooling == JIMM_POOL_CLS ? 1 : 0;
   const int od = vision_out_dim(m);
   std::vector<int> tok;
-  size_t t0 = 0;  // the chunk's first token row
+  size_t t0 = 0, sq0 = 0;  // the chunk's first token row; the sum of S_b^2 over the samples before it
   for (int b0 = 0; b0 < B;) {
     tok.assign(1, 0);
     int b1 = b0, max_S = 0;
@@ -1494,9 +1531,10 @@ static int vision_packed(jimm_model* m, const ImageSrc& src, int in_dtype, int B
       ++b1;
     }
     float* dst = out ? out + static_cast<size_t>(b0) * od : nullptr;
-    const TokenSink at = sink ? sink->at(t0) : TokenSink{};
+    const TokenSink at = sink ? sink->at(t0, sq0) : TokenSink{};
     JIMM_TRY(run_vision_packed(m, src.from(b0), in_dtype, b1 - b0, tok.data(), max_S, dst, s, sink ? &at : nullptr));
     t0 += tok.back();
+    sq0 += sum_squares(tok);
     b0 = b1;
   }
   return 0;
@@ -1508,7 +1546,7 @@ static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* o
     const int32_t* src = ids + static_cast<size_t>(b0) * T;
     float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
     if (!sink) return exec_text(m, src, nb, T, dst, s);
-    const TokenSink at = sink->at(static_cast<size_t>(b0) * T);
+    const TokenSink at = sink->at(static_cast<size_t>(b0) * T, static_cast<size_t>(b0) * T * T);
     return run_text(m, src, nb, T, dst, s, &at);
   });
 }
@@ -1520,7 +1558,7 @@ static int text_chunks(jimm_model* m, const int32_t* ids, int B, int T, float* o
 static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len, float* out, cudaStream_t s, const TokenSink* sink) {
   const int budget = m->max_batch * m->txt.T;
   std::vector<int> tok;
-  size_t r0 = 0;  // the chunk's first row of ids
+  size_t r0 = 0, sq0 = 0;  // the chunk's first row of ids; the sum of len^2 over the sequences before it
   for (int b0 = 0; b0 < B;) {
     tok.assign(1, 0);
     int b1 = b0, max_S = 0;
@@ -1530,9 +1568,10 @@ static int text_packed(jimm_model* m, const int32_t* ids, int B, const int* len,
       ++b1;
     }
     float* dst = out ? out + static_cast<size_t>(b0) * m->txt.D : nullptr;
-    const TokenSink at = sink ? sink->at(r0) : TokenSink{};
+    const TokenSink at = sink ? sink->at(r0, sq0) : TokenSink{};
     JIMM_TRY(run_text_packed(m, ids + r0, b1 - b0, tok.data(), max_S, dst, s, sink ? &at : nullptr));
     r0 += tok.back();
+    sq0 += sum_squares(tok);
     b0 = b1;
   }
   return 0;
@@ -1573,9 +1612,47 @@ static int tokens_sink(const char* fn, const jimm_tokens_req_t* req, const Encod
   return 0;
 }
 
-// The kinds of forward call: the pooled output (jimm_encode_*), the same on a ViT / tower handle only (jimm_vit_forward*), and the
-// hidden states of a request with the pooled output optional (jimm_image_tokens* / jimm_text_tokens*)
-enum CallKind { CALL_ENCODE, CALL_VIT, CALL_TOKENS };
+// The request of an attention call (fn names it) on the tower with encoder `enc` (map_head: the tower pools with a MAP head), as the
+// sink of its chunks.  pooled or a JIMM_ATTN_MAP request: every block runs.
+static int attn_sink(const char* fn, const jimm_attn_req_t* req, const Encoder& enc, bool map_head, bool pooled, TokenSink* sink) {
+  const int L = enc.c.L;
+  if (!req || !req->blocks || !req->out) { set_last_error("%s: null request", fn); return JIMM_EINVAL; }
+  if (req->n < 1 || req->n > L + 1) { set_last_error("%s: %d attention requests, outside 1 .. L + 1 = %d", fn, req->n, L + 1); return JIMM_EINVAL; }
+  if (req->out_dtype != JIMM_F32 && req->out_dtype != JIMM_F16 && req->out_dtype != JIMM_BF16) {
+    set_last_error("%s: output dtype %d; attention weights are JIMM_F32, JIMM_F16 or JIMM_BF16", fn, req->out_dtype);
+    return JIMM_EINVAL;
+  }
+  int blocks = pooled ? L : 0;
+  bool map = false;
+  for (int j = 0; j < req->n; ++j) {
+    const int k = req->blocks[j];
+    if (k == JIMM_ATTN_MAP) {
+      if (!map_head) { set_last_error("%s: request %d asks for JIMM_ATTN_MAP on a tower without a MAP head", fn, j); return JIMM_EINVAL; }
+      map = true;
+    } else if (k < 0 || k >= L) {
+      set_last_error("%s: request %d asks for block %d, outside 0 .. %d (or JIMM_ATTN_MAP)", fn, j, k, L - 1);
+      return JIMM_EINVAL;
+    }
+    if (!req->out[j] || reinterpret_cast<uintptr_t>(req->out[j]) % 16 != 0) {
+      set_last_error("%s: output buffer %d is null or not 16-byte aligned", fn, j);
+      return JIMM_EINVAL;
+    }
+    blocks = std::max(blocks, k == JIMM_ATTN_MAP ? L : k + 1);
+  }
+  *sink = TokenSink{};
+  sink->an = req->n;
+  sink->ablocks = req->blocks;
+  sink->aout = req->out;
+  sink->aout_type = req->out_dtype;
+  sink->map = map;
+  sink->blocks = blocks;
+  return 0;
+}
+
+// The kinds of forward call: the pooled output (jimm_encode_*), the same on a ViT / tower handle only (jimm_vit_forward*), the hidden
+// states of a request with the pooled output optional (jimm_image_tokens* / jimm_text_tokens*), and the attention weights of a request,
+// the same (jimm_image_attn* / jimm_text_attn*)
+enum CallKind { CALL_ENCODE, CALL_VIT, CALL_TOKENS, CALL_ATTN };
 
 static int null_argument(const char* fn) {
   set_last_error("%s: null argument", fn);
@@ -1629,7 +1706,7 @@ static int image_shapes(jimm_model* m, const char* fn, ImageSrc* src, int in_dty
 
 // Every vision call on device images (fn names it): the checks in the order include/jimm_b200.h states, then the chunker of the form.
 static int image_call(jimm_model* m, const char* fn, CallKind kind, ImageSrc src, int in_dtype, int B, float* out, const jimm_tokens_req_t* req,
-                      void* stream) {
+                      void* stream, const jimm_attn_req_t* areq = nullptr) {
   JIMM_TRY(check_ready(m, B));
   JIMM_TRY(check_image_dtype(in_dtype));
   if (src.form != IMG_ROWS) {
@@ -1640,14 +1717,16 @@ static int image_call(jimm_model* m, const char* fn, CallKind kind, ImageSrc src
   }
   TokenSink sink;
   if (kind == CALL_TOKENS) JIMM_TRY(tokens_sink(fn, req, m->vis.enc, m->vis.ln_post, m->vis.eps_outer, out != nullptr, &sink));
+  if (kind == CALL_ATTN) JIMM_TRY(attn_sink(fn, areq, m->vis.enc, m->vis.pooling == JIMM_POOL_MAP, out != nullptr, &sink));
+  const bool sinks = kind == CALL_TOKENS || kind == CALL_ATTN;
   const bool inputs = src.form == IMG_LIST ? src.imgs && src.Hs && src.Ws : src.img && (src.form == IMG_DENSE || src.grid);
-  if (B > 0 && (!inputs || (kind != CALL_TOKENS && !out))) return null_argument(fn);
+  if (B > 0 && (!inputs || (!sinks && !out))) return null_argument(fn);
   std::vector<int> cut;
   PatchGrid* grid = nullptr;
   JIMM_TRY(image_shapes(m, fn, &src, in_dtype, B, &cut, &grid));
   JIMM_TRY(set_device(m));
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const TokenSink* sk = kind == CALL_TOKENS ? &sink : nullptr;
+  const TokenSink* sk = sinks ? &sink : nullptr;
   if (src.form == IMG_DENSE) return vision_chunks(m, src, in_dtype, B, grid, out, s, sk);
   return vision_packed(m, src, in_dtype, B, out, s, sk);
 }
@@ -1662,16 +1741,18 @@ struct TextSrc {
 
 // Every text call on device ids (fn names it), on the pattern of image_call
 static int text_call(jimm_model* m, const char* fn, CallKind kind, const TextSrc& src, int B, float* out, const jimm_tokens_req_t* req,
-                     void* stream) {
+                     void* stream, const jimm_attn_req_t* areq = nullptr) {
   JIMM_TRY(check_ready(m, B));
   JIMM_TRY(check_text(m));
   TokenSink sink;
   if (kind == CALL_TOKENS) JIMM_TRY(tokens_sink(fn, req, m->txt.enc, m->txt.ln_final, m->txt.eps_outer, out != nullptr, &sink));
-  if (B > 0 && (!src.ids || (src.packed && !src.len) || (kind != CALL_TOKENS && !out))) return null_argument(fn);
+  if (kind == CALL_ATTN) JIMM_TRY(attn_sink(fn, areq, m->txt.enc, false, out != nullptr, &sink));
+  const bool sinks = kind == CALL_TOKENS || kind == CALL_ATTN;
+  if (B > 0 && (!src.ids || (src.packed && !src.len) || (!sinks && !out))) return null_argument(fn);
   JIMM_TRY(src.packed ? check_lens(m, B, src.len) : check_text_len(m, src.T));
   JIMM_TRY(set_device(m));
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const TokenSink* sk = kind == CALL_TOKENS ? &sink : nullptr;
+  const TokenSink* sk = sinks ? &sink : nullptr;
   if (src.packed) return text_packed(m, src.ids, B, src.len, out, s, sk);
   return text_chunks(m, src.ids, B, src.T, out, s, sk);
 }
@@ -1733,6 +1814,28 @@ int jimm_text_tokens(jimm_model_t* m, const int32_t* ids, int B, int T, const ji
 
 int jimm_text_tokens_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_tokens_req_t* req, float* pooled, void* stream) {
   return text_call(m, "jimm_text_tokens_packed", CALL_TOKENS, TextSrc{ids, 0, len, true}, B, pooled, req, stream);
+}
+
+int jimm_image_attn(jimm_model_t* m, const void* img, int in_dtype, int B, int H, int W, const jimm_attn_req_t* req, float* pooled, void* stream) {
+  return image_call(m, "jimm_image_attn", CALL_ATTN, ImageSrc::dense(img, H, W), in_dtype, B, pooled, nullptr, stream, req);
+}
+
+int jimm_image_attn_packed(jimm_model_t* m, const void* const* imgs, int in_dtype, int B, const int* H, const int* W, const jimm_attn_req_t* req,
+                           float* pooled, void* stream) {
+  return image_call(m, "jimm_image_attn_packed", CALL_ATTN, ImageSrc::list(imgs, H, W), in_dtype, B, pooled, nullptr, stream, req);
+}
+
+int jimm_image_attn_patches(jimm_model_t* m, const void* patches, int in_dtype, int B, int N, const int* grid, const jimm_attn_req_t* req,
+                            float* pooled, void* stream) {
+  return image_call(m, "jimm_image_attn_patches", CALL_ATTN, ImageSrc::rows(patches, N, grid), in_dtype, B, pooled, nullptr, stream, req);
+}
+
+int jimm_text_attn(jimm_model_t* m, const int32_t* ids, int B, int T, const jimm_attn_req_t* req, float* pooled, void* stream) {
+  return text_call(m, "jimm_text_attn", CALL_ATTN, TextSrc{ids, T, nullptr, false}, B, pooled, nullptr, stream, req);
+}
+
+int jimm_text_attn_packed(jimm_model_t* m, const int32_t* ids, int B, const int* len, const jimm_attn_req_t* req, float* pooled, void* stream) {
+  return text_call(m, "jimm_text_attn_packed", CALL_ATTN, TextSrc{ids, 0, len, true}, B, pooled, nullptr, stream, req);
 }
 
 int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const float* txt_e, int Bt, float* logits, void* stream) {

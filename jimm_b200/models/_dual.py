@@ -5,7 +5,7 @@ from __future__ import annotations
 import torch
 
 from .. import _lib, nn
-from .._runtime import Texts, _call, prep_ids, prep_layers, prep_texts, tokens_result
+from .._runtime import Texts, _call, prep_blocks, prep_ids, prep_layers, prep_texts, tokens_result
 from ..common.transformer import Transformer, g_wrap
 from ..common.vit import _NativeOwner, tower_config_fields
 
@@ -74,13 +74,33 @@ class DualTower(_NativeOwner, nn.Module):
         bfloat16), every row as computed, those after an EOT or padding included; a list of sequences gives a list of [L_i, width].
         Without None or return_pooled only the blocks up to the deepest request run.  return_pooled: also return encode_text's result,
         bit for bit: (tokens, pooled)."""
-        req = prep_layers(layers, self.transformer_layers, dtype)
+        return self._text_tokens(text, prep_layers(layers, self.transformer_layers, dtype), return_pooled, False)
+
+    def encode_image_attentions(self, image, blocks=None, *, dtype=torch.float32, return_pooled: bool = False,
+                                interpolate_pos_encoding: bool = False):
+        """Self-attention weights of the vision tower (HF's output_attentions) on the inputs encode_image takes: as
+        VisionTransformerBase.forward_attentions ("map" on SigLIP's MAP head).  return_pooled: also return encode_image's result, bit
+        for bit."""
+        return self._vision_tokens(image, blocks, dtype, return_pooled, interpolate_pos_encoding, attn=True)
+
+    def encode_text_attentions(self, text, blocks=None, *, dtype=torch.float32, return_pooled: bool = False):
+        """Self-attention weights of the text tower (HF's output_attentions) on the inputs encode_text takes.  blocks: an int k in
+        [-L, L-1], None (every block in order, a tuple) or a list / tuple of ints, giving a tuple in request order.  Each result is
+        [batch, heads, T, T] of `dtype` (float32, float16 or bfloat16), every row as computed, those after an EOT or padding included;
+        CLIP's text tower is causal, its entries above the diagonal 0.  A list of sequences gives a list of [heads, L_i, L_i].  Without
+        return_pooled only the blocks up to the deepest request run.  return_pooled: also return encode_text's result, bit for bit."""
+        return self._text_tokens(text, prep_blocks(blocks, self.transformer_layers, dtype, False), return_pooled, True)
+
+    def _text_tokens(self, text, req, return_pooled: bool, attn: bool):
+        """A per-token (NativeModel.text_tokens) or, attn, attention call (NativeModel.text_attn) of request req on the text inputs,
+        checked before any handle is built."""
         text = self._texts(text)
         if not isinstance(text, Texts):
             text = prep_ids(text)
             if not 1 <= text.shape[1] <= self.context_length:
                 raise ValueError(f"sequence length {text.shape[1]} outside 1 .. context_length={self.context_length}")
-        toks, pooled = self.native().text_tokens(text, req, return_pooled)
+        n = self.native()
+        toks, pooled = (n.text_attn if attn else n.text_tokens)(text, req, return_pooled)
         return tokens_result(toks, req, pooled, return_pooled)
 
     def __call__(self, image, text, interpolate_pos_encoding: bool = False) -> torch.Tensor:

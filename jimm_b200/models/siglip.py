@@ -92,6 +92,13 @@ class SigLIP(DualTower):
         return self._vision_tokens(image, layers, dtype, return_pooled, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,
                                    pixel_attention_mask=pixel_attention_mask)
 
+    def encode_image_attentions(self, image, blocks=None, *, dtype=torch.float32, return_pooled: bool = False,
+                                interpolate_pos_encoding: bool = False, spatial_shapes=None, pixel_attention_mask=None):
+        """As DualTower.encode_image_attentions, with the NaFlex image inputs of encode_image: on pixel_values with spatial_shapes each
+        sample's result is [heads, n_b, n_b] ("map": [heads, 1, n_b]), n_b = rows_b * cols_b its patches, row-major."""
+        return self._vision_tokens(image, blocks, dtype, return_pooled, interpolate_pos_encoding or self.naflex, attn=True,
+                                   spatial_shapes=spatial_shapes, pixel_attention_mask=pixel_attention_mask)
+
     def __call__(self, image, text, spatial_shapes=None, pixel_attention_mask=None, interpolate_pos_encoding: bool = False) -> torch.Tensor:
         """As DualTower.__call__, with the NaFlex image inputs of encode_image (single process only)."""
         return self._dual_call(image, text, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,

@@ -63,6 +63,11 @@ class VisionTransformer(_NativeOwner, nn.Module):
         __call__ takes.  return_pooled: also return the logits __call__ gives on the same input, bit for bit: (tokens, logits)."""
         return self._vision_tokens(x, layers, dtype, return_pooled, interpolate_pos_encoding)
 
+    def forward_attentions(self, x, blocks=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False):
+        """Self-attention weights of the encoder's blocks (HF's output_attentions; VisionTransformerBase.forward_attentions), on the
+        inputs __call__ takes.  return_pooled: also return the logits __call__ gives on the same input, bit for bit: (weights, logits)."""
+        return self._vision_tokens(x, blocks, dtype, return_pooled, interpolate_pos_encoding, attn=True)
+
     @classmethod
     def from_pretrained(cls, model_name_or_path: str, use_pytorch: bool = False, mesh=None, dtype=torch.float32) -> "VisionTransformer":
         """Load a HF `ViTForImageClassification` checkpoint (models/vit.py:105-273): same config parsing, shape
