@@ -438,8 +438,33 @@ JIMM_API int jimm_preproc_output_size(const jimm_preproc_t* p, int H, int W, int
  * through an 8-bit intermediate allocated in stream order per call, at most 64 MB per chunk of images; same bytes. */
 JIMM_API int jimm_preproc_run(jimm_preproc_t* p, const uint8_t* img, int B, int H, int W, void* out, int out_dtype, void* stream);
 JIMM_API int jimm_preproc_destroy(jimm_preproc_t* p);
+/* ---- SigLIP 2 NaFlex front-end: transformers' Siglip2ImageProcessor (PIL backend) on the GPU ----
+ * Every frame gets its own output size from the patch budget, is resized with Pillow's 8-bit arithmetic, rescaled, normalised and
+ * written as patch rows, bit-exact with the processor's pixel_values / pixel_attention_mask / spatial_shapes.
+ * jimm_preproc_naflex_grid (host only, no handle, no GPU): the processor's size rule (get_image_size_for_max_num_patches) in double
+ *   precision -- the patch grid gh x gw of an H x W frame (output size gh*patch x gw*patch).  JIMM_EINVAL for patch < 1,
+ *   max_num_patches < 1, an edge < 1, H x W x 3 >= 2^31 bytes, or a grid of more than max_num_patches patches (extreme strips,
+ *   for which the processor itself emits more rows than max_num_patches).
+ * jimm_preproc_create_naflex: cfg's resample (2 bilinear | 3 bicubic), rescale_factor, mean and std; height, width, shortest_edge,
+ *   crop_h and crop_w must be 0.  jimm_preproc_run and jimm_preproc_output_size refuse such a handle; jimm_preproc_run_naflex
+ *   refuses a fixed-size one.
+ * jimm_preproc_run_naflex: imgs a host array of B device pointers, image i contiguous uint8 RGB [H[i], W[i], 3] at any alignment;
+ *   pixel_values device [B, max_num_patches, patch*patch*3] of out_dtype (JIMM_F32 | JIMM_F16 | JIMM_BF16, aligned as for
+ *   jimm_preproc_run), each row a patch in (py, px, c) order, sample b's rows gh*gw .. max_num_patches - 1 zero; mask (nullable)
+ *   device int32 [B, max_num_patches], 1 on the patch rows; grid (nullable) host int [B][2] = (gh, gw), written before the call
+ *   returns.  fp16 / bf16 are the fp32 values rounded to nearest even.  Every refusal (JIMM_EINVAL) happens before anything is
+ *   enqueued; B = 0 is a no-op.  The call never waits for the stream: Pillow's tables are built on the device into scratch
+ *   allocated in stream order, plus an 8-bit intermediate of at most 64 MB per chunk for frames whose fused plan does not fit in
+ *   shared memory. */
+JIMM_API int jimm_preproc_naflex_grid(int patch, int max_num_patches, int H, int W, int* gh, int* gw);
+JIMM_API int jimm_preproc_create_naflex(const jimm_preproc_config_t* cfg, int patch, int device, jimm_preproc_t** out);
+JIMM_API int jimm_preproc_run_naflex(jimm_preproc_t* p, const uint8_t* const* imgs, int B, const int* H, const int* W, int max_num_patches,
+                                     void* pixel_values, int out_dtype, int32_t* mask, int* grid, void* stream);
 /* Host-only test entry: Pillow's resampling windows and 22-bit fixed-point weights for one axis. */
 JIMM_API int jimm_k_resample_coeffs(int in_size, int out_size, int resample, int* ksize, int* first, int* count, int* kk, int kk_capacity);
+/* Test entry: the same tables as built on the device by the NaFlex front-end (first, count [out_size], kk [out_size][ksize] on the host;
+ * synchronises). */
+JIMM_API int jimm_k_resample_coeffs_device(int in_size, int out_size, int resample, int* first, int* count, int* kk, int kk_capacity);
 /* Host-only test entry: the plan jimm_preproc_run uses for H x W frames.  path 0: one fused kernel with TY output rows per CTA, smem
  * bytes of shared memory, chosen under shared-memory budget tier 0 / 1 / 2 (72 / 110 / 200 KB); path 1: two passes (tier -1, smem 0). */
 JIMM_API int jimm_k_preproc_plan(const jimm_preproc_config_t* cfg, int H, int W, int* path, int* tier, int* TY, long long* smem);

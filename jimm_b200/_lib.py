@@ -155,7 +155,11 @@ SIGNATURES = {
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),
     "jimm_preproc_destroy": (_i, [_vp]),
+    "jimm_preproc_naflex_grid": (_i, [_i, _i, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
+    "jimm_preproc_create_naflex": (_i, [C.POINTER(PreprocConfig), _i, _i, C.POINTER(_vp)]),
+    "jimm_preproc_run_naflex": (_i, [_vp, C.POINTER(_vp), _i, C.POINTER(_i), C.POINTER(_i), _i, _vp, _i, _vp, C.POINTER(_i), _vp]),
     "jimm_k_resample_coeffs": (_i, [_i, _i, _i, C.POINTER(_i), _ip, _ip, _ip, _i]),
+    "jimm_k_resample_coeffs_device": (_i, [_i, _i, _i, _ip, _ip, _ip, _i]),
     "jimm_k_preproc_plan": (_i, [C.POINTER(PreprocConfig), _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_longlong)]),
 }
 

@@ -154,7 +154,16 @@ class _NativeOwner:
     def set_preprocessor(self, preprocessor):
         """Attach a `jimm_b200.preprocess.ImagePreprocessor`: the model then also accepts raw uint8 RGB frames [B,H,W,3] (host or
         CUDA) -- examples/vit_inference.py:27-37's `processor(images=...)` + transpose runs on the GPU, and host batches cross PCIe
-        as bytes instead of fp32 pixel values."""
+        as bytes instead of fp32 pixel values.  A `NaFlexPreprocessor` goes with SigLIP 2 NaFlex models only, at the model's patch
+        size (ValueError otherwise)."""
+        from ..preprocess import NaFlexPreprocessor
+
+        if isinstance(preprocessor, NaFlexPreprocessor):
+            if not getattr(self, "naflex", False):
+                raise ValueError("a NaFlexPreprocessor feeds SigLIP 2 NaFlex models (SigLIP(..., naflex=True)) only; use ImagePreprocessor")
+            patch = self._native_config().patch
+            if preprocessor.patch_size != patch:
+                raise ValueError(f"the NaFlex front-end cuts {preprocessor.patch_size}-pixel patches, the model takes {patch}-pixel patches")
         object.__setattr__(self, "_preproc", preprocessor)
         if self._native is not None:
             self._native.preproc = preprocessor

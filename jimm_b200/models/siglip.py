@@ -11,7 +11,7 @@ from .. import _lib, nn
 from ..common.transformer import g_wrap
 from ..common import hf_loader as L
 from ..common.utils import load_params_and_config
-from .._runtime import prep_patches
+from .._runtime import _as_tensor, prep_patches
 from ..common.vit import VisionTransformerBase, tower_config_fields
 from ._dual import DualTower, build_text_tower
 
@@ -77,30 +77,78 @@ class SigLIP(DualTower):
         n = self._native
         return prep_patches(images, spatial_shapes, pixel_attention_mask, n.cfg if n is not None else self._native_config())
 
+    def _frames(self, image, spatial_shapes, pixel_attention_mask) -> bool:
+        """Whether a call's image input is uint8 RGB frames for the attached NaFlex front-end: a [B, H, W, 3] batch or a list of
+        [H, W, 3] frames on a NaFlex model.  Such frames with a fixed-size ImagePreprocessor attached are a ValueError: it would not
+        give each image its own patch grid."""
+        if not self.naflex or spatial_shapes is not None or pixel_attention_mask is not None:
+            return False
+        first = image[0] if isinstance(image, (list, tuple)) and len(image) else image
+        if isinstance(first, (list, tuple)) or _as_tensor(first).dtype != torch.uint8:
+            return False
+        from ..preprocess import NaFlexPreprocessor
+
+        if not isinstance(self._preproc, NaFlexPreprocessor):
+            raise ValueError("uint8 frames into a SigLIP 2 NaFlex model need model.set_preprocessor(NaFlexPreprocessor(...)): a fixed-size "
+                             "ImagePreprocessor does not give each image its own patch grid")
+        return True
+
+    def _frames_call(self, frames, fn):
+        """fn(pixel_values, spatial_shapes) on uint8 frames in chunks of max_batch: one front-end call per chunk, in the model's operand
+        dtype, so the intermediate holds at most max_batch x max_num_patches patch rows.  The chunks' results are joined in order, and
+        come back to the host for host frames."""
+        xs = frames if isinstance(frames, (list, tuple)) else _as_tensor(frames)
+        if not isinstance(xs, (list, tuple)) and xs.ndim == 3:
+            xs = xs[None]
+        first = xs[0] if len(xs) else None
+        host = first is not None and not _as_tensor(first).is_cuda
+        dtype = {_lib.F32: torch.float32, _lib.BF16: torch.bfloat16}.get(self._compute_dtype, torch.float16)
+        parts = []
+        for b0 in range(0, max(len(xs), 1), self._max_batch):
+            r = self._preproc(xs[b0:b0 + self._max_batch], dtype=dtype)
+            parts.append(fn(r["pixel_values"], r["spatial_shapes"]))
+        return _host(_join(parts)) if host else _join(parts)
+
     def encode_image(self, image, interpolate_pos_encoding: bool = False, spatial_shapes=None, pixel_attention_mask=None) -> torch.Tensor:
         """As DualTower.encode_image.  On a NaFlex model: `image` is the HF processor's pixel_values [B, N, P*P*3] when spatial_shapes
         [B, 2] = (patch rows, patch columns) is given -- sample b's first rows_b * cols_b rows are its patches, the rest padding that is
-        never read; a pixel_attention_mask, if given, must be the prefix mask those shapes imply (ValueError otherwise) -- else NHWC images
-        of any size (interpolate_pos_encoding is implied)."""
+        never read; a pixel_attention_mask, if given, must be the prefix mask those shapes imply (ValueError otherwise) -- or, with a
+        NaFlexPreprocessor attached, uint8 RGB frames (a [B, H, W, 3] batch or a list of frames of any sizes), which the front-end turns
+        into exactly those inputs; else NHWC images of any size (interpolate_pos_encoding is implied)."""
+        if self._frames(image, spatial_shapes, pixel_attention_mask):
+            return self._frames_call(image, lambda pv, ss: self.encode_image(pv, spatial_shapes=ss))
         return self._vision(image, interpolate_pos_encoding or self.naflex, encode=True, spatial_shapes=spatial_shapes,
                             pixel_attention_mask=pixel_attention_mask)
 
     def encode_image_tokens(self, image, layers=None, *, dtype=torch.float32, return_pooled: bool = False, interpolate_pos_encoding: bool = False,
                             spatial_shapes=None, pixel_attention_mask=None):
         """As DualTower.encode_image_tokens, with the NaFlex image inputs of encode_image: on pixel_values with spatial_shapes each
-        sample's result is [rows_b * cols_b, D] (no CLS token), its patches row-major."""
+        sample's result is [rows_b * cols_b, D] (no CLS token), its patches row-major; uint8 frames as encode_image takes them."""
+        if self._frames(image, spatial_shapes, pixel_attention_mask):
+            return self._frames_call(image, lambda pv, ss: self.encode_image_tokens(pv, layers, dtype=dtype, return_pooled=return_pooled,
+                                                                                    spatial_shapes=ss))
         return self._vision_tokens(image, layers, dtype, return_pooled, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,
                                    pixel_attention_mask=pixel_attention_mask)
 
     def encode_image_attentions(self, image, blocks=None, *, dtype=torch.float32, return_pooled: bool = False,
                                 interpolate_pos_encoding: bool = False, spatial_shapes=None, pixel_attention_mask=None):
         """As DualTower.encode_image_attentions, with the NaFlex image inputs of encode_image: on pixel_values with spatial_shapes each
-        sample's result is [heads, n_b, n_b] ("map": [heads, 1, n_b]), n_b = rows_b * cols_b its patches, row-major."""
+        sample's result is [heads, n_b, n_b] ("map": [heads, 1, n_b]), n_b = rows_b * cols_b its patches, row-major; uint8 frames as
+        encode_image takes them."""
+        if self._frames(image, spatial_shapes, pixel_attention_mask):
+            return self._frames_call(image, lambda pv, ss: self.encode_image_attentions(pv, blocks, dtype=dtype, return_pooled=return_pooled,
+                                                                                        spatial_shapes=ss))
         return self._vision_tokens(image, blocks, dtype, return_pooled, interpolate_pos_encoding or self.naflex, attn=True,
                                    spatial_shapes=spatial_shapes, pixel_attention_mask=pixel_attention_mask)
 
     def __call__(self, image, text, spatial_shapes=None, pixel_attention_mask=None, interpolate_pos_encoding: bool = False) -> torch.Tensor:
-        """As DualTower.__call__, with the NaFlex image inputs of encode_image (single process only)."""
+        """As DualTower.__call__, with the NaFlex image inputs of encode_image (single process only).  uint8 frames: the logits of
+        encode_image(frames) against encode_text(text)."""
+        if self._frames(image, spatial_shapes, pixel_attention_mask):
+            ie, te = self.encode_image(image), self.encode_text(text)
+            n = self.native(max(len(ie), len(te)), require=True)
+            out = n.logits(ie, te)
+            return out.cpu() if not ie.is_cuda and not te.is_cuda else out
         return self._dual_call(image, text, interpolate_pos_encoding or self.naflex, spatial_shapes=spatial_shapes,
                                pixel_attention_mask=pixel_attention_mask)
 
@@ -173,3 +221,19 @@ class SigLIP(DualTower):
             rules += L.block_rules(f"{v}transformer.blocks.layers.{i}.", f"{v}encoder.layers.{i}.", L.CLIP_BLOCK)
         L.apply_mapping(model, hf, rules, missing="strict", shape_error=ValueError, what="SigLIP ")
         return model
+
+
+def _join(parts):
+    """The results of a call's chunks as one result: tensors concatenated, per-sample lists chained, tuples joined per position."""
+    a = parts[0]
+    if isinstance(a, torch.Tensor):
+        return torch.cat(parts) if len(parts) > 1 else a
+    if isinstance(a, list):
+        return [x for p in parts for x in p]
+    return tuple(_join([p[i] for p in parts]) for i in range(len(a)))
+
+
+def _host(r):
+    if isinstance(r, torch.Tensor):
+        return r.cpu()
+    return [_host(x) for x in r] if isinstance(r, list) else tuple(_host(x) for x in r)

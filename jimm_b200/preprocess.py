@@ -188,3 +188,128 @@ def plan(height: int, width: int, **config):
     path, tier, ty, smem = C.c_int(), C.c_int(), C.c_int(), C.c_longlong()
     _lib.check(lib.jimm_k_preproc_plan(C.byref(cfg), int(height), int(width), C.byref(path), C.byref(tier), C.byref(ty), C.byref(smem)))
     return path.value, tier.value, ty.value, smem.value
+
+
+def naflex_grid(height: int, width: int, patch_size: int = 16, max_num_patches: int = 256):
+    """Host-only: the patch grid (rows, columns) of transformers' Siglip2 size rule (get_image_size_for_max_num_patches) for a
+    height x width frame.  Raises ValueError for a frame the front-end refuses or a grid of more than max_num_patches patches."""
+    gh, gw = C.c_int(), C.c_int()
+    _lib.check(_lib.load().jimm_preproc_naflex_grid(int(patch_size), int(max_num_patches), int(height), int(width), C.byref(gh),
+                                                     C.byref(gw)))
+    return gh.value, gw.value
+
+
+class NaFlexPreprocessor:
+    """Mirror of transformers' `Siglip2ImageProcessor` (PIL backend) for uint8 RGB frames of any size on the GPU: each frame resized to
+    its own patch grid under the max_num_patches budget, rescaled, normalised and written as patch rows, every frame of a call in
+    one set of launches (csrc/preprocess.cu).  The result is the processor's three tensors, bit for bit, so it also feeds a
+    HuggingFace model."""
+
+    def __init__(self, patch_size: int = 16, max_num_patches: int = 256, resample: int = BILINEAR, rescale_factor: float = 1 / 255,
+                 image_mean: Sequence[float] = (0.5, 0.5, 0.5), image_std: Sequence[float] = (0.5, 0.5, 0.5), device: Optional[int] = None,
+                 do_resize: bool = True, do_rescale: bool = True, do_normalize: bool = True, **unused):
+        if not (do_resize and do_rescale and do_normalize):
+            raise ValueError("the GPU front-end implements the full resize -> rescale -> normalize pipeline of the Siglip2 processor")
+        if int(resample) not in (BILINEAR, BICUBIC):
+            raise ValueError(f"resample must be PIL BILINEAR (2) or BICUBIC (3), got {resample}")
+        if len(image_mean) != 3 or len(image_std) != 3:
+            raise ValueError("mean must have 3 elements if it is an iterable")
+        if not all(image_std):
+            raise ValueError("std evaluated to zero, leading to division by zero.")
+        if int(patch_size) < 1 or int(max_num_patches) < 1:
+            raise ValueError(f"patch_size and max_num_patches must be at least 1, got {patch_size} and {max_num_patches}")
+        cfg = _lib.PreprocConfig()
+        cfg.resample = int(resample)
+        cfg.rescale_factor = float(rescale_factor)
+        cfg.mean = (C.c_float * 3)(*[float(v) for v in image_mean])
+        cfg.std = (C.c_float * 3)(*[float(v) for v in image_std])
+        self.patch_size, self.max_num_patches = int(patch_size), int(max_num_patches)
+        if not torch.cuda.is_available():
+            raise _lib.JimmError("jimm_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
+        self.lib = _lib.load()
+        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else int(device))
+        self.cfg = cfg
+        self.handle = C.c_void_p()
+        _lib.check(self.lib.jimm_preproc_create_naflex(C.byref(cfg), self.patch_size, self.device.index, C.byref(self.handle)))
+
+    @classmethod
+    def from_pretrained(cls, path: str, **kw):
+        """Read a Siglip2 `preprocessor_config.json` from a checkpoint directory (or the file itself)."""
+        f = os.path.join(path, "preprocessor_config.json") if os.path.isdir(path) else path
+        if not os.path.exists(f):
+            raise ValueError(f"preprocessor_config.json not found at {path}")
+        with open(f) as fh:
+            c = json.load(fh)
+        keys = ("patch_size", "max_num_patches", "resample", "rescale_factor", "image_mean", "image_std", "do_resize", "do_rescale",
+                "do_normalize")
+        args = {k: c[k] for k in keys if k in c and c[k] is not None}
+        args.update(kw)
+        return cls(**args)
+
+    def grid(self, height: int, width: int, max_num_patches: Optional[int] = None):
+        """The (rows, columns) patch grid of a height x width frame (the size rule; host only)."""
+        return naflex_grid(height, width, self.patch_size, self.max_num_patches if max_num_patches is None else max_num_patches)
+
+    def __call__(self, frames: Union[torch.Tensor, np.ndarray, Sequence], dtype: torch.dtype = torch.float32,
+                 max_num_patches: Optional[int] = None) -> dict:
+        """uint8 RGB frames -- a [B, H, W, 3] batch, one [H, W, 3] frame, or a list of [H, W, 3] frames of different sizes, on the host or
+        CUDA -- -> {"pixel_values": CUDA [B, max_num_patches, P*P*3] of dtype, "pixel_attention_mask": CUDA int32 [B, max_num_patches],
+        "spatial_shapes": CPU int64 [B, 2]}.  max_num_patches: the processor's per-call keyword (default: the constructor's)."""
+        if dtype not in _OUT_CODE:
+            raise ValueError(f"unsupported output dtype {dtype}")
+        N = self.max_num_patches if max_num_patches is None else int(max_num_patches)
+        if isinstance(frames, (list, tuple)):
+            xs = [f if isinstance(f, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(f)) for f in frames]
+            xs = [x[0] if x.ndim == 4 and x.shape[0] == 1 else x for x in xs]
+        else:
+            x = frames if isinstance(frames, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(frames))
+            xs = [x] if x.ndim == 3 else list(x) if x.ndim == 4 else [x]
+        for i, x in enumerate(xs):
+            if x.dtype != torch.uint8:
+                raise ValueError(f"frame {i}: expected uint8 RGB, got {x.dtype}")
+            if x.ndim != 3 or x.shape[2] != 3:
+                raise ValueError(f"frame {i}: expected shape [height, width, 3], got {tuple(x.shape)}")
+        B, P = len(xs), self.patch_size
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            if isinstance(frames, torch.Tensor) and frames.ndim == 4:
+                xd = frames.to(self.device, non_blocking=True).contiguous()
+                ds = list(xd) if B else []
+            else:
+                ds = [x.to(self.device, non_blocking=True).contiguous() for x in xs]
+            pv = torch.empty((B, N, P * P * 3), dtype=dtype, device=self.device)
+            mask = torch.empty((B, N), dtype=torch.int32, device=self.device)
+            grid = (C.c_int * max(2 * B, 1))()
+            if B:
+                _lib.check(self.lib.jimm_preproc_run_naflex(
+                    self.handle, (C.c_void_p * B)(*[d.data_ptr() for d in ds]), B, (C.c_int * B)(*[d.shape[0] for d in ds]),
+                    (C.c_int * B)(*[d.shape[1] for d in ds]), N, C.c_void_p(pv.data_ptr()), _OUT_CODE[dtype], C.c_void_p(mask.data_ptr()),
+                    grid, C.c_void_p(st.cuda_stream)))
+                for d in ds:
+                    d.record_stream(st)
+        shapes = torch.tensor(list(grid)[:2 * B], dtype=torch.int64).reshape(B, 2)
+        return {"pixel_values": pv, "pixel_attention_mask": mask, "spatial_shapes": shapes}
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.jimm_preproc_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def resample_coeffs_device(in_size: int, out_size: int, resample: int):
+    """Pillow's tables as the NaFlex front-end builds them on the GPU (test hook): (first, count, kk) as resample_coeffs returns."""
+    lib = _lib.load()
+    ks = C.c_int()
+    _lib.check(lib.jimm_k_resample_coeffs(in_size, out_size, resample, C.byref(ks), None, None, None, 0))
+    first = np.zeros(out_size, np.int32)
+    count = np.zeros(out_size, np.int32)
+    kk = np.zeros((out_size, ks.value), np.int32)
+    _lib.check(lib.jimm_k_resample_coeffs_device(in_size, out_size, resample, first.ctypes.data_as(C.c_void_p),
+                                                 count.ctypes.data_as(C.c_void_p), kk.ctypes.data_as(C.c_void_p), kk.size))
+    return first, count, kk
