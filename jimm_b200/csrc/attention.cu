@@ -83,7 +83,7 @@ __device__ __forceinline__ void load_tile(uint32_t smem_base, const T* __restric
   }
 }
 
-// Shared memory of a CTA: static up to 48 KB, else dynamic (opted in by attn_launch, 1 KB of slack for the 1024-byte alignment).
+// Shared memory of a CTA: static up to 48 KB, else dynamic (opted in by attn_launch_k, 1 KB of slack for the 1024-byte alignment).
 template <int BYTES, bool STATIC = (BYTES <= 48 * 1024)>
 struct AttnSmem {
   static __device__ __forceinline__ uint8_t* get() {
@@ -99,6 +99,99 @@ struct AttnSmem<BYTES, false> {
   }
 };
 
+// The rows of sample b: rows row0 .. row0 + S - 1 of qkv / out.  Dense: B samples of S_arg rows each.  PACKED: sample b is rows
+// seq_off[b] .. seq_off[b + 1] - 1 (read after pdl_wait: the offsets may come from the previous kernel).
+template <bool PACKED>
+__device__ __forceinline__ void sample_rows(int b, int S_arg, const int* __restrict__ seq_off, size_t& row0, int& S) {
+  if constexpr (PACKED) {
+    row0 = static_cast<size_t>(seq_off[b]);
+    S = seq_off[b + 1] - seq_off[b];
+  } else {
+    row0 = static_cast<size_t>(b) * S_arg;
+    S = S_arg;
+  }
+}
+
+// S = Q K^T of one 64-key tile (64 x 64 per warpgroup, both operands K-major in shared memory): this warp's 16 query rows in the
+// m16n8 accumulator layout, s[n-block][e] = the score of row g + 8 (e >> 1) and key 8 n-block + 2 t4 + (e & 1) (g = lane / 4, t4 = lane % 4).
+template <typename T, int DP>
+__device__ __forceinline__ void score_tile(float (&s)[8][4], uint64_t qdesc, uint32_t sK) {
+  using L = HeadTile<DP>;
+  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  float (&s_acc)[32] = reinterpret_cast<float (&)[32]>(s);
+  const uint64_t kdesc = make_wgmma_desc<L::SW>(sK, 16);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) s_acc[i] = 0.f;
+  wgmma_fence_operands(s_acc);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < DP / 16; ++ks)  // 16 head dims (32 B) per step
+    wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + L::kstep(ks), kdesc + L::kstep(ks), ks != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_operands(s_acc);
+}
+
+// Scores of keys at or past S, and (CAUSAL) of keys above the diagonal, to -inf.  k0: the tile's first key, q0: the CTA's first query
+// row, row_lo: this thread's first row (the other is row_lo + 8).  Tiles with no such key are left alone.
+template <bool CAUSAL>
+__device__ __forceinline__ void mask_tile(float (&s)[8][4], int k0, int q0, int row_lo, int t4, int S) {
+  if ((k0 + KT > S) || (CAUSAL && (k0 + KT - 1 > q0))) {
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = k0 + nt * 8 + t4 * 2 + (e & 1);
+        const int qrow = row_lo + (e >> 1) * 8;
+        const bool ok = key < S && (!CAUSAL || key <= qrow);
+        if (!ok) s[nt][e] = -INFINITY;
+      }
+    }
+  }
+}
+
+// One online-softmax step over a masked score tile, for this thread's two rows: the row max (over the quad that shares the rows)
+// updates m_run, s becomes p = exp2(s scale_log2 - m_run scale_log2) in place, and l_run, this thread's share of the row sums, is
+// rescaled to the new max and adds the tile's p.  Returns alpha, the factor that rescaled l_run (and must rescale what else the earlier
+// tiles summed).  A row with every key masked so far keeps m_run = -inf and gets p = 0.
+__device__ __forceinline__ float2 softmax_step(float (&s)[8][4], float (&m_run)[2], float (&l_run)[2], float scale_log2) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    mx[0] = fmaxf(mx[0], fmaxf(s[nt][0], s[nt][1]));
+    mx[1] = fmaxf(mx[1], fmaxf(s[nt][2], s[nt][3]));
+  }
+  float alpha[2], moff[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    const float mnew = fmaxf(m_run[r], mx[r]);
+    const float muse = (mnew == -INFINITY) ? 0.f : mnew;
+    alpha[r] = exp2f((m_run[r] - muse) * scale_log2);  // m_run = -inf -> 0
+    m_run[r] = mnew;
+    moff[r] = muse * scale_log2;
+    l_run[r] *= alpha[r];
+  }
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    s[nt][0] = exp2f(s[nt][0] * scale_log2 - moff[0]);
+    s[nt][1] = exp2f(s[nt][1] * scale_log2 - moff[0]);
+    s[nt][2] = exp2f(s[nt][2] * scale_log2 - moff[1]);
+    s[nt][3] = exp2f(s[nt][3] * scale_log2 - moff[1]);
+    l_run[0] += s[nt][0] + s[nt][1];
+    l_run[1] += s[nt][2] + s[nt][3];
+  }
+  return make_float2(alpha[0], alpha[1]);
+}
+
+// 1 / l of one of this thread's rows: l, this thread's share of the row sum, added over the quad that shares the row
+__device__ __forceinline__ float row_inv_sum(float l) {
+  l += __shfl_xor_sync(0xffffffffu, l, 1);
+  l += __shfl_xor_sync(0xffffffffu, l, 2);
+  return 1.0f / l;
+}
+
 // Head width d (a multiple of 8, d <= DP); the tiles are padded to DP columns with zeros.  scale_log2 = log2(e) / sqrt(d).
 // PACKED: sample b is rows seq_off[b] .. seq_off[b + 1] - 1 of qkv / out (S_arg unused); query tiles past a sample's end exit at once.
 template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED = false>
@@ -111,15 +204,14 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, i
   const int qt = blockIdx.x, h = blockIdx.y, b = reverse ? static_cast<int>(gridDim.z) - 1 - static_cast<int>(blockIdx.z) : static_cast<int>(blockIdx.z);
   const int D = H * d;
   const size_t ld = static_cast<size_t>(3) * D;
-  int S = S_arg;
-  size_t row0 = static_cast<size_t>(b) * S_arg;
   if constexpr (PACKED) {
     pdl_launch_dependents();
     pdl_wait();  // the offsets may come from the previous kernel
-    row0 = static_cast<size_t>(seq_off[b]);
-    S = seq_off[b + 1] - seq_off[b];
-    if (qt * QT >= S) return;
   }
+  size_t row0;
+  int S;
+  sample_rows<PACKED>(b, S_arg, seq_off, row0, S);
+  if (PACKED && qt * QT >= S) return;
   const T* base = qkv + row0 * ld + h * d;
   const T* gq = base;
   const T* gk = base + D;
@@ -165,66 +257,14 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, i
     __syncthreads();
     const uint32_t sK = sK0 + buf * L::BYTES, sV = sV0 + buf * L::BYTES;
 
-    // ---- S = Q K^T (64 x 64 per warpgroup; this warp's 16 rows in the m16n8 accumulator layout, s[n-block][e]) ----
     float s[8][4];
-    float (&s_acc)[32] = reinterpret_cast<float (&)[32]>(s);
-    const uint64_t kdesc = make_wgmma_desc<L::SW>(sK, 16);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s_acc[i] = 0.f;
-    wgmma_fence_operands(s_acc);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < DP / 16; ++ks)  // 16 head dims (32 B) per step
-      wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + L::kstep(ks), kdesc + L::kstep(ks), ks != 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_operands(s_acc);
-    // ---- mask + online softmax ----
-    const int k0 = j * KT;
-    const bool need_mask = (k0 + KT > S) || (CAUSAL && (k0 + KT - 1 > q0));
-    if (need_mask) {
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = k0 + nt * 8 + t4 * 2 + (e & 1);
-          const int qrow = row_lo + (e >> 1) * 8;
-          const bool ok = key < S && (!CAUSAL || key <= qrow);
-          if (!ok) s[nt][e] = -INFINITY;
-        }
-      }
-    }
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      mx[0] = fmaxf(mx[0], fmaxf(s[nt][0], s[nt][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[nt][2], s[nt][3]));
-    }
-    float alpha[2], moff[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float mnew = fmaxf(m_run[r], mx[r]);
-      const float muse = (mnew == -INFINITY) ? 0.f : mnew;
-      alpha[r] = exp2f((m_run[r] - muse) * scale_log2);  // m_run = -inf -> 0
-      m_run[r] = mnew;
-      moff[r] = muse * scale_log2;
-      l_run[r] *= alpha[r];
-    }
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      s[nt][0] = exp2f(s[nt][0] * scale_log2 - moff[0]);
-      s[nt][1] = exp2f(s[nt][1] * scale_log2 - moff[0]);
-      s[nt][2] = exp2f(s[nt][2] * scale_log2 - moff[1]);
-      s[nt][3] = exp2f(s[nt][3] * scale_log2 - moff[1]);
-      l_run[0] += s[nt][0] + s[nt][1];
-      l_run[1] += s[nt][2] + s[nt][3];
-    }
+    score_tile<T, DP>(s, qdesc, sK);
+    mask_tile<CAUSAL>(s, j * KT, q0, row_lo, t4, S);
+    const float2 alpha = softmax_step(s, m_run, l_run, scale_log2);
 #pragma unroll
     for (int nt = 0; nt < DP / 8; ++nt) {
-      o[nt][0] *= alpha[0]; o[nt][1] *= alpha[0];
-      o[nt][2] *= alpha[1]; o[nt][3] *= alpha[1];
+      o[nt][0] *= alpha.x; o[nt][1] *= alpha.x;
+      o[nt][2] *= alpha.y; o[nt][3] *= alpha.y;
     }
     // ---- O += P V: A = P (keys 16 kk .. 16 kk + 15 of this warp's rows), B = V rows of those keys (MN-major, 16 rows per step) ----
     uint32_t pf[4][4];
@@ -248,14 +288,7 @@ attention_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, i
   }
 
   // ---- finalise: O /= l, store columns < d ----
-  float inv[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    float l = l_run[r];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    inv[r] = 1.0f / l;
-  }
+  const float inv[2] = {row_inv_sum(l_run[0]), row_inv_sum(l_run[1])};
   OutT* obase = out + row0 * D + h * d;
   if constexpr (sizeof(OutT) == 2) {
     // stage this warp's 16 x DP tile through its (now free) Q rows so the global stores are whole 16-byte chunks of a row
@@ -305,47 +338,55 @@ static int padded_head_dim(int d) { return d <= 16 ? 16 : d <= 32 ? 32 : d <= 64
 // The softmax scale 1 / sqrt(d) (flax: query / sqrt(depth)) times log2(e), in fp32: 0.125f * log2(e) for d = 64.
 static float attn_scale_log2(int d) { return static_cast<float>(1.0 / std::sqrt(static_cast<double>(d))) * 1.4426950408889634f; }
 
-// seq_off null: B samples of S rows each; else the packed form (S = the longest sample, sample b = rows seq_off[b] .. seq_off[b + 1] - 1)
-template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED>
-static int attn_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse, const int* seq_off) {
-  constexpr int SMEM = HeadTile<DP>::SMEM;
-  constexpr size_t dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
-  auto* kernel = attention_kernel<T, OutT, CAUSAL, DP, PACKED>;
+// Calls f(CAUSAL, DP, PACKED), each a std::integral_constant: the compiled variant of a wgmma attention kernel that runs head width d,
+// causal or not, on B samples of S rows each (seq_off null) or in the packed form (S = the longest sample, sample b = rows seq_off[b]
+// .. seq_off[b + 1] - 1).  Packed and causal: the query tile, the key count n_kv and the mask are all relative to the sample's first
+// row (row0), so each sample is masked as it is alone.
+template <typename F>
+static int attn_variant(int d, int causal, const int* seq_off, F&& f) {
+  auto at_width = [&](auto c, auto p) -> int {
+    switch (padded_head_dim(d)) {
+      case 16: return f(c, std::integral_constant<int, 16>{}, p);
+      case 32: return f(c, std::integral_constant<int, 32>{}, p);
+      case 64: return f(c, std::integral_constant<int, 64>{}, p);
+      case 80: return f(c, std::integral_constant<int, 80>{}, p);
+      case 96: return f(c, std::integral_constant<int, 96>{}, p);
+      default: return f(c, std::integral_constant<int, 128>{}, p);
+    }
+  };
+  if (seq_off && causal) return at_width(std::true_type{}, std::true_type{});
+  if (seq_off) return at_width(std::false_type{}, std::true_type{});
+  if (causal) return at_width(std::true_type{}, std::false_type{});
+  return at_width(std::false_type{}, std::false_type{});
+}
+
+// Launches Kernel, one warpgroup CTA per 64 query rows of each (sample, head), with SMEM bytes of shared memory: static up to 48 KB,
+// else dynamic (opted in, with 1 KB of slack for AttnSmem's 1024-byte alignment).
+template <auto Kernel, int SMEM, typename... Args>
+static int attn_launch_k(int B, int S, int H, cudaStream_t stream, Args... args) {
+  constexpr int dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
   if constexpr (dyn > 0) {
-    static DeviceOnce attr_set;
-    if (int rc = attr_set.run([&]() -> int {
-          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
-          return 0;
-        }))
-      return rc;
+    if (int rc = smem_opt_in<Kernel>(dyn)) return rc;
   }
-  dim3 grid((S + QT - 1) / QT, H, B);
-  JIMM_CUDA_CHECK(launch_k(kernel, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d,
-                           attn_scale_log2(d), reverse, seq_off));
+  JIMM_CUDA_CHECK(launch_k(Kernel, dim3((S + QT - 1) / QT, H, B), dim3(128), dyn, stream, 1, true, args...));
   note_launch();
   return 0;
 }
 
-template <typename T, typename OutT, bool CAUSAL, bool PACKED>
-static int attn_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, int reverse, const int* seq_off) {
-  switch (padded_head_dim(d)) {
-    case 16: return attn_launch_dp<T, OutT, CAUSAL, 16, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-    case 32: return attn_launch_dp<T, OutT, CAUSAL, 32, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-    case 64: return attn_launch_dp<T, OutT, CAUSAL, 64, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-    case 80: return attn_launch_dp<T, OutT, CAUSAL, 80, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-    case 96: return attn_launch_dp<T, OutT, CAUSAL, 96, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-    default: return attn_launch_dp<T, OutT, CAUSAL, 128, PACKED>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-  }
-}
-
-// Packed and causal: the query tile, the key count n_kv and the mask are all relative to the sample's first row (row0), so each sample is
-// masked as it is alone.
-template <typename T, typename OutT>
-static int attn_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, int reverse, const int* seq_off) {
-  if (seq_off && causal) return attn_launch_causal<T, OutT, true, true>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-  if (seq_off) return attn_launch_causal<T, OutT, false, true>(qkv, out, B, S, H, d, stream, reverse, seq_off);
-  if (causal) return attn_launch_causal<T, OutT, true, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
-  return attn_launch_causal<T, OutT, false, false>(qkv, out, B, S, H, d, stream, reverse, nullptr);
+template <typename T>
+struct Type {
+  using type = T;
+};
+// Calls f(Type<T>{}, Type<OutT>{}) for the (io, out) dtype pairs of the flash and MAP kernels.
+template <typename F>
+static int io_out_dispatch(const char* name, int io_type, int out_type, F&& f) {
+  if (io_type == DT_F16 && out_type == DT_F16) return f(Type<__half>{}, Type<__half>{});
+  if (io_type == DT_F16 && out_type == DT_F32) return f(Type<__half>{}, Type<float>{});
+  if (io_type == DT_F16 && out_type == DT_TF32) return f(Type<__half>{}, Type<tf32_t>{});
+  if (io_type == DT_BF16 && out_type == DT_BF16) return f(Type<__nv_bfloat16>{}, Type<__nv_bfloat16>{});
+  if (io_type == DT_BF16 && out_type == DT_F32) return f(Type<__nv_bfloat16>{}, Type<float>{});
+  set_last_error("%s: unsupported dtype combination io=%d out=%d", name, io_type, out_type);
+  return -1;
 }
 
 static bool head_dim_ok(int d) { return d >= 8 && d <= 128 && d % 8 == 0; }
@@ -355,13 +396,15 @@ static int attn_dispatch(const void* qkv, int io_type, void* out, int out_type, 
   if (!head_dim_ok(head_dim)) { set_last_error("attention: head_dim %d is not a multiple of 8 in [8, 128]", head_dim); return -1; }
   if (B <= 0 || S <= 0) return 0;
   if (B > 65535 || H > 65535) { set_last_error("attention: grid too large (B=%d H=%d)", B, H); return -1; }
-  if (io_type == DT_F16 && out_type == DT_F16) return attn_launch<__half, __half>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
-  if (io_type == DT_F16 && out_type == DT_F32) return attn_launch<__half, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
-  if (io_type == DT_F16 && out_type == DT_TF32) return attn_launch<__half, tf32_t>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return attn_launch<__nv_bfloat16, __nv_bfloat16>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
-  if (io_type == DT_BF16 && out_type == DT_F32) return attn_launch<__nv_bfloat16, float>(qkv, out, B, S, H, head_dim, causal, stream, reverse, seq_off);
-  set_last_error("attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
-  return -1;
+  return io_out_dispatch("attention", io_type, out_type, [&](auto io, auto o) {
+    using T = typename decltype(io)::type;
+    using OutT = typename decltype(o)::type;
+    return attn_variant(head_dim, causal, seq_off, [&](auto c, auto dp, auto p) {
+      constexpr int DP = decltype(dp)::value;
+      return attn_launch_k<attention_kernel<T, OutT, decltype(c)::value, DP, decltype(p)::value>, HeadTile<DP>::SMEM>(
+          B, S, H, stream, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, head_dim, attn_scale_log2(head_dim), reverse, seq_off);
+    });
+  });
 }
 
 int attention_run(const void* qkv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, int causal, cudaStream_t stream, int reverse) {
@@ -403,12 +446,11 @@ attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, 
   uint32_t* stage = reinterpret_cast<uint32_t*>(smem + 3 * L::BYTES);
   pdl_launch_dependents();
   pdl_wait();  // qkv is the QKV GEMM's output (and the offsets may come from the previous kernel)
-  int S = S_arg;
-  size_t row0 = static_cast<size_t>(b) * S_arg;
+  size_t row0;
+  int S;
+  sample_rows<PACKED>(b, S_arg, seq_off, row0, S);
   size_t obase = static_cast<size_t>(b) * H * S_arg * S_arg;
   if constexpr (PACKED) {
-    row0 = static_cast<size_t>(seq_off[b]);
-    S = seq_off[b + 1] - seq_off[b];
     if (qt * QT >= S) return;
     // H * sum_{j<b} S_j^2, reduced over the CTA
     unsigned long long acc = 0;
@@ -432,16 +474,14 @@ attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, 
   const int n_all = (S + KT - 1) / KT;
   const int n_kv = CAUSAL ? min(n_all, qt + 1) : n_all;  // the tiles with a key at or below the diagonal
 
-  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   const uint64_t qdesc = make_wgmma_desc<L::SW>(sQ, 16);
   const int g = lane >> 2, t4 = lane & 3;
   const int row_lo = q0 + warp * 16 + g;  // this thread's two query rows: row_lo, row_lo + 8
 
-  // S = Q K^T of key tile j (this warp's 16 rows, m16n8 accumulator layout), masked to -inf past S and above the diagonal.  The K tile
-  // of step `it` of a pass is in buffer it & 1; the next one is prefetched while this one is used.
-  auto scores = [&](int j, int it, int n_it, float (&s)[8][4]) {
-    const int buf = it & 1;
-    if (it + 1 < n_it) {
+  // S = Q K^T of key tile j, masked.  The K tile of step j of a pass is in buffer j & 1; the next one is prefetched while this one is used.
+  auto scores = [&](int j, float (&s)[8][4]) {
+    const int buf = j & 1;
+    if (j + 1 < n_kv) {
       load_tile<T, DP>(sK0 + (buf ^ 1) * L::BYTES, gk, ld, (j + 1) * KT, S, d, tid);
       cp_async_commit();
       cp_async_wait<1>();
@@ -450,68 +490,25 @@ attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, 
     }
     fence_proxy_async_smem();
     __syncthreads();
-    float (&s_acc)[32] = reinterpret_cast<float (&)[32]>(s);
-    const uint64_t kdesc = make_wgmma_desc<L::SW>(sK0 + buf * L::BYTES, 16);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s_acc[i] = 0.f;
-    wgmma_fence_operands(s_acc);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < DP / 16; ++ks) wgmma_m64n64k16_ss<BF16>(s_acc, qdesc + L::kstep(ks), kdesc + L::kstep(ks), ks != 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_operands(s_acc);
+    score_tile<T, DP>(s, qdesc, sK0 + buf * L::BYTES);
     __syncthreads();  // every warp is done reading buf before it is refilled by the next step's prefetch
-    const int k0 = j * KT;
-    if ((k0 + KT > S) || (CAUSAL && (k0 + KT - 1 > q0))) {
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = k0 + nt * 8 + t4 * 2 + (e & 1);
-          if (!(key < S && (!CAUSAL || key <= row_lo + (e >> 1) * 8))) s[nt][e] = -INFINITY;
-        }
-    }
+    mask_tile<CAUSAL>(s, j * KT, q0, row_lo, t4, S);
   };
 
-  // ---- pass 1: row max and sum ----
+  // ---- pass 1: row max and sum (the flash kernel's softmax steps; p and alpha are not needed) ----
   load_tile<T, DP>(sQ, gq, ld, q0, S, d, tid);
   load_tile<T, DP>(sK0, gk, ld, 0, S, d, tid);
   cp_async_commit();
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   for (int j = 0; j < n_kv; ++j) {
     float s[8][4];
-    scores(j, j, n_kv, s);
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      mx[0] = fmaxf(mx[0], fmaxf(s[nt][0], s[nt][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[nt][2], s[nt][3]));
-    }
-    float moff[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float mnew = fmaxf(m_run[r], mx[r]);
-      const float muse = (mnew == -INFINITY) ? 0.f : mnew;
-      l_run[r] *= exp2f((m_run[r] - muse) * scale_log2);
-      m_run[r] = mnew;
-      moff[r] = muse * scale_log2;
-    }
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      l_run[0] += exp2f(s[nt][0] * scale_log2 - moff[0]) + exp2f(s[nt][1] * scale_log2 - moff[0]);
-      l_run[1] += exp2f(s[nt][2] * scale_log2 - moff[1]) + exp2f(s[nt][3] * scale_log2 - moff[1]);
-    }
+    scores(j, s);
+    softmax_step(s, m_run, l_run, scale_log2);
   }
   float inv[2], moff[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    float l = l_run[r];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    inv[r] = 1.0f / l;
+    inv[r] = row_inv_sum(l_run[r]);
     moff[r] = (m_run[r] == -INFINITY ? 0.f : m_run[r]) * scale_log2;
   }
 
@@ -525,7 +522,7 @@ attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, 
     const int k0 = j * KT, cols = min(KT, S - k0);
     if (j < n_kv) {
       float s[8][4];
-      scores(j, j, n_kv, s);
+      scores(j, s);
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
@@ -556,44 +553,13 @@ attn_probs_kernel(const T* __restrict__ qkv, OutT* __restrict__ out, int S_arg, 
   }
 }
 
-template <typename T, typename OutT, bool CAUSAL, int DP, bool PACKED>
-static int probs_launch_dp(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
-  constexpr int SMEM = ProbsSmem<DP, static_cast<int>(sizeof(OutT))>::BYTES;
-  constexpr size_t dyn = SMEM <= 48 * 1024 ? 0 : SMEM + 1024;
-  auto* kernel = attn_probs_kernel<T, OutT, CAUSAL, DP, PACKED>;
-  if constexpr (dyn > 0) {
-    static DeviceOnce attr_set;
-    if (int rc = attr_set.run([&]() -> int {
-          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
-          return 0;
-        }))
-      return rc;
-  }
-  dim3 grid((S + QT - 1) / QT, H, B);
-  JIMM_CUDA_CHECK(launch_k(kernel, grid, dim3(128), dyn, stream, 1, true, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d,
-                           attn_scale_log2(d), seq_off));
-  note_launch();
-  return 0;
-}
-
-template <typename T, typename OutT, bool CAUSAL, bool PACKED>
-static int probs_launch_causal(const void* qkv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off) {
-  switch (padded_head_dim(d)) {
-    case 16: return probs_launch_dp<T, OutT, CAUSAL, 16, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-    case 32: return probs_launch_dp<T, OutT, CAUSAL, 32, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-    case 64: return probs_launch_dp<T, OutT, CAUSAL, 64, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-    case 80: return probs_launch_dp<T, OutT, CAUSAL, 80, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-    case 96: return probs_launch_dp<T, OutT, CAUSAL, 96, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-    default: return probs_launch_dp<T, OutT, CAUSAL, 128, PACKED>(qkv, out, B, S, H, d, stream, seq_off);
-  }
-}
-
 template <typename T, typename OutT>
 static int probs_launch(const void* qkv, void* out, int B, int S, int H, int d, int causal, cudaStream_t stream, const int* seq_off) {
-  if (seq_off && causal) return probs_launch_causal<T, OutT, true, true>(qkv, out, B, S, H, d, stream, seq_off);
-  if (seq_off) return probs_launch_causal<T, OutT, false, true>(qkv, out, B, S, H, d, stream, seq_off);
-  if (causal) return probs_launch_causal<T, OutT, true, false>(qkv, out, B, S, H, d, stream, nullptr);
-  return probs_launch_causal<T, OutT, false, false>(qkv, out, B, S, H, d, stream, nullptr);
+  return attn_variant(d, causal, seq_off, [&](auto c, auto dp, auto p) {
+    constexpr int DP = decltype(dp)::value;
+    return attn_launch_k<attn_probs_kernel<T, OutT, decltype(c)::value, DP, decltype(p)::value>, ProbsSmem<DP, static_cast<int>(sizeof(OutT))>::BYTES>(
+        B, S, H, stream, static_cast<const T*>(qkv), static_cast<OutT*>(out), S, H, d, attn_scale_log2(d), seq_off);
+  });
 }
 
 template <typename T>
@@ -726,33 +692,19 @@ int map_attention_max_seq(int device, int* max_S) {
   return 0;
 }
 
+// smem_max: the bytes of the longest sequence map_attention_max_seq allows on this device, which the kernel is opted in to once
 template <typename T, typename OutT, bool PACKED>
 static int map_launch_k(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off, void* probs,
-                        int probs_type) {
-  auto* kernel = map_attention_kernel<T, OutT, PACKED>;
+                        int probs_type, int smem_max) {
+  constexpr auto kernel = map_attention_kernel<T, OutT, PACKED>;
   const size_t smem = (kMapSmemFloats + S) * sizeof(float);
-  if (smem > 48 * 1024) {  // opt in once per device to all the shared memory map_attention_max_seq counts on
-    static DeviceOnce attr_set;
-    if (int rc = attr_set.run([&]() -> int {
-          int dev = 0, max_S = 0;
-          JIMM_CUDA_CHECK(cudaGetDevice(&dev));
-          if (int rc = map_attention_max_seq(dev, &max_S)) return rc;
-          JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>((kMapSmemFloats + max_S) * sizeof(float))));
-          return 0;
-        }))
-      return rc;
+  if (smem > 48 * 1024) {
+    if (int rc = smem_opt_in<kernel>(smem_max)) return rc;
   }
   const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(d)));  // 0.125f for d = 64
   kernel<<<dim3(H, B), 256, smem, stream>>>(q, static_cast<const T*>(kv), static_cast<OutT*>(out), S, H, d, qscale, seq_off, probs, probs_type);
   JIMM_LAUNCH_CHECK();
   return 0;
-}
-
-template <typename T, typename OutT>
-static int map_launch(const float* q, const void* kv, void* out, int B, int S, int H, int d, cudaStream_t stream, const int* seq_off, void* probs,
-                      int probs_type) {
-  if (seq_off) return map_launch_k<T, OutT, true>(q, kv, out, B, S, H, d, stream, seq_off, probs, probs_type);
-  return map_launch_k<T, OutT, false>(q, kv, out, B, S, H, d, stream, nullptr, probs, probs_type);
 }
 
 static int map_dispatch(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,
@@ -767,13 +719,13 @@ static int map_dispatch(const float* q, const void* kv, int io_type, void* out, 
     set_last_error("map_attention: probs dtype %d", probs_type);
     return -1;
   }
-  if (io_type == DT_F16 && out_type == DT_F16) return map_launch<__half, __half>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
-  if (io_type == DT_F16 && out_type == DT_F32) return map_launch<__half, float>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
-  if (io_type == DT_F16 && out_type == DT_TF32) return map_launch<__half, tf32_t>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
-  if (io_type == DT_BF16 && out_type == DT_BF16) return map_launch<__nv_bfloat16, __nv_bfloat16>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
-  if (io_type == DT_BF16 && out_type == DT_F32) return map_launch<__nv_bfloat16, float>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type);
-  set_last_error("map_attention: unsupported dtype combination io=%d out=%d", io_type, out_type);
-  return -1;
+  const int smem_max = (kMapSmemFloats + max_S) * static_cast<int>(sizeof(float));
+  return io_out_dispatch("map_attention", io_type, out_type, [&](auto io, auto o) {
+    using T = typename decltype(io)::type;
+    using OutT = typename decltype(o)::type;
+    if (seq_off) return map_launch_k<T, OutT, true>(q, kv, out, B, S, H, head_dim, stream, seq_off, probs, probs_type, smem_max);
+    return map_launch_k<T, OutT, false>(q, kv, out, B, S, H, head_dim, stream, nullptr, probs, probs_type, smem_max);
+  });
 }
 
 int map_attention_run(const float* q, const void* kv, int io_type, void* out, int out_type, int B, int S, int H, int head_dim, cudaStream_t stream,

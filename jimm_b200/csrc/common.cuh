@@ -97,6 +97,17 @@ struct DeviceOnce {
   }
 };
 
+// Opts Kernel in to `bytes` of dynamic shared memory per block, which a launch needs above 48 KB: once per device, through its own
+// DeviceOnce (Kernel is a template argument so that every kernel has one).
+template <auto Kernel>
+int smem_opt_in(int bytes) {
+  static DeviceOnce once;
+  return once.run([&]() -> int {
+    JIMM_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    return 0;
+  });
+}
+
 // ----------------------------------------------------------------------------
 // device helpers
 // ----------------------------------------------------------------------------

@@ -765,11 +765,11 @@ static EpiDev to_dev(const GemmEpilogue& e, int M, int N) {
 
 template <typename T, int OUT, int ACT>
 static int launch_one(const GemmPlan* p, int M, cudaStream_t stream) {
-  auto* kernel = gemm_wgmma_kernel<T, OUT, ACT>;
+  constexpr auto kernel = gemm_wgmma_kernel<T, OUT, ACT>;
   constexpr int TM = tile_rows(Traits<T>::DTYPE);
-  static DeviceOnce attr_set;
-  if (int rc = attr_set.run([&]() -> int {
-        JIMM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  if (int rc = smem_opt_in<kernel>(SMEM_BYTES)) return rc;
+  static DeviceOnce regs_checked;
+  if (int rc = regs_checked.run([&]() -> int {
         // setmaxnreg moves registers within the launch allocation: with fewer than KERNEL_REGS per thread, an increase would wait forever
         cudaFuncAttributes fa;
         JIMM_CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));

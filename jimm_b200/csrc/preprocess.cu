@@ -527,12 +527,7 @@ int get_plan(jimm_preproc* p, int H, int W, SizePlan** out) {
 
 template <typename OUT>
 int launch(const KernelArgs& a, const SizePlan& s, int B, cudaStream_t stream) {
-  static DeviceOnce attr_set;
-  if (int rc = attr_set.run([]() -> int {
-        JIMM_CUDA_CHECK(cudaFuncSetAttribute(preprocess_kernel<OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        return 0;
-      }))
-    return rc;
+  if (int rc = smem_opt_in<preprocess_kernel<OUT>>(200 * 1024)) return rc;
   const dim3 grid((s.oh + s.TY - 1) / s.TY, B);
   JIMM_CUDA_CHECK(launch_k(preprocess_kernel<OUT>, grid, dim3(kThreads), s.smem, stream, 1, false, a));
   note_launch();
@@ -858,11 +853,7 @@ int nf_launch(K kernel, NfLaunch& L, const std::vector<const NfWork*>& ws, const
 template <typename OUT>
 int nf_enqueue(const jimm_preproc* p, std::vector<NfWork>& work, const std::vector<NfImage>& all, int B, int maxp, void* pixel_values,
                int32_t* mask, cudaStream_t st) {
-  static DeviceOnce attr_set;
-  JIMM_TRY(attr_set.run([]() -> int {
-    JIMM_CUDA_CHECK(cudaFuncSetAttribute(nf_fused_kernel<OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    return 0;
-  }));
+  JIMM_TRY(smem_opt_in<nf_fused_kernel<OUT>>(200 * 1024));
   const int P = p->naflex_patch;
   long long tab_ints = 0;
   for (NfWork& w : work) {

@@ -17,6 +17,7 @@ import torch
 import jimm_oracle as O
 import naflex_oracle as NF
 import tokens_oracle as TO
+from gpu_util import record_parity
 
 
 @dataclass
@@ -117,3 +118,69 @@ def naflex_attn(p: O.Params, cfg: O.DualCfg, pixel_values, spatial_shapes, sem: 
         blocks, mw = vision_attn(pb, "vision_model.", img, t, sem)
         out.append(([w[0] for w in blocks], mw[0]))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------- the attention kernel
+# fp64 references of one attention call on the fused qkv buffer [B * S, 3 * H * d] (q, k, v of head h at columns h d, D + h d, 2 D + h d),
+# for the kernel tests: exact softmax attention, and the attention kernel's own steps restated in fp64.
+def _scale_log2(d):
+    """The kernel's fp32 constant: fl(fl(1 / sqrt(d)) * fl(log2 e))."""
+    return float(torch.tensor(1.0 / math.sqrt(d), dtype=torch.float32) * torch.tensor(1.4426950408889634, dtype=torch.float32))
+
+
+def _attn_ref(qkv, B, S, H, d, causal):
+    q, k, v = qkv.double().reshape(B, S, 3, H, d).permute(2, 0, 3, 1, 4)
+    w = (q / math.sqrt(d)) @ k.transpose(-1, -2)
+    if causal:
+        w = w.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
+    return (torch.softmax(w, -1) @ v).permute(0, 2, 1, 3).reshape(B * S, H * d)
+
+
+def _attn_tile_ref(qkv, B, S, H, d, causal):
+    """attention_kernel restated in fp64: 64-key tiles from key 0, a running row maximum m of the raw scores q.k, alpha =
+    exp2((m_old - m_new) c), p = exp2(s c - m_new c), l = l alpha + sum(p) with p unrounded, o = o alpha + round(p) . v, with p
+    rounded to the operand type as the kernel packs it for the P.V MMA (c = _scale_log2(d)).  A causal row sees no key past itself, so
+    the tiles after its own add nothing (alpha = 1, p = 0) and need no special case."""
+    c = _scale_log2(d)
+    q, k, v = qkv.double().reshape(B, S, 3, H, d).permute(2, 0, 3, 1, 4)
+    s = q @ k.transpose(-1, -2)
+    if causal:
+        s = s.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
+    m = torch.full((B, H, S, 1), float("-inf"), dtype=torch.float64, device=qkv.device)
+    l = torch.zeros_like(m)
+    o = torch.zeros(B, H, S, d, dtype=torch.float64, device=qkv.device)
+    for k0 in range(0, S, 64):
+        sj = s[..., k0:k0 + 64]
+        m_new = torch.maximum(m, sj.amax(-1, keepdim=True))
+        alpha = torch.exp2((m - m_new) * c)  # m = -inf on the first tile: alpha = 0
+        p = torch.exp2(sj * c - m_new * c)
+        l = l * alpha + p.sum(-1, keepdim=True)
+        o = o * alpha + p.to(qkv.dtype).double() @ v[..., k0:k0 + 64, :]
+        m = m_new
+    return (o / l).permute(0, 2, 1, 3).reshape(B * S, H * d)
+
+
+# Worst values over seven runs of test_attention, test_attention_split_variant and test_attention_lazy_rescale_path (inputs are
+# unseeded) on an H100 80GB HBM3 at a 400 W power limit: per row 6.5e-4 (fp16) and 3.9e-3 (bf16), bias 1.3e-6 and 4.0e-6.  The
+# per-row floor is one ulp of P on a row's dominant key: the kernel's fp32 p and the fp64 p now and then round to neighbouring
+# operand values.  Those flips have no sign, so the bias is their sampling noise (largest for bf16 at small S); a P packer that
+# truncates instead of rounding moved it to 3.5e-5 .. 1.9e-3 (unchanged only at S = 1, where most p are exactly 1).  Per-row bounds
+# are 3x, bias bounds 4-5x the worst value.
+TILE_ROW_TOL = {torch.float16: 2e-3, torch.bfloat16: 1.2e-2}
+TILE_BIAS_TOL = {torch.float16: 5e-6, torch.bfloat16: 2e-5}
+EXACT_TOL = {torch.float16: 3e-3, torch.bfloat16: 2e-2}  # against _attn_ref
+
+
+def _check_tile_faithful(case, out, qkv, B, S, H, d, causal, ref=None):
+    """The fp32 output against _attn_tile_ref (or `ref`, the same computed another way): the largest error of any (sample, head, query
+    row) relative to that row's largest |ref|, and the mean error along sign(ref) relative to mean |ref| (a P packer that truncates
+    instead of rounding to nearest biases every output towards zero by about half an ulp of the operand type)."""
+    ref = (_attn_tile_ref(qkv, B, S, H, d, causal) if ref is None else ref).reshape(B, S, H, d)
+    e = out.double().reshape(B, S, H, d) - ref
+    row = float((e.abs().amax(-1) / ref.abs().amax(-1)).max())
+    bias = float((e * ref.sign()).mean() / ref.abs().mean())
+    dn = str(qkv.dtype).replace("torch.", "")
+    record_parity(case, "per-row", dn, "tile-faithful fp64", TILE_ROW_TOL[qkv.dtype], row)
+    record_parity(case, "bias", dn, "tile-faithful fp64", TILE_BIAS_TOL[qkv.dtype], abs(bias))
+    assert row < TILE_ROW_TOL[qkv.dtype], (case, "per-row", row)
+    assert abs(bias) < TILE_BIAS_TOL[qkv.dtype], (case, "bias", bias)

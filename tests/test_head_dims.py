@@ -17,7 +17,8 @@ import pytest
 import torch
 
 import jimm_oracle as O
-from gpu_util import BF16, CODE, F16, F32, check, check_parity, ptr, record_parity, stream
+from attn_oracle import EXACT_TOL, _attn_ref, _check_tile_faithful
+from gpu_util import BF16, CODE, F16, F32, check, check_parity, ptr, stream
 from test_kernel_paths_gpu import SENTINEL, TF32, rna_tf32 as _rna_tf32
 
 DEV = "cuda"
@@ -109,11 +110,6 @@ def test_oracle_matches_hf_siglip_text_d72():
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU: attention kernel
-def _scale_log2(d):
-    """The kernel's fp32 constant: fl(fl(1 / sqrt(d)) * fl(log2 e))."""
-    return float(torch.tensor(1.0 / math.sqrt(d), dtype=torch.float32) * torch.tensor(1.4426950408889634, dtype=torch.float32))
-
-
 def _qkv(B, S, H, d, dtype, seed):
     """Odd heads hold values 6x larger than even ones: a padded column that is not zero-filled reads the next head's (or for the last
     q head, the first k head's) values into Q K^T."""
@@ -122,55 +118,6 @@ def _qkv(B, S, H, d, dtype, seed):
     x[:, :, 1::2] *= 6.0
     x[:, :, 0::2] *= 1.5
     return x.reshape(B * S, 3 * H * d).to(DEV).to(dtype)
-
-
-def _attn_ref(qkv, B, S, H, d, causal):
-    q, k, v = qkv.double().reshape(B, S, 3, H, d).permute(2, 0, 3, 1, 4)
-    w = (q / math.sqrt(d)) @ k.transpose(-1, -2)
-    if causal:
-        w = w.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
-    return (torch.softmax(w, -1) @ v).permute(0, 2, 1, 3).reshape(B * S, H * d)
-
-
-def _attn_tile_ref(qkv, B, S, H, d, causal):
-    """attention_kernel restated in fp64 (test_kernels_gpu._attn_tile_ref with head width d and scale constant c = _scale_log2(d)):
-    64-key tiles from key 0, a running row maximum m of the raw scores, alpha = exp2((m_old - m_new) c), p = exp2(s c - m_new c),
-    l = l alpha + sum(p), o = o alpha + round(p) . v with p rounded to the operand type."""
-    c = _scale_log2(d)
-    q, k, v = qkv.double().reshape(B, S, 3, H, d).permute(2, 0, 3, 1, 4)
-    s = q @ k.transpose(-1, -2)
-    if causal:
-        s = s.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
-    m = torch.full((B, H, S, 1), float("-inf"), dtype=torch.float64, device=qkv.device)
-    l = torch.zeros_like(m)
-    o = torch.zeros(B, H, S, d, dtype=torch.float64, device=qkv.device)
-    for k0 in range(0, S, 64):
-        sj = s[..., k0:k0 + 64]
-        m_new = torch.maximum(m, sj.amax(-1, keepdim=True))
-        alpha = torch.exp2((m - m_new) * c)
-        p = torch.exp2(sj * c - m_new * c)
-        l = l * alpha + p.sum(-1, keepdim=True)
-        o = o * alpha + p.to(qkv.dtype).double() @ v[..., k0:k0 + 64, :]
-        m = m_new
-    return (o / l).permute(0, 2, 1, 3).reshape(B * S, H * d)
-
-
-# the per-row and bias bounds of test_kernels_gpu.py
-TILE_ROW_TOL = {torch.float16: 2e-3, torch.bfloat16: 1.2e-2}
-TILE_BIAS_TOL = {torch.float16: 5e-6, torch.bfloat16: 2e-5}
-EXACT_TOL = {torch.float16: 3e-3, torch.bfloat16: 2e-2}
-
-
-def _check_tile_faithful(case, out, qkv, B, S, H, d, causal):
-    ref = _attn_tile_ref(qkv, B, S, H, d, causal).reshape(B, S, H, d)
-    e = out.double().reshape(B, S, H, d) - ref
-    row = float((e.abs().amax(-1) / ref.abs().amax(-1)).max())
-    bias = float((e * ref.sign()).mean() / ref.abs().mean())
-    dn = str(qkv.dtype).replace("torch.", "")
-    record_parity(case, "per-row", dn, "tile-faithful fp64", TILE_ROW_TOL[qkv.dtype], row)
-    record_parity(case, "bias", dn, "tile-faithful fp64", TILE_BIAS_TOL[qkv.dtype], abs(bias))
-    assert row < TILE_ROW_TOL[qkv.dtype], (case, "per-row", row)
-    assert abs(bias) < TILE_BIAS_TOL[qkv.dtype], (case, "bias", bias)
 
 
 def attention_hd(lib, qkv, out, out_code, B, S, H, d, causal, reverse=0):

@@ -6,7 +6,8 @@ import math
 import pytest
 import torch
 
-from gpu_util import BF16, CODE, F16, F32, check, gelu_tanh, gemm, ptr, quick_gelu, record_parity, rel_err, stream
+from attn_oracle import _attn_ref, _check_tile_faithful
+from gpu_util import BF16, CODE, F16, F32, check, gelu_tanh, gemm, ptr, quick_gelu, rel_err, stream
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -145,80 +146,20 @@ def test_layernorm_gather_rows_and_eps(lib):
     assert torch.all(out == 0)
 
 
-def _attn_ref(qkv, B, S, H, causal):
-    D = H * 64
-    q, k, v = qkv.double().reshape(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    w = (q / 8.0) @ k.transpose(-1, -2)
-    if causal:
-        w = w.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
-    return (torch.softmax(w, -1) @ v).permute(0, 2, 1, 3).reshape(B * S, D)
-
-
-SCALE_LOG2 = float(torch.tensor(0.125, dtype=torch.float32) * torch.tensor(1.4426950408889634, dtype=torch.float32))  # the kernel's fp32 constant
-
-
-def _attn_tile_ref(qkv, B, S, H, causal):
-    """attention_kernel restated in fp64: 64-key tiles from key 0, a running row maximum m of the raw scores q.k, alpha =
-    exp2((m_old - m_new) c), p = exp2(s c - m_new c), l = l alpha + sum(p) with p unrounded, o = o alpha + round(p) . v, with p
-    rounded to the operand type as the kernel packs it for the P.V MMA.  A causal row sees no key past itself, so the tiles after
-    its own add nothing (alpha = 1, p = 0) and need no special case."""
-    q, k, v = qkv.double().reshape(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    s = q @ k.transpose(-1, -2)
-    if causal:
-        s = s.masked_fill(~torch.tril(torch.ones(S, S, dtype=torch.bool, device=qkv.device)), float("-inf"))
-    m = torch.full((B, H, S, 1), float("-inf"), dtype=torch.float64, device=qkv.device)
-    l = torch.zeros_like(m)
-    o = torch.zeros(B, H, S, 64, dtype=torch.float64, device=qkv.device)
-    for k0 in range(0, S, 64):
-        sj = s[..., k0:k0 + 64]
-        m_new = torch.maximum(m, sj.amax(-1, keepdim=True))
-        alpha = torch.exp2((m - m_new) * SCALE_LOG2)  # m = -inf on the first tile: alpha = 0
-        p = torch.exp2(sj * SCALE_LOG2 - m_new * SCALE_LOG2)
-        l = l * alpha + p.sum(-1, keepdim=True)
-        o = o * alpha + p.to(qkv.dtype).double() @ v[..., k0:k0 + 64, :]
-        m = m_new
-    return (o / l).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-
-
-# Worst values over seven runs of test_attention, test_attention_split_variant and test_attention_lazy_rescale_path (inputs are
-# unseeded) on an H100 80GB HBM3 at a 400 W power limit: per row 6.5e-4 (fp16) and 3.9e-3 (bf16), bias 1.3e-6 and 4.0e-6.  The
-# per-row floor is one ulp of P on a row's dominant key: the kernel's fp32 p and the fp64 p now and then round to neighbouring
-# operand values.  Those flips have no sign, so the bias is their sampling noise (largest for bf16 at small S); a P packer that
-# truncates instead of rounding moved it to 3.5e-5 .. 1.9e-3 (unchanged only at S = 1, where most p are exactly 1).  Per-row bounds
-# are 3x, bias bounds 4-5x the worst value.
-TILE_ROW_TOL = {torch.float16: 2e-3, torch.bfloat16: 1.2e-2}
-TILE_BIAS_TOL = {torch.float16: 5e-6, torch.bfloat16: 2e-5}
-
-
-def _check_tile_faithful(case, out, qkv, B, S, H, causal):
-    """The fp32 output against _attn_tile_ref: the largest error of any (sample, head, query row) relative to that row's largest
-    |ref|, and the mean error along sign(ref) relative to mean |ref| (a P packer that truncates instead of rounding to nearest
-    biases every output towards zero by about half an ulp of the operand type)."""
-    ref = _attn_tile_ref(qkv, B, S, H, causal).reshape(B, S, H, 64)
-    d = out.double().reshape(B, S, H, 64) - ref
-    row = float((d.abs().amax(-1) / ref.abs().amax(-1)).max())
-    bias = float((d * ref.sign()).mean() / ref.abs().mean())
-    dn = str(qkv.dtype).replace("torch.", "")
-    record_parity(case, "per-row", dn, "tile-faithful fp64", TILE_ROW_TOL[qkv.dtype], row)
-    record_parity(case, "bias", dn, "tile-faithful fp64", TILE_BIAS_TOL[qkv.dtype], abs(bias))
-    assert row < TILE_ROW_TOL[qkv.dtype], (case, "per-row", row)
-    assert abs(bias) < TILE_BIAS_TOL[qkv.dtype], (case, "bias", bias)
-
-
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("S", [1, 16, 50, 64, 77, 128, 129, 144, 197, 200, 256, 257, 384, 385, 577, 700, 1024])
 @pytest.mark.parametrize("causal", [0, 1])
 def test_attention(lib, dtype, S, causal):
     B, H = 3, 2
     qkv = (torch.randn(B * S, 3 * H * 64, device=DEV) * 1.5).to(dtype)
-    ref = _attn_ref(qkv, B, S, H, causal)
+    ref = _attn_ref(qkv, B, S, H, 64, causal)
     for out_dtype in (dtype, torch.float32):
         out = torch.empty(B * S, H * 64, dtype=out_dtype, device=DEV)
         check(lib, lib.jimm_k_attention(ptr(qkv), CODE[dtype], ptr(out), CODE[out_dtype], B, S, H, causal, stream()))
         # P is rounded to the operand dtype before P.V (as in any tensor-core flash kernel)
         tol = 3e-3 if dtype == torch.float16 else 2e-2
         assert rel_err(out, ref) < tol, (S, causal, out_dtype, rel_err(out, ref))
-    _check_tile_faithful(f"attention B={B} S={S} H={H} causal={causal}", out, qkv, B, S, H, causal)
+    _check_tile_faithful(f"attention B={B} S={S} H={H} causal={causal}", out, qkv, B, S, H, 64, causal)
 
 
 @pytest.mark.parametrize("S,causal", [(130, 1), (197, 0), (256, 1), (577, 0)])
@@ -229,7 +170,7 @@ def test_attention_flash_kernel_forced(lib, S, causal):
     qkv = (torch.randn(B * S, 3 * H * 64, device=DEV) * 1.5).half()
     out = torch.empty(B * S, H * 64, dtype=torch.float16, device=DEV)
     check(lib, lib.jimm_k_attention(ptr(qkv), F16, ptr(out), F16, B, S, H, causal, stream()))
-    assert rel_err(out, _attn_ref(qkv, B, S, H, causal)) < 3e-3
+    assert rel_err(out, _attn_ref(qkv, B, S, H, 64, causal)) < 3e-3
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -239,13 +180,13 @@ def test_attention_split_variant(lib, dtype, S, causal):
     widths.  (No variant is selected: there is one attention kernel; the test keeps its id so its history stays comparable.)"""
     B, H = 30, 6
     qkv = (torch.randn(B * S, 3 * H * 64, device=DEV) * 1.5).to(dtype)
-    ref = _attn_ref(qkv, B, S, H, causal)
+    ref = _attn_ref(qkv, B, S, H, 64, causal)
     tol = 3e-3 if dtype == torch.float16 else 2e-2
     for out_dtype in (dtype, torch.float32):
         out = torch.empty(B * S, H * 64, dtype=out_dtype, device=DEV)
         check(lib, lib.jimm_k_attention(ptr(qkv), CODE[dtype], ptr(out), CODE[out_dtype], B, S, H, causal, stream()))
         assert rel_err(out, ref) < tol, (S, causal, out_dtype, rel_err(out, ref))
-    _check_tile_faithful(f"attention B={B} S={S} H={H} causal={causal}", out, qkv, B, S, H, causal)
+    _check_tile_faithful(f"attention B={B} S={S} H={H} causal={causal}", out, qkv, B, S, H, 64, causal)
 
 
 def test_attention_many_items_persistent(lib):
@@ -254,7 +195,7 @@ def test_attention_many_items_persistent(lib):
     qkv = (torch.randn(B * S, 3 * H * 64, device=DEV)).half()
     out = torch.empty(B * S, H * 64, dtype=torch.float16, device=DEV)
     check(lib, lib.jimm_k_attention(ptr(qkv), F16, ptr(out), F16, B, S, H, 0, stream()))
-    assert rel_err(out, _attn_ref(qkv, B, S, H, 0)) < 3e-3
+    assert rel_err(out, _attn_ref(qkv, B, S, H, 64, 0)) < 3e-3
 
 
 def test_attention_long_many_units_persistent(lib):
@@ -263,7 +204,7 @@ def test_attention_long_many_units_persistent(lib):
     qkv = (torch.randn(B * S, 3 * H * 64, device=DEV)).half()
     out = torch.empty(B * S, H * 64, dtype=torch.float16, device=DEV)
     check(lib, lib.jimm_k_attention(ptr(qkv), F16, ptr(out), F16, B, S, H, 0, stream()))
-    assert rel_err(out, _attn_ref(qkv, B, S, H, 0)) < 3e-3
+    assert rel_err(out, _attn_ref(qkv, B, S, H, 64, 0)) < 3e-3
 
 
 @pytest.mark.parametrize("S", [197, 256, 300, 576, 1024])
@@ -281,10 +222,10 @@ def test_attention_lazy_rescale_path(lib, S):
     qkv = torch.stack([q, k, v], dim=2).reshape(B * S, 3 * H * 64).to(DEV).half()
     out = torch.empty(B * S, H * 64, dtype=torch.float32, device=DEV)
     check(lib, lib.jimm_k_attention(ptr(qkv), F16, ptr(out), F32, B, S, H, 0, stream()))
-    ref = _attn_ref(qkv, B, S, H, 0)
+    ref = _attn_ref(qkv, B, S, H, 64, 0)
     assert torch.isfinite(out).all()
     assert rel_err(out, ref) < 5e-3, rel_err(out, ref)
-    _check_tile_faithful(f"attention (rising scores) B={B} S={S} H={H}", out, qkv, B, S, H, 0)
+    _check_tile_faithful(f"attention (rising scores) B={B} S={S} H={H}", out, qkv, B, S, H, 64, 0)
 
 
 def test_attention_large_scores_stable(lib):
@@ -293,7 +234,7 @@ def test_attention_large_scores_stable(lib):
     out = torch.empty(B * S, 64, dtype=torch.float32, device=DEV)
     check(lib, lib.jimm_k_attention(ptr(qkv), F16, ptr(out), F32, B, S, H, 0, stream()))
     assert torch.isfinite(out).all()
-    assert rel_err(out, _attn_ref(qkv, B, S, H, 0)) < 5e-3
+    assert rel_err(out, _attn_ref(qkv, B, S, H, 64, 0)) < 5e-3
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])

@@ -25,7 +25,8 @@ import torch
 import interp_oracle as I
 import jimm_oracle as O
 from gpu_util import BF16, CODE, F16, F32, TORCH, check, check_parity, ptr, record_parity, rel_err, stream
-from test_head_dims import EXACT_TOL, TILE_BIAS_TOL, TILE_ROW_TOL, _attn_ref, _attn_tile_ref, _qkv, _run_all_outputs
+from attn_oracle import EXACT_TOL, _attn_ref, _attn_tile_ref, _check_tile_faithful
+from test_head_dims import _qkv, _run_all_outputs
 from test_kernel_paths_gpu import SENTINEL, TF32, rna_tf32
 
 pytestmark = pytest.mark.gpu
@@ -70,18 +71,10 @@ def _per_head(fn, qkv, B, S, H, d, causal):
 
 
 def _check_long(case, out, qkv, B, S, H, d, causal):
-    """out (fp32) against exact fp64 and, with the per-row and bias bounds of test_kernels_gpu.py, against the tile-faithful fp64."""
+    """out (fp32) against exact fp64 and against the tile-faithful fp64."""
     io = qkv.dtype
     check_parity(case, "out", io, "exact fp64", out, _per_head(_attn_ref, qkv, B, S, H, d, causal), EXACT_TOL[io])
-    ref = _per_head(_attn_tile_ref, qkv, B, S, H, d, causal).reshape(B, S, H, d)
-    e = out.double().reshape(B, S, H, d) - ref
-    row = float((e.abs().amax(-1) / ref.abs().amax(-1)).max())
-    bias = float((e * ref.sign()).mean() / ref.abs().mean())
-    dn = str(io).replace("torch.", "")
-    record_parity(case, "per-row", dn, "tile-faithful fp64", TILE_ROW_TOL[io], row)
-    record_parity(case, "bias", dn, "tile-faithful fp64", TILE_BIAS_TOL[io], abs(bias))
-    assert row < TILE_ROW_TOL[io], (case, "per-row", row)
-    assert abs(bias) < TILE_BIAS_TOL[io], (case, "bias", bias)
+    _check_tile_faithful(case, out, qkv, B, S, H, d, causal, ref=_per_head(_attn_tile_ref, qkv, B, S, H, d, causal))
 
 
 LONG_S = [1025, 2048, 2305, 4097, 8464]
