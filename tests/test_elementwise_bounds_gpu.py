@@ -31,16 +31,13 @@ import pytest
 import torch
 
 import fp8_oracle as F
-from gpu_util import BF16, CODE, F16, F32, check, gemm, ptr, record_parity, stream
+from bounds_util import OUT, U, assert_within
+from gpu_util import CODE, F16, check, gemm, ptr, record_parity, stream
 from test_fp8_gpu import gemm8
-from test_kernel_paths_gpu import SENTINEL, TF32, gemm_ex, rna_tf32
+from test_kernel_paths_gpu import SENTINEL, gemm_ex, rna_tf32
 
 DEV = "cuda"
-U = 2.0 ** -24
 LOG2E = 1.0 / math.log(2.0)
-# output type: (torch dtype, type code of the jimm_k_* entry points, unit roundoff, half the smallest subnormal step)
-OUT = {"f16": (torch.float16, F16, 2.0 ** -11, 2.0 ** -25), "bf16": (torch.bfloat16, BF16, 2.0 ** -8, 2.0 ** -134),
-       "f32": (torch.float32, F32, 2.0 ** -24, 2.0 ** -150), "tf32": (torch.float32, TF32, 2.0 ** -11, 2.0 ** -137)}
 OPS = ["f16", "bf16", "tf32"]
 OP_DTYPE = {"f16": torch.float16, "bf16": torch.bfloat16, "tf32": torch.float32}
 SLOPE = [1.0, 1.13, 1.1]
@@ -51,23 +48,6 @@ C_ACC = {"f16": 3e-6, "bf16": 3e-6, "tf32": 6e-6, "e4m3": 2.4e-4}
 
 
 # ---------------------------------------------------------------------------------------------------------------- the per-element check
-def assert_within(case, what, out, ref, bound, dtype="fp32"):
-    """Assert |out - ref| <= bound at every element (NaN in out - ref fails); record and return max |out - ref| / bound."""
-    out, ref = torch.as_tensor(out).double(), torch.as_tensor(ref).double()
-    bound = torch.as_tensor(bound, dtype=torch.float64, device=out.device).expand_as(out)
-    err = (out - ref).abs()
-    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
-    ratio = torch.nan_to_num(ratio, nan=math.inf, posinf=math.inf)
-    flat = int(ratio.argmax())
-    worst = float(ratio.flatten()[flat])
-    record_parity(case, what, dtype, "fp64", 1.0, worst)
-    if not worst <= 1.0:
-        idx = tuple(int(i) for i in np.unravel_index(flat, tuple(out.shape)))
-        o, r, b = (float(t.flatten()[flat]) for t in (out, ref, bound))
-        raise AssertionError(f"{case} / {what} [{dtype}]: |out - ref| / bound = {worst:.3g} at {idx}: out={o!r} ref={r!r} bound={b!r}")
-    return worst
-
-
 def test_assert_within_flags_one_element():
     """CPU: an exact result passes with ratio 0; one element off by 1.5 x its bound fails and the message names it; NaN fails."""
     g = torch.Generator().manual_seed(0)
