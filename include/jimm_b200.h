@@ -477,6 +477,21 @@ JIMM_API int jimm_k_preproc_plan(const jimm_preproc_config_t* cfg, int H, int W,
  * per row (8 when cols <= 8192), for at most 256 MB of rows at a time (or one row, if a row needs more). */
 JIMM_API int jimm_postprocess(const float* logits, int rows, int cols, int ld, int mode, float* probs, int ldp, int32_t* order, int32_t* argmax,
                               void* stream);
+/* Top-k of each logits row (1 <= k <= cols): indices (int32 [rows, k]) are the first k columns of jimm_postprocess's order -- equal
+ * scores larger index first, every NaN above +inf, -0 tied with +0 -- values (fp32 [rows, k]) the logits at those columns, bit for
+ * bit, and probs (nullable, fp32 [rows, k]) mode 0's probabilities there, bit for bit.  k <= 1024: a row of up to 32768 columns is
+ * selected in one CTA from one read (radix select, then a sort of the k survivors); a wider row keeps k candidates per 8192-column
+ * segment in scratch (8 k bytes per segment per row, at most 256 MB of rows at a time) and merges them.  k > 1024: the prefix of the
+ * full order, sorted in scratch (4 bytes per column per row, at most 256 MB of rows at a time, plus the sort's own).  Scratch is
+ * allocated in stream order on `stream`. */
+JIMM_API int jimm_topk(const float* logits, int rows, int cols, int ld, int k, float* values, int32_t* indices, float* probs, void* stream);
+/* Gallery search of a CLIP / SigLIP model: for each of the Q queries (device fp32 [Q, E], un-normalised embeddings as
+ * jimm_encode_image / jimm_encode_text return them) its k best gallery rows (device fp32 [N, E], the other tower's embeddings) by
+ * the model's own score, as jimm_topk would pick them from the [Q, N] jimm_contrastive_logits matrix -- values fp32 [Q, k], indices
+ * int32 [Q, k] -- bit for bit, without that matrix: scores go through bounded score blocks in stream-ordered scratch (under 0.5 GB
+ * at E <= 1024 for any N).  E is the model's embedding width; 1 <= k <= min(N, 1024). */
+JIMM_API int jimm_search(jimm_model_t* m, const float* queries, int Q, const float* gallery, int N, int k, float* values, int32_t* indices,
+                         void* stream);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads
  * its own 16 KB tiles; 1: the CTAs of a cluster load the same tile each; 2: same tile, each loads 1/cluster of it and multicasts. */
 JIMM_API int jimm_k_l2_probe(const void* buf, int rows, int mode, int cluster, int iters, float* ms, void* stream);

@@ -151,6 +151,8 @@ SIGNATURES = {
     "jimm_k_upload_kernel": (_i, [_vp, _i, _i, _i, _i, _vp, _i, C.c_longlong, _i, _vp]),
     "jimm_k_l2_probe": (_i, [_vp, _i, _i, _i, _i, C.POINTER(C.c_float), _vp]),
     "jimm_postprocess": (_i, [_fp, _i, _i, _i, _i, _fp, _i, _ip, _ip, _vp]),
+    "jimm_topk": (_i, [_fp, _i, _i, _i, _i, _fp, _ip, _fp, _vp]),
+    "jimm_search": (_i, [_vp, _fp, _i, _fp, _i, _i, _fp, _ip, _vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),

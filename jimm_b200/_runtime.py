@@ -538,6 +538,31 @@ class NativeModel:
         self._run("jimm_contrastive_logits", img_e, Bi, txt_e, Bt, out)
         return out
 
+    def search(self, queries, gallery, k: int):
+        """The k best gallery rows of each query by the model's score (jimm_search): fp32 [Q, k] scores and int32 [Q, k] indices,
+        bit for bit the top_k of the logits matrix the contrastive head would give for the two sets.  Both [*, E] embedding sets of
+        float32 / float16 / bfloat16 on the device or the host; the result is on the host when both were."""
+        q, g = _as_tensor(queries), _as_tensor(gallery)
+        E = self.text_out
+        for name, t in (("queries", q), ("gallery", g)):
+            if t.ndim != 2 or t.shape[1] != E:
+                raise ValueError(f"search: expected {name} of shape [rows, {E}] (the model's embedding width), got {tuple(t.shape)}")
+            if t.dtype not in _TORCH_TO_CODE:
+                raise ValueError(f"search: {name} must be float32, float16 or bfloat16, got {t.dtype}")
+            if t.shape[0] > 2**31 - 1:
+                raise ValueError(f"search: at most {2**31 - 1} {name} rows, got {t.shape[0]}")
+        Q, N = q.shape[0], g.shape[0]
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= min(N, 1024):
+            raise ValueError(f"search: k must be an int in 1 .. min(gallery rows={N}, 1024), got {k!r}")
+        k = int(k)
+        host = not q.is_cuda and not g.is_cuda
+        qd = q.to(self.device, torch.float32, non_blocking=True).contiguous()
+        gd = g.to(self.device, torch.float32, non_blocking=True).contiguous()
+        values = torch.empty((Q, k), dtype=torch.float32, device=self.device)
+        indices = torch.empty((Q, k), dtype=torch.int32, device=self.device)
+        self._run("jimm_search", qd, Q, gd, N, k, values, indices)
+        return self._back(values, host).result(), self._back(indices, host).result()
+
     def dual(self, images, text, interpolate: bool = False) -> torch.Tensor:
         """CLIP.__call__ / SigLIP.__call__ on one GPU, on Images or on a tensor / list prepared here, and on a [B, T] ids tensor or a
         list of token sequences (Texts).  The result is on the host when the images and the ids were.  A list of sequences runs the

@@ -78,6 +78,14 @@ int l2_normalize_run(const float* x, float* out, int ldo, int B, int E, cudaStre
 int logits_run(const float* img, const float* txt, const float* logit_scale, const float* logit_bias, float* logits, int Bi, int Bt,
                int E, int ldl, cudaStream_t stream);
 
+// postprocess.cu.  Top-k of each logits row: the first k entries of jimm_postprocess's order (1 <= k <= cols), their values and,
+// probs non-null, their softmax probabilities -- bit for bit.  Scratch is allocated in stream order on `stream`.
+int topk_run(const float* logits, int rows, int cols, int ld, int k, float* values, int32_t* indices, float* probs, cudaStream_t stream);
+// Top-k of each query's scores against the gallery (1 <= k <= min(N, 1024)) with no [Q, N] buffer: every score is the one
+// l2_normalize_run + logits_run give for that pair (queries on the image side, gallery on the text side, or the other way round).
+int search_run(const float* queries, int Q, const float* gallery, int N, int E, const float* logit_scale, const float* logit_bias, int k,
+               float* values, int32_t* indices, cudaStream_t stream);
+
 // dst[n*K + k] = cast(src[k*N + n])   (flax (in,out) kernel -> K-major [N,K] operand)
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);
 int cast_run(const float* src, void* dst, int out_type, size_t n, cudaStream_t stream);

@@ -1850,6 +1850,16 @@ int jimm_contrastive_logits(jimm_model_t* m, const float* img_e, int Bi, const f
   return logits_run(m->ws.nrm_i, m->ws.nrm_t, m->logit_scale, m->logit_bias, logits, Bi, Bt, E, Bt, s);
 }
 
+int jimm_search(jimm_model_t* m, const float* queries, int Q, const float* gallery, int N, int k, float* values, int32_t* indices, void* stream) {
+  JIMM_TRY(check_ready(m, Q));
+  JIMM_TRY(check_text(m));
+  if (N < 1 || k < 1 || k > N || k > 1024) { set_last_error("search: k=%d outside 1 .. min(N=%d, 1024)", k, N); return JIMM_EINVAL; }
+  if (!gallery || (Q > 0 && (!queries || !values || !indices))) { set_last_error("search: null queries, gallery, values or indices"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  if (Q == 0) return 0;
+  return search_run(queries, Q, gallery, N, m->txt.D, m->logit_scale, m->logit_bias, k, values, indices, static_cast<cudaStream_t>(stream));
+}
+
 // Fork the text tower onto the model's side stream (ordered after everything already enqueued on `s`), returning the stream it runs
 // on; join_text() makes `s` wait for it.  Profiling (per-GEMM events) and JIMM_DUAL_STREAMS=0 keep the towers on one stream.
 static int fork_text(jimm_model* m, cudaStream_t s, cudaStream_t* ts) {

@@ -13,6 +13,7 @@
 
 #include "../../include/jimm_b200.h"
 #include "common.cuh"
+#include "kernels.cuh"
 
 namespace jimm {
 namespace {
@@ -41,8 +42,13 @@ __device__ __forceinline__ u64 sort_key(const float* x, long long i) {
   return (static_cast<u64>(order_key(x[i])) << 32) | static_cast<uint32_t>(i);
 }
 
-// Bitonic sort of n (a power of two) keys in shared memory, descending, by the whole CTA.
-__device__ void bitonic_sort_desc(u64* keys, int n) {
+struct KeyIsValue {
+  __device__ __forceinline__ u64 operator()(u64 v) const { return v; }
+};
+
+// Bitonic sort of n (a power of two) keys in shared memory, descending by key(.), by the whole CTA.
+template <typename Key = KeyIsValue>
+__device__ void bitonic_sort_desc(u64* keys, int n, Key key = {}) {
   for (int k = 2; k <= n; k <<= 1) {
     for (int j = k >> 1; j > 0; j >>= 1) {
       for (int i = threadIdx.x; i < n; i += kThreads) {
@@ -50,7 +56,7 @@ __device__ void bitonic_sort_desc(u64* keys, int n) {
         if (l > i) {
           const u64 a = keys[i], b = keys[l];
           const bool desc = (i & k) == 0;
-          if (desc ? a < b : a > b) {
+          if (desc ? key(a) < key(b) : key(a) > key(b)) {
             keys[i] = b;
             keys[l] = a;
           }
@@ -59,6 +65,26 @@ __device__ void bitonic_sort_desc(u64* keys, int n) {
       __syncthreads();
     }
   }
+}
+
+// Softmax denominator of a row: sum of exp(x[i]), per-thread strided sums reduced by a shuffle tree per warp and the warps' sums in
+// order by thread 0.  Called by the whole CTA; every thread gets the total.  zero_shot's probabilities and top_k's are both
+// exp(x) / this sum, so they agree bit for bit.
+__device__ __forceinline__ float row_exp_sum(const float* __restrict__ x, int cols, float* red, float* total) {
+  const int tid = threadIdx.x;
+  float s = 0.f;
+  for (long long i = tid; i < cols; i += kThreads) s += expf(x[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((tid & 31) == 0) red[tid >> 5] = s;
+  __syncthreads();
+  if (tid == 0) {
+    float t = 0.f;
+    for (int w = 0; w < kThreads / 32; ++w) t += red[w];
+    *total = t;
+  }
+  __syncthreads();
+  return *total;
 }
 
 __global__ void __launch_bounds__(kThreads) postprocess_kernel(const float* __restrict__ logits, int cols, int ld, int mode, float* __restrict__ probs,
@@ -77,19 +103,7 @@ __global__ void __launch_bounds__(kThreads) postprocess_kernel(const float* __re
     if (mode == 1) {
       for (long long i = tid; i < cols; i += kThreads) p[i] = 1.0f / (1.0f + expf(-x[i]));
     } else {
-      float s = 0.f;
-      for (long long i = tid; i < cols; i += kThreads) s += expf(x[i]);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if ((tid & 31) == 0) red[tid >> 5] = s;
-      __syncthreads();
-      if (tid == 0) {
-        float t = 0.f;
-        for (int w = 0; w < kThreads / 32; ++w) t += red[w];
-        total = t;
-      }
-      __syncthreads();
-      const float t = total;
+      const float t = row_exp_sum(x, cols, red, &total);
       for (long long i = tid; i < cols; i += kThreads) p[i] = expf(x[i]) / t;
     }
   }
@@ -229,7 +243,312 @@ int sort_wide_rows(const float* logits, int rows, int cols, int ld, int32_t* ord
   return rc;
 }
 
+// ---- top-k: the first k entries of the descending order, selected without sorting the row ----
+// A candidate is (float bits << 32 | column): the value as stored (-0 and NaN payloads included) and its column.  Its sort key is the
+// order's (order_key << 32 | column), so candidates compare exactly like the full sort's keys; kPadCand (column 0xffffffff, never a
+// real column) has key 0, below every real one.
+constexpr int kSelectMaxK = 1024;   // largest k selected in shared memory; beyond it top_k takes the prefix of the full sort
+constexpr int kRowCols = 32768;     // rows up to this wide are selected in one CTA from one read (128 KB of keys)
+constexpr int kSegCols = 8192;      // wider rows: segments of this many columns, k candidates each, then one merge
+constexpr u64 kPadCand = 0xffffffffull;
+
+struct CandKey {
+  __device__ __forceinline__ u64 operator()(u64 c) const {
+    const uint32_t col = static_cast<uint32_t>(c & 0xffffffffu);
+    return col == 0xffffffffu ? 0ull : (static_cast<u64>(order_key(__uint_as_float(static_cast<uint32_t>(c >> 32)))) << 32) | col;
+  }
+};
+
+struct SelectSmem {
+  uint32_t hist[kThreads / 32][256];  // one histogram per warp: fewer collisions on the shared atomics
+  uint32_t digit, remaining;
+  int count;
+  float red[kThreads / 32], total;
+};
+
+// The k-th largest of n unique 64-bit keys key(i), 1 <= k <= n: one 8-bit digit per pass from the top, each pass a histogram of the
+// keys that share the digits chosen so far.  Every key's low word (a column) is below 2^lo_bits, so the passes over its higher
+// digits (all zero) are skipped.
+template <typename Key>
+__device__ u64 radix_select(Key key, long long n, int k, int lo_bits, SelectSmem& s) {
+  static_assert(kThreads == 256, "one bin per thread");
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  u64 prefix = 0, mask = 0;
+  uint32_t remaining = static_cast<uint32_t>(k);
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    if (shift < 32 && shift >= lo_bits) continue;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) s.hist[w][tid] = 0;
+    __syncthreads();
+    for (long long i = tid; i < n; i += kThreads) {
+      const u64 v = key(i);
+      if ((v & mask) == prefix) atomicAdd(&s.hist[warp][(v >> shift) & 255], 1u);
+    }
+    __syncthreads();
+    uint32_t t = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) t += s.hist[w][tid];
+    __syncthreads();
+    s.hist[0][tid] = t;
+    __syncthreads();
+    if (warp == 0) {  // lane l holds bins 255 - 8l down to 248 - 8l; find the bin where the count from the top reaches `remaining`
+      uint32_t c[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += (c[j] = s.hist[0][255 - 8 * lane - j]);
+      uint32_t inc = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += u;
+      }
+      uint32_t acc = inc - sum;
+      if (acc < remaining && remaining <= inc) {
+        int d = -1;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (d < 0) {
+            if (acc + c[j] >= remaining) d = j;
+            else acc += c[j];
+          }
+        }
+        s.digit = 255 - 8 * lane - d;
+        s.remaining = remaining - acc;
+      }
+    }
+    __syncthreads();
+    prefix |= static_cast<u64>(s.digit) << shift;
+    mask |= 0xffull << shift;
+    remaining = s.remaining;
+  }
+  return prefix;
+}
+
+// The candidates cand(i) of the keys key(i) >= kth (the min(n, k) best when kth is the k-th key, or every one when kth is 0) into
+// surv[], padded with kPadCand to npow2 (a power of two >= k) and sorted descending.
+template <typename Key, typename Cand>
+__device__ void collect_sorted(Key key, Cand cand, long long n, u64 kth, int k, int npow2, u64* surv, SelectSmem& s) {
+  if (threadIdx.x == 0) s.count = 0;
+  __syncthreads();
+  for (long long i = threadIdx.x; i < n; i += kThreads)
+    if (key(i) >= kth) surv[atomicAdd(&s.count, 1)] = cand(i);
+  for (long long i = min(n, static_cast<long long>(k)) + threadIdx.x; i < npow2; i += kThreads) surv[i] = kPadCand;
+  __syncthreads();
+  bitonic_sort_desc(surv, npow2, CandKey{});
+}
+
+// The first k sorted candidates of a row: as candidates into cand_out, or as values (the stored bits), columns and, when probs is
+// set, exp(value) / total -- zero_shot's probability at that column.
+__device__ void emit_row(const u64* surv, int k, u64* cand_out, float* values, int32_t* indices, float* probs, float total) {
+  for (int i = threadIdx.x; i < k; i += kThreads) {
+    const u64 c = surv[i];
+    if (cand_out) {
+      cand_out[i] = c;
+    } else {
+      const float v = __uint_as_float(static_cast<uint32_t>(c >> 32));
+      values[i] = v;
+      indices[i] = static_cast<int32_t>(c & 0xffffffffu);
+      if (probs) probs[i] = expf(v) / total;
+    }
+  }
+}
+
+// grid (segments, rows): segment s of row r is the columns [s * seg, min((s + 1) * seg, cols)) of x's row r, numbered from col_base.
+// Its keys are staged once in shared memory; its k best (all of them, padded, when it is narrower) go to cand + r * cand_ld + s * k,
+// or -- cand null, one segment spanning the row -- straight to the row's outputs (row stride k).
+__global__ void __launch_bounds__(kThreads) topk_segment_kernel(const float* __restrict__ logits, int cols, int ld, int seg, int k, int col_base,
+                                                              int lo_bits, int npow2, u64* __restrict__ cand, long long cand_ld,
+                                                              float* __restrict__ values, int32_t* __restrict__ indices, float* __restrict__ probs) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  u64* surv = reinterpret_cast<u64*>(smem_raw);                   // [npow2]
+  uint32_t* keys = reinterpret_cast<uint32_t*>(surv + npow2);     // [seg]
+  __shared__ SelectSmem s;
+  const int row = blockIdx.y;
+  const float* x = logits + static_cast<size_t>(row) * ld;
+  const int c0 = blockIdx.x * seg;
+  const int n = min(seg, cols - c0);
+  for (int i = threadIdx.x; i < n; i += kThreads) keys[i] = order_key(x[c0 + i]);
+  __syncthreads();
+  const uint32_t base = static_cast<uint32_t>(col_base + c0);
+  auto key = [&](long long i) { return (static_cast<u64>(keys[i]) << 32) | (base + static_cast<uint32_t>(i)); };
+  auto cand_of = [&](long long i) { return (static_cast<u64>(__float_as_uint(x[c0 + i])) << 32) | (base + static_cast<uint32_t>(i)); };
+  const u64 kth = n > k ? radix_select(key, n, k, lo_bits, s) : 0ull;
+  collect_sorted(key, cand_of, n, kth, k, npow2, surv, s);
+  if (cand) {
+    emit_row(surv, k, cand + row * cand_ld + static_cast<long long>(blockIdx.x) * k, nullptr, nullptr, nullptr, 0.f);
+  } else {
+    const float t = probs ? row_exp_sum(x, cols, s.red, &s.total) : 0.f;
+    const size_t o = static_cast<size_t>(row) * k;
+    emit_row(surv, k, nullptr, values + o, indices + o, probs ? probs + o : nullptr, t);
+  }
+}
+
+// grid (rows): the k best of the n candidates at cand + r * cand_ld (at least k of them real), to out_cand + r * cand_ld (which may
+// be where they came from: every read is done before the first write) or, out_cand null, to the outputs (row stride k); probs
+// need the logits row x (cols wide, stride ld) for the softmax denominator.
+__global__ void __launch_bounds__(kThreads) topk_merge_kernel(const u64* cand, long long cand_ld, long long n, int k, int lo_bits, int npow2,
+                                                            u64* out_cand, const float* __restrict__ logits, int cols, int ld,
+                                                            float* __restrict__ values, int32_t* __restrict__ indices, float* __restrict__ probs) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  u64* surv = reinterpret_cast<u64*>(smem_raw);  // [npow2]
+  __shared__ SelectSmem s;
+  const int row = blockIdx.x;
+  const u64* c = cand + row * cand_ld;
+  auto key = [&](long long i) { return CandKey{}(c[i]); };
+  auto cand_of = [&](long long i) { return c[i]; };
+  collect_sorted(key, cand_of, n, radix_select(key, n, k, lo_bits, s), k, npow2, surv, s);
+  if (out_cand) {
+    emit_row(surv, k, out_cand + row * cand_ld, nullptr, nullptr, nullptr, 0.f);
+  } else {
+    const float t = probs ? row_exp_sum(logits + static_cast<size_t>(row) * ld, cols, s.red, &s.total) : 0.f;
+    const size_t o = static_cast<size_t>(row) * k;
+    emit_row(surv, k, nullptr, values + o, indices + o, probs ? probs + o : nullptr, t);
+  }
+}
+
+// grid (rows): the first k columns of each row's full order (k > kSelectMaxK), with their values and probabilities.
+__global__ void __launch_bounds__(kThreads) topk_gather_kernel(const int32_t* __restrict__ order, int cols, const float* __restrict__ logits, int ld,
+                                                             int k, float* __restrict__ values, int32_t* __restrict__ indices, float* __restrict__ probs) {
+  __shared__ float red[kThreads / 32], total;
+  const int row = blockIdx.x;
+  const float* x = logits + static_cast<size_t>(row) * ld;
+  const float t = probs ? row_exp_sum(x, cols, red, &total) : 0.f;
+  const size_t o = static_cast<size_t>(row) * k;
+  for (int i = threadIdx.x; i < k; i += kThreads) {
+    const int32_t j = order[static_cast<size_t>(row) * cols + i];
+    const float v = x[j];
+    values[o + i] = v;
+    indices[o + i] = j;
+    if (probs) probs[o + i] = expf(v) / t;
+  }
+}
+
+int bit_width(long long cols) {  // bits of the largest column index, cols - 1
+  int b = 0;
+  while ((1ll << b) < cols) ++b;
+  return b;
+}
+
+int pow2_at_least(int k) {
+  int p = 1;
+  while (p < k) p <<= 1;
+  return p;
+}
+
+// Segment kernel over rows [0, rows) of `logits` in grid-sized groups; shared memory for `seg`-column segments and k survivors.
+int launch_segments(const float* logits, int rows, int cols, int ld, int seg, int k, int col_base, int lo_bits, u64* cand, long long cand_ld,
+                    float* values, int32_t* indices, float* probs, cudaStream_t st) {
+  const int npow2 = pow2_at_least(k);
+  const size_t smem = static_cast<size_t>(npow2) * sizeof(u64) + static_cast<size_t>(seg) * sizeof(uint32_t);
+  if (const int rc = smem_opt_in<topk_segment_kernel>(kSelectMaxK * sizeof(u64) + kRowCols * sizeof(uint32_t))) return rc;
+  const unsigned segs = static_cast<unsigned>((static_cast<long long>(cols) + seg - 1) / seg);
+  for (int r0 = 0; r0 < rows; r0 += 65535) {
+    const int g = std::min(65535, rows - r0);
+    const size_t o = static_cast<size_t>(r0) * k;
+    JIMM_CUDA_CHECK(launch_k(topk_segment_kernel, dim3(segs, g), dim3(kThreads), smem, st, 1, false, logits + static_cast<size_t>(r0) * ld, cols, ld,
+                             seg, k, col_base, lo_bits, npow2, cand ? cand + r0 * cand_ld : nullptr, cand_ld, cand ? nullptr : values + o,
+                             cand ? nullptr : indices + o, cand || !probs ? nullptr : probs + o));
+    note_launch();
+  }
+  return 0;
+}
+
+int launch_merge(const u64* cand, int rows, long long cand_ld, long long n, int k, int lo_bits, u64* out_cand, const float* logits, int cols, int ld,
+                 float* values, int32_t* indices, float* probs, cudaStream_t st) {
+  const int npow2 = pow2_at_least(k);
+  JIMM_CUDA_CHECK(launch_k(topk_merge_kernel, dim3(rows), dim3(kThreads), static_cast<size_t>(npow2) * sizeof(u64), st, 1, false, cand, cand_ld, n,
+                           k, lo_bits, npow2, out_cand, logits, cols, ld, values, indices, probs));
+  note_launch();
+  return 0;
+}
+
+int free_scratch(void* p, cudaStream_t st, int rc) {
+  const cudaError_t fe = cudaFreeAsync(p, st);
+  if (rc == 0 && fe != cudaSuccess) { set_last_error("cudaFreeAsync -> %s", cudaGetErrorString(fe)); return JIMM_ECUDA; }
+  return rc;
+}
+
 }  // namespace
+
+int topk_run(const float* logits, int rows, int cols, int ld, int k, float* values, int32_t* indices, float* probs, cudaStream_t st) {
+  if (k > kSelectMaxK) {  // the prefix of the full order, sorted in scratch for as many rows at a time as fit in kScratchBytes
+    const int group = static_cast<int>(std::min<size_t>(std::max<size_t>(kScratchBytes / (static_cast<size_t>(cols) * sizeof(int32_t)), 1), rows));
+    int32_t* order = nullptr;
+    JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&order), static_cast<size_t>(group) * cols * sizeof(int32_t), st));
+    int rc = 0;
+    for (int r0 = 0; r0 < rows && rc == 0; r0 += group) {
+      const int g = std::min(group, rows - r0);
+      const float* x = logits + static_cast<size_t>(r0) * ld;
+      const size_t o = static_cast<size_t>(r0) * k;
+      rc = jimm_postprocess(x, g, cols, ld, 0, nullptr, cols, order, nullptr, st);
+      if (rc == 0) {
+        const cudaError_t e = launch_k(topk_gather_kernel, dim3(g), dim3(kThreads), 0, st, 1, false, order, cols, x, ld, k, values + o, indices + o,
+                                       probs ? probs + o : nullptr);
+        if (e != cudaSuccess) { set_last_error("topk_gather_kernel -> %s", cudaGetErrorString(e)); rc = JIMM_ECUDA; }
+        else note_launch();
+      }
+    }
+    return free_scratch(order, st, rc);
+  }
+  const int lo = bit_width(cols);
+  if (cols <= kRowCols) return launch_segments(logits, rows, cols, ld, cols, k, 0, lo, nullptr, 0, values, indices, probs, st);
+  // wider rows: k candidates per segment in scratch, for as many rows at a time as fit in kScratchBytes, then one merge per row
+  const long long segs = (static_cast<long long>(cols) + kSegCols - 1) / kSegCols, cand_ld = segs * k;
+  const size_t row_bytes = static_cast<size_t>(cand_ld) * sizeof(u64);
+  const int group = static_cast<int>(std::min<size_t>(std::max<size_t>(kScratchBytes / row_bytes, 1), std::min(rows, 65535)));
+  u64* cand = nullptr;
+  JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&cand), group * row_bytes, st));
+  int rc = 0;
+  for (int r0 = 0; r0 < rows && rc == 0; r0 += group) {
+    const int g = std::min(group, rows - r0);
+    const float* x = logits + static_cast<size_t>(r0) * ld;
+    const size_t o = static_cast<size_t>(r0) * k;
+    rc = launch_segments(x, g, cols, ld, kSegCols, k, 0, lo, cand, cand_ld, nullptr, nullptr, nullptr, st);
+    if (rc == 0) rc = launch_merge(cand, g, cand_ld, cand_ld, k, lo, nullptr, x, cols, ld, values + o, indices + o, probs ? probs + o : nullptr, st);
+  }
+  return free_scratch(cand, st, rc);
+}
+
+// Gallery search: the scores of a chunk of queries against a chunk of gallery rows are the contrastive head's own -- the same
+// l2_normalize and logits kernels, so every score is the bit pattern model(x, t) holds at that (image, text) pair -- written to a
+// bounded score block and reduced at once to k candidates per (query, segment).  Each query's candidate row holds its running best
+// k in slot 0 and the current chunk's segments after it; one merge per gallery chunk folds them back into slot 0, and the last one
+// writes the outputs.  Scratch is the same for every N: kSearchRows x (E + kSearchCols) floats, kSearchCols x E floats and
+// kSearchRows x (1 + kSearchCols / kSegCols) x k candidates -- at most about 450 MB at E = 768 and k = 1024.  The block costs 8 bytes
+// of memory traffic per score against 2E FMA flops, so the search stays bound by the FMAs.
+int search_run(const float* queries, int Q, const float* gallery, int N, int E, const float* logit_scale, const float* logit_bias, int k,
+               float* values, int32_t* indices, cudaStream_t st) {
+  constexpr int kSearchRows = 2048, kSearchCols = 32768;
+  static_assert(kSearchCols % kSegCols == 0 && kSearchCols >= kSelectMaxK, "a chunk is whole segments and holds k candidates");
+  const int qc = std::min(Q, kSearchRows), gc = std::min(N, kSearchCols);
+  const long long cand_ld = (1 + (gc + kSegCols - 1) / kSegCols) * static_cast<long long>(k);
+  const size_t cand_bytes = (static_cast<size_t>(qc) * cand_ld * sizeof(u64) + 255) / 256 * 256;  // the float rows start 16-byte aligned
+  const size_t floats = static_cast<size_t>(qc) * E + static_cast<size_t>(gc) * E + static_cast<size_t>(qc) * gc;
+  u64* cand = nullptr;
+  JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&cand), cand_bytes + floats * sizeof(float), st));
+  float* nq = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(cand) + cand_bytes);
+  float* ng = nq + static_cast<size_t>(qc) * E;
+  float* block = ng + static_cast<size_t>(gc) * E;
+  const int lo = bit_width(N);
+  int rc = 0;
+  for (int q0 = 0; q0 < Q && rc == 0; q0 += qc) {
+    const int qn = std::min(qc, Q - q0);
+    rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
+    for (int g0 = 0; g0 < N && rc == 0; g0 += gc) {
+      const int gn = std::min(gc, N - g0);
+      const bool first = g0 == 0, last = N - g0 == gn;
+      const long long segs = (gn + kSegCols - 1) / kSegCols;
+      const size_t o = static_cast<size_t>(q0) * k;
+      if (rc == 0) rc = l2_normalize_run(gallery + static_cast<size_t>(g0) * E, ng, E, gn, E, st);
+      if (rc == 0) rc = logits_run(nq, ng, logit_scale, logit_bias, block, qn, gn, E, gn, st);
+      if (rc == 0) rc = launch_segments(block, qn, gn, gn, kSegCols, k, g0, lo, cand + k, cand_ld, nullptr, nullptr, nullptr, st);
+      if (rc == 0)
+        rc = launch_merge(first ? cand + k : cand, qn, cand_ld, (first ? 0 : k) + segs * k, k, lo, last ? nullptr : cand, nullptr, 0, 0,
+                          last ? values + o : nullptr, last ? indices + o : nullptr, nullptr, st);
+    }
+  }
+  return free_scratch(cand, st, rc);
+}
+
 }  // namespace jimm
 
 using namespace jimm;
@@ -254,4 +573,12 @@ extern "C" int jimm_postprocess(const float* logits, int rows, int cols, int ld,
   }
   if (order && wide) return sort_wide_rows(logits, rows, cols, ld, order, st);
   return 0;
+}
+
+extern "C" int jimm_topk(const float* logits, int rows, int cols, int ld, int k, float* values, int32_t* indices, float* probs, void* stream) {
+  if (rows < 0 || cols <= 0 || ld < cols) { set_last_error("top_k: bad shape rows=%d cols=%d ld=%d", rows, cols, ld); return JIMM_EINVAL; }
+  if (k < 1 || k > cols) { set_last_error("top_k: k=%d outside 1 .. cols=%d", k, cols); return JIMM_EINVAL; }
+  if (rows > 0 && (!logits || !values || !indices)) { set_last_error("top_k: null logits, values or indices"); return JIMM_EINVAL; }
+  if (rows == 0) return 0;
+  return topk_run(logits, rows, cols, ld, k, values, indices, probs, static_cast<cudaStream_t>(stream));
 }

@@ -131,6 +131,14 @@ class DualTower(_NativeOwner, nn.Module):
         n = self.native(max(len(im.x), Bt), require=True, hw=im.hw if interpolate_pos_encoding else None)
         return n.dual(im, text)
 
+    def search(self, queries, gallery, k: int):
+        """Top-k retrieval without the score matrix: for each query embedding its k best gallery embeddings by this model's logit,
+        `scores, indices` ([Q, k] fp32 and int32).  queries [Q, E] and gallery [N, E] are encode_image / encode_text outputs, either
+        side either tower, fp32 / fp16 / bf16 on the device or the host (host results when both are on the host).  Bit for bit,
+        search(encode_image(x), encode_text(t), k) == top_k(model(x, t), k) and search(encode_text(t), encode_image(x), k) ==
+        top_k(model(x, t).T, k), at any Q and N; 1 <= k <= min(N, 1024).  Single GPU."""
+        return self.native().search(queries, gallery, k)
+
     def set_comm(self, mode: str):
         """'peer' (default, fused NVLink peer-store kernel) | 'nccl' (torch.distributed all_gather baseline) | 'off'."""
         if mode not in ("peer", "nccl", "off"):
