@@ -492,6 +492,34 @@ JIMM_API int jimm_topk(const float* logits, int rows, int cols, int ld, int k, f
  * at E <= 1024 for any N).  E is the model's embedding width; 1 <= k <= min(N, 1024). */
 JIMM_API int jimm_search(jimm_model_t* m, const float* queries, int Q, const float* gallery, int N, int k, float* values, int32_t* indices,
                          void* stream);
+/* Gallery index of a CLIP / SigLIP model: a gallery normalised once and kept on the device, searched many times.
+ * jimm_index_create: an empty index for m's embedding width E (a multiple of 8 up to 8192, which every model width is) on m's device.
+ *   jimm_index_add and jimm_index_search read the model the index is bound to (its logit_scale / logit_bias at every search), so that
+ *   model must outlive every such call.
+ * jimm_index_rebind: binds the index to another model of the same width on the same device (JIMM_EINVAL otherwise), e.g. the handle
+ *   rebuilt from the same parameters; the stored rows stay.  After the bound model is destroyed, only jimm_index_rebind and
+ *   jimm_index_destroy may be called.
+ * jimm_index_add: appends n rows (device fp32 [n, E], un-normalised embeddings as jimm_search's gallery); row numbering continues.
+ *   The index stores each row normalised by the contrastive head's l2_normalize (fp32), an fp16 copy and an upper bound on the
+ *   normalised row's norm: 6 E + 4 bytes per row, in storage that grows geometrically.  At most 2^31 - 1 rows in all.
+ * jimm_index_search: jimm_search(m, queries, Q, all rows added so far, N, k, ...) bit for bit, 1 <= k <= min(N, 1024).  Each query's
+ *   exact best k over the first 32768 rows seeds a threshold; the other rows are screened in fp16 on the tensor cores against it with a
+ *   proven error bound, and only the rows that can still reach the best k are scored exactly (see INTEGRATION.md, "Gallery index").
+ *   stats (nullable, host) receives the work done.  The call waits for `stream` once per screened chunk of 65536 rows.
+ * Adds and searches on different streams must be ordered by the caller.  jimm_index_destroy waits for the index's device; it never
+ * reads the model. */
+typedef struct jimm_index jimm_index_t;
+typedef struct jimm_search_stats {
+  long long rows_rescored;    /* (query, row) pairs the screen passed and the rescorer scored exactly */
+  long long fallbacks;        /* (query, screen chunk) pairs that passed too many rows and went through the exact block step */
+  long long chunks_screened;  /* screen launches: (query chunk of up to 2048, gallery chunk of up to 65536) pairs */
+} jimm_search_stats;
+JIMM_API int jimm_index_create(jimm_model_t* m, jimm_index_t** out);
+JIMM_API int jimm_index_rebind(jimm_index_t* idx, jimm_model_t* m);
+JIMM_API int jimm_index_add(jimm_index_t* idx, const float* rows, int n, void* stream);
+JIMM_API int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, float* values, int32_t* indices, jimm_search_stats* stats,
+                               void* stream);
+JIMM_API int jimm_index_destroy(jimm_index_t* idx);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads
  * its own 16 KB tiles; 1: the CTAs of a cluster load the same tile each; 2: same tile, each loads 1/cluster of it and multicasts. */
 JIMM_API int jimm_k_l2_probe(const void* buf, int rows, int mode, int cluster, int iters, float* ms, void* stream);

@@ -56,6 +56,12 @@ class AttnReq(C.Structure):
     _fields_ = [("n", C.c_int), ("blocks", C.POINTER(C.c_int)), ("out", C.POINTER(C.c_void_p)), ("out_dtype", C.c_int)]
 
 
+class SearchStats(C.Structure):
+    """jimm_search_stats: the work of one jimm_index_search"""
+
+    _fields_ = [("rows_rescored", C.c_longlong), ("fallbacks", C.c_longlong), ("chunks_screened", C.c_longlong)]
+
+
 # name -> (restype, argtypes): every symbol include/jimm_b200.h declares
 class PreprocConfig(C.Structure):
     """jimm_preproc_config_t"""
@@ -153,6 +159,11 @@ SIGNATURES = {
     "jimm_postprocess": (_i, [_fp, _i, _i, _i, _i, _fp, _i, _ip, _ip, _vp]),
     "jimm_topk": (_i, [_fp, _i, _i, _i, _i, _fp, _ip, _fp, _vp]),
     "jimm_search": (_i, [_vp, _fp, _i, _fp, _i, _i, _fp, _ip, _vp]),
+    "jimm_index_create": (_i, [_vp, C.POINTER(_vp)]),
+    "jimm_index_rebind": (_i, [_vp, _vp]),
+    "jimm_index_add": (_i, [_vp, _fp, _i, _vp]),
+    "jimm_index_search": (_i, [_vp, _fp, _i, _i, _fp, _ip, C.c_void_p, _vp]),
+    "jimm_index_destroy": (_i, [_vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),

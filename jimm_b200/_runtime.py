@@ -6,7 +6,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
-from typing import Dict, List, NamedTuple, Optional, Tuple, Union
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -538,23 +538,31 @@ class NativeModel:
         self._run("jimm_contrastive_logits", img_e, Bi, txt_e, Bt, out)
         return out
 
+    def _embeddings(self, name: str, x) -> torch.Tensor:
+        """A [rows, E] embedding set of a search or an index, checked: float32 / float16 / bfloat16, at most 2^31 - 1 rows."""
+        t = _as_tensor(x)
+        E = self.text_out
+        if t.ndim != 2 or t.shape[1] != E:
+            raise ValueError(f"search: expected {name} of shape [rows, {E}] (the model's embedding width), got {tuple(t.shape)}")
+        if t.dtype not in _TORCH_TO_CODE:
+            raise ValueError(f"search: {name} must be float32, float16 or bfloat16, got {t.dtype}")
+        if t.shape[0] > 2**31 - 1:
+            raise ValueError(f"search: at most {2**31 - 1} {name} rows, got {t.shape[0]}")
+        return t
+
+    @staticmethod
+    def _search_k(k, N: int) -> int:
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= min(N, 1024):
+            raise ValueError(f"search: k must be an int in 1 .. min(gallery rows={N}, 1024), got {k!r}")
+        return int(k)
+
     def search(self, queries, gallery, k: int):
         """The k best gallery rows of each query by the model's score (jimm_search): fp32 [Q, k] scores and int32 [Q, k] indices,
         bit for bit the top_k of the logits matrix the contrastive head would give for the two sets.  Both [*, E] embedding sets of
         float32 / float16 / bfloat16 on the device or the host; the result is on the host when both were."""
-        q, g = _as_tensor(queries), _as_tensor(gallery)
-        E = self.text_out
-        for name, t in (("queries", q), ("gallery", g)):
-            if t.ndim != 2 or t.shape[1] != E:
-                raise ValueError(f"search: expected {name} of shape [rows, {E}] (the model's embedding width), got {tuple(t.shape)}")
-            if t.dtype not in _TORCH_TO_CODE:
-                raise ValueError(f"search: {name} must be float32, float16 or bfloat16, got {t.dtype}")
-            if t.shape[0] > 2**31 - 1:
-                raise ValueError(f"search: at most {2**31 - 1} {name} rows, got {t.shape[0]}")
+        q, g = self._embeddings("queries", queries), self._embeddings("gallery", gallery)
         Q, N = q.shape[0], g.shape[0]
-        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= min(N, 1024):
-            raise ValueError(f"search: k must be an int in 1 .. min(gallery rows={N}, 1024), got {k!r}")
-        k = int(k)
+        k = self._search_k(k, N)
         host = not q.is_cuda and not g.is_cuda
         qd = q.to(self.device, torch.float32, non_blocking=True).contiguous()
         gd = g.to(self.device, torch.float32, non_blocking=True).contiguous()
@@ -562,6 +570,11 @@ class NativeModel:
         indices = torch.empty((Q, k), dtype=torch.int32, device=self.device)
         self._run("jimm_search", qd, Q, gd, N, k, values, indices)
         return self._back(values, host).result(), self._back(indices, host).result()
+
+    def index(self, gallery=None) -> "GalleryIndex":
+        """A gallery index on this handle (jimm_index_create), holding `gallery`'s rows when given; it raises once this handle is
+        closed."""
+        return GalleryIndex(lambda: self, gallery)
 
     def dual(self, images, text, interpolate: bool = False) -> torch.Tensor:
         """CLIP.__call__ / SigLIP.__call__ on one GPU, on Images or on a tensor / list prepared here, and on a [B, T] ids tensor or a
@@ -615,6 +628,78 @@ class NativeModel:
         out = torch.empty((B, world * B), dtype=torch.float32, device=self.device)
         self._run("jimm_comm_contrastive_logits", img_e, txt_e, B, out)
         return out
+
+
+class GalleryIndex:
+    """A gallery normalised once and kept on the GPU (jimm_index_*): search(queries, k) is NativeModel.search(queries, every row added
+    so far, k) on the model's current handle, bit for bit.  `native` returns that handle: a model's `native` method, which rebuilds it
+    when its parameters or batch bound change.  Each add / search rebinds the index to the handle `native` gives (jimm_index_rebind,
+    same width and device; the stored rows stay), so it scores with the model's current logit_scale / logit_bias and never reads a
+    handle the model has destroyed.  Holding `native` keeps the model alive."""
+
+    def __init__(self, native: Callable[[], NativeModel], gallery=None):
+        self._native = native
+        m = native()
+        self._bound, self._lib, self._device = m, m.lib, m.device
+        self.handle = C.c_void_p()
+        _lib.check(m.lib.jimm_index_create(m.handle, C.byref(self.handle)))
+        self._rows = 0
+        if gallery is not None:
+            self.add(gallery)
+
+    def _model(self) -> NativeModel:
+        """The handle the index scores with now, bound to it."""
+        if not self.handle:
+            raise _lib.JimmError("gallery index: closed")
+        m = self._native()
+        if not m.handle:
+            raise _lib.JimmError("gallery index: its model handle has been closed")
+        if m is not self._bound:
+            _lib.check(self._lib.jimm_index_rebind(self.handle, m.handle))
+            self._bound = m
+        return m
+
+    def add(self, rows) -> "GalleryIndex":
+        """Append [n, E] embeddings (float32 / float16 / bfloat16, device or host); their indices continue from len(self)."""
+        m = self._model()
+        g = m._embeddings("gallery", rows)
+        n = g.shape[0]
+        if self._rows + n > 2**31 - 1:
+            raise ValueError(f"index: at most {2**31 - 1} rows, {self._rows} + {n} given")
+        gd = g.to(m.device, torch.float32, non_blocking=True).contiguous()
+        _call(m.lib, m.device, "jimm_index_add", self.handle, gd, n)
+        self._rows += n
+        return self
+
+    def __len__(self) -> int:
+        return self._rows
+
+    def search(self, queries, k: int):
+        """The k best rows of the index for each query: fp32 [Q, k] scores and int32 [Q, k] row indices, on the host when the queries
+        were."""
+        m = self._model()
+        q = m._embeddings("queries", queries)
+        k = m._search_k(k, self._rows)
+        Q = q.shape[0]
+        qd = q.to(m.device, torch.float32, non_blocking=True).contiguous()
+        values = torch.empty((Q, k), dtype=torch.float32, device=m.device)
+        indices = torch.empty((Q, k), dtype=torch.int32, device=m.device)
+        _call(m.lib, m.device, "jimm_index_search", self.handle, qd, Q, k, values, indices, None)
+        host = not q.is_cuda
+        return m._back(values, host).result(), m._back(indices, host).result()
+
+    def close(self):
+        """Free the stored rows (jimm_index_destroy reads only the index's own device, never the model)."""
+        if getattr(self, "handle", None):
+            with torch.cuda.device(self._device):
+                self._lib.jimm_index_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class NativeSubModule:

@@ -26,6 +26,8 @@
 //       never reads the residual).
 //   OUT_GENERIC: everything else (position-embedding row-add + row remap of the patch GEMM, heads with unaligned N,
 //       fp32 stores to caller buffers): LSU stores from the registers, run-time flags.
+//   OUT_SCREEN: the gallery index's screen (fp16 only): no output, each (row, column) whose score may reach the row's threshold is
+//       appended to the row's candidate list (see "screening epilogue").
 //
 // Reference ops served (SURVEY.md 8a): a1 patch-embed conv-as-GEMM (common/vit.py:153-165,228-236),
 // a4 fused q/k/v projections (common/transformer.py:67-79), a6 out-proj + residual (:130),
@@ -59,7 +61,7 @@ static constexpr int EPI_STAGE_BYTES = EPI_WARPS * EPI_BUFS * EPI_BUF_BYTES;  //
 static constexpr int NUM_THREADS = 384;
 static constexpr int KERNEL_REGS = 168;  // per thread at launch: 64 K registers / 384 threads, in the allocation unit of 8
 
-enum OutKind : int { OUT_GENERIC = 0, OUT_H16 = 1, OUT_BF16 = 2, OUT_TF32 = 3, OUT_F32_ADD = 4, OUT_F32 = 5 };
+enum OutKind : int { OUT_GENERIC = 0, OUT_H16 = 1, OUT_BF16 = 2, OUT_TF32 = 3, OUT_F32_ADD = 4, OUT_F32 = 5, OUT_SCREEN = 6 };
 
 struct EpiDev {
   const float* bias;
@@ -79,6 +81,8 @@ struct EpiDev {
   float ln_eps;
   const float* a_scale;  // e4m3 operands: dequantisation scales (see GemmEpilogue)
   const float* b_scale;
+  // OUT_SCREEN reads its GemmScreen from the fields above (gemm_screen_run): t = bias, nq = a_scale, ng = b_scale, cnt = ln_cnt,
+  // list = out, cap = ldo.  The struct keeps its size, so every other kernel's parameters keep their offsets.
 };
 
 template <int ACT>
@@ -385,6 +389,52 @@ __device__ __forceinline__ void epilogue_generic(const EpiDev& epi, const float 
   }
 }
 
+// ---- screening epilogue of the gallery index (fp16 operands) ------------------------------------------------------------------------
+// A row i is a normalised query q (fp32) rounded to fp16 as q^, B row j a normalised gallery row g rounded as g^; nq >= ||q||_2 and
+// ng >= ||g||_2 are the index's norm bounds (+inf for a row with a non-finite value, whose fp16 copy is zeros).  The exact score's
+// accumulator is acc = the fp32 fmaf chain of q_k g_k, k ascending (logits_tile); the screen holds a = the wgmma's sum of q^_k g^_k.
+// delta >= |a - acc|, with u = 2^-11 (fp16 unit roundoff), s = 2^-25 sqrt(E) and E = K:
+//   * the fp16 operands: q^_k = q_k (1 + e) + h with |e| <= u, |h| <= 2^-25 (half the fp16 subnormal step), likewise g^_k, so
+//     |sum q^ g^ - sum q g| <= (2u + u^2) sum |q g| + (1 + 2u) 2^-25 (sum |q| + sum |g|) + E 2^-50
+//                           <= (2u + u^2) nq ng + (1 + 2u) s (nq + ng) + E 2^-50              (Cauchy-Schwarz, sum |q| <= sqrt(E) ||q||);
+//   * the fmaf chain, one rounding per step: |acc - sum q g| <= gamma_E sum |q g| <= gamma_E nq ng, gamma_E = E 2^-24 / (1 - E 2^-24);
+//   * the tensor core's own accumulation, not assumed to be IEEE: |a - sum q^ g^| <= c_tc sum |q^ g^| <= c_tc nq^ ng^ with
+//     nq^ = (1 + u) nq + s >= ||q^||, so <= c_tc ((1 + u)^2 nq ng + (1 + u) s (nq + ng) + s^2).  c_tc = E 2^-22; the GPU tests measure
+//     the fp16 wgmma's accumulation against that constant on adversarial operands.
+// So delta = c1 nq ng + c2 (nq + ng) + c3 with c1 = 2u + u^2 + gamma_E + c_tc (1 + u)^2, c2 = (1 + 2u) s + c_tc (1 + u) s and
+// c3 = E 2^-50 + c_tc s^2, computed in double and rounded up by 2^-20 relative (screen_bound, gemm.cuh), which covers the
+// four fp32 roundings of the expression below.  At E = 768: c1 = 1.2e-3.  Then acc >= t implies a + delta >= acc >= t, and
+// fl(a + delta) >= t (t is a float, rounding is monotone): a row is dropped only if acc < t.  A non-finite bound makes delta +inf or
+// NaN, and `!(a + delta < t)` keeps the row.
+template <int NC>
+__device__ __forceinline__ void epilogue_screen(const EpiDev& epi, const float (&acc)[NC / 2], int lane, int row_base, int n_tile0, int K) {
+  const ScreenBound c = screen_bound(K);
+  int* list = static_cast<int*>(epi.out);
+  const int g = lane >> 2, t4 = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row_base + g + 8 * h;
+    if (row >= epi.M) continue;
+    const float t = __ldg(epi.bias + row), nq = __ldg(epi.a_scale + row);
+    const float d0 = c.c1 * nq, d1 = c.c2 * nq + c.c3;
+#pragma unroll
+    for (int j = 0; j < NC / 8; ++j) {
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int col = n_tile0 + 8 * j + 2 * t4 + q;
+        if (col < epi.N) {
+          const float ng = __ldg(epi.b_scale + col);
+          const float delta = fmaf(d0, ng, fmaf(c.c2, ng, d1));
+          if (!(acc[4 * j + 2 * h + q] + delta < t)) {
+            const int pos = atomicAdd(epi.ln_cnt + row, 1);
+            if (pos < epi.ldo) list[static_cast<size_t>(row) * epi.ldo + pos] = col;
+          }
+        }
+      }
+    }
+  }
+}
+
 // ---- e4m3 operands ---------------------------------------------------------------------------------------------------------------
 // The e4m3 wgmma does not accumulate in full fp32: its sums of products lose low-order bits (about 5e-4 of sum |a b| at K = 768..2048
 // on an H100, measured with m64n256k32), which puts an FP8 model at about a third of its whole FP8 error away from an exact-accumulation
@@ -440,7 +490,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   if (warp_idx == 0 && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    if constexpr (OUT != OUT_GENERIC) tma_prefetch_desc(&map_c);
+    if constexpr (OUT != OUT_GENERIC && OUT != OUT_SCREEN) tma_prefetch_desc(&map_c);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], EPI_WARPS);
@@ -540,6 +590,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       const int n_tile0 = n_blk * BN + wg * WG_DN;
       if constexpr (OUT == OUT_GENERIC) {
         epilogue_generic<SCALED, NC>(epi, acc, lane, row_base, n_tile0);
+      } else if constexpr (OUT == OUT_SCREEN) {
+        epilogue_screen<NC>(epi, acc, lane, row_base, n_tile0, K);
       } else {
         // split by columns, a consumer warpgroup's columns can lie wholly past N
         if (row_base < M && (WG_DN == 0 || n_tile0 < N))
@@ -560,7 +612,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         atomicAdd(&lnq->done, 1);
       }
     }
-    if constexpr (OUT != OUT_GENERIC) {
+    if constexpr (OUT != OUT_GENERIC && OUT != OUT_SCREEN) {
       if (lane == 0) tma_store_wait_all();
     }
   }
@@ -841,6 +893,24 @@ int gemm_plan_run(const GemmPlan* p0, int M_override, cudaStream_t stream, int r
   }
   set_last_error("gemm: bad dtype %d", p->dtype);
   return -1;
+}
+
+int gemm_screen_run(const void* A, int M, const void* B, int N, int K, const GemmScreen& screen, cudaStream_t stream) {
+  if (M <= 0 || N <= 0 || K <= 0) { set_last_error("gemm screen: bad shape %dx%dx%d", M, N, K); return -1; }
+  if (!screen.t || !screen.nq || !screen.ng || !screen.cnt || !screen.list || screen.cap < 1) {
+    set_last_error("gemm screen: null threshold, bound, counter or list, or cap < 1");
+    return -1;
+  }
+  GemmPlan p;
+  if (int rc = make_tensor_map_2d(&p.map_a, DT_F16, A, M, K, K, tile_rows(DT_F16))) return rc;
+  if (int rc = make_tensor_map_2d(&p.map_b, DT_F16, B, N, K, K, BN)) return rc;
+  memset(&p.map_c, 0, sizeof(p.map_c));
+  p.M = M; p.N = N; p.K = K; p.dtype = DT_F16;
+  // the screen travels in the epilogue fields epilogue_screen reads (see EpiDev)
+  p.epi.mode = 0;
+  p.epi.bias = screen.t; p.epi.a_scale = screen.nq; p.epi.b_scale = screen.ng; p.epi.ln_cnt = screen.cnt;
+  p.epi.out = screen.list; p.epi.ldo = screen.cap;
+  return launch_one<__half, OUT_SCREEN, ACT_NONE>(&p, M, stream);
 }
 
 int gemm_simt_run(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmEpilogue& epi,

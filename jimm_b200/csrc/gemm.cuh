@@ -9,6 +9,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 namespace jimm {
@@ -65,6 +66,34 @@ struct GemmEpilogue {
   const float* b_scale = nullptr;
 };
 
+// Screening epilogue of the gallery index (fp16 operands; see epilogue_screen in gemm.cu): no output is written.  Column j of row i is
+// kept when acc_ij + delta_ij >= t[i] (or the comparison is unordered), delta_ij = c1 nq[i] ng[j] + c2 (nq[i] + ng[j]) + c3 at K = E
+// (screen_bound); a kept j goes to list[i * cap + atomicAdd(&cnt[i], 1)] when that slot is below cap.  cnt[i] > cap afterwards means
+// row i's list overflowed.
+struct GemmScreen {
+  const float* t = nullptr;   // [M] per-row thresholds
+  const float* nq = nullptr;  // [M] row norm bounds of A
+  const float* ng = nullptr;  // [N] row norm bounds of B
+  int* cnt = nullptr;         // [M] zero before the launch
+  int* list = nullptr;        // [M, cap] column indices
+  int cap = 0;
+};
+
+// c_tc / E: the bound on the fp16 wgmma's accumulation error per unit of sum |q^ g^| and of K (measured by the GPU tests)
+constexpr double kTcAccumPerK = 0x1p-22;
+
+// The screen's bound delta = c1 nq ng + c2 (nq + ng) + c3 on |fp16 wgmma sum - fp32 fmaf chain| at width E (derivation at
+// epilogue_screen, gemm.cu), each constant rounded up by 2^-20 relative.
+struct ScreenBound {
+  float c1, c2, c3;
+};
+__host__ __device__ inline ScreenBound screen_bound(int E) {
+  const double u = 0x1p-11, s = 0x1p-25 * sqrt(static_cast<double>(E)), gam = E * 0x1p-24 / (1.0 - E * 0x1p-24), ctc = E * kTcAccumPerK;
+  const double up = 1.0 + 0x1p-20;
+  return {static_cast<float>((2 * u + u * u + gam + ctc * (1 + u) * (1 + u)) * up), static_cast<float>(((1 + 2 * u) * s + ctc * (1 + u) * s) * up),
+          static_cast<float>((E * 0x1p-50 + ctc * s * s) * up)};
+}
+
 struct GemmPlan {
   CUtensorMap map_a, map_b, map_c;  // map_c: output (mode 2 only)
   int M = 0, N = 0, K = 0;
@@ -89,6 +118,10 @@ int gemm_plan_run(const GemmPlan* plan, int M_override, cudaStream_t stream, int
 // unless JIMM_GEMM_IMPL=simt is set for bisection).
 int gemm_simt_run(int dtype, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmEpilogue& epi,
                   cudaStream_t stream);
+
+// The screen of the gallery index: fp16 A [M, K] . B [N, K]^T (both K-major, row stride K, 16-byte aligned) on the same mainloop, ring,
+// tiles and schedule as every other 16-bit GEMM, through the GemmScreen epilogue.
+int gemm_screen_run(const void* A, int M, const void* B, int N, int K, const GemmScreen& screen, cudaStream_t stream);
 
 // 1 when gemm_plan_run(plan, M_override) will apply the plan's fused LayerNorm (fp32 reduce-add epilogue)
 int gemm_fuses_ln(const GemmPlan* plan, int M_override);

@@ -86,6 +86,20 @@ int topk_run(const float* logits, int rows, int cols, int ld, int k, float* valu
 int search_run(const float* queries, int Q, const float* gallery, int N, int E, const float* logit_scale, const float* logit_bias, int k,
                float* values, int32_t* indices, cudaStream_t stream);
 
+// Gallery index (postprocess.cu): rows of width E (a multiple of 8 up to 8192, as every model width is) normalised once and stored with
+// an fp16 copy and per-row norm bounds; a search screens them on the tensor cores and rescores the survivors exactly, and gives search_run's bits for the same queries against
+// every row added so far (1 <= k <= min(rows, 1024)).  The store's memory is allocated in stream order on the add's stream; the caller
+// orders adds and searches on different streams.  stats (nullable, zeroed by the caller): rows rescored, (query, chunk) pairs that fell
+// back to the exact block step, and chunks screened.  A search waits for its stream once per screened chunk.
+struct GalleryStore;
+int gallery_create(int E, GalleryStore** out);
+long long gallery_rows(const GalleryStore* g);
+int gallery_width(const GalleryStore* g);
+int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t stream);
+int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, float* values,
+                   int32_t* indices, long long* stats, cudaStream_t stream);
+void gallery_destroy(GalleryStore* g);
+
 // dst[n*K + k] = cast(src[k*N + n])   (flax (in,out) kernel -> K-major [N,K] operand)
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);
 int cast_run(const float* src, void* dst, int out_type, size_t n, cudaStream_t stream);

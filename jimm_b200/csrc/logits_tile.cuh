@@ -13,6 +13,10 @@ namespace jimm {
 
 static constexpr int LOGITS_LDS = 68;  // shared-memory row stride (floats)
 
+// The logit of one pair from its dot-product accumulator: one fused multiply-add, fl(sc * acc + bs), rounded once.  The gallery
+// index's rescorer (postprocess.cu) computes its scores through this same function, so they are these bits.
+__device__ __forceinline__ float logit_value(float sc, float acc, float bs) { return __fmaf_rn(sc, acc, bs); }
+
 // out[i, j] = sc * <A[i, :E], B[j, :E]> + bs   for the 64x64 tile at (i0, j0); row strides lda / ldb / ldl (elements).
 // CG_LOADS: read the operands with ld.global.cg (data written by peer GPUs into local memory; bypass L1).
 template <bool CG_LOADS>
@@ -74,7 +78,7 @@ __device__ __forceinline__ void logits_tile(const float* __restrict__ A, size_t 
 #pragma unroll
     for (int w = 0; w < 4; ++w) {
       const int i = i0 + ty * 4 + u, j = j0 + tx * 4 + w;
-      if (i < Bi && j < Bt) out[static_cast<size_t>(i) * ldl + j] = sc * acc[u][w] + bs;
+      if (i < Bi && j < Bt) out[static_cast<size_t>(i) * ldl + j] = logit_value(sc, acc[u][w], bs);
     }
 }
 

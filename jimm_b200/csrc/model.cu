@@ -1860,6 +1860,70 @@ int jimm_search(jimm_model_t* m, const float* queries, int Q, const float* galle
   return search_run(queries, Q, gallery, N, m->txt.D, m->logit_scale, m->logit_bias, k, values, indices, static_cast<cudaStream_t>(stream));
 }
 
+// The gallery index: the model it scores with, the device its rows live on and the stored rows (postprocess.cu owns their formats).
+// Only add and search read m; destroy needs the device alone, so an index outlives a model it has been rebound away from.
+struct jimm_index {
+  jimm_model* m = nullptr;
+  int device = 0;
+  GalleryStore* store = nullptr;
+};
+
+int jimm_index_create(jimm_model_t* m, jimm_index_t** out) {
+  JIMM_TRY(check_ready(m, 0));
+  JIMM_TRY(check_text(m));
+  if (!out) { set_last_error("index: null output handle"); return JIMM_EINVAL; }
+  GalleryStore* store = nullptr;
+  JIMM_TRY(gallery_create(m->txt.D, &store));
+  *out = new jimm_index{m, m->device, store};
+  return 0;
+}
+
+int jimm_index_rebind(jimm_index_t* idx, jimm_model_t* m) {
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  JIMM_TRY(check_ready(m, 0));
+  JIMM_TRY(check_text(m));
+  if (m->device != idx->device || m->txt.D != gallery_width(idx->store)) {
+    set_last_error("index rebind: the model (device %d, width %d) does not match the index (device %d, width %d)", m->device, m->txt.D,
+                   idx->device, gallery_width(idx->store));
+    return JIMM_EINVAL;
+  }
+  idx->m = m;
+  return 0;
+}
+
+int jimm_index_add(jimm_index_t* idx, const float* rows, int n, void* stream) {
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  if (n < 0 || (n > 0 && !rows)) { set_last_error("index add: n=%d rows=%p", n, static_cast<const void*>(rows)); return JIMM_EINVAL; }
+  if (gallery_rows(idx->store) + n > 2147483647ll) {
+    set_last_error("index add: %lld + %d rows exceed 2^31 - 1", gallery_rows(idx->store), n);
+    return JIMM_EINVAL;
+  }
+  JIMM_TRY(set_device(idx->m));
+  return gallery_add(idx->store, rows, n, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, float* values, int32_t* indices, jimm_search_stats* stats, void* stream) {
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  jimm_model* m = idx->m;
+  JIMM_TRY(check_ready(m, Q));
+  const long long N = gallery_rows(idx->store);
+  if (N < 1 || k < 1 || k > N || k > 1024) { set_last_error("search: k=%d outside 1 .. min(N=%lld, 1024)", k, N); return JIMM_EINVAL; }
+  if (Q > 0 && (!queries || !values || !indices)) { set_last_error("search: null queries, values or indices"); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  long long st[3] = {0, 0, 0};
+  const int rc = Q == 0 ? 0 : gallery_search(idx->store, queries, Q, m->logit_scale, m->logit_bias, k, values, indices, st, static_cast<cudaStream_t>(stream));
+  if (stats) { stats->rows_rescored = st[0]; stats->fallbacks = st[1]; stats->chunks_screened = st[2]; }
+  return rc;
+}
+
+int jimm_index_destroy(jimm_index_t* idx) {
+  if (!idx) return 0;
+  JIMM_CUDA_CHECK(cudaSetDevice(idx->device));
+  gallery_destroy(idx->store);
+  delete idx;
+  return 0;
+}
+
 // Fork the text tower onto the model's side stream (ordered after everything already enqueued on `s`), returning the stream it runs
 // on; join_text() makes `s` wait for it.  Profiling (per-GEMM events) and JIMM_DUAL_STREAMS=0 keep the towers on one stream.
 static int fork_text(jimm_model* m, cudaStream_t s, cudaStream_t* ts) {

@@ -10,10 +10,12 @@
 // so any correct descending sort of them is numpy's stable argsort reversed, and the maximum of (order_key, -index) is the first
 // maximum.
 #include <algorithm>
+#include <cfloat>
 
 #include "../../include/jimm_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
+#include "logits_tile.cuh"
 
 namespace jimm {
 namespace {
@@ -467,6 +469,24 @@ int free_scratch(void* p, cudaStream_t st, int rc) {
   return rc;
 }
 
+// The exact block step of a search: the scores of qn normalised queries nq against gn normalised gallery rows ng (gallery rows g0 ..
+// g0 + gn - 1) through the contrastive head's logits kernel into `block` [qn, gn], reduced to k candidates per segment in each cand row
+// after slot 0, and merged into slot 0, the row's running best k (first: there is none yet).  last: the merge writes values / indices
+// (row stride k) instead.
+constexpr int kSearchRows = 2048, kSearchCols = 32768;  // one score block: queries x gallery rows
+static_assert(kSearchCols % kSegCols == 0 && kSearchCols >= kSelectMaxK, "a chunk is whole segments and holds k candidates");
+
+int block_step(const float* nq, int qn, const float* ng, int gn, int g0, int E, const float* logit_scale, const float* logit_bias, int k, int lo,
+               float* block, u64* cand, long long cand_ld, bool first, bool last, float* values, int32_t* indices, cudaStream_t st) {
+  const long long segs = (gn + kSegCols - 1) / kSegCols;
+  int rc = logits_run(nq, ng, logit_scale, logit_bias, block, qn, gn, E, gn, st);
+  if (rc == 0) rc = launch_segments(block, qn, gn, gn, kSegCols, k, g0, lo, cand + k, cand_ld, nullptr, nullptr, nullptr, st);
+  if (rc == 0)
+    rc = launch_merge(first ? cand + k : cand, qn, cand_ld, (first ? 0 : k) + segs * k, k, lo, last ? nullptr : cand, nullptr, 0, 0,
+                      last ? values : nullptr, last ? indices : nullptr, nullptr, st);
+  return rc;
+}
+
 }  // namespace
 
 int topk_run(const float* logits, int rows, int cols, int ld, int k, float* values, int32_t* indices, float* probs, cudaStream_t st) {
@@ -517,8 +537,6 @@ int topk_run(const float* logits, int rows, int cols, int ld, int k, float* valu
 // of memory traffic per score against 2E FMA flops, so the search stays bound by the FMAs.
 int search_run(const float* queries, int Q, const float* gallery, int N, int E, const float* logit_scale, const float* logit_bias, int k,
                float* values, int32_t* indices, cudaStream_t st) {
-  constexpr int kSearchRows = 2048, kSearchCols = 32768;
-  static_assert(kSearchCols % kSegCols == 0 && kSearchCols >= kSelectMaxK, "a chunk is whole segments and holds k candidates");
   const int qc = std::min(Q, kSearchRows), gc = std::min(N, kSearchCols);
   const long long cand_ld = (1 + (gc + kSegCols - 1) / kSegCols) * static_cast<long long>(k);
   const size_t cand_bytes = (static_cast<size_t>(qc) * cand_ld * sizeof(u64) + 255) / 256 * 256;  // the float rows start 16-byte aligned
@@ -535,18 +553,334 @@ int search_run(const float* queries, int Q, const float* gallery, int N, int E, 
     rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
     for (int g0 = 0; g0 < N && rc == 0; g0 += gc) {
       const int gn = std::min(gc, N - g0);
-      const bool first = g0 == 0, last = N - g0 == gn;
-      const long long segs = (gn + kSegCols - 1) / kSegCols;
       const size_t o = static_cast<size_t>(q0) * k;
       if (rc == 0) rc = l2_normalize_run(gallery + static_cast<size_t>(g0) * E, ng, E, gn, E, st);
-      if (rc == 0) rc = logits_run(nq, ng, logit_scale, logit_bias, block, qn, gn, E, gn, st);
-      if (rc == 0) rc = launch_segments(block, qn, gn, gn, kSegCols, k, g0, lo, cand + k, cand_ld, nullptr, nullptr, nullptr, st);
       if (rc == 0)
-        rc = launch_merge(first ? cand + k : cand, qn, cand_ld, (first ? 0 : k) + segs * k, k, lo, last ? nullptr : cand, nullptr, 0, 0,
-                          last ? values + o : nullptr, last ? indices + o : nullptr, nullptr, st);
+        rc = block_step(nq, qn, ng, gn, g0, E, logit_scale, logit_bias, k, lo, block, cand, cand_ld, g0 == 0, N - g0 == gn, values + o,
+                        indices + o, st);
     }
   }
   return free_scratch(cand, st, rc);
+}
+
+// ---- gallery index: normalised rows stored once, screened on the tensor cores in fp16, survivors rescored exactly ----
+// A search gives the bits search_run gives for the same queries against every row added so far.  Per chunk of kSearchRows queries:
+//   1. the queries are normalised by l2_normalize_run, and get an fp16 copy and a norm bound (prep_rows_kernel);
+//   2. seed: the first min(N, kSearchCols) stored rows go through block_step, the exact block step of search_run, which gives each
+//      query a running exact best k;
+//   3. each query's threshold t_i (threshold_kernel) is a lower bound on the accumulator of any row that can still enter its best k;
+//   4. the other rows are screened kScreenCols at a time by the fp16 GEMM with the screening epilogue (gemm.cu, which also derives the
+//      bound delta on |fp16 wgmma sum - fp32 accumulator|): a row survives when a + delta >= t_i;
+//   5. the survivors are rescored exactly (rescore_kernel: the fmaf chain and logit_value of logits_tile) and merged into the best k,
+//      and t_i is recomputed, so later chunks are screened harder.  A query with more than kScreenCap survivors in a chunk falls back to
+//      block_step on that chunk.
+// Dropped rows provably score below the running k-th; every other row is scored by the logits kernel's own arithmetic, on the stored
+// normalised rows -- the bits search_run computes -- so the result is search_run's.
+namespace {
+
+constexpr int kScreenCols = 65536;  // gallery rows per screen launch
+constexpr int kScreenCap = 4096;    // survivors kept per query and screen chunk; more fall back to the exact block step
+constexpr float kMaxBound = 1024.f;  // rows of larger norm are treated as non-finite (their fp16 copy could overflow)
+
+// One warp per row of x (normalised, fp32 [n, E]): the fp16 copy h and bound[r] >= ||x_r||_2, the sum of squares taken in double (each
+// square exact, E <= 8192 additions: relative error below 2^-39) and rounded up by 2^-30.  A row with a non-finite value or a norm above
+// kMaxBound gets bound +inf and zeros in h: it passes every screen and is always scored exactly.
+__global__ void __launch_bounds__(256) prep_rows_kernel(const float* __restrict__ x, int n, int E, __half* __restrict__ h,
+                                                        float* __restrict__ bound) {
+  const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= n) return;
+  const float* r = x + row * E;
+  double s = 0.0;
+  bool finite = true;
+  for (int i = lane; i < E; i += 32) {
+    const float v = r[i];
+    finite = finite && isfinite(v);
+    s += static_cast<double>(v) * v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float nb = __double2float_ru(sqrt(s) * (1.0 + 0x1p-30));
+  const bool ok = __all_sync(0xffffffffu, finite) && nb <= kMaxBound;
+  __half* hr = h + row * E;
+  for (int i = lane; i < E; i += 32) hr[i] = ok ? __float2half_rn(r[i]) : __float2half_rn(0.f);
+  if (lane == 0) bound[row] = ok ? nb : INFINITY;
+}
+
+int prep_rows_run(const float* x, int n, int E, __half* h, float* bound, cudaStream_t st) {
+  if (n <= 0) return 0;
+  JIMM_CUDA_CHECK(launch_k(prep_rows_kernel, dim3(static_cast<unsigned>((n + 7) / 8)), dim3(256), 0, st, 1, false, x, n, E, h, bound));
+  note_launch();
+  return 0;
+}
+
+// t[i] for each of qn queries from its running k-th score s_k (slot k - 1 of its sorted candidate row).  A row enters the best k only if
+// its score s = fl(sc acc + bs) (logit_value: one rounding) is >= s_k -- a tie enters too, since a later row has the larger index.
+// Rounding to nearest is monotone, so s >= s_k needs sc acc + bs >= s_k - 2^-24 |s_k| - 2^-150, i.e. (sc > 0)
+//   acc >= (s_k - bs) / sc - (2^-24 |s_k| + 2^-150) / sc.
+// t = (s_k - bs) / sc - m in double, m = 2^-20 (|s_k| + |bs|) / sc + 2^-20, then rounded down to fp32.  The double arithmetic errs by
+// under 2^-50 (|s_k| + |bs|) / sc, and with sc >= 2^-60 the 2^-150 / sc term is below 2^-90, so m covers both with room to spare and
+// t <= that lower bound.  Non-finite s_k, with sc and bs finite:
+//   * s_k = +inf: s = +inf needs sc acc + bs >= FLT_MAX, so s_k = FLT_MAX in the formula gives a valid (weaker) bound;
+//   * s_k NaN (NaN ranks above every number, so the running best k is all NaN): a number can no longer enter, only another NaN score.
+//     With sc and bs finite, fl(sc acc + bs) is NaN only if acc is, which needs a non-finite value in the query or the row; the index
+//     gives such a row or query norm bound +inf, and delta is then +inf or NaN, which passes any t.  So t = +inf: only those rows survive;
+//   * s_k = -inf: every row ties or beats it, t = -inf.
+// If sc or bs is not finite, or sc < 2^-60, t = -inf: every row survives and the chunk goes exact.
+__global__ void threshold_kernel(const u64* __restrict__ cand, long long cand_ld, int qn, int k, const float* __restrict__ logit_scale,
+                                 const float* __restrict__ logit_bias, float* __restrict__ t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= qn) return;
+  const float sk = __uint_as_float(static_cast<uint32_t>(cand[i * cand_ld + k - 1] >> 32));
+  const float sc = expf(*logit_scale);
+  const float bs = logit_bias ? *logit_bias : 0.f;
+  float ti = -INFINITY;
+  if (isfinite(sc) && isfinite(bs)) {
+    if (isnan(sk)) {
+      ti = INFINITY;
+    } else if (sk != -INFINITY && sc >= 0x1p-60f) {
+      const double s = fmin(static_cast<double>(sk), static_cast<double>(FLT_MAX));
+      const double a = fabs(s) + fabs(static_cast<double>(bs));
+      const double td = (s - bs) / sc - (0x1p-20 * a / sc + 0x1p-20);
+      ti = __double2float_rd(td);
+    }
+  }
+  t[i] = ti;
+}
+
+// After a screen: per query whose list overflowed (cnt > cap) its index in ovl; info[0] = the largest count of the others, info[1] =
+// the number of overflowed queries, info[2] = the others' counts summed.  One CTA.
+__global__ void __launch_bounds__(1024) screen_info_kernel(const int* __restrict__ cnt, int qn, int cap, int* __restrict__ ovl, int* __restrict__ info) {
+  __shared__ int smax, snov, ssum;
+  if (threadIdx.x == 0) smax = snov = ssum = 0;
+  __syncthreads();
+  for (int i = threadIdx.x; i < qn; i += blockDim.x) {
+    const int c = cnt[i];
+    if (c > cap) {
+      ovl[atomicAdd(&snov, 1)] = i;
+    } else if (c > 0) {
+      atomicMax(&smax, c);
+      atomicAdd(&ssum, c);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) { info[0] = smax; info[1] = snov; info[2] = ssum; }
+}
+
+// grid (ceil(width / 128), qn): slot s < width of query i's candidates after its running best k.  A surviving row j of the chunk
+// (list[i][s], s < cnt[i] <= cap) gets its exact score -- the fmaf chain over k ascending of logits_tile and logit_value with the
+// same sc and bs as logits_kernel -- as the candidate (score bits << 32 | g0 + j); other slots get kPadCand.
+__global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ nq, const float* __restrict__ ng, int E, const int* __restrict__ cnt,
+                                                      const int* __restrict__ list, int cap, int width, int g0, const float* __restrict__ logit_scale,
+                                                      const float* __restrict__ logit_bias, u64* __restrict__ cand, long long cand_ld, int k) {
+  extern __shared__ __align__(16) float qrow[];  // [E]
+  const int i = blockIdx.y;
+  const float* q = nq + static_cast<size_t>(i) * E;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) qrow[e] = q[e];
+  __syncthreads();
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= width) return;
+  const int c = cnt[i];
+  u64 out = kPadCand;
+  if (c <= cap && s < c) {
+    const int j = list[static_cast<size_t>(i) * cap + s];
+    const float4* g = reinterpret_cast<const float4*>(ng + static_cast<size_t>(j) * E);  // E % 4 == 0 (checked by gallery_create)
+    float acc = 0.f;
+    for (int e = 0; e < E; e += 4) {
+      const float4 v = __ldg(g + e / 4);
+      acc = fmaf(qrow[e], v.x, acc);
+      acc = fmaf(qrow[e + 1], v.y, acc);
+      acc = fmaf(qrow[e + 2], v.z, acc);
+      acc = fmaf(qrow[e + 3], v.w, acc);
+    }
+    if (E % 16 != 0) acc = fmaf(0.f, 0.f, acc);  // logits_tile's zero-padded last K step (turns a -0 into +0)
+    const float sc = expf(*logit_scale);
+    const float bs = logit_bias ? *logit_bias : 0.f;
+    out = (static_cast<u64>(__float_as_uint(logit_value(sc, acc, bs))) << 32) | static_cast<uint32_t>(g0 + j);
+  }
+  cand[i * cand_ld + k + s] = out;
+}
+
+// grid (nover): copy overflowed query ovl[r]'s normalised row and running best k into row r of fq / fcand (to_chunk), or the best k back.
+__global__ void __launch_bounds__(256) fallback_copy_kernel(const int* __restrict__ ovl, int E, int k, float* nq, float* fq, u64* cand,
+                                                            long long cand_ld, u64* fcand, long long fcand_ld, int to_chunk) {
+  const int r = blockIdx.x, i = ovl[r];
+  if (to_chunk) {
+    for (int e = threadIdx.x; e < E; e += blockDim.x) fq[static_cast<size_t>(r) * E + e] = nq[static_cast<size_t>(i) * E + e];
+    for (int s = threadIdx.x; s < k; s += blockDim.x) fcand[r * fcand_ld + s] = cand[i * cand_ld + s];
+  } else {
+    for (int s = threadIdx.x; s < k; s += blockDim.x) cand[i * cand_ld + s] = fcand[r * fcand_ld + s];
+  }
+}
+
+}  // namespace
+
+struct GalleryStore {
+  int E = 0;
+  long long n = 0, cap = 0;
+  float* rows = nullptr;   // [cap, E] normalised by l2_normalize_run: the bits search_run computes
+  __half* half = nullptr;  // [cap, E] fp16 copy, the screen's B operand
+  float* bound = nullptr;  // [cap] norm bounds (prep_rows_kernel)
+};
+
+int gallery_create(int E, GalleryStore** out) {
+  if (E <= 0 || E % 8 != 0 || E > 1024 * 8) { set_last_error("index: embedding width %d must be a multiple of 8 in 8 .. 8192", E); return JIMM_EINVAL; }
+  *out = new GalleryStore();
+  (*out)->E = E;
+  return 0;
+}
+
+long long gallery_rows(const GalleryStore* g) { return g->n; }
+
+int gallery_width(const GalleryStore* g) { return g->E; }
+
+int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t st) {
+  if (n <= 0) return 0;
+  const int E = g->E;
+  const long long need = g->n + n;
+  if (need > g->cap) {  // grow geometrically: copy the stored rows over, free the old storage in stream order
+    const long long cap = std::max(need, std::max(2 * g->cap, 1024ll));
+    float* r = nullptr;
+    __half* h = nullptr;
+    float* b = nullptr;
+    auto fail = [&](cudaError_t e, const char* what) {
+      cudaGetLastError();
+      if (r) cudaFreeAsync(r, st);
+      if (h) cudaFreeAsync(h, st);
+      if (b) cudaFreeAsync(b, st);
+      set_last_error("index: %s growing to %lld rows of width %d -> %s", what, cap, E, cudaGetErrorString(e));
+      return e == cudaErrorMemoryAllocation ? JIMM_ENOMEM : JIMM_ECUDA;
+    };
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&r), static_cast<size_t>(cap) * E * sizeof(float), st);
+    if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&h), static_cast<size_t>(cap) * E * sizeof(__half), st);
+    if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&b), static_cast<size_t>(cap) * sizeof(float), st);
+    if (e != cudaSuccess) return fail(e, "allocation");
+    if (g->n > 0) {
+      e = cudaMemcpyAsync(r, g->rows, static_cast<size_t>(g->n) * E * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(h, g->half, static_cast<size_t>(g->n) * E * sizeof(__half), cudaMemcpyDeviceToDevice, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(b, g->bound, static_cast<size_t>(g->n) * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) return fail(e, "copy");
+    }
+    if (g->rows) {  // the new storage holds every row from here on
+      cudaFreeAsync(g->rows, st);
+      cudaFreeAsync(g->half, st);
+      cudaFreeAsync(g->bound, st);
+    }
+    g->rows = r; g->half = h; g->bound = b; g->cap = cap;
+  }
+  constexpr int kPiece = 1 << 20;  // rows per l2_normalize_run (its warp index is an int)
+  for (int r0 = 0; r0 < n; r0 += kPiece) {
+    const int m = std::min(kPiece, n - r0);
+    const size_t at = static_cast<size_t>(g->n + r0);
+    if (int rc = l2_normalize_run(rows + static_cast<size_t>(r0) * E, g->rows + at * E, E, m, E, st)) return rc;
+    if (int rc = prep_rows_run(g->rows + at * E, m, E, g->half + at * E, g->bound + at, st)) return rc;
+  }
+  g->n = need;
+  return 0;
+}
+
+void gallery_destroy(GalleryStore* g) {
+  if (!g) return;
+  cudaDeviceSynchronize();  // cudaFree does not wait for the work still using stream-ordered allocations
+  cudaFree(g->rows);
+  cudaFree(g->half);
+  cudaFree(g->bound);
+  delete g;
+}
+
+int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, float* values,
+                   int32_t* indices, long long* stats, cudaStream_t st) {
+  const int E = g->E, N = static_cast<int>(g->n);
+  const int qc = std::min(Q, kSearchRows), seed = std::min(N, kSearchCols);
+  const bool screen = N > seed;
+  const long long seed_ld = k + (seed + kSegCols - 1) / kSegCols * static_cast<long long>(k);
+  const long long cand_ld = screen ? k + std::max<long long>(kScreenCap, kSearchCols / kSegCols * static_cast<long long>(k)) : seed_ld;
+  const long long fcand_ld = k + kSearchCols / kSegCols * static_cast<long long>(k);
+  // scratch: 256-byte aligned pieces of one stream-ordered allocation
+  size_t off = 0;
+  auto piece = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
+  const size_t o_cand = piece(static_cast<size_t>(qc) * cand_ld * sizeof(u64));
+  const size_t o_nq = piece(static_cast<size_t>(qc) * E * sizeof(float));
+  const size_t o_block = piece(static_cast<size_t>(qc) * seed * sizeof(float));
+  size_t o_fcand = 0, o_fq = 0, o_hq = 0, o_nbq = 0, o_t = 0, o_cnt = 0, o_ovl = 0, o_list = 0, o_info = 0;
+  if (screen) {
+    o_fcand = piece(static_cast<size_t>(qc) * fcand_ld * sizeof(u64));
+    o_fq = piece(static_cast<size_t>(qc) * E * sizeof(float));
+    o_hq = piece(static_cast<size_t>(qc) * E * sizeof(__half));
+    o_nbq = piece(static_cast<size_t>(qc) * sizeof(float));
+    o_t = piece(static_cast<size_t>(qc) * sizeof(float));
+    o_cnt = piece(static_cast<size_t>(qc) * sizeof(int));
+    o_ovl = piece(static_cast<size_t>(qc) * sizeof(int));
+    o_list = piece(static_cast<size_t>(qc) * kScreenCap * sizeof(int));
+    o_info = piece(4 * sizeof(int));
+  }
+  uint8_t* base = nullptr;
+  JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&base), off, st));
+  u64* cand = reinterpret_cast<u64*>(base + o_cand);
+  float* nq = reinterpret_cast<float*>(base + o_nq);
+  float* block = reinterpret_cast<float*>(base + o_block);
+  u64* fcand = reinterpret_cast<u64*>(base + o_fcand);
+  float* fq = reinterpret_cast<float*>(base + o_fq);
+  __half* hq = reinterpret_cast<__half*>(base + o_hq);
+  float* nbq = reinterpret_cast<float*>(base + o_nbq);
+  float* t = reinterpret_cast<float*>(base + o_t);
+  int* cnt = reinterpret_cast<int*>(base + o_cnt);
+  int* ovl = reinterpret_cast<int*>(base + o_ovl);
+  int* list = reinterpret_cast<int*>(base + o_list);
+  int* info = reinterpret_cast<int*>(base + o_info);
+  GemmScreen sd;
+  sd.t = t; sd.nq = nbq; sd.cnt = cnt; sd.list = list; sd.cap = kScreenCap;
+  const int lo = bit_width(N);
+  int rc = 0;
+  auto threshold = [&](int qn) -> int {
+    JIMM_CUDA_CHECK(launch_k(threshold_kernel, dim3((qn + 255) / 256), dim3(256), 0, st, 1, false, cand, cand_ld, qn, k, logit_scale, logit_bias, t));
+    note_launch();
+    return 0;
+  };
+  // Gallery rows g0 .. g0 + gn - 1 against the current qn queries: screen, rescore the survivors, send overflowed queries through the
+  // exact block step, tighten the thresholds.  Every error is returned, so the caller frees the scratch.
+  auto screen_chunk = [&](int qn, int g0) -> int {
+    const int gn = std::min(kScreenCols, N - g0);
+    sd.ng = g->bound + g0;
+    JIMM_CUDA_CHECK(cudaMemsetAsync(cnt, 0, static_cast<size_t>(qn) * sizeof(int), st));
+    if (int e = gemm_screen_run(hq, qn, g->half + static_cast<size_t>(g0) * E, gn, E, sd, st)) return e;
+    JIMM_CUDA_CHECK(launch_k(screen_info_kernel, dim3(1), dim3(1024), 0, st, 1, false, cnt, qn, kScreenCap, ovl, info));
+    note_launch();
+    int h[3];
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(h, info, sizeof(h), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int width = h[0], nover = h[1];
+    if (stats) { stats[0] += h[2]; stats[1] += nover; stats[2] += 1; }
+    if (width > 0) {
+      JIMM_CUDA_CHECK(launch_k(rescore_kernel, dim3((width + 127) / 128, qn), dim3(128), static_cast<size_t>(E) * sizeof(float), st, 1, false, nq,
+                               g->rows + static_cast<size_t>(g0) * E, E, cnt, list, kScreenCap, width, g0, logit_scale, logit_bias, cand, cand_ld, k));
+      note_launch();
+      if (int e = launch_merge(cand, qn, cand_ld, k + width, k, lo, cand, nullptr, 0, 0, nullptr, nullptr, nullptr, st)) return e;
+    }
+    if (nover > 0) {  // those queries' chunk goes through the exact block step, in kSearchCols pieces
+      JIMM_CUDA_CHECK(launch_k(fallback_copy_kernel, dim3(nover), dim3(256), 0, st, 1, false, ovl, E, k, nq, fq, cand, cand_ld, fcand, fcand_ld, 1));
+      note_launch();
+      for (int s0 = 0; s0 < gn; s0 += kSearchCols)
+        if (int e = block_step(fq, nover, g->rows + static_cast<size_t>(g0 + s0) * E, std::min(kSearchCols, gn - s0), g0 + s0, E, logit_scale,
+                               logit_bias, k, lo, block, fcand, fcand_ld, false, false, nullptr, nullptr, st))
+          return e;
+      JIMM_CUDA_CHECK(launch_k(fallback_copy_kernel, dim3(nover), dim3(256), 0, st, 1, false, ovl, E, k, nq, fq, cand, cand_ld, fcand, fcand_ld, 0));
+      note_launch();
+    }
+    return width > 0 || nover > 0 ? threshold(qn) : 0;
+  };
+  for (int q0 = 0; q0 < Q && rc == 0; q0 += qc) {
+    const int qn = std::min(qc, Q - q0);
+    const size_t o = static_cast<size_t>(q0) * k;
+    rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
+    if (rc == 0) rc = block_step(nq, qn, g->rows, seed, 0, E, logit_scale, logit_bias, k, lo, block, cand, cand_ld, true, !screen, values + o, indices + o, st);
+    if (!screen) continue;
+    if (rc == 0) rc = prep_rows_run(nq, qn, E, hq, nbq, st);
+    if (rc == 0) rc = threshold(qn);
+    for (int g0 = seed; g0 < N && rc == 0; g0 += kScreenCols) rc = screen_chunk(qn, g0);
+    if (rc == 0) rc = launch_merge(cand, qn, cand_ld, k, k, lo, nullptr, nullptr, 0, 0, values + o, indices + o, nullptr, st);
+  }
+  return free_scratch(base, st, rc);
 }
 
 }  // namespace jimm

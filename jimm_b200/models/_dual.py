@@ -5,7 +5,7 @@ from __future__ import annotations
 import torch
 
 from .. import _lib, nn
-from .._runtime import Texts, _call, prep_blocks, prep_ids, prep_layers, prep_texts, tokens_result
+from .._runtime import GalleryIndex, Texts, _call, prep_blocks, prep_ids, prep_layers, prep_texts, tokens_result
 from ..common.transformer import Transformer, g_wrap
 from ..common.vit import _NativeOwner, tower_config_fields
 
@@ -138,6 +138,16 @@ class DualTower(_NativeOwner, nn.Module):
         search(encode_image(x), encode_text(t), k) == top_k(model(x, t), k) and search(encode_text(t), encode_image(x), k) ==
         top_k(model(x, t).T, k), at any Q and N; 1 <= k <= min(N, 1024).  Single GPU."""
         return self.native().search(queries, gallery, k)
+
+    def index(self, gallery=None):
+        """A gallery index: `gallery` ([N, E] embeddings as search takes them, fp32 / fp16 / bf16, device or host) normalised once and
+        kept on the GPU.  `index.add(rows)` appends (indices continue), `len(index)` counts the rows, and `index.search(queries, k)`
+        equals search(queries, every row added so far, k) bit for bit, with host results for host queries.  Each search screens the
+        gallery on the tensor cores in fp16 and scores exactly only the rows that can still reach the best k.  The index keeps this
+        model alive and follows its native handle: after a rebuild (a larger batch, set_flat_param, ...) the next add / search binds
+        the stored rows to the new handle, so results stay equal to search with the model's current logit_scale / logit_bias.
+        Single GPU; widths as the model has them (multiples of 8)."""
+        return GalleryIndex(self.native, gallery)
 
     def set_comm(self, mode: str):
         """'peer' (default, fused NVLink peer-store kernel) | 'nccl' (torch.distributed all_gather baseline) | 'off'."""
