@@ -520,6 +520,30 @@ JIMM_API int jimm_index_add(jimm_index_t* idx, const float* rows, int n, void* s
 JIMM_API int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, float* values, int32_t* indices, jimm_search_stats* stats,
                                void* stream);
 JIMM_API int jimm_index_destroy(jimm_index_t* idx);
+/* Threshold search of a gallery index.  Scores are the ones jimm_index_search ranks (fp32, on the model's score scale: exp(logit_scale)
+ * cos + logit_bias); a pair is a hit when its score >= threshold in IEEE order (a NaN score never is; -0 >= +0).  threshold must not be
+ * NaN (JIMM_EINVAL); +inf and -inf are allowed.
+ * jimm_index_range_search: for each of the Q queries (device fp32 [Q, E], as jimm_index_search takes them) every row added so far whose
+ *   score is >= threshold, in ascending row order.  Rows: Q.
+ * jimm_index_pairs: for each stored row i every stored row j > i whose score against it is >= threshold (score(i, j) and score(j, i) are
+ *   the same bits), in ascending j.  Rows: the rows added so far.
+ * Both screen in fp16 on the tensor cores against a fixed accumulator bound and rescore the survivors exactly, as jimm_index_search
+ *   does; stats (nullable, host) receives the work done.  They wait for `stream` once per screened chunk of 65536 rows and once per
+ *   chunk of 2048 query rows, size the result from the counts and return it in *out, a jimm_hits_t the caller destroys.  If the hits
+ *   do not fit in device memory the call returns JIMM_ENOMEM, names the hits reached, frees what it allocated in stream order and sets
+ *   *out to NULL; the index is unchanged.  Device memory: 8 bytes per hit and 8 per row in the result, and as much again for one
+ *   query chunk's staged hits while it runs.
+ * jimm_hits_size: the result's rows and hits (host values, no wait).
+ * jimm_hits_copy: CSR into caller memory (device or host): offsets int64 [rows + 1] (offsets[0] = 0), scores fp32 [total], indices
+ *   int32 [total] (the row numbers of the hits), enqueued on `stream`.
+ * jimm_hits_destroy: waits for the result's device, then frees it. */
+typedef struct jimm_hits jimm_hits_t;
+JIMM_API int jimm_index_range_search(jimm_index_t* idx, const float* queries, int Q, float threshold, jimm_hits_t** out,
+                                     jimm_search_stats* stats, void* stream);
+JIMM_API int jimm_index_pairs(jimm_index_t* idx, float threshold, jimm_hits_t** out, jimm_search_stats* stats, void* stream);
+JIMM_API int jimm_hits_size(const jimm_hits_t* h, int* rows, long long* total);
+JIMM_API int jimm_hits_copy(const jimm_hits_t* h, int64_t* offsets, float* scores, int32_t* indices, void* stream);
+JIMM_API int jimm_hits_destroy(jimm_hits_t* h);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads
  * its own 16 KB tiles; 1: the CTAs of a cluster load the same tile each; 2: same tile, each loads 1/cluster of it and multicasts. */
 JIMM_API int jimm_k_l2_probe(const void* buf, int rows, int mode, int cluster, int iters, float* ms, void* stream);

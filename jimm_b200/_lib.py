@@ -164,6 +164,11 @@ SIGNATURES = {
     "jimm_index_add": (_i, [_vp, _fp, _i, _vp]),
     "jimm_index_search": (_i, [_vp, _fp, _i, _i, _fp, _ip, C.c_void_p, _vp]),
     "jimm_index_destroy": (_i, [_vp]),
+    "jimm_index_range_search": (_i, [_vp, _fp, _i, _f, C.POINTER(_vp), C.c_void_p, _vp]),
+    "jimm_index_pairs": (_i, [_vp, _f, C.POINTER(_vp), C.c_void_p, _vp]),
+    "jimm_hits_size": (_i, [_vp, C.POINTER(_i), C.POINTER(C.c_longlong)]),
+    "jimm_hits_copy": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "jimm_hits_destroy": (_i, [_vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),

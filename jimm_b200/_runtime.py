@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 import os
 from typing import Callable, Dict, List, NamedTuple, Optional, Tuple, Union
 
@@ -632,7 +633,8 @@ class NativeModel:
 
 class GalleryIndex:
     """A gallery normalised once and kept on the GPU (jimm_index_*): search(queries, k) is NativeModel.search(queries, every row added
-    so far, k) on the model's current handle, bit for bit.  `native` returns that handle: a model's `native` method, which rebuilds it
+    so far, k) on the model's current handle, bit for bit; range_search(queries, threshold) and pairs(threshold) give every score at or
+    above a threshold.  `native` returns that handle: a model's `native` method, which rebuilds it
     when its parameters or batch bound change.  Each add / search rebinds the index to the handle `native` gives (jimm_index_rebind,
     same width and device; the stored rows stay), so it scores with the model's current logit_scale / logit_bias and never reads a
     handle the model has destroyed.  Holding `native` keeps the model alive."""
@@ -687,6 +689,60 @@ class GalleryIndex:
         _call(m.lib, m.device, "jimm_index_search", self.handle, qd, Q, k, values, indices, None)
         host = not q.is_cuda
         return m._back(values, host).result(), m._back(indices, host).result()
+
+    @staticmethod
+    def _threshold(threshold) -> float:
+        """A threshold on the model's score scale as a Python float; the C call rounds it to fp32 (nearest) once."""
+        if isinstance(threshold, bool) or not isinstance(threshold, numbers.Real):
+            raise ValueError(f"index: the threshold must be a real number, got {threshold!r}")
+        try:
+            t = float(threshold)
+        except OverflowError:  # an integer beyond every float: fp32 rounds it to an infinity
+            t = math.copysign(math.inf, threshold)
+        if math.isnan(t):
+            raise ValueError("index: the threshold is NaN")
+        return t
+
+    def _hits(self, m: NativeModel, name: str, *args):
+        """Run jimm_index_range_search / jimm_index_pairs and copy its jimm_hits_t into device tensors: offsets int64 [rows + 1], scores
+        fp32 [total] and indices int32 [total]."""
+        h = C.c_void_p()
+        _call(m.lib, m.device, name, self.handle, *args, C.byref(h), None)
+        try:
+            rows, total = C.c_int(), C.c_longlong()
+            _lib.check(m.lib.jimm_hits_size(h, C.byref(rows), C.byref(total)))
+            offsets = torch.empty(rows.value + 1, dtype=torch.int64, device=m.device)
+            scores = torch.empty(total.value, dtype=torch.float32, device=m.device)
+            indices = torch.empty(total.value, dtype=torch.int32, device=m.device)
+            _call(m.lib, m.device, "jimm_hits_copy", h, offsets, scores, indices)
+        finally:
+            with torch.cuda.device(m.device):
+                m.lib.jimm_hits_destroy(h)
+        return offsets, scores, indices
+
+    def range_search(self, queries, threshold):
+        """Every row of the index whose score against each query is >= threshold (a real number on the model's score scale,
+        exp(logit_scale) * cos + logit_bias, rounded to fp32), in CSR: offsets int64 [Q + 1], scores fp32 [nnz] and row indices int32
+        [nnz], each query's hits in ascending row order; on the host when the queries were.  Bit for bit the entries >= threshold of the
+        score matrix model.search ranks; a NaN score is never a hit."""
+        m = self._model()
+        q = m._embeddings("queries", queries)
+        t = self._threshold(threshold)
+        Q = q.shape[0]
+        qd = q.to(m.device, torch.float32, non_blocking=True).contiguous()
+        out = self._hits(m, "jimm_index_range_search", qd, Q, t)
+        host = not q.is_cuda
+        return tuple(m._back(x, host).result() for x in out)
+
+    def pairs(self, threshold):
+        """Every pair of stored rows i < j whose score is >= threshold: `i, j, scores` (int32, int32, fp32), ordered by i then j, on the
+        device.  The upper triangle of range_search(every raw row added, threshold), without the raw rows."""
+        m = self._model()
+        t = self._threshold(threshold)
+        offsets, scores, j = self._hits(m, "jimm_index_pairs", t)
+        rows = offsets.numel() - 1
+        i = torch.repeat_interleave(torch.arange(rows, dtype=torch.int32, device=m.device), offsets.diff(), output_size=j.numel())
+        return i, j, scores
 
     def close(self):
         """Free the stored rows (jimm_index_destroy reads only the index's own device, never the model)."""

@@ -8,6 +8,8 @@
 
 #include "gemm.cuh"
 
+struct jimm_hits;  // the C ABI's jimm_hits_t (postprocess.cu)
+
 namespace jimm {
 
 // nnx.LayerNorm (fast variance, fp32 statistics) over fp32 rows.  SURVEY 8a row a3.
@@ -99,6 +101,12 @@ int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t stream);
 int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, float* values,
                    int32_t* indices, long long* stats, cudaStream_t stream);
 void gallery_destroy(GalleryStore* g);
+// Every (query, stored row) pair whose score is >= threshold, in CSR (jimm_hits, postprocess.cu), each row's hits in ascending stored-row
+// order: the Q queries against every stored row, or (pairs) the stored rows against the later ones, Q = rows.  The same screen and
+// rescore as gallery_search with the threshold fixed; stats as there.  The call waits for its stream once per screened chunk and once
+// per chunk of kSearchRows queries.  On failure *out is null and everything allocated is freed in stream order.
+int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs, float threshold, const float* logit_scale,
+                  const float* logit_bias, jimm_hits** out, long long* stats, cudaStream_t stream);
 
 // dst[n*K + k] = cast(src[k*N + n])   (flax (in,out) kernel -> K-major [N,K] operand)
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);

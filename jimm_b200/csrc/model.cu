@@ -1916,6 +1916,33 @@ int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, flo
   return rc;
 }
 
+// Shared checks and dispatch of jimm_index_range_search (queries) and jimm_index_pairs (queries null, Q = 0).
+static int index_range(jimm_index_t* idx, const float* queries, int Q, bool pairs, float threshold, jimm_hits_t** out, jimm_search_stats* stats,
+                       void* stream) {
+  const char* what = pairs ? "pairs" : "range search";
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  if (!out) { set_last_error("%s: null output handle", what); return JIMM_EINVAL; }
+  *out = nullptr;
+  jimm_model* m = idx->m;
+  JIMM_TRY(check_ready(m, Q));
+  if (threshold != threshold) { set_last_error("%s: the threshold is NaN", what); return JIMM_EINVAL; }
+  if (Q > 0 && !queries) { set_last_error("%s: null queries", what); return JIMM_EINVAL; }
+  JIMM_TRY(set_device(m));
+  long long st[3] = {0, 0, 0};
+  const int rc = gallery_range(idx->store, queries, Q, pairs, threshold, m->logit_scale, m->logit_bias, out, st, static_cast<cudaStream_t>(stream));
+  if (stats) { stats->rows_rescored = st[0]; stats->fallbacks = st[1]; stats->chunks_screened = st[2]; }
+  return rc;
+}
+
+int jimm_index_range_search(jimm_index_t* idx, const float* queries, int Q, float threshold, jimm_hits_t** out, jimm_search_stats* stats,
+                            void* stream) {
+  return index_range(idx, queries, Q, false, threshold, out, stats, stream);
+}
+
+int jimm_index_pairs(jimm_index_t* idx, float threshold, jimm_hits_t** out, jimm_search_stats* stats, void* stream) {
+  return index_range(idx, nullptr, 0, true, threshold, out, stats, stream);
+}
+
 int jimm_index_destroy(jimm_index_t* idx) {
   if (!idx) return 0;
   JIMM_CUDA_CHECK(cudaSetDevice(idx->device));

@@ -11,6 +11,7 @@
 // maximum.
 #include <algorithm>
 #include <cfloat>
+#include <vector>
 
 #include "../../include/jimm_b200.h"
 #include "common.cuh"
@@ -627,13 +628,8 @@ int prep_rows_run(const float* x, int n, int E, __half* h, float* bound, cudaStr
 //     gives such a row or query norm bound +inf, and delta is then +inf or NaN, which passes any t.  So t = +inf: only those rows survive;
 //   * s_k = -inf: every row ties or beats it, t = -inf.
 // If sc or bs is not finite, or sc < 2^-60, t = -inf: every row survives and the chunk goes exact.
-__global__ void threshold_kernel(const u64* __restrict__ cand, long long cand_ld, int qn, int k, const float* __restrict__ logit_scale,
-                                 const float* __restrict__ logit_bias, float* __restrict__ t) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= qn) return;
-  const float sk = __uint_as_float(static_cast<uint32_t>(cand[i * cand_ld + k - 1] >> 32));
-  const float sc = expf(*logit_scale);
-  const float bs = logit_bias ? *logit_bias : 0.f;
+// The same bound serves a fixed threshold (range search): a row is a hit only if its score is >= s_k := the threshold.
+__device__ __forceinline__ float acc_lower_bound(float sk, float sc, float bs) {
   float ti = -INFINITY;
   if (isfinite(sc) && isfinite(bs)) {
     if (isnan(sk)) {
@@ -645,7 +641,17 @@ __global__ void threshold_kernel(const u64* __restrict__ cand, long long cand_ld
       ti = __double2float_rd(td);
     }
   }
-  t[i] = ti;
+  return ti;
+}
+
+__global__ void threshold_kernel(const u64* __restrict__ cand, long long cand_ld, int qn, int k, const float* __restrict__ logit_scale,
+                                 const float* __restrict__ logit_bias, float* __restrict__ t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= qn) return;
+  const float sk = __uint_as_float(static_cast<uint32_t>(cand[i * cand_ld + k - 1] >> 32));
+  const float sc = expf(*logit_scale);
+  const float bs = logit_bias ? *logit_bias : 0.f;
+  t[i] = acc_lower_bound(sk, sc, bs);
 }
 
 // After a screen: per query whose list overflowed (cnt > cap) its index in ovl; info[0] = the largest count of the others, info[1] =
@@ -667,9 +673,28 @@ __global__ void __launch_bounds__(1024) screen_info_kernel(const int* __restrict
   if (threadIdx.x == 0) { info[0] = smax; info[1] = snov; info[2] = ssum; }
 }
 
+// The exact score of normalised query row qrow (shared memory) against stored row grow: the fmaf chain over k ascending of
+// logits_tile and logit_value with the same sc and bs as logits_kernel.
+__device__ __forceinline__ float rescore_value(const float* qrow, const float* __restrict__ grow, int E, const float* __restrict__ logit_scale,
+                                               const float* __restrict__ logit_bias) {
+  const float4* g = reinterpret_cast<const float4*>(grow);  // E % 4 == 0 (checked by gallery_create)
+  float acc = 0.f;
+  for (int e = 0; e < E; e += 4) {
+    const float4 v = __ldg(g + e / 4);
+    acc = fmaf(qrow[e], v.x, acc);
+    acc = fmaf(qrow[e + 1], v.y, acc);
+    acc = fmaf(qrow[e + 2], v.z, acc);
+    acc = fmaf(qrow[e + 3], v.w, acc);
+  }
+  if (E % 16 != 0) acc = fmaf(0.f, 0.f, acc);  // logits_tile's zero-padded last K step (turns a -0 into +0)
+  const float sc = expf(*logit_scale);
+  const float bs = logit_bias ? *logit_bias : 0.f;
+  return logit_value(sc, acc, bs);
+}
+
 // grid (ceil(width / 128), qn): slot s < width of query i's candidates after its running best k.  A surviving row j of the chunk
-// (list[i][s], s < cnt[i] <= cap) gets its exact score -- the fmaf chain over k ascending of logits_tile and logit_value with the
-// same sc and bs as logits_kernel -- as the candidate (score bits << 32 | g0 + j); other slots get kPadCand.
+// (list[i][s], s < cnt[i] <= cap) gets its exact score (rescore_value) as the candidate (score bits << 32 | g0 + j); other slots get
+// kPadCand.
 __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ nq, const float* __restrict__ ng, int E, const int* __restrict__ cnt,
                                                       const int* __restrict__ list, int cap, int width, int g0, const float* __restrict__ logit_scale,
                                                       const float* __restrict__ logit_bias, u64* __restrict__ cand, long long cand_ld, int k) {
@@ -684,19 +709,8 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
   u64 out = kPadCand;
   if (c <= cap && s < c) {
     const int j = list[static_cast<size_t>(i) * cap + s];
-    const float4* g = reinterpret_cast<const float4*>(ng + static_cast<size_t>(j) * E);  // E % 4 == 0 (checked by gallery_create)
-    float acc = 0.f;
-    for (int e = 0; e < E; e += 4) {
-      const float4 v = __ldg(g + e / 4);
-      acc = fmaf(qrow[e], v.x, acc);
-      acc = fmaf(qrow[e + 1], v.y, acc);
-      acc = fmaf(qrow[e + 2], v.z, acc);
-      acc = fmaf(qrow[e + 3], v.w, acc);
-    }
-    if (E % 16 != 0) acc = fmaf(0.f, 0.f, acc);  // logits_tile's zero-padded last K step (turns a -0 into +0)
-    const float sc = expf(*logit_scale);
-    const float bs = logit_bias ? *logit_bias : 0.f;
-    out = (static_cast<u64>(__float_as_uint(logit_value(sc, acc, bs))) << 32) | static_cast<uint32_t>(g0 + j);
+    const float v = rescore_value(qrow, ng + static_cast<size_t>(j) * E, E, logit_scale, logit_bias);
+    out = (static_cast<u64>(__float_as_uint(v)) << 32) | static_cast<uint32_t>(g0 + j);
   }
   cand[i * cand_ld + k + s] = out;
 }
@@ -710,6 +724,183 @@ __global__ void __launch_bounds__(256) fallback_copy_kernel(const int* __restric
     for (int s = threadIdx.x; s < k; s += blockDim.x) fcand[r * fcand_ld + s] = cand[i * cand_ld + s];
   } else {
     for (int s = threadIdx.x; s < k; s += blockDim.x) cand[i * cand_ld + s] = fcand[r * fcand_ld + s];
+  }
+}
+
+// ---- range search: every row whose score is >= a fixed threshold ----
+constexpr int kRangeThreads = kThreads;  // bitonic_sort_desc strides by kThreads
+
+struct KeyAscending {  // bitonic_sort_desc by this key sorts ascending
+  __device__ __forceinline__ u64 operator()(u64 v) const { return ~v; }
+};
+
+// Exclusive prefix sum of v over the CTA (blockDim.x a multiple of 32, at most 1024), in thread order; *total gets the sum.  Every
+// thread of the CTA calls it; *total may be read until the next call.
+template <typename T>
+__device__ T block_exclusive_scan(T v, T* warp_sums, T* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  T x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sums[w] = x;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    T run = 0;
+    for (int i = 0; i < nw; ++i) {
+      const T s = warp_sums[i];
+      warp_sums[i] = run;
+      run += s;
+    }
+    *total = run;
+  }
+  __syncthreads();
+  const T r = warp_sums[w] + x - v;
+  __syncthreads();
+  return r;
+}
+
+// t[i] = acc_lower_bound(threshold) for each of qn rows: a row whose accumulator is below t scores below the threshold.
+__global__ void range_threshold_kernel(int qn, float threshold, const float* __restrict__ logit_scale, const float* __restrict__ logit_bias,
+                                       float* __restrict__ t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= qn) return;
+  t[i] = acc_lower_bound(threshold, expf(*logit_scale), logit_bias ? *logit_bias : 0.f);
+}
+
+// After a screen of gn rows, one CTA: each query's staging room pos[i] (exclusive prefix sum of cnt[i], or of gn when its list overflowed
+// (cnt[i] > cap)), the overflowed queries in ascending order in ovl, info[0] = their number, info[1] = the summed room, info[2] = the
+// summed counts of the others (rows rescored) and info[3] = the largest of those counts.
+__global__ void __launch_bounds__(1024) range_info_kernel(const int* __restrict__ cnt, int qn, int cap, int gn, int* __restrict__ ovl,
+                                                          int* __restrict__ pos, int* __restrict__ info) {
+  __shared__ int warp_sums[32], total, smax;
+  if (threadIdx.x == 0) smax = 0;
+  __syncthreads();
+  int room = 0, nover = 0, rescored = 0;
+  for (int b = 0; b < qn; b += blockDim.x) {
+    const int i = b + threadIdx.x;
+    const int c = i < qn ? cnt[i] : 0;
+    const bool over = c > cap;
+    if (!over && c > 0) atomicMax(&smax, c);
+    const int p = block_exclusive_scan(over ? gn : c, warp_sums, &total);
+    if (i < qn) pos[i] = room + p;
+    room += total;
+    const int o = block_exclusive_scan(over ? 1 : 0, warp_sums, &total);
+    if (over) ovl[nover + o] = i;
+    nover += total;
+    block_exclusive_scan(over ? 0 : c, warp_sums, &total);
+    rescored += total;
+  }
+  if (threadIdx.x == 0) { info[0] = nover; info[1] = room; info[2] = rescored; info[3] = smax; }
+}
+
+// Keeps the hits of one round of blockDim.x candidates, in thread order: hit (score v, row j) goes to out[base + its rank].  Returns the
+// round's number of hits.
+__device__ __forceinline__ int keep_hits(bool hit, float v, int j, float* __restrict__ out_score, int32_t* __restrict__ out_index, long long base,
+                                         int* warp_sums, int* total) {
+  const int r = block_exclusive_scan(hit ? 1 : 0, warp_sums, total);
+  if (hit) { out_score[base + r] = v; out_index[base + r] = j; }
+  return *total;
+}
+
+// grid (qn): query i's screen survivors in chunk g0 (list[i][s], s < cnt[i] <= cap) sorted ascending in shared memory, scored by
+// rescore_value, and those with score >= threshold -- and, pairs (row0 >= 0), stored row g0 + j > row0 + i -- written in row order to
+// the staging at pos[i]; count[i] = their number.  An overflowed query (cnt[i] > cap) is left to range_block_kernel.
+__global__ void __launch_bounds__(kRangeThreads) range_rescore_kernel(const float* __restrict__ nq, const float* __restrict__ ng, int E,
+                                                                      const int* __restrict__ cnt, const int* __restrict__ list, int cap, int g0,
+                                                                      int row0, float threshold, const float* __restrict__ logit_scale,
+                                                                      const float* __restrict__ logit_bias, const int* __restrict__ pos,
+                                                                      float* __restrict__ st_score, int32_t* __restrict__ st_index,
+                                                                      int* __restrict__ count) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  float* qrow = reinterpret_cast<float*>(smem_raw);                  // [E]
+  u64* keys = reinterpret_cast<u64*>(smem_raw + static_cast<size_t>(E) * sizeof(float));  // [npow2]: row, then score bits << 32 | row
+  __shared__ int warp_sums[32], total;
+  const int i = blockIdx.x;
+  const int c = cnt[i];
+  if (c > cap || c == 0) return;  // the block step takes an overflowed query; count[i] stays 0 for an empty one
+  int npow2 = 1;
+  while (npow2 < c) npow2 <<= 1;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) qrow[e] = nq[static_cast<size_t>(i) * E + e];
+  for (int s = threadIdx.x; s < npow2; s += blockDim.x) keys[s] = s < c ? static_cast<u64>(list[static_cast<size_t>(i) * cap + s]) : ~0ull;
+  __syncthreads();
+  bitonic_sort_desc(keys, npow2, KeyAscending{});  // ascending rows, the padding (~0) last
+  for (int s = threadIdx.x; s < c; s += blockDim.x) {
+    const int j = static_cast<int>(keys[s]);
+    const float v = rescore_value(qrow, ng + static_cast<size_t>(j) * E, E, logit_scale, logit_bias);
+    keys[s] = (static_cast<u64>(__float_as_uint(v)) << 32) | static_cast<uint32_t>(j);
+  }
+  __syncthreads();
+  long long base = pos[i];
+  for (int s0 = 0; s0 < c; s0 += blockDim.x) {
+    const int s = s0 + threadIdx.x;
+    const u64 kv = s < c ? keys[s] : 0ull;
+    const float v = __uint_as_float(static_cast<uint32_t>(kv >> 32));
+    const int j = g0 + static_cast<int>(static_cast<uint32_t>(kv));
+    const bool hit = s < c && v >= threshold && (row0 < 0 || j > row0 + i);
+    base += keep_hits(hit, v, j, st_score, st_index, base, warp_sums, &total);
+  }
+  if (threadIdx.x == 0) count[i] = static_cast<int>(base - pos[i]);
+}
+
+// grid (nover): row r of the exact score block [nover, cols] (query ovl[r], stored rows col0 ..) -- the entries >= threshold, and for
+// pairs (row0 >= 0) those of stored row col0 + c > row0 + ovl[r], in column order, appended to the query's staging after the count[i]
+// hits its earlier pieces of the chunk left there.
+__global__ void __launch_bounds__(kRangeThreads) range_block_kernel(const float* __restrict__ block, int cols, const int* __restrict__ ovl, int col0,
+                                                                    int row0, float threshold, const int* __restrict__ pos,
+                                                                    float* __restrict__ st_score, int32_t* __restrict__ st_index,
+                                                                    int* __restrict__ count) {
+  __shared__ int warp_sums[32], total;
+  const int r = blockIdx.x, i = ovl[r];
+  const float* x = block + static_cast<size_t>(r) * cols;
+  long long base = static_cast<long long>(pos[i]) + count[i];
+  for (int c0 = 0; c0 < cols; c0 += blockDim.x) {
+    const int c = c0 + threadIdx.x;
+    const float v = c < cols ? x[c] : 0.f;
+    const bool hit = c < cols && v >= threshold && (row0 < 0 || col0 + c > row0 + i);
+    base += keep_hits(hit, v, col0 + c, st_score, st_index, base, warp_sums, &total);
+  }
+  if (threadIdx.x == 0) count[i] = static_cast<int>(base - pos[i]);
+}
+
+// One CTA, at the end of a query chunk: with count[c * qn + i] the hits of query i in gallery chunk c, offsets[i] = base + the hits of
+// the queries before i (offsets[qn] = base + all of them) and dst[c * qn + i] = where the hits of (i, c) go: after offsets[i] and the
+// query's hits in chunks before c.
+__global__ void __launch_bounds__(1024) range_offsets_kernel(const int* __restrict__ count, int nch, int qn, long long base,
+                                                             long long* __restrict__ offsets, long long* __restrict__ dst) {
+  __shared__ long long warp_sums[32], total;
+  long long run = base;
+  for (int b = 0; b < qn; b += blockDim.x) {
+    const int i = b + threadIdx.x;
+    long long n = 0;
+    if (i < qn)
+      for (int c = 0; c < nch; ++c) n += count[static_cast<size_t>(c) * qn + i];
+    const long long o = run + block_exclusive_scan(n, warp_sums, &total);
+    if (i < qn) {
+      offsets[i] = o;
+      long long d = o;
+      for (int c = 0; c < nch; ++c) {
+        dst[static_cast<size_t>(c) * qn + i] = d;
+        d += count[static_cast<size_t>(c) * qn + i];
+      }
+    }
+    run += total;
+  }
+  if (threadIdx.x == 0) offsets[qn] = run;
+}
+
+// grid (qn): the count[i] staged hits of query i in one gallery chunk, from pos[i] to the result at dst[i] - base.
+__global__ void __launch_bounds__(kRangeThreads) range_gather_kernel(const float* __restrict__ st_score, const int32_t* __restrict__ st_index,
+                                                                     const int* __restrict__ pos, const int* __restrict__ count,
+                                                                     const long long* __restrict__ dst, long long base, float* __restrict__ score,
+                                                                     int32_t* __restrict__ index) {
+  const int i = blockIdx.x, n = count[i];
+  const long long from = pos[i], to = dst[i] - base;
+  for (int s = threadIdx.x; s < n; s += blockDim.x) {
+    score[to + s] = st_score[from + s];
+    index[to + s] = st_index[from + s];
   }
 }
 
@@ -885,6 +1076,220 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
 
 }  // namespace jimm
 
+// The hits of one range search or pairs call, in CSR: one segment per query chunk, each in its own device storage.
+struct jimm_hits {
+  struct Segment {
+    int rows = 0;                   // rows of the segment; its offsets [rows + 1] count from the first row of the result
+    long long start = 0, nnz = 0;   // offsets[0] and the segment's hits
+    long long* offsets = nullptr;   // device
+    float* scores = nullptr;        // device: scores fp32 [nnz], then indices int32 [nnz]
+  };
+  int device = 0, rows = 0;
+  long long total = 0;
+  std::vector<Segment> segs;
+};
+
+namespace jimm {
+
+void hits_free(jimm_hits* h, cudaStream_t st) {  // in stream order
+  for (auto& s : h->segs) {
+    cudaFreeAsync(s.offsets, st);
+    if (s.scores) cudaFreeAsync(s.scores, st);
+  }
+  delete h;
+}
+
+int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs, float threshold, const float* logit_scale,
+                  const float* logit_bias, jimm_hits** out, long long* stats, cudaStream_t st) {
+  const int E = g->E, N = static_cast<int>(g->n);
+  if (pairs) Q = N;
+  *out = nullptr;
+  int device = 0;
+  JIMM_CUDA_CHECK(cudaGetDevice(&device));
+  jimm_hits* hits = new jimm_hits();
+  hits->device = device;
+  hits->rows = Q;
+  if (Q == 0) { *out = hits; return 0; }
+  const int qc = std::min(Q, kSearchRows), nch = (N + kScreenCols - 1) / kScreenCols;
+  // scratch: 256-byte aligned pieces of one stream-ordered allocation
+  size_t off = 0;
+  auto piece = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
+  const size_t o_nq = pairs ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(float));
+  const size_t o_hq = pairs ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(__half));
+  const size_t o_nbq = pairs ? 0 : piece(static_cast<size_t>(qc) * sizeof(float));
+  const size_t o_fq = piece(static_cast<size_t>(qc) * E * sizeof(float));
+  const size_t o_block = piece(static_cast<size_t>(qc) * std::min(N, kSearchCols) * sizeof(float));
+  const size_t o_t = piece(static_cast<size_t>(qc) * sizeof(float));
+  const size_t o_cnt = piece(static_cast<size_t>(qc) * sizeof(int));
+  const size_t o_ovl = piece(static_cast<size_t>(qc) * sizeof(int));
+  const size_t o_list = piece(static_cast<size_t>(qc) * kScreenCap * sizeof(int));
+  const size_t o_info = piece(4 * sizeof(int));
+  const size_t o_pos = piece(static_cast<size_t>(nch) * qc * sizeof(int));
+  const size_t o_count = piece(static_cast<size_t>(nch) * qc * sizeof(int));
+  const size_t o_dst = piece(static_cast<size_t>(nch) * qc * sizeof(long long));
+  uint8_t* base = nullptr;
+  std::vector<float*> stage(nch, nullptr);  // per gallery chunk: staged scores [room], then indices [room], of the current query chunk
+  std::vector<int> stage_room(nch, 0);
+  long long done = 0;                       // hits of the query chunks before the current one
+  auto free_stage = [&]() {
+    for (auto& p : stage) {
+      if (p) cudaFreeAsync(p, st);
+      p = nullptr;
+    }
+    std::fill(stage_room.begin(), stage_room.end(), 0);
+  };
+  // every failure frees what the call allocated, in stream order
+  auto fail = [&](int rc) {
+    free_stage();
+    hits_free(hits, st);
+    return base ? free_scratch(base, st, rc) : rc;
+  };
+  auto alloc = [&](void** p, size_t bytes, const char* what) -> int {
+    const cudaError_t e = cudaMallocAsync(p, bytes, st);
+    if (e == cudaSuccess) return 0;
+    cudaGetLastError();
+    *p = nullptr;
+    set_last_error("%s: %s of %zu bytes after %lld hits -> %s", pairs ? "pairs" : "range search", what, bytes, done, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? JIMM_ENOMEM : JIMM_ECUDA;
+  };
+  if (int rc = alloc(reinterpret_cast<void**>(&base), off, "scratch")) return fail(rc);
+  float* nq = reinterpret_cast<float*>(base + o_nq);
+  __half* hq = reinterpret_cast<__half*>(base + o_hq);
+  float* nbq = reinterpret_cast<float*>(base + o_nbq);
+  float* fq = reinterpret_cast<float*>(base + o_fq);
+  float* block = reinterpret_cast<float*>(base + o_block);
+  float* t = reinterpret_cast<float*>(base + o_t);
+  int* cnt = reinterpret_cast<int*>(base + o_cnt);
+  int* ovl = reinterpret_cast<int*>(base + o_ovl);
+  int* list = reinterpret_cast<int*>(base + o_list);
+  int* info = reinterpret_cast<int*>(base + o_info);
+  int* pos = reinterpret_cast<int*>(base + o_pos);
+  int* count = reinterpret_cast<int*>(base + o_count);
+  long long* dst = reinterpret_cast<long long*>(base + o_dst);
+  GemmScreen sd;
+  sd.t = t; sd.cnt = cnt; sd.list = list; sd.cap = kScreenCap;
+  const int max_smem = static_cast<int>(8192 * sizeof(float) + kScreenCap * sizeof(u64));
+  if (int rc = smem_opt_in<range_rescore_kernel>(max_smem)) return fail(rc);
+  auto check_launch = [&](cudaError_t e, const char* what) -> int {
+    if (e == cudaSuccess) { note_launch(); return 0; }
+    set_last_error("%s -> %s", what, cudaGetErrorString(e));
+    return JIMM_ECUDA;
+  };
+  // Query rows q0 .. q0 + qn - 1 (normalised in qrows, fp16 copies qh, bounds qb) against gallery chunk c: screen, then the survivors'
+  // hits (rescored) and the overflowed queries' hits (exact block step) staged in row order, their counts in count[c * qn + i].
+  auto range_chunk = [&](int qn, int q0, float* qrows, const __half* qh, int c) -> int {
+    const int g0 = c * kScreenCols, gn = std::min(kScreenCols, N - g0);
+    if (pairs && g0 + gn - 1 <= q0) return 0;  // no row of the chunk lies above any query row's diagonal
+    const int row0 = pairs ? q0 : -1;
+    int* pos_c = pos + static_cast<size_t>(c) * qn;
+    int* count_c = count + static_cast<size_t>(c) * qn;
+    sd.ng = g->bound + g0;
+    JIMM_CUDA_CHECK(cudaMemsetAsync(cnt, 0, static_cast<size_t>(qn) * sizeof(int), st));
+    if (int e = gemm_screen_run(qh, qn, g->half + static_cast<size_t>(g0) * E, gn, E, sd, st)) return e;
+    if (int e = check_launch(launch_k(range_info_kernel, dim3(1), dim3(1024), 0, st, 1, false, cnt, qn, kScreenCap, gn, ovl, pos_c, info),
+                             "range_info_kernel"))
+      return e;
+    int h[4];
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(h, info, sizeof(h), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int nover = h[0], room = h[1], rescored = h[2], widest = h[3];
+    if (stats) { stats[0] += rescored; stats[1] += nover; stats[2] += 1; }
+    if (room == 0) return 0;
+    if (int e = alloc(reinterpret_cast<void**>(&stage[c]), static_cast<size_t>(room) * (sizeof(float) + sizeof(int32_t)), "staging")) return e;
+    stage_room[c] = room;
+    float* ss = stage[c];
+    int32_t* si = reinterpret_cast<int32_t*>(ss + room);
+    if (widest > 0) {
+      const size_t smem = static_cast<size_t>(E) * sizeof(float) + static_cast<size_t>(pow2_at_least(widest)) * sizeof(u64);
+      if (int e = check_launch(launch_k(range_rescore_kernel, dim3(qn), dim3(kRangeThreads), smem, st, 1, false, qrows,
+                                        g->rows + static_cast<size_t>(g0) * E, E, cnt, list, kScreenCap, g0, row0, threshold, logit_scale,
+                                        logit_bias, pos_c, ss, si, count_c),
+                               "range_rescore_kernel"))
+        return e;
+    }
+    if (nover > 0) {  // those queries' chunk goes through the exact block step, in kSearchCols pieces
+      if (int e = check_launch(launch_k(fallback_copy_kernel, dim3(nover), dim3(256), 0, st, 1, false, ovl, E, 0, qrows, fq, nullptr, 0ll,
+                                        nullptr, 0ll, 1),
+                               "fallback_copy_kernel"))
+        return e;
+      for (int s0 = 0; s0 < gn; s0 += kSearchCols) {
+        const int pw = std::min(kSearchCols, gn - s0);
+        if (int e = logits_run(fq, g->rows + static_cast<size_t>(g0 + s0) * E, logit_scale, logit_bias, block, nover, pw, E, pw, st)) return e;
+        if (int e = check_launch(launch_k(range_block_kernel, dim3(nover), dim3(kRangeThreads), 0, st, 1, false, block, pw, ovl, g0 + s0, row0,
+                                          threshold, pos_c, ss, si, count_c),
+                                 "range_block_kernel"))
+          return e;
+      }
+    }
+    return 0;
+  };
+  // The end of a query chunk: offsets from the counts, then the staged hits gathered into the chunk's segment in (query, row) order.
+  auto assemble = [&](int qn) -> int {
+    jimm_hits::Segment seg;
+    seg.rows = qn;
+    seg.start = done;
+    if (int e = alloc(reinterpret_cast<void**>(&seg.offsets), static_cast<size_t>(qn + 1) * sizeof(long long), "result offsets")) return e;
+    hits->segs.push_back(seg);
+    jimm_hits::Segment& sg = hits->segs.back();
+    if (int e = check_launch(launch_k(range_offsets_kernel, dim3(1), dim3(1024), 0, st, 1, false, count, nch, qn, done, sg.offsets, dst),
+                             "range_offsets_kernel"))
+      return e;
+    long long end = 0;
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(&end, sg.offsets + qn, sizeof(end), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    sg.nnz = end - done;
+    if (sg.nnz > 0) {
+      if (int e = alloc(reinterpret_cast<void**>(&sg.scores), static_cast<size_t>(sg.nnz) * (sizeof(float) + sizeof(int32_t)), "result")) return e;
+      int32_t* idx = reinterpret_cast<int32_t*>(sg.scores + sg.nnz);
+      for (int c = 0; c < nch; ++c) {
+        if (!stage[c]) continue;
+        const int* pos_c = pos + static_cast<size_t>(c) * qn;
+        const int* count_c = count + static_cast<size_t>(c) * qn;
+        const float* ss = stage[c];
+        const int32_t* si = reinterpret_cast<const int32_t*>(ss + stage_room[c]);
+        if (int e = check_launch(launch_k(range_gather_kernel, dim3(qn), dim3(kRangeThreads), 0, st, 1, false, ss, si, pos_c, count_c,
+                                          dst + static_cast<size_t>(c) * qn, done, sg.scores, idx),
+                                 "range_gather_kernel"))
+          return e;
+      }
+    }
+    done = end;
+    return 0;
+  };
+  if (int rc = check_launch(launch_k(range_threshold_kernel, dim3((qc + 255) / 256), dim3(256), 0, st, 1, false, qc, threshold, logit_scale,
+                                     logit_bias, t),
+                            "range_threshold_kernel"))
+    return fail(rc);
+  for (int q0 = 0; q0 < Q; q0 += qc) {
+    const int qn = std::min(qc, Q - q0);
+    float* qrows = nq;
+    const __half* qh = hq;
+    int rc = 0;
+    if (pairs) {  // the stored rows themselves: normalised, with their fp16 copies and bounds
+      qrows = g->rows + static_cast<size_t>(q0) * E;
+      qh = g->half + static_cast<size_t>(q0) * E;
+      sd.nq = g->bound + q0;
+    } else {
+      sd.nq = nbq;
+      rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
+      if (rc == 0) rc = prep_rows_run(nq, qn, E, hq, nbq, st);
+    }
+    if (rc == 0 && nch > 0) {
+      const cudaError_t e = cudaMemsetAsync(count, 0, static_cast<size_t>(nch) * qn * sizeof(int), st);
+      if (e != cudaSuccess) { set_last_error("cudaMemsetAsync -> %s", cudaGetErrorString(e)); rc = JIMM_ECUDA; }
+    }
+    for (int c = 0; c < nch && rc == 0; ++c) rc = range_chunk(qn, q0, qrows, qh, c);
+    if (rc == 0) rc = assemble(qn);
+    if (rc != 0) return fail(rc);
+    free_stage();
+  }
+  hits->total = done;
+  *out = hits;
+  return free_scratch(base, st, 0);
+}
+
+}  // namespace jimm
+
 using namespace jimm;
 
 extern "C" int jimm_postprocess(const float* logits, int rows, int cols, int ld, int mode, float* probs, int ldp, int32_t* order, int32_t* argmax,
@@ -915,4 +1320,40 @@ extern "C" int jimm_topk(const float* logits, int rows, int cols, int ld, int k,
   if (rows > 0 && (!logits || !values || !indices)) { set_last_error("top_k: null logits, values or indices"); return JIMM_EINVAL; }
   if (rows == 0) return 0;
   return topk_run(logits, rows, cols, ld, k, values, indices, probs, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int jimm_hits_size(const jimm_hits_t* h, int* rows, long long* total) {
+  if (!h || !rows || !total) { set_last_error("hits: null handle, rows or total"); return JIMM_EINVAL; }
+  *rows = h->rows;
+  *total = h->total;
+  return 0;
+}
+
+extern "C" int jimm_hits_copy(const jimm_hits_t* h, int64_t* offsets, float* scores, int32_t* indices, void* stream) {
+  if (!h || !offsets || (h->total > 0 && (!scores || !indices))) { set_last_error("hits copy: null handle, offsets, scores or indices"); return JIMM_EINVAL; }
+  JIMM_CUDA_CHECK(cudaSetDevice(h->device));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (h->segs.empty()) JIMM_CUDA_CHECK(cudaMemsetAsync(offsets, 0, sizeof(int64_t), st));
+  long long row = 0;
+  for (const auto& s : h->segs) {  // consecutive segments share one offset: the first's last is the next one's first
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(offsets + row, s.offsets, static_cast<size_t>(s.rows + 1) * sizeof(int64_t), cudaMemcpyDefault, st));
+    if (s.nnz > 0) {
+      JIMM_CUDA_CHECK(cudaMemcpyAsync(scores + s.start, s.scores, static_cast<size_t>(s.nnz) * sizeof(float), cudaMemcpyDefault, st));
+      JIMM_CUDA_CHECK(cudaMemcpyAsync(indices + s.start, s.scores + s.nnz, static_cast<size_t>(s.nnz) * sizeof(int32_t), cudaMemcpyDefault, st));
+    }
+    row += s.rows;
+  }
+  return 0;
+}
+
+extern "C" int jimm_hits_destroy(jimm_hits_t* h) {
+  if (!h) return 0;
+  JIMM_CUDA_CHECK(cudaSetDevice(h->device));
+  cudaDeviceSynchronize();  // cudaFree does not wait for the work still using stream-ordered allocations
+  for (auto& s : h->segs) {
+    cudaFree(s.offsets);
+    if (s.scores) cudaFree(s.scores);
+  }
+  delete h;
+  return 0;
 }
