@@ -544,6 +544,30 @@ JIMM_API int jimm_index_pairs(jimm_index_t* idx, float threshold, jimm_hits_t** 
 JIMM_API int jimm_hits_size(const jimm_hits_t* h, int* rows, long long* total);
 JIMM_API int jimm_hits_copy(const jimm_hits_t* h, int64_t* offsets, float* scores, int32_t* indices, void* stream);
 JIMM_API int jimm_hits_destroy(jimm_hits_t* h);
+/* Removing rows and searching a subset of a gallery index.  A row keeps its number from jimm_index_add until jimm_index_compact, removed
+ * or not, and numbers are never reused.
+ * jimm_index_remove: marks rows ids (device int32 [n], any order, duplicates allowed) removed; *removed (host) = the rows newly removed.
+ *   An id outside 0 .. rows - 1 is JIMM_EINVAL and removes nothing.  Waits for `stream` once.  Removed rows keep their memory.
+ * jimm_index_live: *live = the rows not removed (host, no wait).
+ * jimm_index_search_keep / _range_search_keep / _pairs_keep: the calls above over the allowed rows -- the live rows with keep[r] != 0
+ *   (keep: device bytes [rows], a bool tensor's memory; NULL keeps every row) -- bit for bit the same call on an index holding only
+ *   those rows, with results in the index's row numbers.  Pairs need both rows allowed, and their result still has one row per stored
+ *   row.  A search with fewer than k allowed rows pads each query's outputs past them with (-inf, -1); k's limit is unchanged.  With
+ *   keep NULL and no row removed they run exactly as the calls without _keep; those calls are these with keep NULL, so after a
+ *   removal they too see only the live rows.  Otherwise each call first lists the allowed rows (4 bytes each, one more wait for
+ *   `stream`) and reads them through a buffer of 65536 rows, (6 E + 4) bytes each; rows_rescored counts allowed rows only.
+ * jimm_index_compact: drops the removed rows: the live ones are renumbered 0 .. live - 1 in order, into new storage of exactly that
+ *   size (the old one freed in stream order).  old_to_new (nullable, device int32 [rows before]) gets each row's new number, -1 for a
+ *   removed row.  JIMM_ENOMEM leaves the index as it was. */
+JIMM_API int jimm_index_remove(jimm_index_t* idx, const int32_t* ids, int n, long long* removed, void* stream);
+JIMM_API int jimm_index_live(const jimm_index_t* idx, long long* live);
+JIMM_API int jimm_index_search_keep(jimm_index_t* idx, const float* queries, int Q, int k, const uint8_t* keep, float* values, int32_t* indices,
+                                    jimm_search_stats* stats, void* stream);
+JIMM_API int jimm_index_range_search_keep(jimm_index_t* idx, const float* queries, int Q, float threshold, const uint8_t* keep, jimm_hits_t** out,
+                                          jimm_search_stats* stats, void* stream);
+JIMM_API int jimm_index_pairs_keep(jimm_index_t* idx, float threshold, const uint8_t* keep, jimm_hits_t** out, jimm_search_stats* stats,
+                                   void* stream);
+JIMM_API int jimm_index_compact(jimm_index_t* idx, int32_t* old_to_new, void* stream);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads
  * its own 16 KB tiles; 1: the CTAs of a cluster load the same tile each; 2: same tile, each loads 1/cluster of it and multicasts. */
 JIMM_API int jimm_k_l2_probe(const void* buf, int rows, int mode, int cluster, int iters, float* ms, void* stream);

@@ -169,6 +169,12 @@ SIGNATURES = {
     "jimm_hits_size": (_i, [_vp, C.POINTER(_i), C.POINTER(C.c_longlong)]),
     "jimm_hits_copy": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "jimm_hits_destroy": (_i, [_vp]),
+    "jimm_index_remove": (_i, [_vp, _vp, _i, C.POINTER(C.c_longlong), _vp]),
+    "jimm_index_live": (_i, [_vp, C.POINTER(C.c_longlong)]),
+    "jimm_index_search_keep": (_i, [_vp, _fp, _i, _i, _vp, _fp, _ip, C.c_void_p, _vp]),
+    "jimm_index_range_search_keep": (_i, [_vp, _fp, _i, _f, _vp, C.POINTER(_vp), C.c_void_p, _vp]),
+    "jimm_index_pairs_keep": (_i, [_vp, _f, _vp, C.POINTER(_vp), C.c_void_p, _vp]),
+    "jimm_index_compact": (_i, [_vp, _vp, _vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),

@@ -634,7 +634,8 @@ class NativeModel:
 class GalleryIndex:
     """A gallery normalised once and kept on the GPU (jimm_index_*): search(queries, k) is NativeModel.search(queries, every row added
     so far, k) on the model's current handle, bit for bit; range_search(queries, threshold) and pairs(threshold) give every score at or
-    above a threshold.  `native` returns that handle: a model's `native` method, which rebuilds it
+    above a threshold.  remove(ids) drops rows from every later call, keep= restricts one call to a subset of the rows, and compact()
+    renumbers the live rows and frees the removed ones.  `native` returns that handle: a model's `native` method, which rebuilds it
     when its parameters or batch bound change.  Each add / search rebinds the index to the handle `native` gives (jimm_index_rebind,
     same width and device; the stored rows stay), so it scores with the model's current logit_scale / logit_bias and never reads a
     handle the model has destroyed.  Holding `native` keeps the model alive."""
@@ -674,19 +675,97 @@ class GalleryIndex:
         return self
 
     def __len__(self) -> int:
+        """Every row ever added (removed ones included) since the last compact(): the next add numbers its rows from here."""
         return self._rows
 
-    def search(self, queries, k: int):
+    @property
+    def num_live(self) -> int:
+        """The rows not removed."""
+        if not self.handle:
+            raise _lib.JimmError("gallery index: closed")
+        live = C.c_longlong()
+        _lib.check(self._lib.jimm_index_live(self.handle, C.byref(live)))
+        return live.value
+
+    def _row_tensor(self, x, what: str) -> torch.Tensor:
+        """x (an int, a sequence, a numpy array or a torch tensor, on the host or the index's device) as a 1-D tensor, checked for its
+        device; an empty sequence is int64."""
+        if isinstance(x, torch.Tensor):
+            t = x
+        else:
+            a = np.asarray(x)
+            if a.size == 0:
+                a = a.astype(np.int64)
+            if a.dtype.kind not in "biu":
+                raise ValueError(f"index: {what} must be integers or bools, got {a.dtype}")
+            t = torch.from_numpy(np.ascontiguousarray(a))
+        if t.is_cuda and t.device != self._device:
+            raise ValueError(f"index: {what} is on {t.device}, the index on {self._device}")
+        return t.reshape(-1)
+
+    def _row_ids(self, t: torch.Tensor, what: str) -> torch.Tensor:
+        """Integer row ids, each in 0 .. len(self) - 1, as int32 on the index's device."""
+        if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex:
+            raise ValueError(f"index: {what} must be integer row ids, got {t.dtype}")
+        t = t.to(torch.int64)
+        if t.numel() > 0:
+            lo, hi = int(t.min()), int(t.max())
+            if lo < 0 or hi >= self._rows:
+                raise ValueError(f"index: {what} must be row ids in 0 .. {self._rows - 1}, got {lo} .. {hi}")
+        return t.to(self._device, torch.int32, non_blocking=True).contiguous()
+
+    def _keep(self, keep) -> Optional[torch.Tensor]:
+        """keep as a bool mask [len(self)] on the index's device (its memory is the byte mask the C calls take), or None."""
+        if keep is None:
+            return None
+        t = self._row_tensor(keep, "keep")
+        if t.dtype == torch.bool:
+            if t.numel() != self._rows:
+                raise ValueError(f"index: a keep mask must have one entry per row ({self._rows}), got {t.numel()}")
+            return t.to(self._device, non_blocking=True).contiguous()
+        ids = self._row_ids(t, "keep")
+        mask = torch.zeros(self._rows, dtype=torch.bool, device=self._device)
+        mask[ids.long()] = True
+        return mask
+
+    def remove(self, ids) -> int:
+        """Remove rows by id (an int, a sequence, a numpy array or an integer tensor, host or device): every later call skips them.
+        Returns the rows newly removed (duplicates and rows already removed count once / not at all).  Row numbers are not reused,
+        and removed rows keep their memory until compact()."""
+        if not self.handle:
+            raise _lib.JimmError("gallery index: closed")
+        ids = self._row_ids(self._row_tensor(ids, "ids"), "ids")
+        removed = C.c_longlong()
+        _call(self._lib, self._device, "jimm_index_remove", self.handle, ids, ids.numel(), C.byref(removed))
+        return removed.value
+
+    def compact(self) -> torch.Tensor:
+        """Drop the removed rows and renumber the live ones in their order, in new storage of their size.  Returns the old-to-new
+        map: int64 [len(self) before] on the index's device, -1 for a removed row."""
+        if not self.handle:
+            raise _lib.JimmError("gallery index: closed")
+        old_to_new = torch.empty(self._rows, dtype=torch.int32, device=self._device)
+        _call(self._lib, self._device, "jimm_index_compact", self.handle, old_to_new)
+        self._rows = self.num_live
+        return old_to_new.to(torch.int64)
+
+    def search(self, queries, k: int, keep=None):
         """The k best rows of the index for each query: fp32 [Q, k] scores and int32 [Q, k] row indices, on the host when the queries
-        were."""
+        were.  Only live rows are searched, and of those only the ones keep selects (a bool mask [len(self)] or row ids, host or
+        device): bit for bit model.search against those rows alone, with their row numbers.  With fewer than k such rows, the columns
+        past them hold (-inf, -1)."""
         m = self._model()
         q = m._embeddings("queries", queries)
         k = m._search_k(k, self._rows)
+        mask = self._keep(keep)
         Q = q.shape[0]
         qd = q.to(m.device, torch.float32, non_blocking=True).contiguous()
         values = torch.empty((Q, k), dtype=torch.float32, device=m.device)
         indices = torch.empty((Q, k), dtype=torch.int32, device=m.device)
-        _call(m.lib, m.device, "jimm_index_search", self.handle, qd, Q, k, values, indices, None)
+        if mask is None:
+            _call(m.lib, m.device, "jimm_index_search", self.handle, qd, Q, k, values, indices, None)
+        else:
+            _call(m.lib, m.device, "jimm_index_search_keep", self.handle, qd, Q, k, mask, values, indices, None)
         host = not q.is_cuda
         return m._back(values, host).result(), m._back(indices, host).result()
 
@@ -720,26 +799,35 @@ class GalleryIndex:
                 m.lib.jimm_hits_destroy(h)
         return offsets, scores, indices
 
-    def range_search(self, queries, threshold):
+    def range_search(self, queries, threshold, keep=None):
         """Every row of the index whose score against each query is >= threshold (a real number on the model's score scale,
         exp(logit_scale) * cos + logit_bias, rounded to fp32), in CSR: offsets int64 [Q + 1], scores fp32 [nnz] and row indices int32
         [nnz], each query's hits in ascending row order; on the host when the queries were.  Bit for bit the entries >= threshold of the
-        score matrix model.search ranks; a NaN score is never a hit."""
+        score matrix model.search ranks; a NaN score is never a hit.  Only live rows that keep selects (as in search) are hits."""
         m = self._model()
         q = m._embeddings("queries", queries)
         t = self._threshold(threshold)
+        mask = self._keep(keep)
         Q = q.shape[0]
         qd = q.to(m.device, torch.float32, non_blocking=True).contiguous()
-        out = self._hits(m, "jimm_index_range_search", qd, Q, t)
+        if mask is None:
+            out = self._hits(m, "jimm_index_range_search", qd, Q, t)
+        else:
+            out = self._hits(m, "jimm_index_range_search_keep", qd, Q, t, mask)
         host = not q.is_cuda
         return tuple(m._back(x, host).result() for x in out)
 
-    def pairs(self, threshold):
+    def pairs(self, threshold, keep=None):
         """Every pair of stored rows i < j whose score is >= threshold: `i, j, scores` (int32, int32, fp32), ordered by i then j, on the
-        device.  The upper triangle of range_search(every raw row added, threshold), without the raw rows."""
+        device.  The upper triangle of range_search(every raw row added, threshold), without the raw rows.  Both rows of a pair are
+        live and selected by keep (as in search)."""
         m = self._model()
         t = self._threshold(threshold)
-        offsets, scores, j = self._hits(m, "jimm_index_pairs", t)
+        mask = self._keep(keep)
+        if mask is None:
+            offsets, scores, j = self._hits(m, "jimm_index_pairs", t)
+        else:
+            offsets, scores, j = self._hits(m, "jimm_index_pairs_keep", t, mask)
         rows = offsets.numel() - 1
         i = torch.repeat_interleave(torch.arange(rows, dtype=torch.int32, device=m.device), offsets.diff(), output_size=j.numel())
         return i, j, scores

@@ -98,15 +98,27 @@ int gallery_create(int E, GalleryStore** out);
 long long gallery_rows(const GalleryStore* g);
 int gallery_width(const GalleryStore* g);
 int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t stream);
-int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, float* values,
-                   int32_t* indices, long long* stats, cudaStream_t stream);
+// keep (nullable): device bytes [rows], nonzero keeps the row.  A search runs over the allowed rows -- live and kept -- as if they were
+// the only rows, and with fewer than k of them the slots past the last are (-inf, -1).  With no filter and no removed rows it runs
+// exactly as before any removal existed; otherwise it waits for its stream once more, to size the allowed rows.
+int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, const uint8_t* keep,
+                   float* values, int32_t* indices, long long* stats, cudaStream_t stream);
 void gallery_destroy(GalleryStore* g);
+// Removed rows keep their number and their storage until gallery_compact.  gallery_remove: clears the live bit of ids[0 .. n) (device,
+// each in 0 .. rows - 1, else JIMM_EINVAL and nothing is removed); *removed = the rows newly removed.  Waits for its stream once.
+// gallery_compact: drops the removed rows into new storage of exactly the live rows, in order, and writes old_to_new (nullable, device
+// [rows]: the new number, -1 for a removed row).  On failure the store is unchanged.
+long long gallery_live(const GalleryStore* g);
+int gallery_remove(GalleryStore* g, const int* ids, int n, long long* removed, cudaStream_t stream);
+int gallery_compact(GalleryStore* g, int32_t* old_to_new, cudaStream_t stream);
 // Every (query, stored row) pair whose score is >= threshold, in CSR (jimm_hits, postprocess.cu), each row's hits in ascending stored-row
 // order: the Q queries against every stored row, or (pairs) the stored rows against the later ones, Q = rows.  The same screen and
 // rescore as gallery_search with the threshold fixed; stats as there.  The call waits for its stream once per screened chunk and once
 // per chunk of kSearchRows queries.  On failure *out is null and everything allocated is freed in stream order.
+// keep as gallery_search: only allowed rows are hits, and for pairs both rows of a pair are allowed; the pairs result still has a
+// row for every stored row.
 int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs, float threshold, const float* logit_scale,
-                  const float* logit_bias, jimm_hits** out, long long* stats, cudaStream_t stream);
+                  const float* logit_bias, const uint8_t* keep, jimm_hits** out, long long* stats, cudaStream_t stream);
 
 // dst[n*K + k] = cast(src[k*N + n])   (flax (in,out) kernel -> K-major [N,K] operand)
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);

@@ -1903,6 +1903,11 @@ int jimm_index_add(jimm_index_t* idx, const float* rows, int n, void* stream) {
 }
 
 int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, float* values, int32_t* indices, jimm_search_stats* stats, void* stream) {
+  return jimm_index_search_keep(idx, queries, Q, k, nullptr, values, indices, stats, stream);
+}
+
+int jimm_index_search_keep(jimm_index_t* idx, const float* queries, int Q, int k, const uint8_t* keep, float* values, int32_t* indices,
+                           jimm_search_stats* stats, void* stream) {
   if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
   jimm_model* m = idx->m;
   JIMM_TRY(check_ready(m, Q));
@@ -1911,14 +1916,15 @@ int jimm_index_search(jimm_index_t* idx, const float* queries, int Q, int k, flo
   if (Q > 0 && (!queries || !values || !indices)) { set_last_error("search: null queries, values or indices"); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   long long st[3] = {0, 0, 0};
-  const int rc = Q == 0 ? 0 : gallery_search(idx->store, queries, Q, m->logit_scale, m->logit_bias, k, values, indices, st, static_cast<cudaStream_t>(stream));
+  const int rc = Q == 0 ? 0 : gallery_search(idx->store, queries, Q, m->logit_scale, m->logit_bias, k, keep, values, indices, st,
+                                             static_cast<cudaStream_t>(stream));
   if (stats) { stats->rows_rescored = st[0]; stats->fallbacks = st[1]; stats->chunks_screened = st[2]; }
   return rc;
 }
 
 // Shared checks and dispatch of jimm_index_range_search (queries) and jimm_index_pairs (queries null, Q = 0).
-static int index_range(jimm_index_t* idx, const float* queries, int Q, bool pairs, float threshold, jimm_hits_t** out, jimm_search_stats* stats,
-                       void* stream) {
+static int index_range(jimm_index_t* idx, const float* queries, int Q, bool pairs, float threshold, const uint8_t* keep, jimm_hits_t** out,
+                       jimm_search_stats* stats, void* stream) {
   const char* what = pairs ? "pairs" : "range search";
   if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
   if (!out) { set_last_error("%s: null output handle", what); return JIMM_EINVAL; }
@@ -1929,18 +1935,47 @@ static int index_range(jimm_index_t* idx, const float* queries, int Q, bool pair
   if (Q > 0 && !queries) { set_last_error("%s: null queries", what); return JIMM_EINVAL; }
   JIMM_TRY(set_device(m));
   long long st[3] = {0, 0, 0};
-  const int rc = gallery_range(idx->store, queries, Q, pairs, threshold, m->logit_scale, m->logit_bias, out, st, static_cast<cudaStream_t>(stream));
+  const int rc = gallery_range(idx->store, queries, Q, pairs, threshold, m->logit_scale, m->logit_bias, keep, out, st, static_cast<cudaStream_t>(stream));
   if (stats) { stats->rows_rescored = st[0]; stats->fallbacks = st[1]; stats->chunks_screened = st[2]; }
   return rc;
 }
 
 int jimm_index_range_search(jimm_index_t* idx, const float* queries, int Q, float threshold, jimm_hits_t** out, jimm_search_stats* stats,
                             void* stream) {
-  return index_range(idx, queries, Q, false, threshold, out, stats, stream);
+  return index_range(idx, queries, Q, false, threshold, nullptr, out, stats, stream);
 }
 
 int jimm_index_pairs(jimm_index_t* idx, float threshold, jimm_hits_t** out, jimm_search_stats* stats, void* stream) {
-  return index_range(idx, nullptr, 0, true, threshold, out, stats, stream);
+  return index_range(idx, nullptr, 0, true, threshold, nullptr, out, stats, stream);
+}
+
+int jimm_index_range_search_keep(jimm_index_t* idx, const float* queries, int Q, float threshold, const uint8_t* keep, jimm_hits_t** out,
+                                 jimm_search_stats* stats, void* stream) {
+  return index_range(idx, queries, Q, false, threshold, keep, out, stats, stream);
+}
+
+int jimm_index_pairs_keep(jimm_index_t* idx, float threshold, const uint8_t* keep, jimm_hits_t** out, jimm_search_stats* stats, void* stream) {
+  return index_range(idx, nullptr, 0, true, threshold, keep, out, stats, stream);
+}
+
+// Removal and compaction touch only the stored rows, so they need the index's device, not its model.
+int jimm_index_remove(jimm_index_t* idx, const int32_t* ids, int n, long long* removed, void* stream) {
+  if (!idx || !removed) { set_last_error("index remove: null handle or count"); return JIMM_EINVAL; }
+  if (n < 0 || (n > 0 && !ids)) { set_last_error("index remove: n=%d ids=%p", n, static_cast<const void*>(ids)); return JIMM_EINVAL; }
+  JIMM_CUDA_CHECK(cudaSetDevice(idx->device));
+  return gallery_remove(idx->store, ids, n, removed, static_cast<cudaStream_t>(stream));
+}
+
+int jimm_index_live(const jimm_index_t* idx, long long* live) {
+  if (!idx || !live) { set_last_error("index live: null handle or count"); return JIMM_EINVAL; }
+  *live = gallery_live(idx->store);
+  return 0;
+}
+
+int jimm_index_compact(jimm_index_t* idx, int32_t* old_to_new, void* stream) {
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  JIMM_CUDA_CHECK(cudaSetDevice(idx->device));
+  return gallery_compact(idx->store, old_to_new, static_cast<cudaStream_t>(stream));
 }
 
 int jimm_index_destroy(jimm_index_t* idx) {

@@ -904,6 +904,147 @@ __global__ void __launch_bounds__(kRangeThreads) range_gather_kernel(const float
   }
 }
 
+// ---- removed rows and filters: a call runs over its allowed rows, the live rows it keeps, numbered 0 .. nA - 1 in ascending row order ----
+// The screen GEMM and the exact kernels read those rows through a chunk buffer (gather_rows_kernel), so they run unchanged on
+// positions, and the positions go back to row ids at the end: the map is monotone, so every order and tie rule carries over.
+constexpr int kAllowRows = 8192;  // rows per CTA of the allowed-id passes: 256 threads, one 32-row word each
+
+// Bit b: row 32 w + b (< n) is live (live null: every row is) and kept (keep null: every row is; else the byte is nonzero).
+__device__ __forceinline__ uint32_t allowed_word(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n, long long w) {
+  const long long r0 = w * 32;
+  if (r0 >= n) return 0u;
+  const int nb = static_cast<int>(min(n - r0, 32ll));
+  uint32_t m = live ? live[w] : 0xffffffffu;
+  if (nb < 32) m &= (1u << nb) - 1u;
+  if (keep) {
+    uint32_t kb = 0;
+    for (int b = 0; b < nb; ++b) kb |= (keep[r0 + b] ? 1u : 0u) << b;
+    m &= kb;
+  }
+  return m;
+}
+
+// grid (ceil(n / kAllowRows)): count[b] = the allowed rows among block b's kAllowRows.
+__global__ void __launch_bounds__(256) allowed_count_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n,
+                                                            int* __restrict__ count) {
+  __shared__ int warp_sums[32], total;
+  const long long w = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  block_exclusive_scan(__popc(allowed_word(live, keep, n, w)), warp_sums, &total);
+  if (threadIdx.x == 0) count[blockIdx.x] = total;
+}
+
+// One CTA: start[b] = the allowed rows before block b (exclusive prefix sum of count over nb blocks), start[nb] = all of them.
+__global__ void __launch_bounds__(1024) allowed_scan_kernel(const int* __restrict__ count, int nb, int* __restrict__ start) {
+  __shared__ int warp_sums[32], total;
+  int run = 0;
+  for (int b0 = 0; b0 < nb; b0 += blockDim.x) {
+    const int b = b0 + threadIdx.x;
+    const int o = block_exclusive_scan(b < nb ? count[b] : 0, warp_sums, &total);
+    if (b < nb) start[b] = run + o;
+    run += total;
+  }
+  if (threadIdx.x == 0) start[nb] = run;
+}
+
+// grid as allowed_count_kernel: block b's allowed rows, ascending, to ids[start[b] ..].
+__global__ void __launch_bounds__(256) allowed_scatter_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n,
+                                                              const int* __restrict__ start, int* __restrict__ ids) {
+  __shared__ int warp_sums[32], total;
+  const long long w = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  uint32_t m = allowed_word(live, keep, n, w);
+  int at = start[blockIdx.x] + block_exclusive_scan(__popc(m), warp_sums, &total);
+  for (; m; m &= m - 1) ids[at++] = static_cast<int>(w * 32 + __ffs(m) - 1);
+}
+
+// One warp per row r < pn: stored row ids[r] -- its normalised fp32 row, fp16 copy and bound -- to row r of rows, half and bound, in
+// 16-byte pieces (E % 8 == 0).
+__global__ void __launch_bounds__(256) gather_rows_kernel(const float* __restrict__ g_rows, const __half* __restrict__ g_half,
+                                                          const float* __restrict__ g_bound, const int* __restrict__ ids, int pn, int E,
+                                                          float* __restrict__ rows, __half* __restrict__ half, float* __restrict__ bound) {
+  const int r = static_cast<int>((static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (r >= pn) return;
+  const size_t j = static_cast<size_t>(ids[r]);
+  const float4* fs = reinterpret_cast<const float4*>(g_rows + j * E);
+  float4* fd = reinterpret_cast<float4*>(rows + static_cast<size_t>(r) * E);
+  for (int e = lane; e < E / 4; e += 32) fd[e] = __ldg(fs + e);
+  const uint4* hs = reinterpret_cast<const uint4*>(g_half + j * E);
+  uint4* hd = reinterpret_cast<uint4*>(half + static_cast<size_t>(r) * E);
+  for (int e = lane; e < E / 8; e += 32) hd[e] = __ldg(hs + e);
+  if (lane == 0) bound[r] = g_bound[j];
+}
+
+// The outputs of a search over positions: index p < na becomes row ids[p]; a padding slot (index -1, from kPadCand, or any slot when
+// na == 0) becomes (-inf, -1).
+__global__ void __launch_bounds__(256) search_ids_kernel(float* __restrict__ values, int32_t* __restrict__ indices, long long n,
+                                                         const int* __restrict__ ids, int na) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = indices[i];
+  if (p >= 0 && p < na) {
+    indices[i] = ids[p];
+  } else {
+    values[i] = -INFINITY;
+    indices[i] = -1;
+  }
+}
+
+// index[i] = ids[index[i]] for the n hits of a range search or pairs call over positions.
+__global__ void __launch_bounds__(256) hits_ids_kernel(int32_t* __restrict__ index, long long n, const int* __restrict__ ids) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) index[i] = ids[index[i]];
+}
+
+// Pairs over positions, query rows q0 .. q0 + qn - 1 (offsets pos_off [qn + 1]), to stored rows lo .. lo + R - 1: the offset of row r
+// is the one of the first position p with ids[p] >= r, so a row that is not allowed gets no hits.  R + 1 threads.
+__global__ void __launch_bounds__(256) pairs_rows_kernel(const int* __restrict__ ids, int q0, int qn, int lo, int R,
+                                                         const long long* __restrict__ pos_off, long long* __restrict__ row_off) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x > R) return;
+  const long long r = static_cast<long long>(lo) + x;
+  int a = q0, b = q0 + qn;  // lower bound of r in ids[q0 .. q0 + qn)
+  while (a < b) {
+    const int c = (a + b) >> 1;
+    if (ids[c] < r) a = c + 1;
+    else b = c;
+  }
+  row_off[x] = pos_off[a - q0];
+}
+
+// The ids of a removal, n of them: info[0] counts those outside [0, rows).
+__global__ void __launch_bounds__(256) remove_check_kernel(const int* __restrict__ ids, int n, long long rows, unsigned long long* __restrict__ info) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && (ids[i] < 0 || ids[i] >= rows)) atomicAdd(info, 1ull);
+}
+
+// Unless remove_check_kernel found a bad id (info[0] != 0): clears bit ids[i] of live, and info[1] counts the bits that were set.
+__global__ void __launch_bounds__(256) remove_kernel(const int* __restrict__ ids, int n, uint32_t* __restrict__ live, unsigned long long* __restrict__ info) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || info[0] != 0) return;
+  const uint32_t bit = 1u << (ids[i] & 31);
+  if (atomicAnd(live + (ids[i] >> 5), ~bit) & bit) atomicAdd(info + 1, 1ull);
+}
+
+// old_to_new[ids[p]] = p for the na live rows (the others were set to -1).
+__global__ void __launch_bounds__(256) compact_map_kernel(const int* __restrict__ ids, int na, int32_t* __restrict__ old_to_new) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < na) old_to_new[ids[p]] = p;
+}
+
+int alloc_async(void** p, size_t bytes, const char* what, cudaStream_t st) {
+  const cudaError_t e = cudaMallocAsync(p, bytes, st);
+  if (e == cudaSuccess) return 0;
+  cudaGetLastError();
+  *p = nullptr;
+  set_last_error("index: %s of %zu bytes -> %s", what, bytes, cudaGetErrorString(e));
+  return e == cudaErrorMemoryAllocation ? JIMM_ENOMEM : JIMM_ECUDA;
+}
+
+int launched(cudaError_t e, const char* what) {
+  if (e == cudaSuccess) { note_launch(); return 0; }
+  set_last_error("%s -> %s", what, cudaGetErrorString(e));
+  return JIMM_ECUDA;
+}
+
 }  // namespace
 
 struct GalleryStore {
@@ -912,7 +1053,80 @@ struct GalleryStore {
   float* rows = nullptr;   // [cap, E] normalised by l2_normalize_run: the bits search_run computes
   __half* half = nullptr;  // [cap, E] fp16 copy, the screen's B operand
   float* bound = nullptr;  // [cap] norm bounds (prep_rows_kernel)
+  // Removed rows: bit r of live is clear.  The bitset exists from the first removal to the next compaction, [ceil(cap / 32)] words
+  // with every bit past n set, so added rows are live as they are.  removed counts the clear bits below n.
+  uint32_t* live = nullptr;
+  long long removed = 0;
 };
+
+namespace {
+
+long long live_words(long long rows) { return (rows + 31) / 32; }
+
+// The ascending ids of the live rows that keep keeps (device bytes [n], nonzero keeps; null keeps every row) in *ids, allocated in
+// stream order for the caller to free (null when there are none), and their number in *na.  Waits for the stream once.
+int allowed_ids(const GalleryStore* g, const uint8_t* keep, int** ids, int* na, cudaStream_t st) {
+  *ids = nullptr;
+  *na = 0;
+  if (g->n == 0) return 0;
+  const int nb = static_cast<int>((g->n + kAllowRows - 1) / kAllowRows);
+  int* count = nullptr;
+  if (int rc = alloc_async(reinterpret_cast<void**>(&count), (2 * static_cast<size_t>(nb) + 1) * sizeof(int), "allowed-row counts", st)) return rc;
+  int* start = count + nb;
+  auto run = [&]() -> int {
+    if (int e = launched(launch_k(allowed_count_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, g->n, count), "allowed_count_kernel"))
+      return e;
+    if (int e = launched(launch_k(allowed_scan_kernel, dim3(1), dim3(1024), 0, st, 1, false, count, nb, start), "allowed_scan_kernel")) return e;
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(na, start + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (*na == 0) return 0;
+    if (int e = alloc_async(reinterpret_cast<void**>(ids), static_cast<size_t>(*na) * sizeof(int), "allowed-row ids", st)) return e;
+    return launched(launch_k(allowed_scatter_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, g->n, start, *ids),
+                    "allowed_scatter_kernel");
+  };
+  const int rc = run();
+  if (rc != 0 && *ids) {
+    cudaFreeAsync(*ids, st);
+    *ids = nullptr;
+  }
+  return free_scratch(count, st, rc);
+}
+
+// Allowed rows p0 .. p0 + pn - 1 (ids[p0 ..]) into the chunk buffer rows / half / bound.
+int gather_rows(const GalleryStore* g, const int* ids, int pn, float* rows, __half* half, float* bound, cudaStream_t st) {
+  if (pn <= 0) return 0;
+  return launched(launch_k(gather_rows_kernel, dim3(static_cast<unsigned>((pn + 7) / 8)), dim3(256), 0, st, 1, false, g->rows, g->half, g->bound,
+                           ids, pn, g->E, rows, half, bound),
+                  "gather_rows_kernel");
+}
+
+// The rows a search or range search reads: every stored row (ids null), or the allowed rows ids[0 .. n) through a chunk buffer of
+// kScreenCols rows.  rows / half / bound point at positions p0 .. of the view after at(p0, pn).
+struct RowView {
+  const GalleryStore* g;
+  const int* ids;
+  int n;
+  float* buf_rows;
+  __half* buf_half;
+  float* buf_bound;
+  float* rows = nullptr;
+  __half* half = nullptr;
+  float* bound = nullptr;
+  int at(int p0, int pn, cudaStream_t st) {
+    if (!ids) {
+      rows = g->rows + static_cast<size_t>(p0) * g->E;
+      half = g->half + static_cast<size_t>(p0) * g->E;
+      bound = g->bound + p0;
+      return 0;
+    }
+    rows = buf_rows;
+    half = buf_half;
+    bound = buf_bound;
+    return gather_rows(g, ids + p0, pn, buf_rows, buf_half, buf_bound, st);
+  }
+};
+
+}  // namespace
 
 int gallery_create(int E, GalleryStore** out) {
   if (E <= 0 || E % 8 != 0 || E > 1024 * 8) { set_last_error("index: embedding width %d must be a multiple of 8 in 8 .. 8192", E); return JIMM_EINVAL; }
@@ -934,17 +1148,20 @@ int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t st) {
     float* r = nullptr;
     __half* h = nullptr;
     float* b = nullptr;
+    uint32_t* l = nullptr;
     auto fail = [&](cudaError_t e, const char* what) {
       cudaGetLastError();
       if (r) cudaFreeAsync(r, st);
       if (h) cudaFreeAsync(h, st);
       if (b) cudaFreeAsync(b, st);
+      if (l) cudaFreeAsync(l, st);
       set_last_error("index: %s growing to %lld rows of width %d -> %s", what, cap, E, cudaGetErrorString(e));
       return e == cudaErrorMemoryAllocation ? JIMM_ENOMEM : JIMM_ECUDA;
     };
     cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&r), static_cast<size_t>(cap) * E * sizeof(float), st);
     if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&h), static_cast<size_t>(cap) * E * sizeof(__half), st);
     if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&b), static_cast<size_t>(cap) * sizeof(float), st);
+    if (e == cudaSuccess && g->live) e = cudaMallocAsync(reinterpret_cast<void**>(&l), live_words(cap) * sizeof(uint32_t), st);
     if (e != cudaSuccess) return fail(e, "allocation");
     if (g->n > 0) {
       e = cudaMemcpyAsync(r, g->rows, static_cast<size_t>(g->n) * E * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -952,10 +1169,19 @@ int gallery_add(GalleryStore* g, const float* rows, int n, cudaStream_t st) {
       if (e == cudaSuccess) e = cudaMemcpyAsync(b, g->bound, static_cast<size_t>(g->n) * sizeof(float), cudaMemcpyDeviceToDevice, st);
       if (e != cudaSuccess) return fail(e, "copy");
     }
+    if (l) {  // the new words live, then the old ones over them (their bits past n are set)
+      e = cudaMemsetAsync(l, 0xff, live_words(cap) * sizeof(uint32_t), st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(l, g->live, live_words(g->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) return fail(e, "copy");
+    }
     if (g->rows) {  // the new storage holds every row from here on
       cudaFreeAsync(g->rows, st);
       cudaFreeAsync(g->half, st);
       cudaFreeAsync(g->bound, st);
+    }
+    if (l) {
+      cudaFreeAsync(g->live, st);
+      g->live = l;
     }
     g->rows = r; g->half = h; g->bound = b; g->cap = cap;
   }
@@ -976,12 +1202,106 @@ void gallery_destroy(GalleryStore* g) {
   cudaFree(g->rows);
   cudaFree(g->half);
   cudaFree(g->bound);
+  cudaFree(g->live);
   delete g;
 }
 
-int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, float* values,
-                   int32_t* indices, long long* stats, cudaStream_t st) {
-  const int E = g->E, N = static_cast<int>(g->n);
+long long gallery_live(const GalleryStore* g) { return g->n - g->removed; }
+
+int gallery_remove(GalleryStore* g, const int* ids, int n, long long* removed, cudaStream_t st) {
+  *removed = 0;
+  if (n == 0) return 0;
+  if (!g->live) {  // the first removal: every row live, and every bit past n set
+    const long long words = live_words(g->cap);
+    if (int rc = alloc_async(reinterpret_cast<void**>(&g->live), words * sizeof(uint32_t), "live bitset", st)) return rc;
+    JIMM_CUDA_CHECK(cudaMemsetAsync(g->live, 0xff, words * sizeof(uint32_t), st));
+  }
+  unsigned long long* info = nullptr;
+  if (int rc = alloc_async(reinterpret_cast<void**>(&info), 2 * sizeof(unsigned long long), "removal counts", st)) return rc;
+  unsigned long long h[2] = {0, 0};
+  auto run = [&]() -> int {
+    JIMM_CUDA_CHECK(cudaMemsetAsync(info, 0, 2 * sizeof(unsigned long long), st));
+    const dim3 grid((n + 255) / 256);
+    if (int e = launched(launch_k(remove_check_kernel, grid, dim3(256), 0, st, 1, false, ids, n, g->n, info), "remove_check_kernel")) return e;
+    if (int e = launched(launch_k(remove_kernel, grid, dim3(256), 0, st, 1, false, ids, n, g->live, info), "remove_kernel")) return e;
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(h, info, sizeof(h), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (h[0] != 0) {
+      set_last_error("index remove: %llu of %d ids outside 0 .. %lld", h[0], n, g->n - 1);
+      return JIMM_EINVAL;
+    }
+    return 0;
+  };
+  const int rc = free_scratch(info, st, run());
+  if (rc == 0) {
+    g->removed += static_cast<long long>(h[1]);
+    *removed = static_cast<long long>(h[1]);
+  }
+  return rc;
+}
+
+int gallery_compact(GalleryStore* g, int32_t* old_to_new, cudaStream_t st) {
+  const int E = g->E;
+  int* ids = nullptr;
+  int na = 0;
+  if (g->removed == 0) {  // nothing to drop: the storage stays, the map is the identity
+    if (old_to_new && g->n > 0) {
+      if (int rc = allowed_ids(g, nullptr, &ids, &na, st)) return rc;
+      const int rc = launched(launch_k(compact_map_kernel, dim3((na + 255) / 256), dim3(256), 0, st, 1, false, ids, na, old_to_new),
+                              "compact_map_kernel");
+      return free_scratch(ids, st, rc);
+    }
+    return 0;
+  }
+  if (int rc = allowed_ids(g, nullptr, &ids, &na, st)) return rc;
+  float* r = nullptr;
+  __half* h = nullptr;
+  float* b = nullptr;
+  auto run = [&]() -> int {
+    if (na > 0) {
+      if (int e = alloc_async(reinterpret_cast<void**>(&r), static_cast<size_t>(na) * E * sizeof(float), "compacted rows", st)) return e;
+      if (int e = alloc_async(reinterpret_cast<void**>(&h), static_cast<size_t>(na) * E * sizeof(__half), "compacted fp16 rows", st)) return e;
+      if (int e = alloc_async(reinterpret_cast<void**>(&b), static_cast<size_t>(na) * sizeof(float), "compacted bounds", st)) return e;
+      constexpr int kPiece = 1 << 20;
+      for (int p0 = 0; p0 < na; p0 += kPiece) {
+        const size_t at = static_cast<size_t>(p0);
+        if (int e = gather_rows(g, ids + p0, std::min(kPiece, na - p0), r + at * E, h + at * E, b + at, st)) return e;
+      }
+    }
+    if (old_to_new) {
+      JIMM_CUDA_CHECK(cudaMemsetAsync(old_to_new, 0xff, static_cast<size_t>(g->n) * sizeof(int32_t), st));
+      if (na > 0)
+        if (int e = launched(launch_k(compact_map_kernel, dim3((na + 255) / 256), dim3(256), 0, st, 1, false, ids, na, old_to_new),
+                             "compact_map_kernel"))
+          return e;
+    }
+    return 0;
+  };
+  const int rc = run();
+  if (ids) cudaFreeAsync(ids, st);
+  if (rc != 0) {  // the index stays as it was
+    if (r) cudaFreeAsync(r, st);
+    if (h) cudaFreeAsync(h, st);
+    if (b) cudaFreeAsync(b, st);
+    return rc;
+  }
+  cudaFreeAsync(g->rows, st);
+  cudaFreeAsync(g->half, st);
+  cudaFreeAsync(g->bound, st);
+  cudaFreeAsync(g->live, st);
+  g->rows = r; g->half = h; g->bound = b; g->live = nullptr;
+  g->n = g->cap = na;
+  g->removed = 0;
+  return 0;
+}
+
+namespace {
+
+// gallery_search over the N rows of a view: every stored row (ids null) or the allowed rows ids[0 .. N), whose positions the outputs
+// then hold.
+int search_rows(const GalleryStore* g, const int* ids, int N, const float* queries, int Q, const float* logit_scale, const float* logit_bias,
+                int k, float* values, int32_t* indices, long long* stats, cudaStream_t st) {
+  const int E = g->E;
   const int qc = std::min(Q, kSearchRows), seed = std::min(N, kSearchCols);
   const bool screen = N > seed;
   const long long seed_ld = k + (seed + kSegCols - 1) / kSegCols * static_cast<long long>(k);
@@ -1005,8 +1325,13 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
     o_list = piece(static_cast<size_t>(qc) * kScreenCap * sizeof(int));
     o_info = piece(4 * sizeof(int));
   }
+  const int vc = ids ? std::min(N, kScreenCols) : 0;  // the view's chunk buffer
+  const size_t o_vrows = piece(static_cast<size_t>(vc) * E * sizeof(float));
+  const size_t o_vhalf = piece(static_cast<size_t>(vc) * E * sizeof(__half));
+  const size_t o_vbound = piece(static_cast<size_t>(vc) * sizeof(float));
   uint8_t* base = nullptr;
   JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&base), off, st));
+  RowView view{g, ids, N, reinterpret_cast<float*>(base + o_vrows), reinterpret_cast<__half*>(base + o_vhalf), reinterpret_cast<float*>(base + o_vbound)};
   u64* cand = reinterpret_cast<u64*>(base + o_cand);
   float* nq = reinterpret_cast<float*>(base + o_nq);
   float* block = reinterpret_cast<float*>(base + o_block);
@@ -1032,9 +1357,10 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
   // exact block step, tighten the thresholds.  Every error is returned, so the caller frees the scratch.
   auto screen_chunk = [&](int qn, int g0) -> int {
     const int gn = std::min(kScreenCols, N - g0);
-    sd.ng = g->bound + g0;
+    if (int e = view.at(g0, gn, st)) return e;
+    sd.ng = view.bound;
     JIMM_CUDA_CHECK(cudaMemsetAsync(cnt, 0, static_cast<size_t>(qn) * sizeof(int), st));
-    if (int e = gemm_screen_run(hq, qn, g->half + static_cast<size_t>(g0) * E, gn, E, sd, st)) return e;
+    if (int e = gemm_screen_run(hq, qn, view.half, gn, E, sd, st)) return e;
     JIMM_CUDA_CHECK(launch_k(screen_info_kernel, dim3(1), dim3(1024), 0, st, 1, false, cnt, qn, kScreenCap, ovl, info));
     note_launch();
     int h[3];
@@ -1044,7 +1370,7 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
     if (stats) { stats[0] += h[2]; stats[1] += nover; stats[2] += 1; }
     if (width > 0) {
       JIMM_CUDA_CHECK(launch_k(rescore_kernel, dim3((width + 127) / 128, qn), dim3(128), static_cast<size_t>(E) * sizeof(float), st, 1, false, nq,
-                               g->rows + static_cast<size_t>(g0) * E, E, cnt, list, kScreenCap, width, g0, logit_scale, logit_bias, cand, cand_ld, k));
+                               view.rows, E, cnt, list, kScreenCap, width, g0, logit_scale, logit_bias, cand, cand_ld, k));
       note_launch();
       if (int e = launch_merge(cand, qn, cand_ld, k + width, k, lo, cand, nullptr, 0, 0, nullptr, nullptr, nullptr, st)) return e;
     }
@@ -1052,7 +1378,7 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
       JIMM_CUDA_CHECK(launch_k(fallback_copy_kernel, dim3(nover), dim3(256), 0, st, 1, false, ovl, E, k, nq, fq, cand, cand_ld, fcand, fcand_ld, 1));
       note_launch();
       for (int s0 = 0; s0 < gn; s0 += kSearchCols)
-        if (int e = block_step(fq, nover, g->rows + static_cast<size_t>(g0 + s0) * E, std::min(kSearchCols, gn - s0), g0 + s0, E, logit_scale,
+        if (int e = block_step(fq, nover, view.rows + static_cast<size_t>(s0) * E, std::min(kSearchCols, gn - s0), g0 + s0, E, logit_scale,
                                logit_bias, k, lo, block, fcand, fcand_ld, false, false, nullptr, nullptr, st))
           return e;
       JIMM_CUDA_CHECK(launch_k(fallback_copy_kernel, dim3(nover), dim3(256), 0, st, 1, false, ovl, E, k, nq, fq, cand, cand_ld, fcand, fcand_ld, 0));
@@ -1064,7 +1390,8 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
     const int qn = std::min(qc, Q - q0);
     const size_t o = static_cast<size_t>(q0) * k;
     rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
-    if (rc == 0) rc = block_step(nq, qn, g->rows, seed, 0, E, logit_scale, logit_bias, k, lo, block, cand, cand_ld, true, !screen, values + o, indices + o, st);
+    if (rc == 0) rc = view.at(0, seed, st);
+    if (rc == 0) rc = block_step(nq, qn, view.rows, seed, 0, E, logit_scale, logit_bias, k, lo, block, cand, cand_ld, true, !screen, values + o, indices + o, st);
     if (!screen) continue;
     if (rc == 0) rc = prep_rows_run(nq, qn, E, hq, nbq, st);
     if (rc == 0) rc = threshold(qn);
@@ -1072,6 +1399,24 @@ int gallery_search(const GalleryStore* g, const float* queries, int Q, const flo
     if (rc == 0) rc = launch_merge(cand, qn, cand_ld, k, k, lo, nullptr, nullptr, 0, 0, values + o, indices + o, nullptr, st);
   }
   return free_scratch(base, st, rc);
+}
+
+}  // namespace
+
+int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, const uint8_t* keep,
+                   float* values, int32_t* indices, long long* stats, cudaStream_t st) {
+  if (!keep && g->removed == 0)
+    return search_rows(g, nullptr, static_cast<int>(g->n), queries, Q, logit_scale, logit_bias, k, values, indices, stats, st);
+  // over the allowed rows' positions, then to row ids; with fewer than k of them the slots past the last are padding
+  int* ids = nullptr;
+  int na = 0;
+  if (int rc = allowed_ids(g, keep, &ids, &na, st)) return rc;
+  int rc = na == 0 ? 0 : search_rows(g, ids, na, queries, Q, logit_scale, logit_bias, k, values, indices, stats, st);
+  const long long n = static_cast<long long>(Q) * k;
+  if (rc == 0 && n > 0)
+    rc = launched(launch_k(search_ids_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, 1, false, values, indices, n, ids, na),
+                  "search_ids_kernel");
+  return ids ? free_scratch(ids, st, rc) : rc;
 }
 
 }  // namespace jimm
@@ -1100,23 +1445,39 @@ void hits_free(jimm_hits* h, cudaStream_t st) {  // in stream order
 }
 
 int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs, float threshold, const float* logit_scale,
-                  const float* logit_bias, jimm_hits** out, long long* stats, cudaStream_t st) {
-  const int E = g->E, N = static_cast<int>(g->n);
-  if (pairs) Q = N;
+                  const float* logit_bias, const uint8_t* keep, jimm_hits** out, long long* stats, cudaStream_t st) {
+  const int E = g->E;
   *out = nullptr;
   int device = 0;
   JIMM_CUDA_CHECK(cudaGetDevice(&device));
+  // A filter or removed rows: the call runs over the N allowed rows' positions (ids), then maps the hits and, for pairs, the result's
+  // rows back to row ids.
+  const bool filtered = keep || g->removed > 0;
+  int* ids = nullptr;
+  int N = static_cast<int>(g->n);
+  if (filtered)
+    if (int rc = allowed_ids(g, keep, &ids, &N, st)) return rc;
+  if (pairs) Q = N;
   jimm_hits* hits = new jimm_hits();
   hits->device = device;
   hits->rows = Q;
-  if (Q == 0) { *out = hits; return 0; }
-  const int qc = std::min(Q, kSearchRows), nch = (N + kScreenCols - 1) / kScreenCols;
+  if (Q == 0 && !(pairs && filtered)) {
+    if (ids) cudaFreeAsync(ids, st);
+    *out = hits;
+    return 0;
+  }
+  const int qc = std::max(std::min(Q, kSearchRows), 1), nch = (N + kScreenCols - 1) / kScreenCols;
   // scratch: 256-byte aligned pieces of one stream-ordered allocation
   size_t off = 0;
   auto piece = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
-  const size_t o_nq = pairs ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(float));
-  const size_t o_hq = pairs ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(__half));
-  const size_t o_nbq = pairs ? 0 : piece(static_cast<size_t>(qc) * sizeof(float));
+  const bool qbuf = !pairs || filtered;  // the queries, or the allowed stored rows of a pairs call, are staged in nq / hq / nbq
+  const size_t o_nq = qbuf ? piece(static_cast<size_t>(qc) * E * sizeof(float)) : 0;
+  const size_t o_hq = qbuf ? piece(static_cast<size_t>(qc) * E * sizeof(__half)) : 0;
+  const size_t o_nbq = qbuf ? piece(static_cast<size_t>(qc) * sizeof(float)) : 0;
+  const int vc = ids ? std::min(N, kScreenCols) : 0;  // the gallery view's chunk buffer
+  const size_t o_vrows = piece(static_cast<size_t>(vc) * E * sizeof(float));
+  const size_t o_vhalf = piece(static_cast<size_t>(vc) * E * sizeof(__half));
+  const size_t o_vbound = piece(static_cast<size_t>(vc) * sizeof(float));
   const size_t o_fq = piece(static_cast<size_t>(qc) * E * sizeof(float));
   const size_t o_block = piece(static_cast<size_t>(qc) * std::min(N, kSearchCols) * sizeof(float));
   const size_t o_t = piece(static_cast<size_t>(qc) * sizeof(float));
@@ -1142,6 +1503,7 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
   auto fail = [&](int rc) {
     free_stage();
     hits_free(hits, st);
+    if (ids) cudaFreeAsync(ids, st);
     return base ? free_scratch(base, st, rc) : rc;
   };
   auto alloc = [&](void** p, size_t bytes, const char* what) -> int {
@@ -1166,6 +1528,8 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
   int* pos = reinterpret_cast<int*>(base + o_pos);
   int* count = reinterpret_cast<int*>(base + o_count);
   long long* dst = reinterpret_cast<long long*>(base + o_dst);
+  RowView view{g, ids, N, reinterpret_cast<float*>(base + o_vrows), reinterpret_cast<__half*>(base + o_vhalf), reinterpret_cast<float*>(base + o_vbound)};
+  RowView qview{g, ids, N, nq, hq, nbq};  // pairs: the query rows
   GemmScreen sd;
   sd.t = t; sd.cnt = cnt; sd.list = list; sd.cap = kScreenCap;
   const int max_smem = static_cast<int>(8192 * sizeof(float) + kScreenCap * sizeof(u64));
@@ -1183,9 +1547,10 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
     const int row0 = pairs ? q0 : -1;
     int* pos_c = pos + static_cast<size_t>(c) * qn;
     int* count_c = count + static_cast<size_t>(c) * qn;
-    sd.ng = g->bound + g0;
+    if (int e = view.at(g0, gn, st)) return e;
+    sd.ng = view.bound;
     JIMM_CUDA_CHECK(cudaMemsetAsync(cnt, 0, static_cast<size_t>(qn) * sizeof(int), st));
-    if (int e = gemm_screen_run(qh, qn, g->half + static_cast<size_t>(g0) * E, gn, E, sd, st)) return e;
+    if (int e = gemm_screen_run(qh, qn, view.half, gn, E, sd, st)) return e;
     if (int e = check_launch(launch_k(range_info_kernel, dim3(1), dim3(1024), 0, st, 1, false, cnt, qn, kScreenCap, gn, ovl, pos_c, info),
                              "range_info_kernel"))
       return e;
@@ -1201,8 +1566,7 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
     int32_t* si = reinterpret_cast<int32_t*>(ss + room);
     if (widest > 0) {
       const size_t smem = static_cast<size_t>(E) * sizeof(float) + static_cast<size_t>(pow2_at_least(widest)) * sizeof(u64);
-      if (int e = check_launch(launch_k(range_rescore_kernel, dim3(qn), dim3(kRangeThreads), smem, st, 1, false, qrows,
-                                        g->rows + static_cast<size_t>(g0) * E, E, cnt, list, kScreenCap, g0, row0, threshold, logit_scale,
+      if (int e = check_launch(launch_k(range_rescore_kernel, dim3(qn), dim3(kRangeThreads), smem, st, 1, false, qrows, view.rows, E, cnt, list, kScreenCap, g0, row0, threshold, logit_scale,
                                         logit_bias, pos_c, ss, si, count_c),
                                "range_rescore_kernel"))
         return e;
@@ -1214,7 +1578,7 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
         return e;
       for (int s0 = 0; s0 < gn; s0 += kSearchCols) {
         const int pw = std::min(kSearchCols, gn - s0);
-        if (int e = logits_run(fq, g->rows + static_cast<size_t>(g0 + s0) * E, logit_scale, logit_bias, block, nover, pw, E, pw, st)) return e;
+        if (int e = logits_run(fq, view.rows + static_cast<size_t>(s0) * E, logit_scale, logit_bias, block, nover, pw, E, pw, st)) return e;
         if (int e = check_launch(launch_k(range_block_kernel, dim3(nover), dim3(kRangeThreads), 0, st, 1, false, block, pw, ovl, g0 + s0, row0,
                                           threshold, pos_c, ss, si, count_c),
                                  "range_block_kernel"))
@@ -1252,8 +1616,49 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
                                  "range_gather_kernel"))
           return e;
       }
+      if (ids && check_launch(launch_k(hits_ids_kernel, dim3(static_cast<unsigned>((sg.nnz + 255) / 256)), dim3(256), 0, st, 1, false, idx,
+                                       sg.nnz, ids),
+                              "hits_ids_kernel"))
+        return JIMM_ECUDA;
     }
     done = end;
+    return 0;
+  };
+  // Filtered pairs: the result's rows are the stored rows 0 .. g->n - 1, so segment s of query positions q0 .. q0 + qn - 1 becomes the
+  // stored rows after the previous segment's up to its last allowed row (the last segment: up to the end), those not allowed empty.
+  auto pairs_rows = [&]() -> int {
+    const int rows = static_cast<int>(g->n);
+    if (hits->segs.empty()) {  // no allowed row
+      jimm_hits::Segment seg;
+      seg.rows = rows;
+      if (int e = alloc(reinterpret_cast<void**>(&seg.offsets), static_cast<size_t>(rows + 1) * sizeof(long long), "result offsets")) return e;
+      hits->segs.push_back(seg);
+      JIMM_CUDA_CHECK(cudaMemsetAsync(seg.offsets, 0, static_cast<size_t>(rows + 1) * sizeof(long long), st));
+    } else {
+      const size_t ns = hits->segs.size();
+      std::vector<int> last(ns, rows - 1);  // the last allowed row of each segment but the last
+      for (size_t s = 0; s + 1 < ns; ++s)
+        JIMM_CUDA_CHECK(cudaMemcpyAsync(&last[s], ids + s * qc + hits->segs[s].rows - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+      JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+      int lo = 0;
+      for (size_t s = 0; s < ns; ++s) {
+        jimm_hits::Segment& sg = hits->segs[s];
+        const int R = last[s] + 1 - lo;
+        long long* ro = nullptr;
+        if (int e = alloc(reinterpret_cast<void**>(&ro), static_cast<size_t>(R + 1) * sizeof(long long), "result offsets")) return e;
+        if (int e = check_launch(launch_k(pairs_rows_kernel, dim3((R + 256) / 256), dim3(256), 0, st, 1, false, ids, static_cast<int>(s * qc), sg.rows,
+                                          lo, R, sg.offsets, ro),
+                                 "pairs_rows_kernel")) {
+          cudaFreeAsync(ro, st);
+          return e;
+        }
+        cudaFreeAsync(sg.offsets, st);
+        sg.offsets = ro;
+        sg.rows = R;
+        lo += R;
+      }
+    }
+    hits->rows = rows;
     return 0;
   };
   if (int rc = check_launch(launch_k(range_threshold_kernel, dim3((qc + 255) / 256), dim3(256), 0, st, 1, false, qc, threshold, logit_scale,
@@ -1266,9 +1671,10 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
     const __half* qh = hq;
     int rc = 0;
     if (pairs) {  // the stored rows themselves: normalised, with their fp16 copies and bounds
-      qrows = g->rows + static_cast<size_t>(q0) * E;
-      qh = g->half + static_cast<size_t>(q0) * E;
-      sd.nq = g->bound + q0;
+      rc = qview.at(q0, qn, st);
+      qrows = qview.rows;
+      qh = qview.half;
+      sd.nq = qview.bound;
     } else {
       sd.nq = nbq;
       rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
@@ -1283,8 +1689,11 @@ int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs
     if (rc != 0) return fail(rc);
     free_stage();
   }
+  if (pairs && filtered)
+    if (int rc = pairs_rows()) return fail(rc);
   hits->total = done;
   *out = hits;
+  if (ids) cudaFreeAsync(ids, st);
   return free_scratch(base, st, 0);
 }
 
