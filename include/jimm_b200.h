@@ -568,6 +568,26 @@ JIMM_API int jimm_index_range_search_keep(jimm_index_t* idx, const float* querie
 JIMM_API int jimm_index_pairs_keep(jimm_index_t* idx, float threshold, const uint8_t* keep, jimm_hits_t** out, jimm_search_stats* stats,
                                    void* stream);
 JIMM_API int jimm_index_compact(jimm_index_t* idx, int32_t* old_to_new, void* stream);
+/* Spherical k-means over the stored rows of a gallery index.  The rows are the normalised rows jimm_index_add stored.  A row takes part
+ * when it is live, kept (keep as jimm_index_search_keep) and its norm bound is at most 2 (zero, non-finite and subnormal-sum rows are
+ * not); the others get assign -1 and score -inf.  score(x, c) = jimm_k_logits(x, c) at logit_scale 0 (exp(0) = 1) and no bias: the
+ * cosine, whatever the model's logit_scale and logit_bias.  Initial means m_0 [C, E]: init_vectors (device fp32 [C, E]), the stored rows
+ * init_ids (device int32 [C], each a row that takes part, repeats allowed), or, both NULL, the rows at the first C positions of
+ * top_k(keys, C) with key 1 + (splitmix64(seed + id) >> 41) 2^-23 for the rows taking part in ascending id (splitmix64(x): the first
+ * output of the generator with state x).  Step t = 0, 1, ..: c_t = l2_normalize(m_t); a_t = each row's best cluster (top_k at k = 1:
+ * equal scores to the larger cluster); stop when t + 1 == iters or t > 0 and a_t == a_{t-1}; else m_{t+1}[j] = fp32(fp64(S_j) 2^-30 /
+ * n_j), S_j[e] = sum over the n_j rows x of cluster j of rint(x[e] 2^30) in int64 (exact, so independent of order), keeping m_t[j] when
+ * n_j = 0 or l2_normalize(m_{t+1}[j]) is not finite.  Outputs (device): centroids fp32 [C, E] = the c_t of the last step, assign int32
+ * [rows], scores fp32 [rows] (each row's score against its centroid), counts int64 [C] (rows per cluster under assign); *iterations
+ * (host) = the steps run.  stats sums jimm_index_search's counters over the steps.  JIMM_EINVAL before any launch for C outside 1 ..
+ * 65536, iters < 1 or both inits given; after a check on the device and before any output is written for init ids that do not take
+ * part (or are outside 0 .. rows - 1), initial centroids whose l2_normalize is not finite, or sampling more clusters than rows taking
+ * part.  Memory, in stream order: 8 C E bytes of sums, 18 C E + 20 C bytes of means, centroids and their fp16 copies, 16 bytes per row
+ * taking part, and a search's scratch per step.  Waits for `stream` to list the rows, to check the initial centroids, once per step
+ * and once per screened chunk of 2048 rows. */
+JIMM_API int jimm_index_kmeans(jimm_index_t* idx, int C, const float* init_vectors, const int32_t* init_ids, unsigned long long seed, int iters,
+                               const uint8_t* keep, float* centroids, int32_t* assign, float* scores, int64_t* counts, int* iterations,
+                               jimm_search_stats* stats, void* stream);
 /* Micro-benchmark (not on the product path): TMA fill bandwidth from L2 with `cluster` CTAs per cluster.  mode 0: every CTA loads
  * its own 16 KB tiles; 1: the CTAs of a cluster load the same tile each; 2: same tile, each loads 1/cluster of it and multicasts. */
 JIMM_API int jimm_k_l2_probe(const void* buf, int rows, int mode, int cluster, int iters, float* ms, void* stream);

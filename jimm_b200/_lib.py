@@ -175,6 +175,7 @@ SIGNATURES = {
     "jimm_index_range_search_keep": (_i, [_vp, _fp, _i, _f, _vp, C.POINTER(_vp), C.c_void_p, _vp]),
     "jimm_index_pairs_keep": (_i, [_vp, _f, _vp, C.POINTER(_vp), C.c_void_p, _vp]),
     "jimm_index_compact": (_i, [_vp, _vp, _vp]),
+    "jimm_index_kmeans": (_i, [_vp, _i, _vp, _vp, C.c_ulonglong, _i, _vp, _fp, _ip, _fp, _vp, C.POINTER(_i), C.c_void_p, _vp]),
     "jimm_preproc_create": (_i, [C.POINTER(PreprocConfig), _i, C.POINTER(_vp)]),
     "jimm_preproc_output_size": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "jimm_preproc_run": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp]),

@@ -631,6 +631,16 @@ class NativeModel:
         return out
 
 
+class KMeans(NamedTuple):
+    """The result of GalleryIndex.kmeans, on the index's device."""
+
+    centroids: torch.Tensor  # fp32 [C, E], unit rows: the centroids the last assignment step used
+    assign: torch.Tensor  # int32 [len(index)]: each row's cluster, -1 for rows that take no part
+    scores: torch.Tensor  # fp32 [len(index)]: each row's score against its centroid, -inf where assign is -1
+    counts: torch.Tensor  # int64 [C]: rows per cluster under assign
+    iterations: int  # assignment steps run (<= iters)
+
+
 class GalleryIndex:
     """A gallery normalised once and kept on the GPU (jimm_index_*): search(queries, k) is NativeModel.search(queries, every row added
     so far, k) on the model's current handle, bit for bit; range_search(queries, threshold) and pairs(threshold) give every score at or
@@ -643,7 +653,7 @@ class GalleryIndex:
     def __init__(self, native: Callable[[], NativeModel], gallery=None):
         self._native = native
         m = native()
-        self._bound, self._lib, self._device = m, m.lib, m.device
+        self._bound, self._lib, self._device, self._width = m, m.lib, m.device, m.text_out
         self.handle = C.c_void_p()
         _lib.check(m.lib.jimm_index_create(m.handle, C.byref(self.handle)))
         self._rows = 0
@@ -768,6 +778,43 @@ class GalleryIndex:
             _call(m.lib, m.device, "jimm_index_search_keep", self.handle, qd, Q, k, mask, values, indices, None)
         host = not q.is_cuda
         return m._back(values, host).result(), m._back(indices, host).result()
+
+    def kmeans(self, n_clusters: int, iters: int = 20, init=None, seed: int = 0, keep=None) -> "KMeans":
+        """Spherical k-means over the stored rows (jimm_index_kmeans): at most `iters` assignment steps of each row to its best centroid
+        by cosine (the model's logit_scale and logit_bias play no part), each followed by the mean of every cluster's rows summed in
+        fixed point, so the result is the same bits on every run.  A row takes part when it is live, selected by keep (as in search)
+        and finite and non-zero; the others get assign -1 and score -inf.  init: None (rows sampled from `seed`), n_clusters integer row
+        ids (host or device, each a row that takes part), or a float32 / float16 / bfloat16 [n_clusters, E] tensor of vectors (host or
+        the index's device).  Stops early when an assignment repeats the previous one.  Returns a KMeans on the index's device."""
+        if not self.handle:
+            raise _lib.JimmError("gallery index: closed")
+        for name, v, lo, hi in (("n_clusters", n_clusters, 1, 65536), ("iters", iters, 1, 2**31 - 1), ("seed", seed, 0, 2**64 - 1)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+                raise ValueError(f"index kmeans: {name} must be an int in {lo} .. {hi}, got {v!r}")
+        Cn, E = int(n_clusters), self._width
+        vectors = ids = None
+        if init is not None:
+            t = _as_tensor(init)
+            if t.is_cuda and t.device != self._device:
+                raise ValueError(f"index kmeans: init is on {t.device}, the index on {self._device}")
+            if t.dtype.is_floating_point:
+                if t.dtype not in _TORCH_TO_CODE or tuple(t.shape) != (Cn, E):
+                    raise ValueError(f"index kmeans: init vectors must be float32 / float16 / bfloat16 of shape [{Cn}, {E}], got {t.dtype} "
+                                     f"{tuple(t.shape)}")
+                vectors = t.to(self._device, torch.float32, non_blocking=True).contiguous()
+            else:
+                if t.ndim != 1 or t.numel() != Cn:
+                    raise ValueError(f"index kmeans: init must be {Cn} row ids or a [{Cn}, {E}] float tensor, got {t.dtype} {tuple(t.shape)}")
+                ids = self._row_ids(t, "init ids")
+        mask = self._keep(keep)
+        centroids = torch.empty((Cn, E), dtype=torch.float32, device=self._device)
+        assign = torch.empty(self._rows, dtype=torch.int32, device=self._device)
+        scores = torch.empty(self._rows, dtype=torch.float32, device=self._device)
+        counts = torch.empty(Cn, dtype=torch.int64, device=self._device)
+        steps = C.c_int()
+        _call(self._lib, self._device, "jimm_index_kmeans", self.handle, Cn, vectors, ids, int(seed), int(iters), mask, centroids, assign,
+              scores, counts, C.byref(steps), None)
+        return KMeans(centroids, assign, scores, counts, steps.value)
 
     @staticmethod
     def _threshold(threshold) -> float:

@@ -119,6 +119,15 @@ int gallery_compact(GalleryStore* g, int32_t* old_to_new, cudaStream_t stream);
 // row for every stored row.
 int gallery_range(const GalleryStore* g, const float* queries, int Q, bool pairs, float threshold, const float* logit_scale,
                   const float* logit_bias, const uint8_t* keep, jimm_hits** out, long long* stats, cudaStream_t stream);
+// Spherical k-means over the clusterable rows (live, kept, norm bound <= 2) with C clusters (1 .. 65536) and at most iters assignment
+// steps; init: vectors (device fp32 [C, E]), row ids (device int32 [C]) or, both null, sampled from seed.  Outputs on the device:
+// centroids fp32 [C, E], assign int32 / scores fp32 [rows] (-1 / -inf for rows that take no part), counts int64 [C]; *iterations
+// (host).  stats as gallery_search, summed over the steps.  JIMM_EINVAL for init ids that are not clusterable, initial centroids with a
+// non-finite l2_normalize, or more sampled clusters than clusterable rows, before any output is written.  Waits for its stream to size
+// the rows, to check the initial centroids, once per screened chunk and once per step.
+int gallery_kmeans(const GalleryStore* g, int C, const float* init_vectors, const int32_t* init_ids, unsigned long long seed, int iters,
+                   const uint8_t* keep, float* centroids, int32_t* assign, float* scores, int64_t* counts, int* iterations, long long* stats,
+                   cudaStream_t stream);
 
 // dst[n*K + k] = cast(src[k*N + n])   (flax (in,out) kernel -> K-major [N,K] operand)
 int transpose_cast_run(const float* src, int K, int N, void* dst, int out_type, int ldd, cudaStream_t stream);

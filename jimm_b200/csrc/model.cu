@@ -1978,6 +1978,26 @@ int jimm_index_compact(jimm_index_t* idx, int32_t* old_to_new, void* stream) {
   return gallery_compact(idx->store, old_to_new, static_cast<cudaStream_t>(stream));
 }
 
+// k-means reads only the stored rows (scores at unit scale and zero bias), so like removal it needs the index's device, not its model.
+int jimm_index_kmeans(jimm_index_t* idx, int C, const float* init_vectors, const int32_t* init_ids, unsigned long long seed, int iters,
+                      const uint8_t* keep, float* centroids, int32_t* assign, float* scores, int64_t* counts, int* iterations,
+                      jimm_search_stats* stats, void* stream) {
+  if (!idx) { set_last_error("index: null handle"); return JIMM_EINVAL; }
+  if (C < 1 || C > 65536) { set_last_error("index kmeans: n_clusters=%d outside 1 .. 65536", C); return JIMM_EINVAL; }
+  if (iters < 1) { set_last_error("index kmeans: iters=%d must be at least 1", iters); return JIMM_EINVAL; }
+  if (init_vectors && init_ids) { set_last_error("index kmeans: give init vectors or init ids, not both"); return JIMM_EINVAL; }
+  if (!centroids || !counts || !iterations || (gallery_rows(idx->store) > 0 && (!assign || !scores))) {
+    set_last_error("index kmeans: null centroids, assign, scores, counts or iterations");
+    return JIMM_EINVAL;
+  }
+  JIMM_CUDA_CHECK(cudaSetDevice(idx->device));
+  long long st[3] = {0, 0, 0};
+  const int rc = gallery_kmeans(idx->store, C, init_vectors, init_ids, seed, iters, keep, centroids, assign, scores, counts, iterations, st,
+                                static_cast<cudaStream_t>(stream));
+  if (stats) { stats->rows_rescored = st[0]; stats->fallbacks = st[1]; stats->chunks_screened = st[2]; }
+  return rc;
+}
+
 int jimm_index_destroy(jimm_index_t* idx) {
   if (!idx) return 0;
   JIMM_CUDA_CHECK(cudaSetDevice(idx->device));

@@ -909,8 +909,12 @@ __global__ void __launch_bounds__(kRangeThreads) range_gather_kernel(const float
 // positions, and the positions go back to row ids at the end: the map is monotone, so every order and tie rule carries over.
 constexpr int kAllowRows = 8192;  // rows per CTA of the allowed-id passes: 256 threads, one 32-row word each
 
-// Bit b: row 32 w + b (< n) is live (live null: every row is) and kept (keep null: every row is; else the byte is nonzero).
-__device__ __forceinline__ uint32_t allowed_word(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n, long long w) {
+constexpr float kClusterBound = 2.f;  // k-means takes the rows whose norm bound is at most this: |x[e]| <= 2, so x[e] 2^30 fits 32 bits
+
+// Bit b: row 32 w + b (< n) is live (live null: every row is), kept (keep null: every row is; else the byte is nonzero) and, bound
+// non-null, clusterable (bound <= kClusterBound).
+__device__ __forceinline__ uint32_t allowed_word(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, const float* __restrict__ bound,
+                                                 long long n, long long w) {
   const long long r0 = w * 32;
   if (r0 >= n) return 0u;
   const int nb = static_cast<int>(min(n - r0, 32ll));
@@ -921,15 +925,20 @@ __device__ __forceinline__ uint32_t allowed_word(const uint32_t* __restrict__ li
     for (int b = 0; b < nb; ++b) kb |= (keep[r0 + b] ? 1u : 0u) << b;
     m &= kb;
   }
+  if (bound) {
+    uint32_t bb = 0;
+    for (int b = 0; b < nb; ++b) bb |= (bound[r0 + b] <= kClusterBound ? 1u : 0u) << b;
+    m &= bb;
+  }
   return m;
 }
 
 // grid (ceil(n / kAllowRows)): count[b] = the allowed rows among block b's kAllowRows.
-__global__ void __launch_bounds__(256) allowed_count_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n,
-                                                            int* __restrict__ count) {
+__global__ void __launch_bounds__(256) allowed_count_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep,
+                                                            const float* __restrict__ bound, long long n, int* __restrict__ count) {
   __shared__ int warp_sums[32], total;
   const long long w = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  block_exclusive_scan(__popc(allowed_word(live, keep, n, w)), warp_sums, &total);
+  block_exclusive_scan(__popc(allowed_word(live, keep, bound, n, w)), warp_sums, &total);
   if (threadIdx.x == 0) count[blockIdx.x] = total;
 }
 
@@ -947,11 +956,12 @@ __global__ void __launch_bounds__(1024) allowed_scan_kernel(const int* __restric
 }
 
 // grid as allowed_count_kernel: block b's allowed rows, ascending, to ids[start[b] ..].
-__global__ void __launch_bounds__(256) allowed_scatter_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep, long long n,
-                                                              const int* __restrict__ start, int* __restrict__ ids) {
+__global__ void __launch_bounds__(256) allowed_scatter_kernel(const uint32_t* __restrict__ live, const uint8_t* __restrict__ keep,
+                                                              const float* __restrict__ bound, long long n, const int* __restrict__ start,
+                                                              int* __restrict__ ids) {
   __shared__ int warp_sums[32], total;
   const long long w = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  uint32_t m = allowed_word(live, keep, n, w);
+  uint32_t m = allowed_word(live, keep, bound, n, w);
   int at = start[blockIdx.x] + block_exclusive_scan(__popc(m), warp_sums, &total);
   for (; m; m &= m - 1) ids[at++] = static_cast<int>(w * 32 + __ffs(m) - 1);
 }
@@ -1063,9 +1073,10 @@ namespace {
 
 long long live_words(long long rows) { return (rows + 31) / 32; }
 
-// The ascending ids of the live rows that keep keeps (device bytes [n], nonzero keeps; null keeps every row) in *ids, allocated in
-// stream order for the caller to free (null when there are none), and their number in *na.  Waits for the stream once.
-int allowed_ids(const GalleryStore* g, const uint8_t* keep, int** ids, int* na, cudaStream_t st) {
+// The ascending ids of the live rows that keep keeps (device bytes [n], nonzero keeps; null keeps every row) and, clusterable, whose
+// norm bound is at most kClusterBound, in *ids, allocated in stream order for the caller to free (null when there are none), and their
+// number in *na.  Waits for the stream once.
+int allowed_ids(const GalleryStore* g, const uint8_t* keep, int** ids, int* na, cudaStream_t st, bool clusterable = false) {
   *ids = nullptr;
   *na = 0;
   if (g->n == 0) return 0;
@@ -1073,15 +1084,16 @@ int allowed_ids(const GalleryStore* g, const uint8_t* keep, int** ids, int* na, 
   int* count = nullptr;
   if (int rc = alloc_async(reinterpret_cast<void**>(&count), (2 * static_cast<size_t>(nb) + 1) * sizeof(int), "allowed-row counts", st)) return rc;
   int* start = count + nb;
+  const float* bound = clusterable ? g->bound : nullptr;
   auto run = [&]() -> int {
-    if (int e = launched(launch_k(allowed_count_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, g->n, count), "allowed_count_kernel"))
+    if (int e = launched(launch_k(allowed_count_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, bound, g->n, count), "allowed_count_kernel"))
       return e;
     if (int e = launched(launch_k(allowed_scan_kernel, dim3(1), dim3(1024), 0, st, 1, false, count, nb, start), "allowed_scan_kernel")) return e;
     JIMM_CUDA_CHECK(cudaMemcpyAsync(na, start + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
     JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
     if (*na == 0) return 0;
     if (int e = alloc_async(reinterpret_cast<void**>(ids), static_cast<size_t>(*na) * sizeof(int), "allowed-row ids", st)) return e;
-    return launched(launch_k(allowed_scatter_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, g->n, start, *ids),
+    return launched(launch_k(allowed_scatter_kernel, dim3(nb), dim3(256), 0, st, 1, false, g->live, keep, bound, g->n, start, *ids),
                     "allowed_scatter_kernel");
   };
   const int rc = run();
@@ -1298,11 +1310,12 @@ int gallery_compact(GalleryStore* g, int32_t* old_to_new, cudaStream_t st) {
 namespace {
 
 // gallery_search over the N rows of a view: every stored row (ids null) or the allowed rows ids[0 .. N), whose positions the outputs
-// then hold.
-int search_rows(const GalleryStore* g, const int* ids, int N, const float* queries, int Q, const float* logit_scale, const float* logit_bias,
-                int k, float* values, int32_t* indices, long long* stats, cudaStream_t st) {
+// then hold.  The queries are raw rows, normalised and prepared here, or (qrows non-null) rows already normalised with their fp16 copies
+// and bounds, read through qrows in chunks of kSearchRows.  The first min(N, seed_cols) rows seed each chunk's best k exactly.
+int search_rows(const GalleryStore* g, const int* ids, int N, const float* queries, RowView* qrows, int Q, int seed_cols, const float* logit_scale,
+                const float* logit_bias, int k, float* values, int32_t* indices, long long* stats, cudaStream_t st) {
   const int E = g->E;
-  const int qc = std::min(Q, kSearchRows), seed = std::min(N, kSearchCols);
+  const int qc = std::min(Q, kSearchRows), seed = std::min(N, seed_cols);
   const bool screen = N > seed;
   const long long seed_ld = k + (seed + kSegCols - 1) / kSegCols * static_cast<long long>(k);
   const long long cand_ld = screen ? k + std::max<long long>(kScreenCap, kSearchCols / kSegCols * static_cast<long long>(k)) : seed_ld;
@@ -1311,14 +1324,15 @@ int search_rows(const GalleryStore* g, const int* ids, int N, const float* queri
   size_t off = 0;
   auto piece = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
   const size_t o_cand = piece(static_cast<size_t>(qc) * cand_ld * sizeof(u64));
-  const size_t o_nq = piece(static_cast<size_t>(qc) * E * sizeof(float));
-  const size_t o_block = piece(static_cast<size_t>(qc) * seed * sizeof(float));
+  const size_t o_nq = qrows ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(float));
+  // the seed block, and with a screen the fallback's kSearchCols pieces
+  const size_t o_block = piece(static_cast<size_t>(qc) * (screen ? std::min(N, kSearchCols) : seed) * sizeof(float));
   size_t o_fcand = 0, o_fq = 0, o_hq = 0, o_nbq = 0, o_t = 0, o_cnt = 0, o_ovl = 0, o_list = 0, o_info = 0;
   if (screen) {
     o_fcand = piece(static_cast<size_t>(qc) * fcand_ld * sizeof(u64));
     o_fq = piece(static_cast<size_t>(qc) * E * sizeof(float));
-    o_hq = piece(static_cast<size_t>(qc) * E * sizeof(__half));
-    o_nbq = piece(static_cast<size_t>(qc) * sizeof(float));
+    o_hq = qrows ? 0 : piece(static_cast<size_t>(qc) * E * sizeof(__half));
+    o_nbq = qrows ? 0 : piece(static_cast<size_t>(qc) * sizeof(float));
     o_t = piece(static_cast<size_t>(qc) * sizeof(float));
     o_cnt = piece(static_cast<size_t>(qc) * sizeof(int));
     o_ovl = piece(static_cast<size_t>(qc) * sizeof(int));
@@ -1333,19 +1347,19 @@ int search_rows(const GalleryStore* g, const int* ids, int N, const float* queri
   JIMM_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&base), off, st));
   RowView view{g, ids, N, reinterpret_cast<float*>(base + o_vrows), reinterpret_cast<__half*>(base + o_vhalf), reinterpret_cast<float*>(base + o_vbound)};
   u64* cand = reinterpret_cast<u64*>(base + o_cand);
-  float* nq = reinterpret_cast<float*>(base + o_nq);
+  float* nq = qrows ? nullptr : reinterpret_cast<float*>(base + o_nq);
   float* block = reinterpret_cast<float*>(base + o_block);
   u64* fcand = reinterpret_cast<u64*>(base + o_fcand);
   float* fq = reinterpret_cast<float*>(base + o_fq);
-  __half* hq = reinterpret_cast<__half*>(base + o_hq);
-  float* nbq = reinterpret_cast<float*>(base + o_nbq);
+  __half* hq = qrows ? nullptr : reinterpret_cast<__half*>(base + o_hq);
+  float* nbq = qrows ? nullptr : reinterpret_cast<float*>(base + o_nbq);
   float* t = reinterpret_cast<float*>(base + o_t);
   int* cnt = reinterpret_cast<int*>(base + o_cnt);
   int* ovl = reinterpret_cast<int*>(base + o_ovl);
   int* list = reinterpret_cast<int*>(base + o_list);
   int* info = reinterpret_cast<int*>(base + o_info);
   GemmScreen sd;
-  sd.t = t; sd.nq = nbq; sd.cnt = cnt; sd.list = list; sd.cap = kScreenCap;
+  sd.t = t; sd.cnt = cnt; sd.list = list; sd.cap = kScreenCap;
   const int lo = bit_width(N);
   int rc = 0;
   auto threshold = [&](int qn) -> int {
@@ -1389,11 +1403,19 @@ int search_rows(const GalleryStore* g, const int* ids, int N, const float* queri
   for (int q0 = 0; q0 < Q && rc == 0; q0 += qc) {
     const int qn = std::min(qc, Q - q0);
     const size_t o = static_cast<size_t>(q0) * k;
-    rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
+    if (qrows) {
+      rc = qrows->at(q0, qn, st);
+      nq = qrows->rows;
+      hq = qrows->half;
+      nbq = qrows->bound;
+    } else {
+      rc = l2_normalize_run(queries + static_cast<size_t>(q0) * E, nq, E, qn, E, st);
+    }
     if (rc == 0) rc = view.at(0, seed, st);
     if (rc == 0) rc = block_step(nq, qn, view.rows, seed, 0, E, logit_scale, logit_bias, k, lo, block, cand, cand_ld, true, !screen, values + o, indices + o, st);
     if (!screen) continue;
-    if (rc == 0) rc = prep_rows_run(nq, qn, E, hq, nbq, st);
+    if (rc == 0 && !qrows) rc = prep_rows_run(nq, qn, E, hq, nbq, st);
+    sd.nq = nbq;
     if (rc == 0) rc = threshold(qn);
     for (int g0 = seed; g0 < N && rc == 0; g0 += kScreenCols) rc = screen_chunk(qn, g0);
     if (rc == 0) rc = launch_merge(cand, qn, cand_ld, k, k, lo, nullptr, nullptr, 0, 0, values + o, indices + o, nullptr, st);
@@ -1406,17 +1428,336 @@ int search_rows(const GalleryStore* g, const int* ids, int N, const float* queri
 int gallery_search(const GalleryStore* g, const float* queries, int Q, const float* logit_scale, const float* logit_bias, int k, const uint8_t* keep,
                    float* values, int32_t* indices, long long* stats, cudaStream_t st) {
   if (!keep && g->removed == 0)
-    return search_rows(g, nullptr, static_cast<int>(g->n), queries, Q, logit_scale, logit_bias, k, values, indices, stats, st);
+    return search_rows(g, nullptr, static_cast<int>(g->n), queries, nullptr, Q, kSearchCols, logit_scale, logit_bias, k, values, indices, stats, st);
   // over the allowed rows' positions, then to row ids; with fewer than k of them the slots past the last are padding
   int* ids = nullptr;
   int na = 0;
   if (int rc = allowed_ids(g, keep, &ids, &na, st)) return rc;
-  int rc = na == 0 ? 0 : search_rows(g, ids, na, queries, Q, logit_scale, logit_bias, k, values, indices, stats, st);
+  int rc = na == 0 ? 0 : search_rows(g, ids, na, queries, nullptr, Q, kSearchCols, logit_scale, logit_bias, k, values, indices, stats, st);
   const long long n = static_cast<long long>(Q) * k;
   if (rc == 0 && n > 0)
     rc = launched(launch_k(search_ids_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, 1, false, values, indices, n, ids, na),
                   "search_ids_kernel");
   return ids ? free_scratch(ids, st, rc) : rc;
+}
+
+// ---- k-means: spherical k-means over the clusterable rows (allowed, norm bound <= kClusterBound) ----
+// Assignment is a gallery search at k = 1 with the roles turned: the rows are the queries (already normalised, with fp16 copies and
+// bounds) and the centroids a small gallery, normalised and prepared once per step, seeded exactly by their first kKmeansSeedCols and
+// screened beyond.  Scores are logit_value(1, acc, 0): a device 0.0f as logit_scale (expf(0) = 1) and no bias.  The update sums the rows
+// of each cluster in fixed point, S[j][e] = sum rint(x[e] 2^30) in int64, so every order of the sums gives the same integers, and the
+// mean is fp32(fp64(S) 2^-30 / n_j).
+namespace {
+
+constexpr int kKmeansSeedCols = 256;  // centroids scored exactly before the screen: the threshold's seed
+constexpr int kSumRows = 64;          // sorted rows per CTA of kmeans_sum_kernel
+
+// splitmix64's first output for the state x: the mix of x + the golden-ratio increment.
+__device__ __forceinline__ u64 splitmix64(u64 x) {
+  u64 z = x + 0x9e3779b97f4a7c15ull;
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
+// keys[p] = 1 + (splitmix64(seed + id) >> 41) 2^-23 for the clusterable row id = ids[p] (ids null: p): a float in [1, 2).
+__global__ void __launch_bounds__(256) kmeans_keys_kernel(const int* __restrict__ ids, int na, u64 seed, float* __restrict__ keys) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= na) return;
+  const u64 id = static_cast<u64>(ids ? ids[p] : p);
+  keys[p] = __uint_as_float(0x3f800000u | static_cast<uint32_t>(splitmix64(seed + id) >> 41));
+}
+
+// One warp per cluster j < C: stored row sel[j] (through map when non-null) into m[j], if it is a clusterable row of the n stored rows;
+// otherwise *bad counts it and m[j] is not written.
+__global__ void __launch_bounds__(256) kmeans_gather_kernel(const int* __restrict__ sel, const int* __restrict__ map, int C, const float* __restrict__ rows,
+                                                            const float* __restrict__ bound, const uint32_t* __restrict__ live,
+                                                            const uint8_t* __restrict__ keep, long long n, int E, float* __restrict__ m,
+                                                            int* __restrict__ bad) {
+  const int j = static_cast<int>((static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= C) return;
+  long long id = sel[j];
+  if (map && id >= 0) id = map[id];
+  const bool ok = id >= 0 && id < n && (!live || ((live[id >> 5] >> (id & 31)) & 1u)) && (!keep || keep[id]) && bound[id] <= kClusterBound;
+  if (!ok) {
+    if (lane == 0) atomicAdd(bad, 1);
+    return;
+  }
+  const float4* s = reinterpret_cast<const float4*>(rows + static_cast<size_t>(id) * E);
+  float4* d = reinterpret_cast<float4*>(m + static_cast<size_t>(j) * E);
+  for (int e = lane; e < E / 4; e += 32) d[e] = s[e];
+}
+
+// One warp per centroid j < C of c (l2_normalize of m_new).  If one of its values is not finite: m_old null (the initial centroids), *bad
+// counts it; otherwise the cluster keeps its previous mean and centroid: m_new[j] = m_old[j], c[j] = c_old[j].
+__global__ void __launch_bounds__(256) kmeans_finite_kernel(float* __restrict__ c, int C, int E, float* __restrict__ m_new, const float* __restrict__ m_old,
+                                                            const float* __restrict__ c_old, int* __restrict__ bad) {
+  const int j = static_cast<int>((static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= C) return;
+  const size_t r = static_cast<size_t>(j) * E;
+  bool finite = true;
+  for (int e = lane; e < E; e += 32) finite = finite && isfinite(c[r + e]);
+  if (__all_sync(0xffffffffu, finite)) return;
+  if (!m_old) {
+    if (lane == 0) atomicAdd(bad, 1);
+    return;
+  }
+  for (int e = lane; e < E; e += 32) {
+    m_new[r + e] = m_old[r + e];
+    c[r + e] = c_old[r + e];
+  }
+}
+
+// *changed += the positions p < n where a[p] != b[p].
+__global__ void __launch_bounds__(256) kmeans_changed_kernel(const int32_t* __restrict__ a, const int32_t* __restrict__ b, int n, int* __restrict__ changed) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const int d = __syncthreads_count(p < n && a[p] != b[p]);
+  if (threadIdx.x == 0 && d > 0) atomicAdd(changed, d);
+}
+
+// Called by every lane of the warp: the lanes holding the same cluster j >= 0 add their number to at[j] with one atomic, so a large
+// cluster does not serialise the warp on one address.  Returns this lane's slot: the old at[j] + its rank among those lanes (lanes
+// with j < 0 add nothing).
+template <typename T>
+__device__ __forceinline__ T warp_claim(T* at, int j) {
+  const unsigned peers = __match_any_sync(0xffffffffu, j);
+  const int lane = threadIdx.x & 31, leader = __ffs(peers) - 1;
+  T base = 0;
+  if (lane == leader && j >= 0) base = atomicAdd(at + j, static_cast<T>(__popc(peers)));
+  base = __shfl_sync(peers, base, leader);
+  return base + static_cast<T>(__popc(peers & ((1u << lane) - 1u)));
+}
+
+// n[a[p]] += 1 for each position p < na.
+__global__ void __launch_bounds__(256) kmeans_count_kernel(const int32_t* __restrict__ a, int na, int* __restrict__ n) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  warp_claim(n, p < na ? a[p] : -1);
+}
+
+// Counting sort of the positions by cluster: order[cursor[a[p]]++] = p (cursor starts at each cluster's first slot).
+__global__ void __launch_bounds__(256) kmeans_order_kernel(const int32_t* __restrict__ a, int na, int* __restrict__ cursor, int* __restrict__ order) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const int j = p < na ? a[p] : -1;
+  const int slot = warp_claim(cursor, j);
+  if (j >= 0) order[slot] = p;
+}
+
+// S[j][e] += rint(x[e] 2^30) over the rows x of cluster j, for kSumRows positions of order per CTA (sorted by cluster): each thread sums
+// its elements of a run of one cluster in an int64 and adds it with one atomic when the cluster changes.  x[e] 2^30 is exact (a power
+// of two scaling) and |x[e]| <= 2, so each term fits 32 bits and each sum stays below 2^62; integer sums do not depend on their order.
+__global__ void __launch_bounds__(256) kmeans_sum_kernel(const int* __restrict__ order, const int32_t* __restrict__ a, const int* __restrict__ ids,
+                                                         const float* __restrict__ rows, int E, int na, unsigned long long* __restrict__ S) {
+  __shared__ int srow[kSumRows], sj[kSumRows];
+  const int r0 = blockIdx.x * kSumRows, nr = min(kSumRows, na - r0);
+  for (int r = threadIdx.x; r < nr; r += blockDim.x) {
+    const int p = order[r0 + r];
+    sj[r] = a[p];
+    srow[r] = ids ? ids[p] : p;
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    long long acc = 0;
+    int cur = sj[0];
+    for (int r = 0; r < nr; ++r) {
+      if (sj[r] != cur) {
+        atomicAdd(S + static_cast<size_t>(cur) * E + e, static_cast<unsigned long long>(acc));
+        acc = 0;
+        cur = sj[r];
+      }
+      acc += __float2ll_rn(rows[static_cast<size_t>(srow[r]) * E + e] * 0x1p30f);
+    }
+    atomicAdd(S + static_cast<size_t>(cur) * E + e, static_cast<unsigned long long>(acc));
+  }
+}
+
+// m_new = fp32_rn(fp64_rn(S) 2^-30 / fp64(n_j)) for the clusters with rows; the others keep m_old.
+__global__ void __launch_bounds__(256) kmeans_mean_kernel(const long long* __restrict__ S, const int* __restrict__ n, const float* __restrict__ m_old,
+                                                          float* __restrict__ m_new, int C, int E) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(C) * E) return;
+  const int cnt = n[i / E];
+  m_new[i] = cnt > 0 ? __double2float_rn(__ddiv_rn(__ll2double_rn(S[i]) * 0x1p-30, static_cast<double>(cnt))) : m_old[i];
+}
+
+// Every stored row r < n: assign -1, score -inf (the rows that take no part keep these).
+__global__ void __launch_bounds__(256) kmeans_clear_kernel(int32_t* __restrict__ assign, float* __restrict__ scores, long long n) {
+  const long long r = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  assign[r] = -1;
+  scores[r] = -INFINITY;
+}
+
+// Position p < na to its row id = ids[p] (ids null: p): assign and score, and counts[a[p]] += 1.
+__global__ void __launch_bounds__(256) kmeans_out_kernel(const int32_t* __restrict__ a, const float* __restrict__ v, const int* __restrict__ ids, int na,
+                                                         int32_t* __restrict__ assign, float* __restrict__ scores, unsigned long long* __restrict__ counts) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const int j = p < na ? a[p] : -1;
+  warp_claim(counts, j);
+  if (j < 0) return;
+  const int id = ids ? ids[p] : p;
+  assign[id] = j;
+  scores[id] = v[p];
+}
+
+unsigned blocks_of(long long n, int per) { return static_cast<unsigned>((n + per - 1) / per); }
+
+}  // namespace
+
+int gallery_kmeans(const GalleryStore* g, int C, const float* init_vectors, const int32_t* init_ids, unsigned long long seed, int iters,
+                   const uint8_t* keep, float* centroids, int32_t* assign, float* scores, int64_t* counts, int* iterations, long long* stats,
+                   cudaStream_t st) {
+  const int E = g->E;
+  const long long rows = g->n;
+  const bool sampled = !init_vectors && !init_ids;
+  // the clusterable rows' ids; when that is every stored row, positions are row ids and the rows are read in place
+  int* ids = nullptr;
+  int na = 0;
+  if (int rc = allowed_ids(g, keep, &ids, &na, st, true)) return rc;
+  if (ids && na == rows) {
+    cudaFreeAsync(ids, st);
+    ids = nullptr;
+  }
+  if (sampled && C > na) {
+    set_last_error("index kmeans: %d clusters sampled from %d clusterable rows", C, na);
+    return ids ? free_scratch(ids, st, JIMM_EINVAL) : JIMM_EINVAL;
+  }
+  const size_t CE = static_cast<size_t>(C) * E, NA = static_cast<size_t>(na);
+  const int qc = std::min(std::max(na, 1), kSearchRows);
+  size_t off = 0;
+  auto piece = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
+  const size_t o_S = piece(CE * sizeof(long long));
+  const size_t o_m = piece(2 * CE * sizeof(float));
+  const size_t o_c = piece(2 * CE * sizeof(float));
+  const size_t o_ch = piece(CE * sizeof(__half));
+  const size_t o_cb = piece(static_cast<size_t>(C) * sizeof(float));
+  const size_t o_n = piece((3 * static_cast<size_t>(C) + 1) * sizeof(int));  // n [C], start [C + 1], cursor [C]
+  const size_t o_a = piece(2 * NA * sizeof(int32_t));
+  const size_t o_v = piece(NA * sizeof(float));
+  const size_t o_ord = piece(NA * sizeof(int));
+  const size_t o_keys = piece(sampled ? NA * sizeof(float) : 0);
+  const size_t o_sel = piece(sampled ? 2 * static_cast<size_t>(C) * sizeof(int) : 0);
+  const size_t o_qr = piece(ids ? static_cast<size_t>(qc) * E * sizeof(float) : 0);
+  const size_t o_qh = piece(ids ? static_cast<size_t>(qc) * E * sizeof(__half) : 0);
+  const size_t o_qb = piece(ids ? static_cast<size_t>(qc) * sizeof(float) : 0);
+  const size_t o_info = piece(4 * sizeof(int));  // zero (the logit_scale 0.0f), bad ids, bad vectors, changed
+  uint8_t* base = nullptr;
+  if (int rc = alloc_async(reinterpret_cast<void**>(&base), off, "k-means scratch", st)) return ids ? free_scratch(ids, st, rc) : rc;
+  long long* S = reinterpret_cast<long long*>(base + o_S);
+  float* m[2] = {reinterpret_cast<float*>(base + o_m), reinterpret_cast<float*>(base + o_m) + CE};
+  float* c[2] = {reinterpret_cast<float*>(base + o_c), reinterpret_cast<float*>(base + o_c) + CE};
+  __half* ch = reinterpret_cast<__half*>(base + o_ch);
+  float* cb = reinterpret_cast<float*>(base + o_cb);
+  int* n = reinterpret_cast<int*>(base + o_n);
+  int* start = n + C;
+  int* cursor = start + C + 1;
+  int32_t* abuf = reinterpret_cast<int32_t*>(base + o_a);
+  float* vals = reinterpret_cast<float*>(base + o_v);
+  int* order = reinterpret_cast<int*>(base + o_ord);
+  float* keys = reinterpret_cast<float*>(base + o_keys);
+  int* sel = reinterpret_cast<int*>(base + o_sel);
+  int* info = reinterpret_cast<int*>(base + o_info);
+  const float* zero = reinterpret_cast<const float*>(info);
+  RowView qv{g, ids, na, reinterpret_cast<float*>(base + o_qr), reinterpret_cast<__half*>(base + o_qh), reinterpret_cast<float*>(base + o_qb)};
+  auto run = [&]() -> int {
+    JIMM_CUDA_CHECK(cudaMemsetAsync(info, 0, 4 * sizeof(int), st));
+    // m_0 and c_0, checked on the device
+    if (init_vectors) {
+      JIMM_CUDA_CHECK(cudaMemcpyAsync(m[0], init_vectors, CE * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    } else {
+      const int* from = init_ids;
+      const int* map = nullptr;
+      if (sampled) {  // the rows at the positions of top_k(keys, C), ties to the larger position
+        if (int e = launched(launch_k(kmeans_keys_kernel, dim3(blocks_of(na, 256)), dim3(256), 0, st, 1, false, ids, na, seed, keys),
+                             "kmeans_keys_kernel"))
+          return e;
+        if (int e = topk_run(keys, 1, na, na, C, reinterpret_cast<float*>(sel + C), sel, nullptr, st)) return e;
+        from = sel;
+        map = ids;
+      }
+      if (int e = launched(launch_k(kmeans_gather_kernel, dim3(blocks_of(C, 8)), dim3(256), 0, st, 1, false, from, map, C, g->rows, g->bound, g->live,
+                                    keep, rows, E, m[0], info + 1),
+                           "kmeans_gather_kernel"))
+        return e;
+    }
+    if (int e = l2_normalize_run(m[0], c[0], E, C, E, st)) return e;
+    if (int e = launched(launch_k(kmeans_finite_kernel, dim3(blocks_of(C, 8)), dim3(256), 0, st, 1, false, c[0], C, E, nullptr, nullptr, nullptr,
+                                  info + 2),
+                         "kmeans_finite_kernel"))
+      return e;
+    int h[2];
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(h, info + 1, sizeof(h), cudaMemcpyDeviceToHost, st));
+    JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (h[0] != 0) {
+      set_last_error("index kmeans: %d of %d init ids are not clusterable rows (live, kept, finite and not zero)", h[0], C);
+      return JIMM_EINVAL;
+    }
+    if (h[1] != 0) {
+      set_last_error("index kmeans: %d of %d initial centroids have a non-finite l2_normalize", h[1], C);
+      return JIMM_EINVAL;
+    }
+    int cur = 0, t = 0;
+    for (;; ++t) {
+      int32_t* a = abuf + (t & 1) * NA;
+      int32_t* prev = abuf + ((t + 1) & 1) * NA;
+      if (int e = prep_rows_run(c[cur], C, E, ch, cb, st)) return e;
+      GalleryStore cs;
+      cs.E = E; cs.n = C; cs.cap = C; cs.rows = c[cur]; cs.half = ch; cs.bound = cb;
+      if (na > 0)
+        if (int e = search_rows(&cs, nullptr, C, nullptr, &qv, na, kKmeansSeedCols, zero, nullptr, 1, vals, a, stats, st)) return e;
+      if (t + 1 == iters) break;
+      if (t > 0) {
+        int changed = 0;
+        if (na > 0 && launched(launch_k(kmeans_changed_kernel, dim3(blocks_of(na, 256)), dim3(256), 0, st, 1, false, a, prev, na, info + 3),
+                               "kmeans_changed_kernel"))
+          return JIMM_ECUDA;
+        JIMM_CUDA_CHECK(cudaMemcpyAsync(&changed, info + 3, sizeof(int), cudaMemcpyDeviceToHost, st));
+        JIMM_CUDA_CHECK(cudaMemsetAsync(info + 3, 0, sizeof(int), st));
+        JIMM_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (changed == 0) break;  // the next means would be these bits again
+      }
+      // m_{t+1}: the rows sorted by cluster (counting sort), summed in fixed point, divided; c_{t+1} = l2_normalize(m_{t+1}), and a
+      // cluster whose new centroid is not finite keeps m_t and c_t
+      JIMM_CUDA_CHECK(cudaMemsetAsync(n, 0, static_cast<size_t>(C) * sizeof(int), st));
+      JIMM_CUDA_CHECK(cudaMemsetAsync(S, 0, CE * sizeof(long long), st));
+      if (na > 0) {
+        if (int e = launched(launch_k(kmeans_count_kernel, dim3(blocks_of(na, 256)), dim3(256), 0, st, 1, false, a, na, n), "kmeans_count_kernel")) return e;
+        if (int e = launched(launch_k(allowed_scan_kernel, dim3(1), dim3(1024), 0, st, 1, false, n, C, start), "allowed_scan_kernel")) return e;
+        JIMM_CUDA_CHECK(cudaMemcpyAsync(cursor, start, static_cast<size_t>(C) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        if (int e = launched(launch_k(kmeans_order_kernel, dim3(blocks_of(na, 256)), dim3(256), 0, st, 1, false, a, na, cursor, order), "kmeans_order_kernel"))
+          return e;
+        if (int e = launched(launch_k(kmeans_sum_kernel, dim3(blocks_of(na, kSumRows)), dim3(256), 0, st, 1, false, order, a, ids, g->rows, E, na,
+                                      reinterpret_cast<unsigned long long*>(S)),
+                             "kmeans_sum_kernel"))
+          return e;
+      }
+      if (int e = launched(launch_k(kmeans_mean_kernel, dim3(blocks_of(static_cast<long long>(CE), 256)), dim3(256), 0, st, 1, false, S, n, m[cur],
+                                    m[cur ^ 1], C, E),
+                           "kmeans_mean_kernel"))
+        return e;
+      if (int e = l2_normalize_run(m[cur ^ 1], c[cur ^ 1], E, C, E, st)) return e;
+      if (int e = launched(launch_k(kmeans_finite_kernel, dim3(blocks_of(C, 8)), dim3(256), 0, st, 1, false, c[cur ^ 1], C, E, m[cur ^ 1], m[cur],
+                                    c[cur], info + 2),
+                           "kmeans_finite_kernel"))
+        return e;
+      cur ^= 1;
+    }
+    // the outputs: c_t, a_t scattered to row ids, counts of a_t
+    int32_t* a = abuf + (t & 1) * NA;
+    JIMM_CUDA_CHECK(cudaMemcpyAsync(centroids, c[cur], CE * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    JIMM_CUDA_CHECK(cudaMemsetAsync(counts, 0, static_cast<size_t>(C) * sizeof(int64_t), st));
+    if (rows > 0 && launched(launch_k(kmeans_clear_kernel, dim3(blocks_of(rows, 256)), dim3(256), 0, st, 1, false, assign, scores, rows),
+                             "kmeans_clear_kernel"))
+      return JIMM_ECUDA;
+    if (na > 0 && launched(launch_k(kmeans_out_kernel, dim3(blocks_of(na, 256)), dim3(256), 0, st, 1, false, a, vals, ids, na, assign, scores,
+                                    reinterpret_cast<unsigned long long*>(counts)),
+                           "kmeans_out_kernel"))
+      return JIMM_ECUDA;
+    *iterations = t + 1;
+    return 0;
+  };
+  const int rc = run();
+  if (ids) cudaFreeAsync(ids, st);
+  return free_scratch(base, st, rc);
 }
 
 }  // namespace jimm
